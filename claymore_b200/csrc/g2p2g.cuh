@@ -36,11 +36,14 @@
 
 namespace cb200 {
 
+// Launch shape.  Measured on one H100 80GB HBM3 SXM (400 W limit) on the 40 M-particle two-sphere scene, g2p2g ms per sub-step:
+// 192 threads x 4 CTAs/SM (80 registers, no spills) 4.0-4.1; 192 x 3 (96 registers) 4.4; 256 x 3 (80) 4.25; 256 x 4 (64, spills) 4.85.
+// The kernel is latency bound: with the spills gone, warps in flight win.
 #ifndef CB200_G2P2G_THREADS
 #define CB200_G2P2G_THREADS 192
 #endif
 #ifndef CB200_G2P2G_MIN_CTAS
-#define CB200_G2P2G_MIN_CTAS 4  // the kernel is latency bound: warps in flight beat spill-free registers
+#define CB200_G2P2G_MIN_CTAS 4
 #endif
 constexpr int kG2P2GThreads = CB200_G2P2G_THREADS;  // >= 192 = 64 cells x 3 stencil slices in phase 2
 static_assert(kG2P2GThreads >= 192 && kG2P2GThreads % 32 == 0, "phase 2 maps one thread to (cell, slice)");
@@ -106,6 +109,13 @@ struct G2P2GSmem {
 // Staged records are XOR-swizzled: cell-major buckets put the p-th particles of consecutive cells 8 slots = 128 B apart,
 // i.e. in the same four banks; unswizzled, phase 2 spent 3-5 wavefronts per 16-byte read (profiles/r01_final_*).
 __device__ __forceinline__ int rec_slot(int slot) { return slot ^ ((slot >> 3) & 7); }
+// threadIdx.x through a volatile read the compiler cannot move: values derived from it are computed where they are used
+// instead of being hoisted out of the block loop (where, at 80 registers, they end up on the stack)
+__device__ __forceinline__ int opaque_tid() {
+	int t;
+	asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+	return t;
+}
 constexpr int kRecMover = 1 << 30;
 constexpr int kRecDrop = 1 << 29;
 
@@ -131,7 +141,6 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 	                                                                // before anything is staged in quads 1-3 of the records
 
 	const Cfg& cfg = a.cfg;
-	const int tid = threadIdx.x;
 	float dt = a.dt, new_dt = a.new_dt;
 	int nblocks = a.block_count;
 	if(a.state) {
@@ -140,12 +149,12 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 		nblocks = a.state->pbc;
 	}
 	if(a.block_list) nblocks = *a.list_count;
-	if(tid == 0) {
+	if(threadIdx.x == 0) {
 		mbar_init(bar, 1);
 		mbar_fence_init();
 		sm.nmovers = 0;
 	}
-	if(tid < 64) sm.cnt[tid] = 0;
+	if(threadIdx.x < 64) sm.cnt[threadIdx.x] = 0;
 	__syncthreads();
 	unsigned phase = 0;
 	const float dx = cfg.dx, dx_inv = cfg.dx_inv, d_inv = cfg.d_inv;
@@ -156,7 +165,7 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 	// atomic's round trip hides behind a whole block, and the queue shift rides on the flush barrier of the block before.
 	// Barriers per (single-chunk) block: S1, S2, B1, B2, two for the arena rounds, B6.
 	int q_pending = 0;
-	if(tid == 0) {
+	if(threadIdx.x == 0) {
 		if(a.work_counter) {
 			sm.cur_blk = atomicAdd(a.work_counter, 1);
 			sm.next_blk = atomicAdd(a.work_counter, 1);
@@ -167,6 +176,7 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 	}
 	__syncthreads();
 	for(;;) {
+		const int tid = opaque_tid();  // (not loop-invariant to the compiler: see opaque_tid)
 		const int qi = sm.cur_blk, qn = sm.next_blk;  // published by the last barrier every thread passed
 		if(qi >= nblocks) break;
 		if(tid == 0) q_pending = a.work_counter ? atomicAdd(a.work_counter, 1) : qn + (int) gridDim.x;
@@ -581,11 +591,14 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				acc_dirty = false;
 			}
 			__syncthreads();  // B1: records, cell counts and the mover list of this chunk are complete; the arena is zero
-			const int lane = tid & 31;
 			// ================= phase 2: cell-parallel accumulation =====================================
-			// thread = (home cell hc, x-slice sl of its 3x3x3 stencil); a half-warp holds the 16 cells of one x-plane
-			const int wrp = tid >> 5;
-			const bool p2 = tid < 192;
+			// thread = (home cell hc, x-slice sl of its 3x3x3 stencil); a half-warp holds the 16 cells of one x-plane.
+			// The thread's cell, weight polynomial and nine arena offsets are derived from a fresh read of the thread index (see
+			// opaque_tid), so they are computed here instead of being kept in registers or on the stack since earlier.
+			const int ptid = opaque_tid();
+			const int lane = ptid & 31;
+			const int wrp = ptid >> 5;
+			const bool p2 = ptid < 192;
 			// warp: (cx, sl) of lanes 0-15 / lanes 16-31 -> node plane X = cx + sl + 1
 			//   w0: (1,0) (0,1) -> 2 2    w1: (2,0) (1,1) -> 3 3    w2: (3,0) (2,1) -> 4 4    w3: (3,1) (2,2) -> 5 5
 			//   w4: (0,0) (3,2) -> 1 6    w5: (0,2) (1,2) -> 3 4
@@ -631,94 +644,99 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				float pa, pb, pc;
 				bspline_poly(sl, pa, pb, pc);
 				const float fi = (float) sl;
-				// accumulators as packed pairs: (mass, momentum x), (momentum y, momentum z) of the 9 nodes of this x-slice
-				f2 acc01[9], acc23[9];
+				// accumulators of the 9 nodes (j, k) of this x-slice: sum of W (times the particle mass at the write-back) and the
+				// three momentum channels
+				float acc[9][4];
 #pragma unroll
-				for(int n9 = 0; n9 < 9; ++n9) acc01[n9] = acc23[n9] = mk2(0.f, 0.f);
-				const f2 c01 = mk2(0.f, 1.f);
+				for(int n9 = 0; n9 < 9; ++n9) acc[n9][0] = acc[n9][1] = acc[n9][2] = acc[n9][3] = 0.f;
 				for(int p = 0; p < n; ++p) {  // (requesting the next particle's index / first quad one iteration ahead measured 0.8 % slower)
 					const int slot = SORTED ? rec_slot(st + p) : (int) sm.idx[st + p];
 					const float4 r0 = sm.rec[0][slot];  // (y, z, x, code)
 					if(__float_as_int(r0.w) & (kRecMover | kRecDrop)) continue;
 					const float4 r1 = sm.rec[1][slot], r2 = sm.rec[2][slot], r3 = sm.rec[3][slot];
-					const float wx = pa + r0.z * (pb + pc * r0.z);
-					// B-spline weights of y and z in one packed pass: wyz[i] = (w_y[i], w_z[i])
-					f2 wyz[3];
-					{
-						const f2 d = mk2(r0.x, r0.y);
-						const f2 e = add2(dup2(1.5f), mul2(d, -1.f));
-						wyz[0] = mul2(mul2(e, e), 0.5f);
-						const f2 g = add2(d, dup2(-1.f));
-						wyz[1] = fma2(mul2(g, -1.f), g, dup2(0.75f));
-						const f2 h = add2(g, dup2(0.5f));
-						wyz[2] = mul2(mul2(h, h), 0.5f);
+					// B-spline weights as polynomials in the local position: two FMA each, with immediates for y and z
+					const float wx = fmaf(fmaf(pc, r0.z, pb), r0.z, pa);
+					float wy[3], wz[3];
+#pragma unroll
+					for(int i = 0; i < 3; ++i) {
+						float qa, qb, qc;
+						bspline_poly(i, qa, qb, qc);
+						wy[i] = fmaf(fmaf(qc, r0.x, qb), r0.x, qa);
+						wz[i] = fmaf(fmaf(qc, r0.y, qb), r0.y, qa);
 					}
-					// (1, momentum x) and (momentum y, momentum z) at node (sl, 0, 0) of the stencil
-					f2 a0 = mk2(1.f, fmaf(fi, r3.y, r3.x));
-					f2 b0 = fma2(mk2(r1.z, r1.w), fi, mk2(r1.x, r1.y));
+					// momentum at node (sl, j, k) of the stencil: q + sl D[:,0] + j D[:,1] + k D[:,2], walked by additions
+					float bx = fmaf(fi, r3.y, r3.x), by = fmaf(fi, r1.z, r1.x), bz = fmaf(fi, r1.w, r1.y);
 #pragma unroll
 					for(int j = 0; j < 3; ++j) {
-						const float wxy = wx * wyz[j].x;
-						f2 ak = a0, bk = b0;
+						const float wxy = wx * wy[j];
+						float px = bx, py = by, pz = bz;
 #pragma unroll
 						for(int k = 0; k < 3; ++k) {
-							const float W = wxy * wyz[k].y;
-							acc01[j * 3 + k] = fma2(ak, W, acc01[j * 3 + k]);
-							acc23[j * 3 + k] = fma2(bk, W, acc23[j * 3 + k]);
+							const float W = wxy * wz[k];
+							float* an = acc[j * 3 + k];
+							an[0] += W;
+							an[1] = fmaf(px, W, an[1]);
+							an[2] = fmaf(py, W, an[2]);
+							an[3] = fmaf(pz, W, an[3]);
 							if(k < 2) {
-								ak = fma2(c01, r3.w, ak);
-								bk = add2(bk, mk2(r2.z, r2.w));
+								px += r3.w;
+								py += r2.z;
+								pz += r2.w;
 							}
 						}
 						if(j < 2) {
-							a0 = fma2(c01, r3.z, a0);
-							b0 = add2(b0, mk2(r2.x, r2.y));
+							bx += r3.z;
+							by += r2.x;
+							bz += r2.y;
 						}
 					}
 				}
-				float acc[9][4];
-#pragma unroll
-				for(int n9 = 0; n9 < 9; ++n9) acc[n9][0] = acc01[n9].x, acc[n9][1] = acc01[n9].y, acc[n9][2] = acc23[n9].x, acc[n9][3] = acc23[n9].y;
 				// Registers -> arena by plain read-add-write, no atomics (a shared float atomicAdd is a compare-and-swap loop: 36 per
 				// thread were 60 % of the kernel's shared-memory wavefronts).  All lanes of a warp execute the same stencil offset
 				// (j, k) on different cells, i.e. on different nodes, and a thread only writes the node plane X of its slice, so
 				// warps (half-warps) that own different planes never meet; the rest is ordered by rounds.
+				// Round 0: w0-w3 (both halves hold the same plane: exchange by shuffle, lanes 0-15 add channels 0-1, lanes 16-31
+				// channels 2-3) and w4 (planes 1 and 6, all four channels per lane); round 1: w5 (planes 3 and 4).  The rounds are
+				// straight-line code: in a loop the accumulators of every warp stay live across its back-edge and spill.
 				const int X = (hc >> 4) + 1 + sl, Y = ((hc >> 2) & 3) + 1, Z = (hc & 3) + 1;
 				const int ox = acc_off_x(X);
-				// round 0: w0-w3 (both halves hold the same plane: exchange by shuffle, lanes 0-15 add channels 0-1, lanes 16-31
-				// channels 2-3) and w4 (planes 1 and 6, all four channels per lane); round 1: w5 (planes 3 and 4)
-#pragma unroll 1
-				for(int round = 0; round < 2; ++round) {
-					if(p2 && round == (wrp == 5)) {
-						const bool pair = wrp < 4;
+				// (the __syncwarp orders a lane's write of one node before another lane's read of it at the next stencil offset)
+				auto add_quad = [&]() {  // all four channels of this thread's nodes
 #pragma unroll
-						for(int j = 0; j < 3; ++j) {
-							const int oxy = ox + acc_off_y(Y + j);
+					for(int j = 0; j < 3; ++j)
 #pragma unroll
-							for(int k = 0; k < 3; ++k) {
-								const int o = oxy + acc_off_z(Z + k);
-								const float v0 = mass * acc[j * 3 + k][0], v1 = acc[j * 3 + k][1], v2 = acc[j * 3 + k][2], v3 = acc[j * 3 + k][3];
-								if(pair) {
-									// partner = same (cy, cz), the other (cx, sl) of this plane: same node
-									const float ra = __shfl_xor_sync(0xffffffffu, hi ? v0 : v2, 16), rb = __shfl_xor_sync(0xffffffffu, hi ? v1 : v3, 16);
-									const int oc = o + (hi ? 128 : 0);
-									const float sa = (hi ? v2 : v0) + ra, sb = (hi ? v3 : v1) + rb;
-									const float m0 = sm.acc[oc], m1 = sm.acc[oc + 64];
-									sm.acc[oc] = m0 + sa;
-									sm.acc[oc + 64] = m1 + sb;
-								} else if(n > 0) {
-									const float m0 = sm.acc[o], m1 = sm.acc[o + 64], m2 = sm.acc[o + 128], m3 = sm.acc[o + 192];
-									sm.acc[o] = m0 + v0;
-									sm.acc[o + 64] = m1 + v1;
-									sm.acc[o + 128] = m2 + v2;
-									sm.acc[o + 192] = m3 + v3;
-								}
-								__syncwarp();
+						for(int k = 0; k < 3; ++k) {
+							if(n > 0) {
+								const int o = ox + acc_off_y(Y + j) + acc_off_z(Z + k);
+								const float m0 = sm.acc[o], m1 = sm.acc[o + 64], m2 = sm.acc[o + 128], m3 = sm.acc[o + 192];
+								sm.acc[o] = fmaf(mass, acc[j * 3 + k][0], m0);
+								sm.acc[o + 64] = m1 + acc[j * 3 + k][1];
+								sm.acc[o + 128] = m2 + acc[j * 3 + k][2];
+								sm.acc[o + 192] = m3 + acc[j * 3 + k][3];
 							}
+							__syncwarp();
 						}
-					}
-					__syncthreads();
+				};
+				if(wrp < 4) {
+#pragma unroll
+					for(int j = 0; j < 3; ++j)
+#pragma unroll
+						for(int k = 0; k < 3; ++k) {
+							// partner = same (cy, cz), the other (cx, sl) of this plane: same node
+							const float v0 = mass * acc[j * 3 + k][0], v1 = acc[j * 3 + k][1], v2 = acc[j * 3 + k][2], v3 = acc[j * 3 + k][3];
+							const float ra = __shfl_xor_sync(0xffffffffu, hi ? v0 : v2, 16), rb = __shfl_xor_sync(0xffffffffu, hi ? v1 : v3, 16);
+							const int oc = ox + acc_off_y(Y + j) + acc_off_z(Z + k) + (hi ? 128 : 0);
+							const float m0 = sm.acc[oc], m1 = sm.acc[oc + 64];
+							sm.acc[oc] = m0 + ((hi ? v2 : v0) + ra);
+							sm.acc[oc + 64] = m1 + ((hi ? v3 : v1) + rb);
+							__syncwarp();
+						}
+				} else if(wrp == 4) {
+					add_quad();
 				}
+				__syncthreads();
+				if(wrp == 5) add_quad();
+				__syncthreads();
 			}
 			// ================= phase 3: particles that changed cell, node-parallel ====================
 			{

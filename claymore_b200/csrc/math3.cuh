@@ -13,17 +13,17 @@ namespace cb200 {
 
 // ------------------------------------------------------------------------------------------------
 // FP32 pairs.  The separable-weight arithmetic of G2P / P2G and the packed 3x3 form carry aligned pairs of values; sm_90a
-// has no packed FP32 FMA, so each pair operation is two scalar FFMA / FMUL / FADD, each rounded once (the _rn forms keep
-// the compiler from contracting a multiply and an add into one FMA).
+// has no packed FP32 FMA, so each pair operation is two scalar FFMA / FMUL / FADD, and the compiler is free to contract a
+// multiply and a following add into one FFMA like any other scalar code.
 // ------------------------------------------------------------------------------------------------
 using f2 = float2;
 __device__ __forceinline__ f2 mk2(float a, float b) { return make_float2(a, b); }
 __device__ __forceinline__ f2 dup2(float a) { return make_float2(a, a); }
 __device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ f2 fma2(f2 a, float s, f2 c) { return make_float2(fmaf(a.x, s, c.x), fmaf(a.y, s, c.y)); }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
-__device__ __forceinline__ f2 mul2(f2 a, float s) { return make_float2(__fmul_rn(a.x, s), __fmul_rn(a.y, s)); }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+__device__ __forceinline__ f2 mul2(f2 a, float s) { return make_float2(a.x * s, a.y * s); }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 
 // quadratic B-spline weights of the 3 nodes covering local position p in [0.5dx, 1.5dx)
 __device__ __forceinline__ void bspline_weights(float p_times_dxinv, float& w0, float& w1, float& w2) {
