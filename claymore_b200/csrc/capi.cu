@@ -104,8 +104,6 @@ int cb200_g2p2g(const cb200_config* c, float dt, float new_dt, int pbc, cb200_pa
 	a.dt = dt;
 	a.new_dt = new_dt;
 	a.block_count = pbc;
-	a.halo_mode = 0;
-	a.halo_marks = nullptr;
 	a.n_models = 1;
 	a.m[0].cur = view(cur);
 	a.m[0].next = view(next);
@@ -118,8 +116,6 @@ int cb200_g2p2g(const cb200_config* c, float dt, float new_dt, int pbc, cb200_pa
 	a.next_grid = next_grid;
 	a.error = nullptr;
 	a.work_counter = nullptr;
-	a.block_list = nullptr;
-	a.list_count = nullptr;
 	return (int) launch_g2p2g(cur.material, a, pbc, (cudaStream_t) stream);
 }
 

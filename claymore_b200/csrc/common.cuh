@@ -101,9 +101,7 @@ struct StepState {
 	int pbc, nbc, ebc;      // counts of the CURRENT partition: particle / +neighbour / +exterior blocks
 	int prev_nbc;           // neighbour count of the partition the next-grid is indexed by
 	int prev_ebc;
-	int work_counter;       // dynamic block scheduler of g2p2g
-	int work_counter2;
-	int work_counter_mat[4];  // one block queue per material launch of a sub-step (all zeroed when the state rolls)
+	int work_counter_mat[4];  // dynamic block queue of g2p2g, one per material launch of a sub-step (all zeroed when the state rolls)
 	int error;              // sticky error bits (see cb200_sim_stats)
 	float dt, next_dt;
 	float max_vel_sq;       // max |v|^2 as float bits (non-negative => int compare is order preserving)
@@ -111,7 +109,6 @@ struct StepState {
 	float frame_time;       // seconds per frame (0 = no clamp)
 	float dt_default;
 	int bin_count[kMaxModels];
-	int halo_count;
 	long long steps;
 	int done_counter;       // CTAs of a launch that have finished ("last CTA does the epilogue"; zero between launches)
 	int frame_roll;         // cb200_sim_step with fps > 0: restart the frame clock on the device when a frame is complete (the

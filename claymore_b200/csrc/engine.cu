@@ -25,56 +25,6 @@
 #include "partition.cuh"
 
 namespace cb200 {
-// mark_overlapping_blocks for every peer (mgsp_tag_kernel) with the end-of-step bookkeeping in its last CTA: global max |v|^2,
-// the halo epoch of this sub-step, the roll of the device-resident step state (finalize_step) and the reset of this rank's
-// local maximum for the next carry.  One launch instead of tag + halo statistics + finalize.
-__global__ void __launch_bounds__(256) mgsp_tag_finalize_kernel(Cfg cfg, MgspView v, const int* table, int* overlap_marks, const int* key_limit, float* local_max_vel, float* global_max_vel, FinalizeArgs fin) {
-	const int limit = *key_limit;
-	float gmax = *local_max_vel;
-	const int epoch = v.epochs[2] + 1, par = epoch & 1;
-	for(int p = 0; p < v.world; ++p) {
-		if(p == v.rank) continue;
-		unsigned char* seg = seg_of(v, v.rank, par, p);
-		InboxHeader* hd = reinterpret_cast<InboxHeader*>(seg);
-		if(threadIdx.x == 0) wait_flag(&hd->flag_keys, epoch);
-		__syncthreads();
-		const int n = *reinterpret_cast<volatile int*>(&hd->key_count);
-		gmax = fmaxf(gmax, *reinterpret_cast<volatile float*>(&hd->max_vel_sq));
-		const int* rk = reinterpret_cast<const int*>(seg + v.L.off_keys);
-		int* outk = v.overlap_keys + (size_t) p * v.L.max_blocks * 3;
-		for(int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-			const int x = rk[3 * i], y = rk[3 * i + 1], z = rk[3 * i + 2];
-			const int bno = table_query(cfg, table, x, y, z);
-			if(bno >= 0 && bno < limit) {
-				atomicOr(overlap_marks + bno, 1 << p);
-				v.peer_bno[(size_t) p * v.L.max_blocks + bno] = i;  // the peer's keys arrive in its block order
-				const int h = atomicAdd(&v.overlap_count[p], 1);
-				if(h < v.L.max_blocks) {
-					outk[3 * h] = x;
-					outk[3 * h + 1] = y;
-					outk[3 * h + 2] = z;
-				}
-			}
-		}
-	}
-	__syncthreads();
-	__shared__ int s_last;
-	if(threadIdx.x == 0) {
-		__threadfence();
-		s_last = atomicAdd(&v.done[3], 1) == (int) gridDim.x - 1;
-	}
-	__syncthreads();
-	if(s_last && threadIdx.x == 0) {
-		__threadfence();
-		v.done[3] = 0;
-		v.epochs[2] = epoch;
-		v.epochs[1] = v.epochs[1] + 1;  // the halo ("my reductions have landed") epoch of this sub-step: published behind g2p2g, awaited by the carry
-		*global_max_vel = gmax;         // every CTA saw every header; the last one publishes
-		finalize_step(fin);             // reads *global_max_vel through fin.next_max_vel
-		*local_max_vel = 0.f;           // for the next sub-step's carry
-	}
-}
-
 int num_sms();
 cudaError_t launch_g2p2g(int material, const G2P2GArgs& a, int block_hint, cudaStream_t s);
 void g2p2g_prepare_all();
@@ -259,14 +209,9 @@ struct cb200_sim {
 	InboxLayout inbox_layout {};
 	unsigned char* inbox_local = nullptr;
 	unsigned char* inbox_peer[kMaxRanks] = {};
-	bool inbox_opened[kMaxRanks] = {};
 	bool peers_ready = false;
-	int* halo_list[2] = {nullptr, nullptr};      // per partition: block numbers of halo / interior particle blocks
-	int* interior_list[2] = {nullptr, nullptr};
-	int* interior_count[2] = {nullptr, nullptr};
 	int* peer_bno = nullptr;                 // [world][max_blocks]
 	float* grid1_peer[kMaxRanks] = {};       // every rank's next grid mapped here (fused remote halo reduction)
-	bool grid1_opened[kMaxRanks] = {};
 	int* mgsp_done = nullptr;    // [4] last-CTA counters
 	int* mgsp_epochs = nullptr;  // [3]
 	// per-kernel timing (cudaEvent pairs around the g2p2g launches; stream mode only)
@@ -327,13 +272,11 @@ int push_state(cb200_sim* s) {
 }
 
 // one launch per material: all models of that material share the staged neighbourhood of a block
-G2P2GArgs make_g2p2g_args(cb200_sim* s, int material, int R, int halo_mode) {
+G2P2GArgs make_g2p2g_args(cb200_sim* s, int material, int R) {
 	const int Rn = R ^ 1;
 	G2P2GArgs a {};
 	a.cfg = s->cfg;
 	a.state = s->d_state;
-	a.halo_mode = halo_mode;
-	a.halo_marks = s->part[R].halo_marks;
 	a.n_models = 0;
 	for(const Model& m : s->models) {
 		if(m.material != material) continue;
@@ -350,19 +293,12 @@ G2P2GArgs make_g2p2g_args(cb200_sim* s, int material, int R, int halo_mode) {
 	a.next_grid = s->grid[1];
 	a.error = &s->d_state->error;
 	// one queue per launch: each material's launch of a sub-step pulls from its own counter
-	a.work_counter = halo_mode == 1 ? &s->d_state->work_counter2 : (halo_mode == 0 ? &s->d_state->work_counter_mat[material] : &s->d_state->work_counter);
-	if(s->desc.mgsp_world > 1 && halo_mode == 0) {
+	a.work_counter = &s->d_state->work_counter_mat[material];
+	if(s->desc.mgsp_world > 1) {
 		a.overlap_marks = s->part[R].overlap_marks;
 		a.peer_bno = s->peer_bno;
 		a.peer_stride = s->desc.max_blocks;
 		for(int r = 0; r < s->desc.mgsp_world; ++r) a.peer_grid[r] = s->grid1_peer[r];
-	}
-	if(halo_mode == 1) {
-		a.block_list = s->halo_list[R];
-		a.list_count = s->part[R].halo_count;
-	} else if(halo_mode == 2) {
-		a.block_list = s->interior_list[R];
-		a.list_count = s->interior_count[R];
 	}
 	return a;
 }
@@ -390,16 +326,10 @@ int enqueue_grid_update(cb200_sim* s, int R) {
 	return (int) cudaGetLastError();
 }
 // ---- phase B: g2p2g --------------------------------------------------------------------------------
-int enqueue_g2p2g(cb200_sim* s, int R, int halo_mode, cudaStream_t st = nullptr) {
-	if(!st) st = s->stream;
-	int n_materials = 0;
+int enqueue_g2p2g(cb200_sim* s, int R) {
+	cudaStream_t st = s->stream;
 	for(int material = 0; material < 4; ++material) {
-		bool any = false;
-		for(const Model& m : s->models) any |= m.material == material;
-		n_materials += any;
-	}
-	for(int material = 0; material < 4; ++material) {
-		const G2P2GArgs a = make_g2p2g_args(s, material, R, halo_mode);
+		const G2P2GArgs a = make_g2p2g_args(s, material, R);
 		if(a.n_models == 0) continue;
 		const bool timed = s->profiling && !s->capturing;
 		if(timed) {
@@ -411,9 +341,7 @@ int enqueue_g2p2g(cb200_sim* s, int R, int halo_mode, cudaStream_t st = nullptr)
 			}
 			CK(cudaEventRecord(s->prof_events[s->prof_used].first, st));
 		}
-		G2P2GArgs b = a;
-		if(n_materials > 1 && halo_mode != 0) b.work_counter = nullptr;  // the split (halo / interior) launches share two counters: static striding
-		CK(launch_g2p2g(material, b, -1, st));
+		CK(launch_g2p2g(material, a, -1, st));
 		if(timed) CK(cudaEventRecord(s->prof_events[s->prof_used++].second, st));
 		++s->launches;
 	}
@@ -486,15 +414,12 @@ int enqueue_rebuild(cb200_sim* s, int R) {
 }
 int mark_phase(cb200_sim* s, int id);
 MgspView mgsp_view(cb200_sim* s);
-int enqueue_halo_publish(cb200_sim* s, int P, const float* local_max);
-int enqueue_halo_tag_reset(cb200_sim* s, int P);
-int enqueue_halo_tag(cb200_sim* s, int P, const int* particle_block_count, const float* local_max, float* global_max);
 
 // End of a sub-step.  Single GPU: carry the grid, register exterior blocks (its last CTA rolls the state); the neighbour count
 // was snapshotted by the last CTA of the neighbour registration.
 // MGSP: the same, interleaved with the end-of-step exchange so that its wait sits behind local work:
 //   reset tags -> carry (+ this rank's max |v|^2 of the new grid) -> clear the next grid -> PUBLISH keys + max
-//   -> register exterior blocks -> WAIT for the peers' messages, tag overlaps, global max -> halo block lists -> roll the state.
+//   -> register exterior blocks -> WAIT for the peers' messages, tag overlaps, global max -> roll the state.
 // A peer may reduce into this rank's next grid as soon as it has seen this rank's message: the clear comes before the publish.
 int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 	const int Rn = R ^ 1;
@@ -510,8 +435,6 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 			a.mgsp = 1;
 			a.view = mgsp_view(s);
 			a.overlap_marks = s->part[Rn].overlap_marks;
-			a.halo_count = s->part[Rn].halo_count;
-			a.interior_count = s->interior_count[Rn];
 		}
 		a.cfg = s->cfg;
 		a.new_count = s->d_scratch + 1;
@@ -557,9 +480,9 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 		register_blocks_kernel<<<grid_blocks(4), 128, 0, st>>>(a);
 		++s->launches;
 	}
+	mark_phase(s, 9);
 	if(mgsp) {
-		mark_phase(s, 9);
-		mgsp_tag_finalize_kernel<<<grid_blocks(1), 256, 0, st>>>(s->cfg, mgsp_view(s), s->part[Rn].index_table, s->part[Rn].overlap_marks, s->d_scratch + 1, local_max, global_max, fin);
+		mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(s->cfg, mgsp_view(s), s->part[Rn].index_table, s->part[Rn].overlap_marks, s->d_scratch + 1, local_max, global_max, 1, fin);
 		++s->launches;
 		mark_phase(s, 8);
 	}
@@ -580,42 +503,9 @@ MgspView mgsp_view(cb200_sim* s) {
 	v.epochs = s->mgsp_epochs;
 	return v;
 }
-// collect_halo_grid_blocks + reduce_halo_grid_blocks (mgsp_benchmark.cuh:723-776) on grid `g`, numbering of partition `P`
-int enqueue_halo_send(cb200_sim* s, int g, int P) {
-	mgsp_pack_send_kernel<<<grid_blocks(2), 256, 0, s->stream>>>(s->cfg, mgsp_view(s), s->grid[g], s->part[P].index_table);
-	++s->launches;
-	return (int) cudaGetLastError();
-}
-int enqueue_halo_reduce(cb200_sim* s, int g, int P) {
-	mgsp_wait_reduce_kernel<<<grid_blocks(2), 256, 0, s->stream>>>(s->cfg, mgsp_view(s), s->grid[g], s->part[P].index_table, &s->d_state->error);
-	++s->launches;
-	return (int) cudaGetLastError();
-}
-// halo_tagging (mgsp_benchmark.cuh:661-720) on partition P whose Partition::count currently equals its neighbour count
-// key_limit: device int holding the neighbour count of partition P (its Partition::count may already include exterior blocks)
-int enqueue_halo_publish(cb200_sim* s, int P, const float* local_max) {
-	cudaStream_t st = s->stream;
-	const MgspView v = mgsp_view(s);
-	mgsp_publish_keys_kernel<<<grid_blocks(1), 256, 0, st>>>(v, s->part[P].active_keys, s->d_scratch + 1, local_max);
-	++s->launches;
-	return (int) cudaGetLastError();
-}
-int enqueue_halo_tag_reset(cb200_sim* s, int P) {
-	mgsp_tag_reset_kernel<<<grid_blocks(1), 256, 0, s->stream>>>(mgsp_view(s), s->part[P].overlap_marks, s->d_scratch + 1, s->part[P].halo_count, s->interior_count[P]);
-	++s->launches;
-	return (int) cudaGetLastError();
-}
-int enqueue_halo_tag(cb200_sim* s, int P, const int* particle_block_count, const float* local_max, float* global_max) {
-	cudaStream_t st = s->stream;
-	const MgspView v = mgsp_view(s);
-	mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(s->cfg, v, s->part[P].index_table, s->part[P].overlap_marks, s->d_scratch + 1, local_max, global_max);
-	collect_halo_blockids_kernel<<<grid_blocks(2), 128, 0, st>>>(s->cfg, count_dev(particle_block_count), s->part[P].index_table, s->part[P].active_keys, s->part[P].overlap_marks, s->part[P].halo_marks, s->part[P].halo_count, nullptr, s->halo_list[P], s->interior_list[P], s->interior_count[P]);
-	s->launches += 2;
-	return (int) cudaGetLastError();
-}
 
-// profiling aid: records an event after a phase (ids: 0 start, 1 grid update, 2 max-vel all-reduce, 3 halo g2p2g, 4 halo send,
-// 5 interior g2p2g, 6 halo wait+reduce, 7 rebuild, 8 halo tagging, 9 carry/exterior/finalize)
+// profiling aid: records an event after a phase (ids: 0 start, 1 grid update, 5 g2p2g, 6 MGSP done publish, 7 rebuild,
+// 9 carry + exterior registration (single GPU: + state roll), 8 MGSP halo tagging + state roll; ids 2-4 are not recorded)
 int mark_phase(cb200_sim* s, int id) {
 	if(!s->profiling || s->capturing) return 0;
 	if(s->phase_used == s->phase_events.size()) {
@@ -634,29 +524,21 @@ int enqueue_substep(cb200_sim* s, int R) {
 	mark_phase(s, 0);
 	if((e = enqueue_grid_update(s, R))) return e;
 	mark_phase(s, 1);
+	// MGSP: no halo / interior split, one g2p2g launch per material as on one GPU: the arena flush of a block reduces into this rank's next grid and, for grid blocks
+	// shared with a peer, straight into that peer's next grid over NVLink (no pack, no send, no unpack kernels; the reference:
+	// halo g2p2g, barrier, collect_grid_blocks + cudaMemcpyPeerAsync, non-halo g2p2g, barrier, reduce_grid_blocks; :421-467,
+	// 723-776).  The key exchange at the end of the previous sub-step doubles as "every rank has cleared its next grid"; the
+	// done flag below as "every remote reduction has landed".
+	if((e = enqueue_g2p2g(s, R))) return e;
+	mark_phase(s, 5);
 	if(s->desc.mgsp_world > 1) {
-		// ONE g2p2g launch: the arena flush of a block reduces into this rank's next grid and, for grid blocks shared with a
-		// peer, straight into that peer's next grid over NVLink (no pack, no send, no unpack kernels; the reference: halo g2p2g,
-		// barrier, collect_grid_blocks + cudaMemcpyPeerAsync, non-halo g2p2g, barrier, reduce_grid_blocks; :421-467, 723-776).
-		// The max-vel all-reduce above doubles as "every rank has cleared its next grid"; the barrier below as "every remote
-		// reduction has landed".
-		if((e = enqueue_g2p2g(s, R, 0))) return e;
-		mark_phase(s, 5);
 		mgsp_done_publish_kernel<<<1, 32, 0, s->stream>>>(mgsp_view(s));  // the wait sits at the head of the grid carry
 		++s->launches;
 		mark_phase(s, 6);
-		if((e = enqueue_rebuild(s, R))) return e;
-		mark_phase(s, 7);
-		if((e = enqueue_carry_and_exterior(s, R))) return e;  // includes the key / max-velocity exchange and the halo tagging (:530)
-		mark_phase(s, 9);
-		return 0;
 	}
-	if((e = enqueue_g2p2g(s, R, 0))) return e;
-	mark_phase(s, 5);
 	if((e = enqueue_rebuild(s, R))) return e;
 	mark_phase(s, 7);
-	if((e = enqueue_carry_and_exterior(s, R))) return e;
-	return 0;
+	return enqueue_carry_and_exterior(s, R);  // MGSP: includes the key / max-velocity exchange and the halo tagging (:530)
 }
 }  // namespace
 
@@ -703,13 +585,11 @@ void preload_kernels() {
 	preload(mgsp_allreduce_maxvel_kernel);
 	preload(mgsp_pack_send_kernel);
 	preload(mgsp_wait_reduce_kernel);
-	preload(mgsp_publish_keys_kernel);
 	preload(mgsp_tag_reset_kernel);
 	preload(mgsp_tag_kernel);
 	preload(mgsp_done_publish_kernel);
 	preload(mgsp_done_wait_kernel);
 	preload(mgsp_clear_publish_kernel);
-	preload(mgsp_tag_finalize_kernel);
 	preload(grid_max_kernel);
 	g2p2g_prepare_all();
 }
@@ -896,11 +776,6 @@ static int sim_create_impl(cb200_sim* s, const cb200_sim_desc* desc, void* strea
 		CK(pool_alloc(&s->mgsp_done, 16 * sizeof(int)));
 		CK(cudaMemsetAsync(s->mgsp_done, 0, 16 * sizeof(int), s->stream));
 		s->mgsp_epochs = s->mgsp_done + 4;
-		for(int i = 0; i < 2; ++i) {
-			CK(pool_alloc(&s->halo_list[i], (mb + 1) * sizeof(int)));
-			CK(pool_alloc(&s->interior_list[i], (mb + 1) * sizeof(int)));
-			s->interior_count[i] = s->mgsp_done + 8 + i;
-		}
 		CK(cudaStreamSynchronize(s->stream));
 	}
 	return 0;
@@ -944,10 +819,6 @@ int cb200_sim_destroy(cb200_sim* s) {
 	g_pool.release(s->peer_bno);
 	g_pool.release(s->inbox_local);
 	g_pool.release(s->mgsp_done);
-	for(int i = 0; i < 2; ++i) {
-		g_pool.release(s->halo_list[i]);
-		g_pool.release(s->interior_list[i]);
-	}
 	g_pinned.put(s->h_state);
 	g_pinned.put(s->h_poll);
 	if(s->poll_event) cudaEventDestroy(s->poll_event);
@@ -1080,14 +951,17 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 		register_blocks_kernel<<<blocks_for((long long) pbc * 8, 128), 128, 0, st>>>(a);
 		CK(cudaMemcpyAsync(&nbc, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToHost, st));
 		CK(cudaStreamSynchronize(st));
-		if(s->desc.mgsp_world > 1) {  // halo_tagging of the initial partition (mgsp_benchmark.cuh:633)
+		if(s->desc.mgsp_world > 1) {  // halo_tagging of the initial partition (mgsp_benchmark.cuh:633), with the kernels of the sub-step
 			if(!s->peers_ready) return (int) cudaErrorNotReady;
-			CK(cudaMemcpyAsync(s->d_scratch + 0, &pbc, sizeof(int), cudaMemcpyHostToDevice, st));
-			CK(cudaMemcpyAsync(s->d_scratch + 1, &nbc, sizeof(int), cudaMemcpyHostToDevice, st));
+			const MgspView v = mgsp_view(s);
+			float* local_max = reinterpret_cast<float*>(s->d_scratch + 3);
+			CK(cudaMemcpyAsync(s->d_scratch + 1, &nbc, sizeof(int), cudaMemcpyHostToDevice, st));  // key count of the exchange
 			CK(cudaMemsetAsync(s->d_scratch + 3, 0, 2 * sizeof(int), st));
-			CK(enqueue_halo_tag_reset(s, Rn));
-			CK(enqueue_halo_publish(s, Rn, reinterpret_cast<float*>(s->d_scratch + 3)));
-			CK(enqueue_halo_tag(s, Rn, s->d_scratch + 0, reinterpret_cast<float*>(s->d_scratch + 3), reinterpret_cast<float*>(s->d_scratch + 4)));
+			mgsp_tag_reset_kernel<<<grid_blocks(1), 256, 0, st>>>(v, s->part[Rn].overlap_marks, s->d_scratch + 1);
+			// the next grid is still all zero from cb200_sim_create: the clear changes nothing, and the flag still goes out behind it
+			mgsp_clear_publish_kernel<<<grid_blocks(2), 256, 0, st>>>(v, s->part[Rn].active_keys, s->d_scratch + 1, local_max, s->grid[1]);
+			mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(cfg, v, s->part[Rn].index_table, s->part[Rn].overlap_marks, s->d_scratch + 1, local_max, reinterpret_cast<float*>(s->d_scratch + 4), 0, FinalizeArgs {});
+			s->launches += 3;
 		}
 		a.lo = -1;
 		a.span = 3;
@@ -1102,14 +976,8 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 	CK(cudaMemcpyAsync(s->part[R].index_table, s->part[Rn].index_table, s->table_entries * sizeof(int), cudaMemcpyDeviceToDevice, st));
 	CK(cudaMemcpyAsync(s->part[R].active_keys, s->part[Rn].active_keys, (size_t) ebc * 3 * sizeof(int), cudaMemcpyDeviceToDevice, st));
 	CK(cudaMemcpyAsync(s->part[R].count, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToDevice, st));
-	if(s->desc.mgsp_world > 1) {  // "need to copy halo tag info as well" (mgsp_benchmark.cuh:639-640)
-		CK(cudaMemcpyAsync(s->part[R].halo_marks, s->part[Rn].halo_marks, (size_t) pbc, cudaMemcpyDeviceToDevice, st));
+	if(s->desc.mgsp_world > 1)  // "need to copy halo tag info as well" (mgsp_benchmark.cuh:639-640)
 		CK(cudaMemcpyAsync(s->part[R].overlap_marks, s->part[Rn].overlap_marks, (size_t) nbc * sizeof(int), cudaMemcpyDeviceToDevice, st));
-		CK(cudaMemcpyAsync(s->part[R].halo_count, s->part[Rn].halo_count, sizeof(int), cudaMemcpyDeviceToDevice, st));
-		CK(cudaMemcpyAsync(s->halo_list[R], s->halo_list[Rn], (size_t) pbc * sizeof(int), cudaMemcpyDeviceToDevice, st));
-		CK(cudaMemcpyAsync(s->interior_list[R], s->interior_list[Rn], (size_t) pbc * sizeof(int), cudaMemcpyDeviceToDevice, st));
-		CK(cudaMemcpyAsync(s->interior_count[R], s->interior_count[Rn], sizeof(int), cudaMemcpyDeviceToDevice, st));
-	}
 	for(Model& m : s->models) {
 		CK(cudaMemcpyAsync(m.pb[Rn].bin_offsets, m.pb[R].bin_offsets, (size_t) (pbc + 1) * sizeof(int), cudaMemcpyDeviceToDevice, st));
 		CK(cudaMemcpyAsync(m.pb[Rn].particle_bucket_sizes, m.pb[R].particle_bucket_sizes, (size_t) pbc * sizeof(int), cudaMemcpyDeviceToDevice, st));
@@ -1122,9 +990,11 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 		s->launches += 2;
 	}
 	CK(cudaGetLastError());
-	if(s->desc.mgsp_world > 1) {  // the rasterised halo blocks are partial sums: reduce them (mgsp_benchmark.cuh:653-654)
-		CK(enqueue_halo_send(s, 0, R));
-		CK(enqueue_halo_reduce(s, 0, R));
+	if(s->desc.mgsp_world > 1) {  // the rasterised halo blocks are partial sums: reduce them (mgsp_benchmark.cuh:653-654, 723-776)
+		mgsp_pack_send_kernel<<<grid_blocks(2), 256, 0, st>>>(cfg, mgsp_view(s), s->grid[0], s->part[R].index_table);
+		mgsp_wait_reduce_kernel<<<grid_blocks(2), 256, 0, st>>>(cfg, mgsp_view(s), s->grid[0], s->part[R].index_table, err);
+		s->launches += 2;
+		CK(cudaGetLastError());
 	}
 	// device-resident step state; initial dt as in main_loop's preamble (gmpm_simulator.cuh:305-315)
 	CK(pull_state(s));
@@ -1382,11 +1252,9 @@ int cb200_sim_mgsp_open_peers(cb200_sim* s, const void* handles) {
 		memcpy(&h, (const unsigned char*) handles + CB200_MGSP_HANDLE_BYTES * r, 64);
 		CK(g_ipc.open(&p, h));
 		s->inbox_peer[r] = (unsigned char*) p;
-		s->inbox_opened[r] = true;
 		memcpy(&h, (const unsigned char*) handles + CB200_MGSP_HANDLE_BYTES * r + 64, 64);
 		CK(g_ipc.open(&p, h));
 		s->grid1_peer[r] = (float*) p;
-		s->grid1_opened[r] = true;
 	}
 	s->peers_ready = true;
 	return 0;
@@ -1403,11 +1271,10 @@ int cb200_sim_mgsp_set_peers(cb200_sim* s, void* const* inbox_ptrs, void* const*
 }
 int cb200_sim_mgsp_halo_counts(cb200_sim* s, int* shared, int* halo_particle_blocks) {
 	if(!s || s->desc.mgsp_world <= 1) return (int) cudaErrorInvalidValue;
-	if(s->setup_done) {  // the halo / interior particle-block lists are statistics only in the fused path: built on demand, not per sub-step
+	if(s->setup_done) {  // the halo particle blocks are statistics only in the fused path: counted on demand, not per sub-step
 		const int P = s->rollid;
 		CK(cudaMemsetAsync(s->part[P].halo_count, 0, sizeof(int), s->stream));
-		CK(cudaMemsetAsync(s->interior_count[P], 0, sizeof(int), s->stream));
-		collect_halo_blockids_kernel<<<grid_blocks(2), 128, 0, s->stream>>>(s->cfg, count_dev(&s->d_state->pbc), s->part[P].index_table, s->part[P].active_keys, s->part[P].overlap_marks, s->part[P].halo_marks, s->part[P].halo_count, nullptr, s->halo_list[P], s->interior_list[P], s->interior_count[P]);
+		collect_halo_blockids_kernel<<<grid_blocks(2), 128, 0, s->stream>>>(s->cfg, count_dev(&s->d_state->pbc), s->part[P].index_table, s->part[P].active_keys, s->part[P].overlap_marks, s->part[P].halo_marks, s->part[P].halo_count, nullptr);
 		++s->launches;
 	}
 	CK(cudaStreamSynchronize(s->stream));

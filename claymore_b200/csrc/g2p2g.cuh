@@ -61,8 +61,6 @@ struct G2P2GArgs {
 	const StepState* state;  // nullable: when set, dt/new_dt/block count come from the device
 	float dt, new_dt;
 	int block_count;
-	int halo_mode;            // 0: all blocks, 1: only halo-marked, 2: only non-halo (MGSP split, mgsp_benchmark.cuh:421-467)
-	const char* halo_marks;
 	int n_models;             // models of the SAME material handled by one launch: the neighbourhood of a block is staged
 	G2P2GModel m[kMaxModels]; // and written back once for all of them (the reference launches g2p2g once per model, :386-396)
 	const int* prev_table;
@@ -72,8 +70,6 @@ struct G2P2GArgs {
 	float* next_grid;
 	int* error;  // nullable
 	int* work_counter;  // nullable: dynamic block queue (device int, zero before the launch); static striding otherwise
-	const int* block_list;  // nullable: compacted list of block numbers to process (MGSP halo / interior lists)
-	const int* list_count;  // its length (device)
 	// MGSP fused halo reduction: a grid block that is also active on peer p (bit p of overlap_marks) receives this CTA's
 	// partial sums on BOTH owners: the arena flush issues a second bulk add-reduction straight into the peer's next grid
 	// (CUDA-IPC mapped, NVLink) at the block number the peer gave that key (peer_bno).  nullptr = single-GPU.
@@ -148,7 +144,6 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 		new_dt = device_compute_dt(cfg, a.state->max_vel_sq, a.state->step_time, a.state->frame_time, a.state->dt_default);
 		nblocks = a.state->pbc;
 	}
-	if(a.block_list) nblocks = *a.list_count;
 	if(threadIdx.x == 0) {
 		mbar_init(bar, 1);
 		mbar_fence_init();
@@ -180,12 +175,10 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 		const int qi = sm.cur_blk, qn = sm.next_blk;  // published by the last barrier every thread passed
 		if(qi >= nblocks) break;
 		if(tid == 0) q_pending = a.work_counter ? atomicAdd(a.work_counter, 1) : qn + (int) gridDim.x;
-		const int blk = a.block_list ? a.block_list[qi] : qi;
+		const int blk = qi;
 		int total_size = 0;
 		for(int mi = 0; mi < a.n_models; ++mi) total_size += a.m[mi].next.particle_bucket_sizes[blk];
-		bool skip = total_size == 0;
-		if(a.halo_mode && !a.block_list) skip |= (a.halo_mode == 1) != (a.halo_marks[blk] != 0);
-		if(skip) {
+		if(total_size == 0) {
 			__syncthreads();
 			if(tid == 0) {
 				sm.cur_blk = qn;

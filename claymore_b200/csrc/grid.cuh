@@ -108,28 +108,18 @@ struct CarryArgs {
 	float* new_grid;
 	float* next_max_vel;    // nullable (MGSP): max |v|^2 the NEXT grid update will find on this rank, so that the all-reduce
 	                        // of it can ride on the end-of-step key exchange instead of being a sync point of its own
-	// MGSP: reset the tagging state of the new partition on the way (reset_overlap_marks / reset_halo_count, hash_table.cuh:60-66);
+	// MGSP: reset the tagging state of the new partition on the way (reset_overlap_marks, hash_table.cuh:64-66);
 	// the launch sits behind mgsp_done_wait_kernel: the old next-grid is complete only when every peer's halo reductions have landed
 	int mgsp;
 	MgspView view;
 	int* overlap_marks;
-	int* halo_count;
-	int* interior_count;
 };
 __global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int n = *a.new_count;
 	const int old_nbc = a.state->nbc;
 	const int g = a.cfg.gsize, bc = a.cfg.boundary;
-	if(a.mgsp) {
-		if(blockIdx.x == 0) {
-			if((int) threadIdx.x < a.view.world) a.view.overlap_count[threadIdx.x] = 0;
-			if(threadIdx.x == 0) {
-				*a.halo_count = 0;
-				*a.interior_count = 0;
-			}
-		}
-	}
+	if(a.mgsp && blockIdx.x == 0 && (int) threadIdx.x < a.view.world) a.view.overlap_count[threadIdx.x] = 0;
 	float gdt = 0.f;
 	if(a.next_max_vel) gdt = a.cfg.gravity * device_compute_dt(a.cfg, a.state->max_vel_sq, a.state->step_time, a.state->frame_time, a.state->dt_default);
 	unsigned vmax = 0u;

@@ -208,8 +208,7 @@ __global__ void mark_overlapping_blocks_kernel(Cfg cfg, Count block_count, int o
 	}
 }
 // collect_blockids_for_halo_reduction :38-62 -- particle blocks whose 2x2x2 footprint touches an overlapping block
-// halo_list / interior_list (nullable) receive the block NUMBERS of the two classes so that g2p2g can walk compact lists
-__global__ void collect_halo_blockids_kernel(Cfg cfg, Count particle_block_count, const int* table, const int* keys, const int* overlap_marks, char* halo_marks, int* halo_count, int* halo_blocks, int* halo_list = nullptr, int* interior_list = nullptr, int* interior_count = nullptr) {
+__global__ void collect_halo_blockids_kernel(Cfg cfg, Count particle_block_count, const int* table, const int* keys, const int* overlap_marks, char* halo_marks, int* halo_count, int* halo_blocks) {
 	const int n = particle_block_count.get();
 	for(int b = blockIdx.x * blockDim.x + threadIdx.x; b < n; b += gridDim.x * blockDim.x) {
 		const int x = keys[3 * b], y = keys[3 * b + 1], z = keys[3 * b + 2];
@@ -219,10 +218,8 @@ __global__ void collect_halo_blockids_kernel(Cfg cfg, Count particle_block_count
 			hit = nno >= 0 && overlap_marks[nno] != 0;
 		}
 		halo_marks[b] = hit ? 1 : 0;
-		if(!hit && interior_list) interior_list[atomicAdd(interior_count, 1)] = b;
 		if(hit) {
 			const int h = atomicAdd(halo_count, 1);
-			if(halo_list) halo_list[h] = b;
 			if(halo_blocks) {
 				halo_blocks[3 * h] = x;
 				halo_blocks[3 * h + 1] = y;

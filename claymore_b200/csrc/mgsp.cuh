@@ -7,14 +7,20 @@
 // while the transfer is in flight, add what arrived.  The reference does this with one host thread per GPU,
 // cudaMemcpyPeerAsync, events and six host barriers per sub-step.
 //
-// This library's form (one process per GPU): every rank exposes an INBOX through CUDA IPC; producers store straight into the
-// consumer's inbox over NVLink from inside the pack kernel (no staging buffer, no copy engine, no host-known sizes),
-// then publish an epoch flag with a system-scope release; consumers spin on their local flag with a system-scope
+// This library's form (one process per GPU): every rank exposes an INBOX and its next grid through CUDA IPC.  A sub-step has no
+// halo / interior split: its one g2p2g launch bulk-reduces every shared grid block straight into the peer's next grid over
+// NVLink (g2p2g.cuh), and the done publish / wait pair below is the barrier behind those reductions.  At the end of the
+// sub-step every rank stores its block keys and its max |v|^2 into the peers' inboxes and tags the blocks it shares with each
+// peer from theirs (mgsp_clear_publish_kernel, mgsp_tag_kernel).  Whole grid blocks travel through the inbox only once, at
+// setup: the halo sums of the rasterised start grid (mgsp_pack_send_kernel, mgsp_wait_reduce_kernel).
+// Producers store straight into the consumer's inbox or grid over NVLink (no staging buffer, no copy engine, no host-known
+// sizes), then publish an epoch flag with a system-scope release; consumers spin on their local flag with a system-scope
 // acquire.  Nothing on this path returns to the host, so the whole sub-step stays a fixed kernel sequence.
 // Inbox segments are double-buffered by epoch parity: a rank can be at most one exchange ahead of a peer (it needs
 // the peer's flag of the previous exchange to get there).
 #pragma once
 #include "common.cuh"
+#include "partition.cuh"
 
 namespace cb200 {
 
@@ -106,7 +112,7 @@ __global__ void mgsp_allreduce_maxvel_kernel(MgspView v, float* max_vel_sq) {
 // flag goes to every peer with a system-scope release, and everybody's is awaited.  The step driver uses it as two halves:
 // the flag is published right behind g2p2g, the wait sits in front of the first kernel that reads the reduced grid (the grid carry),
 // behind the partition rebuild -- a rank that finishes its g2p2g late costs its peers nothing as long as it is less late than their
-// rebuild takes.  epochs[1] is advanced by the tag kernel.
+// rebuild takes.  epochs[1] is advanced by the tag kernel (mgsp_wait_reduce_kernel at setup).
 __global__ void mgsp_done_publish_kernel(MgspView v) {
 	const int epoch = v.epochs[1] + 1, par = epoch & 1;
 	const int t = threadIdx.x;
@@ -212,37 +218,10 @@ __global__ void __launch_bounds__(256) mgsp_wait_reduce_kernel(Cfg cfg, MgspView
 }
 
 // ---- key all-gather for halo tagging (halo_tagging, mgsp_benchmark.cuh:661-720) -----------------------------------
+// Clears this rank's next grid (new numbering) and publishes the keys in ONE launch.  The flag goes out only after every CTA has
+// finished both loops, so a peer that sees it may reduce into the cleared grid.
 // The message also carries this rank's max |v|^2 of the grid the NEXT sub-step starts from (computed by the carry kernel), so
 // that the tag kernel, which waits for every peer's message anyway, yields the global maximum: one sync point per sub-step less.
-__global__ void __launch_bounds__(256) mgsp_publish_keys_kernel(MgspView v, const int* keys, const int* key_count, const float* local_max_vel) {
-	const int epoch = v.epochs[2] + 1, par = epoch & 1;
-	const int n3 = min(*key_count, v.L.max_blocks) * 3;
-	for(int p = 0; p < v.world; ++p) {
-		if(p == v.rank) continue;
-		int* rk = reinterpret_cast<int*>(seg_of(v, p, par, v.rank) + v.L.off_keys);
-		for(int i = blockIdx.x * blockDim.x + threadIdx.x; i < n3; i += gridDim.x * blockDim.x) rk[i] = keys[i];
-	}
-	__threadfence_system();
-	__syncthreads();
-	__shared__ int s_last;
-	if(threadIdx.x == 0) s_last = atomicAdd(&v.done[2], 1) == (int) gridDim.x - 1;
-	__syncthreads();
-	if(s_last) {
-		__threadfence_system();
-		if((int) threadIdx.x < v.world && (int) threadIdx.x != v.rank) {
-			InboxHeader* h = reinterpret_cast<InboxHeader*>(seg_of(v, threadIdx.x, par, v.rank));
-			h->key_count = n3 / 3;
-			h->max_vel_sq = *local_max_vel;
-			__threadfence_system();
-			st_release_sys(&h->flag_keys, epoch);
-		}
-		if(threadIdx.x == 0) v.done[2] = 0;
-	}
-}
-
-// Step-driver form: clears this rank's next grid (new numbering) and publishes the keys in ONE launch.  The flag goes out only
-// after every CTA has finished both loops, so a peer that sees it may reduce into the cleared grid (the order the two separate
-// kernels had).
 __global__ void __launch_bounds__(256) mgsp_clear_publish_kernel(MgspView v, const int* keys, const int* key_count, const float* local_max_vel, float* clear_grid) {
 	const int epoch = v.epochs[2] + 1, par = epoch & 1;
 	const int nk = min(*key_count, v.L.max_blocks);
@@ -275,23 +254,23 @@ __global__ void __launch_bounds__(256) mgsp_clear_publish_kernel(MgspView v, con
 	}
 }
 
-// reset of the per-step tagging state (reset_overlap_marks / reset_halo_count, hash_table.cuh:60-66)
-__global__ void mgsp_tag_reset_kernel(MgspView v, int* overlap_marks, const int* key_count, int* halo_count, int* interior_count) {
+// reset of the tagging state at setup (reset_overlap_marks, hash_table.cuh:64-66); the step driver resets it in the grid carry
+__global__ void mgsp_tag_reset_kernel(MgspView v, int* overlap_marks, const int* key_count) {
 	const int n = *key_count;
 	for(int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		overlap_marks[i] = 0;
 		for(int p = 0; p < v.world; ++p) v.peer_bno[(size_t) p * v.L.max_blocks + i] = -1;
 	}
 	if(blockIdx.x == 0 && (int) threadIdx.x < v.world) v.overlap_count[threadIdx.x] = 0;
-	if(blockIdx.x == 0 && threadIdx.x == 0) {
-		*halo_count = 0;
-		*interior_count = 0;
-	}
 }
 
-// mark_overlapping_blocks for every peer (halo_kernels.cuh:22-35), keys read from my inbox
+// mark_overlapping_blocks for every peer (halo_kernels.cuh:22-35), keys read from my inbox; the last CTA publishes the global
+// max |v|^2 of the peers' messages.
 // key_limit: only blocks numbered below it (particle + neighbour blocks) can overlap; exterior blocks registered meanwhile are ignored
-__global__ void __launch_bounds__(256) mgsp_tag_kernel(Cfg cfg, MgspView v, const int* table, int* overlap_marks, const int* key_limit, const float* local_max_vel, float* global_max_vel) {
+// do_finalize (end of a sub-step): the last CTA also advances the halo epoch of this sub-step, rolls the device-resident step state
+// (finalize_step) and resets this rank's local maximum for the next carry.  Setup runs without it: there mgsp_wait_reduce_kernel
+// advances the halo epoch.
+__global__ void __launch_bounds__(256) mgsp_tag_kernel(Cfg cfg, MgspView v, const int* table, int* overlap_marks, const int* key_limit, float* local_max_vel, float* global_max_vel, int do_finalize, FinalizeArgs fin) {
 	const int limit = *key_limit;
 	float gmax = *local_max_vel;
 	const int epoch = v.epochs[2] + 1, par = epoch & 1;
@@ -322,12 +301,21 @@ __global__ void __launch_bounds__(256) mgsp_tag_kernel(Cfg cfg, MgspView v, cons
 	}
 	__syncthreads();
 	__shared__ int s_last;
-	if(threadIdx.x == 0) s_last = atomicAdd(&v.done[3], 1) == (int) gridDim.x - 1;
+	if(threadIdx.x == 0) {
+		__threadfence();
+		s_last = atomicAdd(&v.done[3], 1) == (int) gridDim.x - 1;
+	}
 	__syncthreads();
 	if(s_last && threadIdx.x == 0) {
+		__threadfence();
 		v.done[3] = 0;
 		v.epochs[2] = epoch;
 		*global_max_vel = gmax;  // every CTA saw every header; the last one publishes
+		if(do_finalize) {
+			v.epochs[1] = v.epochs[1] + 1;  // the halo ("my reductions have landed") epoch of this sub-step: published behind g2p2g, awaited by the carry
+			finalize_step(fin);             // reads *global_max_vel through fin.next_max_vel
+			*local_max_vel = 0.f;           // for the next sub-step's carry
+		}
 	}
 }
 

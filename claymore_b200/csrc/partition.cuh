@@ -453,8 +453,6 @@ __device__ __forceinline__ void finalize_step(const FinalizeArgs& a) {
 	s->step_time += next_dt;
 	if(s->frame_roll && s->frame_time > 0.f && s->step_time >= s->frame_time) s->step_time = 0.f;
 	s->max_vel_sq = a.next_max_vel ? *a.next_max_vel : 0.f;
-	s->work_counter = 0;
-	s->work_counter2 = 0;
 	for(int m = 0; m < 4; ++m) s->work_counter_mat[m] = 0;
 	s->steps += 1;
 }

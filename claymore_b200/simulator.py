@@ -199,13 +199,15 @@ class GmpmSimulator:
         check(self.L.cb200_sim_profile_read(self.h, C.byref(ms), C.byref(n)), "profile_read")
         return ms.value, n.value
 
-    PHASES = ("-", "grid_update", "maxvel_allreduce", "halo_g2p2g", "halo_send", "g2p2g", "halo_wait_reduce", "rebuild", "halo_tagging", "carry_exterior_finalize")
+    # phase id of cb200_sim_profile_phases -> name, in sub-step order; ids 6 and 8 are recorded by multi-GPU (MGSP) runs only
+    PHASES = {1: "grid_update", 5: "g2p2g", 6: "halo_done_publish", 7: "rebuild", 9: "carry_exterior_finalize", 8: "halo_tagging"}
+    MGSP_PHASES = (6, 8)
 
     def profile_phases(self):
         """{phase: summed ms} over the sub-steps issued while profile(True) was on (call before profile_read)."""
         out = (C.c_double * 10)()
         check(self.L.cb200_sim_profile_phases(self.h, out), "profile_phases")
-        return {n: out[i] for i, n in enumerate(self.PHASES) if i}
+        return {n: out[i] for i, n in self.PHASES.items() if self.mgsp_world > 1 or i not in self.MGSP_PHASES}
 
     @property
     def launch_count(self):

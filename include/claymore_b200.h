@@ -203,8 +203,8 @@ CB200_API long long cb200_sim_launch_count(cb200_sim* sim);
  * cudaEvent pair around every g2p2g launch; profile_read synchronises and returns the summed duration */
 CB200_API int cb200_sim_profile(cb200_sim* sim, int enable);
 CB200_API int cb200_sim_profile_read(cb200_sim* sim, double* g2p2g_ms_total, int* launches);
-/* summed milliseconds per sub-step phase while profiling was on: out_ms[10] = {-, grid update, max-vel all-reduce, halo g2p2g,
- * halo send, interior (or only) g2p2g, halo wait+reduce, partition rebuild, halo tagging, carry/exterior/finalize} */
+/* summed milliseconds per sub-step phase while profiling was on: out_ms[10] = {-, grid update, -, -, -, g2p2g,
+ * MGSP done publish, partition rebuild, MGSP halo tagging, carry/exterior/finalize}; slots marked - stay 0 */
 CB200_API int cb200_sim_profile_phases(cb200_sim* sim, double* out_ms);
 
 /* MGSP static particle partition, one process per GPU (Projects/MGSP/mgsp_benchmark.cuh:309-559, 661-776).

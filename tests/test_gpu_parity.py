@@ -63,6 +63,18 @@ def test_engine_matches_oracle_small_cube(oracle, cuda_lib, material, use_graph)
     esim.close()
 
 
+def test_profile_phases_cover_the_single_gpu_substep(cuda_lib):
+    """Every phase a single-GPU sub-step records gets time, the grid carry and exterior registration included."""
+    esim = scenes.build_engine(scenes.small_cube())
+    esim.profile(True)
+    esim.step(3)
+    phases = esim.profile_phases()
+    esim.profile(False)
+    assert set(phases) == {"grid_update", "g2p2g", "rebuild", "carry_exterior_finalize"}
+    assert all(ms > 0 for ms in phases.values()), phases
+    esim.close()
+
+
 def test_engine_two_models_colliding(oracle, cuda_lib):
     scene = scenes.two_cubes_colliding()
     osim = scenes.build_oracle(oracle, scene, dt=2e-4)
