@@ -22,8 +22,11 @@
 //                shared memory (XOR-swizzled slots) and counting-sorted by cell with native integer shared atomics;
 //       phase 2  cell-parallel: thread (cell, x-slice) walks the particles of its cell and accumulates its 9 nodes x
 //                4 channels in registers: 108 adds per CELL, not per particle; registers -> arena by plain
-//                read-add-write in two rounds of plane-disjoint (half-)warps, no atomics;
-//       phase 3  the few particles that changed cell in this step are scattered node-parallel (atomics);
+//                read-add-write in two rounds of plane-disjoint (half-)warps, no atomics.  A particle that changed cell
+//                but stayed in the particle block has the stencil of the cell it moved to and is accumulated there
+//                (any order: counting-sorted by that cell; SORTED fixed-corotated: an arrival list of up to 8 per cell);
+//       phase 3  the rest of the particles that changed cell in this step (leaving the particle block, or beyond a cell's
+//                arrival list) are scattered node-parallel (atomics);
 //   * the arena has the grid-block layout, so the write-back is eight 1-KiB cp.reduce.async.bulk f32-add operations
 //     executed by the TMA unit, not 2048 SM-issued global atomics (:910-936); in MGSP mode a second bulk reduction
 //     per shared grid block goes straight into the peer GPU's grid over NVLink;
@@ -114,6 +117,15 @@ __device__ __forceinline__ int opaque_tid() {
 }
 constexpr int kRecMover = 1 << 30;
 constexpr int kRecDrop = 1 << 29;
+// SORTED fixed-corotated: per-cell capacity of the arrival lists of in-block movers (sm.cnt / sm.idx, unused by the sorted path otherwise)
+constexpr int kArrivals = 8;
+static_assert(64 * kArrivals <= kChunk, "arrival lists live in sm.idx");
+// the stencil base (0..5 per axis, arena node coordinates) packed in a record code: in this particle block when it is 1..4 on every
+// axis, and then the particle is accumulated by the phase-2 thread of cell code_cell
+__device__ __forceinline__ bool code_in_block(int code) {
+	return ((code & 7) - 1u < 4u) & (((code >> 3) & 7) - 1u < 4u) & (((code >> 6) & 7) - 1u < 4u);
+}
+__device__ __forceinline__ int code_cell(int code) { return (((code & 7) - 1) << 4) | ((((code >> 3) & 7) - 1) << 2) | (((code >> 6) & 7) - 1); }
 
 // quadratic B-spline weight of stencil node i as a polynomial in d = local position / dx in [0.5, 1.5)
 __device__ __forceinline__ void bspline_poly(int i, float& a, float& b, float& c) {
@@ -129,6 +141,10 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 	constexpr int BINF = (MAT == CB200_J_FLUID) ? 128 : 512;
 	constexpr int T = kG2P2GThreads;
 	constexpr int ITERS = (kChunk + T - 1) / T;
+	// SORTED: in-block movers go to per-cell arrival lists that phase 2 walks.  Only the fixed-corotated build has them: in the
+	// others (whose kernels are larger or whose phase 1 is shorter) the extra code cost 2-5 % on sand and fluid scenes that have no
+	// movers (H100, DESIGN section 2.1), so their movers all take phase 3 as before.
+	constexpr bool ARRIVALS = SORTED && MAT == CB200_FIXED_COROTATED;
 
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	G2P2GSmem& sm = *reinterpret_cast<G2P2GSmem*>(smem_raw);
@@ -548,9 +564,9 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				if(oob) {  // moved more than one cell: the reference drops the contribution (mgmpm_kernels.cuh:881-885)
 					code = kRecDrop;
 					if(a.error) atomicOr(a.error, kErrLostParticle);
-				} else if(moved) {
-					code |= kRecMover;
-					sm.movers[atomicAdd(&sm.nmovers, 1)] = (unsigned short) slot;
+				} else if(moved && (SORTED || !code_in_block(code))) {
+					code |= kRecMover;  // SORTED: the home-range walk of phase 2 skips every mover
+					if constexpr(!ARRIVALS) sm.movers[atomicAdd(&sm.nmovers, 1)] = (unsigned short) slot;
 				}
 				// momentum of node (i, j, k) of the particle's stencil: q + i D[:,0] + j D[:,1] + k D[:,2], with q = m v - D x_p
 				const float q0 = fmaf(mass, velx, -fmaf(D.s[2], lp[2], fmaf(D.s[1], lp[1], D.s[0] * lp[0])));
@@ -560,10 +576,22 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				sm.rec[1][rs] = make_float4(q12.x, q12.y, D.p[0].x, D.p[0].y);
 				sm.rec[2][rs] = make_float4(D.p[1].x, D.p[1].y, D.p[2].x, D.p[2].y);
 				sm.rec[3][rs] = make_float4(q0, D.s[0], D.s[1], D.s[2]);
-				// counting sort by the cell the particle came from (its accumulation home)
-				if constexpr(!SORTED) {
-					const int hc = ((ab[0] - 1) << 4) | ((ab[1] - 1) << 2) | (ab[2] - 1);
-					const int cr = (hc << 16) | atomicAdd(&sm.cnt[hc], 1);
+				// A particle is accumulated by the phase-2 thread of the cell its stencil starts from (code_cell): its home cell, or for
+				// a mover the new cell when that lies in this particle block (lp is relative to the new base).  Movers that leave the
+				// block are scattered by phase 3.
+				if constexpr(ARRIVALS) {
+					// the home ranges come from the cell-major bucket, so a cell's arrivals get a list of their own (sm.idx, unused
+					// otherwise); the ones beyond its kArrivals entries go to phase 3
+					if(code & kRecMover) {
+						const int dc = code_cell(code);
+						const int k = code_in_block(code) ? atomicAdd(&sm.cnt[dc], 1) : kArrivals;
+						if(k < kArrivals) sm.idx[dc * kArrivals + k] = (unsigned short) rec_slot(slot);
+						else sm.movers[atomicAdd(&sm.nmovers, 1)] = (unsigned short) slot;
+					}
+				} else if constexpr(!SORTED) {
+					// counting sort by accumulation cell: an in-block mover is an ordinary phase-2 particle of its new cell
+					int cr = -1;
+					if(!(code & (kRecMover | kRecDrop))) cr = (code_cell(code) << 16) | atomicAdd(&sm.cnt[code_cell(code)], 1);
 					if(it == 0) cr0 = cr;
 					else if(it == 1) cr1 = cr;
 					else cr2 = cr;
@@ -596,13 +624,18 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 			//   w0: (1,0) (0,1) -> 2 2    w1: (2,0) (1,1) -> 3 3    w2: (3,0) (2,1) -> 4 4    w3: (3,1) (2,2) -> 5 5
 			//   w4: (0,0) (3,2) -> 1 6    w5: (0,2) (1,2) -> 3 4
 			const int hi = lane >> 4;
-			const int cx = wrp < 3 ? wrp + 1 - hi : (wrp == 3 ? 3 - hi : (wrp == 4 ? 3 * hi : hi));
 			const int sl = wrp < 3 ? hi : (wrp == 3 ? 1 + hi : (wrp == 4 ? 2 * hi : 2));
-			const int hc = ((cx & 3) << 4) | (lane & 15);
+			// (a function of the thread index: re-derived from a fresh read after the home-range loop, so it is not held across it)
+			auto cell_of = [](int t) {
+				const int w = t >> 5, h = (t >> 4) & 1;
+				const int cx = w < 3 ? w + 1 - h : (w == 3 ? 3 - h : (w == 4 ? 3 * h : h));
+				return ((cx & 3) << 4) | (t & 15);
+			};
+			int hc = cell_of(ptid);
 			int n, st;
 			if constexpr(SORTED) {
 				// the bucket is cell-major, so the staged slots of this chunk are already grouped by home cell: cell hc owns the
-				// slots [offs[hc], offs[hc + 1]) - c0, clipped to the chunk.  No counting sort, no index array, no second barrier.
+				// slots [offs[hc], offs[hc + 1]) - c0, clipped to the chunk.  No counting sort, no second barrier.
 				const int lo = min(max((int) sm.offs[hc] - c0, 0), nchunk), hiE = min(max((int) sm.offs[hc + 1] - c0, 0), nchunk);
 				st = lo;
 				n = p2 ? hiE - lo : 0;
@@ -642,10 +675,7 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				float acc[9][4];
 #pragma unroll
 				for(int n9 = 0; n9 < 9; ++n9) acc[n9][0] = acc[n9][1] = acc[n9][2] = acc[n9][3] = 0.f;
-				for(int p = 0; p < n; ++p) {  // (requesting the next particle's index / first quad one iteration ahead measured 0.8 % slower)
-					const int slot = SORTED ? rec_slot(st + p) : (int) sm.idx[st + p];
-					const float4 r0 = sm.rec[0][slot];  // (y, z, x, code)
-					if(__float_as_int(r0.w) & (kRecMover | kRecDrop)) continue;
+				auto accumulate = [&](int slot, const float4 r0) {  // r0 = rec[0][slot] = (y, z, x, code)
 					const float4 r1 = sm.rec[1][slot], r2 = sm.rec[2][slot], r3 = sm.rec[3][slot];
 					// B-spline weights as polynomials in the local position: two FMA each, with immediates for y and z
 					const float wx = fmaf(fmaf(pc, r0.z, pb), r0.z, pa);
@@ -682,6 +712,25 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 							by += r2.x;
 							bz += r2.y;
 						}
+					}
+				};
+				for(int p = 0; p < n; ++p) {  // (requesting the next particle's index / first quad one iteration ahead measured 0.8 % slower)
+					const int slot = SORTED ? rec_slot(st + p) : (int) sm.idx[st + p];
+					const float4 r0 = sm.rec[0][slot];  // (y, z, x, code)
+					if(__float_as_int(r0.w) & (kRecMover | kRecDrop)) continue;  // phase 3, or (SORTED) another cell's arrival
+					accumulate(slot, r0);
+				}
+				if constexpr(ARRIVALS) {
+					hc = cell_of(opaque_tid());
+					// then the movers that arrived in this cell.  A warp none of whose cells has one skips the pass, so a sub-step
+					// without movers runs the home-range loop alone.
+					const int na = p2 ? min(sm.cnt[hc], kArrivals) : 0;
+					if(__any_sync(0xffffffffu, na > 0)) {
+						for(int p = 0; p < na; ++p) {
+							const int slot = sm.idx[hc * kArrivals + p];
+							accumulate(slot, sm.rec[0][slot]);
+						}
+						n += na;  // (the write-back below skips threads of cells without particles)
 					}
 				}
 				// Registers -> arena by plain read-add-write, no atomics (a shared float atomicAdd is a compare-and-swap loop: 36 per
@@ -730,6 +779,8 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				__syncthreads();
 				if(wrp == 5) add_quad();
 				__syncthreads();
+				// arrival counts for the next chunk / block (ordered before its phase 1 by the barrier that starts it)
+				if(ARRIVALS && tid < 64) sm.cnt[tid] = 0;
 			}
 			// ================= phase 3: particles that changed cell, node-parallel ====================
 			{
