@@ -7,6 +7,6 @@ It fails loudly when the CUDA library is missing: there is no CPU fallback.
 """
 from ._capi import (CB200Error, Config, ParticleBuffer, Partition, SimDesc, SimStats, J_FLUID, FIXED_COROTATED, SAND, NACC, lib, lib_path, build_library)
 from .simulator import GmpmSimulator
-from . import samplers, scene, scenes
+from . import levelset, samplers, scene, scenes
 
-__all__ = ["CB200Error", "Config", "ParticleBuffer", "Partition", "SimDesc", "SimStats", "J_FLUID", "FIXED_COROTATED", "SAND", "NACC", "lib", "lib_path", "build_library", "GmpmSimulator", "samplers", "scene", "scenes"]
+__all__ = ["CB200Error", "Config", "ParticleBuffer", "Partition", "SimDesc", "SimStats", "J_FLUID", "FIXED_COROTATED", "SAND", "NACC", "lib", "lib_path", "build_library", "GmpmSimulator", "levelset", "samplers", "scene", "scenes"]

@@ -66,6 +66,15 @@ class SimStats(C.Structure):
                 ("error", C.c_int), ("steps", C.c_longlong)]
 
 
+STICKY, SLIP, SEPARATE = 0, 1, 2   # BoundaryT, Projects/MGSP/boundary_condition.cuh:18-22
+
+
+class Collider(C.Structure):
+    """cb200_collider: SignedDistanceGrid's members (Projects/MGSP/boundary_condition.cuh:28-35) + the device field pointer."""
+    _fields_ = [("sdf", C.c_void_p), ("rot_mat", C.c_float * 9), ("trans", C.c_float * 3), ("trans_vel", C.c_float * 3), ("omega", C.c_float * 3),
+                ("dsdt", C.c_float), ("scale", C.c_float), ("friction", C.c_float), ("type", C.c_int)]
+
+
 def lib_path():
     return _LIB
 
@@ -87,6 +96,7 @@ _CFG = C.POINTER(Config)
 _SIGNATURES = {
     "cb200_g2p2g": [_CFG, _F, _F, _I, ParticleBuffer, ParticleBuffer, Partition, Partition, _P, _P, _P],
     "cb200_update_grid_velocity_query_max": [_CFG, _I, _P, Partition, _F, _P, _P],
+    "cb200_update_grid_velocity_query_max_collider": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), _F, _P, _P],
     "cb200_clear_grid": [_I, _P, _P],
     "cb200_cell_bucket_to_block": [_CFG, _I, _P, _P, _P, _P, _P],
     "cb200_mark_active_grid_blocks": [_I, _P, _P, _P],
@@ -130,6 +140,9 @@ _SIGNATURES = {
     "cb200_sim_particle_state": [_P, _I, _P, C.POINTER(_I)],
     "cb200_sim_active_keys": [_P, _P, _I, C.POINTER(_I)],
     "cb200_sim_grid": [_P, _P, _I, C.POINTER(_I)],
+    "cb200_sim_set_collider": [_P, C.POINTER(Collider), _P],
+    "cb200_sim_clear_collider": [_P],
+    "cb200_sim_time": [_P, C.POINTER(C.c_double)],
     "cb200_sim_mgsp_inbox": [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_size_t)],
     "cb200_sim_mgsp_ipc_handle": [_P, _P],
     "cb200_sim_mgsp_open_peers": [_P, _P],

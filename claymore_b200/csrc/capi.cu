@@ -133,7 +133,28 @@ int cb200_update_grid_velocity_query_max(const cb200_config* c, int block_count,
 	a.max_vel = max_vel;
 	a.clear_grid = nullptr;
 	a.n_clear = 0;
-	grid_update_kernel<<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a);
+	grid_update_kernel<false><<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a);
+	return (int) cudaGetLastError();
+}
+
+int cb200_update_grid_velocity_query_max_collider(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, float time, float* max_vel, void* stream) {
+	CB_CFG(c);
+	if(!collider_valid(collider) || !collider->sdf) return (int) cudaErrorInvalidValue;
+	if(block_count <= 0) return 0;
+	GridUpdateArgs a {};
+	a.cfg = cfg;
+	a.state = nullptr;
+	a.nbc = block_count;
+	a.ebc = 0;
+	a.dt = dt;
+	a.grid = grid;
+	a.keys = partition.active_keys;
+	a.max_vel = max_vel;
+	a.clear_grid = nullptr;
+	a.n_clear = 0;
+	a.col = *collider;
+	a.time = time;
+	grid_update_kernel<true><<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a);
 	return (int) cudaGetLastError();
 }
 

@@ -113,6 +113,7 @@ struct StepState {
 	int done_counter;       // CTAs of a launch that have finished ("last CTA does the epilogue"; zero between launches)
 	int frame_roll;         // cb200_sim_step with fps > 0: restart the frame clock on the device when a frame is complete (the
 	                        // reference's outer frame loop, gmpm_simulator.cuh:323); 0 while cb200_sim_advance_frame drives the frames
+	double sim_time;        // simulated time since initial_setup: the sum of every finished sub-step's dt (places a moving collider)
 };
 
 enum : int { kErrBlockCapacity = 1, kErrBinCapacity = 2, kErrLostParticle = 4, kErrCellOverflow = 8, kErrHaloMap = 16 };

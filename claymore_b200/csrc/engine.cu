@@ -231,6 +231,10 @@ struct cb200_sim {
 	bool poll_pending = false;
 	int steps_since_poll = 15;  // the first sub-step polls
 	int grow_events = 0;
+	// signed-distance collider (cb200_sim_set_collider): parameters, and the device field this simulator owns
+	bool has_collider = false;
+	ColliderView collider {};
+	float* sdf = nullptr;
 };
 
 namespace {
@@ -321,7 +325,12 @@ int enqueue_grid_update(cb200_sim* s, int R) {
 	}
 	gu.n_clear = (int) s->models.size();
 	for(size_t m = 0; m < s->models.size(); ++m) gu.clear_counts[m] = s->models[m].pb[Rn].cell_particle_counts;
-	grid_update_kernel<<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu);
+	if(s->has_collider) {  // placed at StepState::sim_time, the start of this sub-step
+		gu.col = s->collider;
+		grid_update_kernel<true><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu);
+	} else {
+		grid_update_kernel<false><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu);
+	}
 	++s->launches;
 	return (int) cudaGetLastError();
 }
@@ -444,7 +453,12 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 		a.old_grid = s->grid[1];
 		a.new_grid = s->grid[0];
 		a.next_max_vel = mgsp ? local_max : nullptr;
-		carry_grid_kernel<<<grid_blocks(4), 256, 0, st>>>(a);
+		if(mgsp && s->has_collider) {  // the predicted max must be the one the next grid update finds
+			a.col = s->collider;
+			carry_grid_kernel<true><<<grid_blocks(4), 256, 0, st>>>(a);
+		} else {
+			carry_grid_kernel<false><<<grid_blocks(4), 256, 0, st>>>(a);
+		}
 		++s->launches;
 	}
 	if(mgsp) {
@@ -565,9 +579,11 @@ void preload_kernels() {
 	preload(g2p2g_kernel<CB200_FIXED_COROTATED, true>);
 	preload(g2p2g_kernel<CB200_SAND, true>);
 	preload(g2p2g_kernel<CB200_NACC, true>);
-	preload(grid_update_kernel);
+	preload(grid_update_kernel<false>);
+	preload(grid_update_kernel<true>);
 	preload(clear_grid_kernel);
-	preload(carry_grid_kernel);
+	preload(carry_grid_kernel<false>);
+	preload(carry_grid_kernel<true>);
 	preload(scan_kernel);
 	preload(summary_kernel);
 	preload(rebuild_kernel);
@@ -590,7 +606,8 @@ void preload_kernels() {
 	preload(mgsp_done_publish_kernel);
 	preload(mgsp_done_wait_kernel);
 	preload(mgsp_clear_publish_kernel);
-	preload(grid_max_kernel);
+	preload(grid_max_kernel<false>);
+	preload(grid_max_kernel<true>);
 	g2p2g_prepare_all();
 }
 int ensure_graph(cb200_sim* s, int R) {
@@ -819,6 +836,7 @@ int cb200_sim_destroy(cb200_sim* s) {
 	g_pool.release(s->peer_bno);
 	g_pool.release(s->inbox_local);
 	g_pool.release(s->mgsp_done);
+	g_pool.release(s->sdf);
 	g_pinned.put(s->h_state);
 	g_pinned.put(s->h_poll);
 	if(s->poll_event) cudaEventDestroy(s->poll_event);
@@ -1007,6 +1025,7 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 	h.dt_default = s->desc.dt_default;
 	h.frame_time = s->desc.fps > 0 ? 1.f / (float) s->desc.fps : 0.f;
 	h.step_time = 0.f;
+	h.sim_time = 0.0;
 	float mv = 0.f;
 	for(const Model& m : s->models) mv = fmaxf(mv, sqrtf(m.v0[0] * m.v0[0] + m.v0[1] * m.v0[1] + m.v0[2] * m.v0[2]));
 	if(s->desc.mgsp_world > 1) {  // every rank must start from the same dt: max over the ranks' initial speeds
@@ -1026,7 +1045,8 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 	CK(push_state(s));
 	if(s->desc.mgsp_world > 1) {
 		// global max |v|^2 of the start grid (later sub-steps get it from the end-of-step exchange of the previous one)
-		grid_max_kernel<<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq);
+		if(s->has_collider) grid_max_kernel<true><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->collider);
+		else grid_max_kernel<false><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, ColliderView {});
 		mgsp_allreduce_maxvel_kernel<<<1, 32, 0, st>>>(mgsp_view(s), &s->d_state->max_vel_sq);
 		s->launches += 2;
 	}
@@ -1199,6 +1219,58 @@ int cb200_sim_grid(cb200_sim* s, float* grid_host, int capacity_blocks, int* n_o
 	return 0;
 }
 long long cb200_sim_launch_count(cb200_sim* s) { return s ? s->launches : 0; }
+
+// The sub-step graphs hold the grid-update and carry launches of the collider state they were captured with: drop them and,
+// once set up, instantiate both roll parities again right away (never later, while an MGSP peer may be waiting on this rank).
+static int recapture(cb200_sim* s) {
+	for(int i = 0; i < 2; ++i) {
+		if(s->graph[i]) cudaGraphExecDestroy(s->graph[i]);
+		s->graph[i] = nullptr;
+	}
+	if(s->setup_done && s->desc.use_graph) {
+		CK(ensure_graph(s, 0));
+		CK(ensure_graph(s, 1));
+	}
+	return 0;
+}
+// init_boundary (mgsp_benchmark.cuh:257-266) + fill_signed_distance_field (boundary_condition.cuh:253-295): the four dense
+// row-major node arrays are re-laid out into 1 KiB blocks on the host and uploaded into a pooled device field.
+int cb200_sim_set_collider(cb200_sim* s, const cb200_collider* params, const float* sdf_host) {
+	if(!s || !collider_valid(params) || (!sdf_host && !s->sdf)) return (int) cudaErrorInvalidValue;
+	CK(cudaStreamSynchronize(s->stream));
+	if(sdf_host) {
+		const int G = s->cfg.gsize, N = 4 * G;
+		const size_t blocks = (size_t) G * G * G, nodes = (size_t) N * N * N;
+		if(!s->sdf) CK(pool_alloc(&s->sdf, blocks * kGridBlockFloats * sizeof(float)));
+		std::vector<float> f(blocks * kGridBlockFloats);
+		for(int ch = 0; ch < 4; ++ch)
+			for(int i = 0; i < N; ++i)
+				for(int j = 0; j < N; ++j)
+					for(int k = 0; k < N; ++k)
+						f[(((size_t) (i >> 2) * G + (j >> 2)) * G + (k >> 2)) * kGridBlockFloats + ch * 64 + (i & 3) * 16 + (j & 3) * 4 + (k & 3)] = sdf_host[ch * nodes + ((size_t) i * N + j) * N + k];
+		CK(cudaMemcpyAsync(s->sdf, f.data(), f.size() * sizeof(float), cudaMemcpyHostToDevice, s->stream));
+		CK(cudaStreamSynchronize(s->stream));
+	}
+	s->collider = *params;
+	s->collider.sdf = s->sdf;
+	s->has_collider = true;
+	return recapture(s);
+}
+int cb200_sim_clear_collider(cb200_sim* s) {
+	if(!s) return (int) cudaErrorInvalidValue;
+	CK(cudaStreamSynchronize(s->stream));
+	s->has_collider = false;
+	s->collider = ColliderView {};
+	g_pool.release(s->sdf);
+	s->sdf = nullptr;
+	return recapture(s);
+}
+int cb200_sim_time(cb200_sim* s, double* time) {
+	if(!s || !time) return (int) cudaErrorInvalidValue;
+	CK(pull_state(s));
+	*time = s->h_state->sim_time;
+	return 0;
+}
 int cb200_trim_pool(void) {
 	g_pool.trim();
 	return 0;

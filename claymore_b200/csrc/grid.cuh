@@ -1,5 +1,6 @@
 // grid.cuh -- sparse-grid block kernels: velocity update + max query (+ fused clears), carry copy.
 #pragma once
+#include "collider.cuh"
 #include "common.cuh"
 #include "mgsp.cuh"
 
@@ -18,14 +19,21 @@ struct GridUpdateArgs {
 	float* clear_grid;       // nullable: next grid, nbc blocks zeroed        (clear_grid, mgmpm_kernels.cuh:106-115)
 	int n_clear;             // number of cell-count arrays to zero over ebc blocks (cudaMemsetAsync at gmpm_simulator.cuh:389)
 	int* clear_counts[kMaxModels];
+	ColliderView col;        // COLLIDE only
+	float time;              // COLLIDE, state == nullptr: time the collider is placed at (the driver reads StepState::sim_time)
 };
 
 // update_grid_velocity_query_max (mgmpm_kernels.cuh:325-420): one warp per grid block, two cells per lane as
 // one 8-byte access per channel; warp max by redux, one atomicMax per CTA on the float's bit pattern.
 // Quirks kept: wall blocks zero the masked component BEFORE gravity is added to y (Appendix B #1);
 // NaN -> +inf (B #3).
+// COLLIDE: the MGSP form with a SignedDistanceGrid (mgmpm_kernels.cuh:323-399): after gravity, cells with mass resolve against
+// the collider (collider.cuh); the max is |v|^2 where that kernel reports 2|v|^2 (Appendix B #11).
+template<bool COLLIDE>
 __global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpdateArgs a) {
 	__shared__ unsigned s_max[kGridThreads / 32];
+	const ColliderFrame* fr = nullptr;
+	if constexpr(COLLIDE) fr = &collider_frame_cta(a.col, a.state ? (float) a.state->sim_time : a.time);
 	const Cfg& cfg = a.cfg;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int nbc = a.state ? a.state->nbc : a.nbc;
@@ -48,6 +56,7 @@ __global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpd
 				v0.x = wx ? 0.f : v0.x * mi;
 				v1.x = (wy ? 0.f : v1.x * mi) + gdt;
 				v2.x = wz ? 0.f : v2.x * mi;
+				if constexpr(COLLIDE) collider_resolve(a.col, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
 				sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
 			}
 			if(m.y > 0.f) {
@@ -55,6 +64,7 @@ __global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpd
 				v0.y = wx ? 0.f : v0.y * mi;
 				v1.y = (wy ? 0.f : v1.y * mi) + gdt;
 				v2.y = wz ? 0.f : v2.y * mi;
+				if constexpr(COLLIDE) collider_resolve(a.col, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
 				sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
 			}
 			if(m.x > 0.f || m.y > 0.f) {
@@ -113,7 +123,9 @@ struct CarryArgs {
 	int mgsp;
 	MgspView view;
 	int* overlap_marks;
+	ColliderView col;  // COLLIDE: the predictor applies the collider at the time the next grid update sees
 };
+template<bool COLLIDE>
 __global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int n = *a.new_count;
@@ -122,6 +134,8 @@ __global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
 	if(a.mgsp && blockIdx.x == 0 && (int) threadIdx.x < a.view.world) a.view.overlap_count[threadIdx.x] = 0;
 	float gdt = 0.f;
 	if(a.next_max_vel) gdt = a.cfg.gravity * device_compute_dt(a.cfg, a.state->max_vel_sq, a.state->step_time, a.state->frame_time, a.state->dt_default);
+	const ColliderFrame* fr = nullptr;
+	if constexpr(COLLIDE) fr = &collider_frame_cta(a.col, (float) (a.state->sim_time + (double) a.state->dt));  // the clock rolls by this sub-step's dt
 	unsigned vmax = 0u;
 	for(int j = blockIdx.x * 8 + warp; j < n; j += gridDim.x * 8) {
 		const int kx = a.new_keys[3 * j], ky = a.new_keys[3 * j + 1], kz = a.new_keys[3 * j + 2];
@@ -138,7 +152,8 @@ __global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
 			if(a.next_max_vel) {
 				const float2* s2 = reinterpret_cast<const float2*>(s);
 				const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
-				vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
+				if constexpr(COLLIDE) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_collide(a.cfg, a.col, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+				else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 			}
 		} else {
 			d[lane] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -152,16 +167,20 @@ __global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
 }
 
 // max |v|^2 the grid update will find, without touching the grid (MGSP start-up)
-__global__ void __launch_bounds__(256) grid_max_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel) {
+template<bool COLLIDE>
+__global__ void __launch_bounds__(256) grid_max_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const ColliderView col) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int g = cfg.gsize, bc = cfg.boundary;
 	const float gdt = cfg.gravity * state->dt;
+	const ColliderFrame* fr = nullptr;
+	if constexpr(COLLIDE) fr = &collider_frame_cta(col, (float) state->sim_time);
 	unsigned vmax = 0u;
 	for(int b = blockIdx.x * 8 + warp; b < state->nbc; b += gridDim.x * 8) {
 		const int kx = keys[3 * b], ky = keys[3 * b + 1], kz = keys[3 * b + 2];
 		const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
 		const float2* s2 = reinterpret_cast<const float2*>(grid + (size_t) b * kGridBlockFloats);
-		vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
+		if constexpr(COLLIDE) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_collide(cfg, col, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+		else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 	}
 	vmax = __reduce_max_sync(0xffffffffu, vmax);
 	if(lane == 0 && vmax) atomicMax(reinterpret_cast<unsigned*>(max_vel), vmax);

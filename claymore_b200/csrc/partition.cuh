@@ -448,6 +448,7 @@ __device__ __forceinline__ void finalize_step(const FinalizeArgs& a) {
 	s->ebc = min(*(volatile const int*) a.new_count, a.max_blocks);
 	for(int m = 0; m < a.n_models; ++m)
 		if(s->bin_count[m] > a.bin_capacity[m]) s->error |= kErrBinCapacity;
+	s->sim_time += (double) s->dt;  // the dt this sub-step ran with
 	s->dt = next_dt;
 	// the reference's loop increment runs after `dt = next_dt` (gmpm_simulator.cuh:324,579): the clock advances by the NEW dt
 	s->step_time += next_dt;

@@ -5,6 +5,14 @@ Projects/GMPM/scenes/scene.json) mapped onto GmpmSimulator.
      "models": [{"type": "particles", "file": ..., "constitutive": "fixed_corotated"|"jfluid"|"nacc"|"sand",
                  "offset": [3], "span": [3], "velocity": [3], + material parameters}]}
 
+     "collider": {"file": <prefix of <prefix>_sdf.bin / _grad_{0,1,2}.bin> | "box" | "sphere" | "plane",
+                  "offset": [3], "span": [3], "normal": [3], "type": "sticky"|"slip"|"separate",
+                  "friction", "velocity": [3], "omega": [3], "scale", "dsdt"}}
+
+A "box" collider spans [offset, offset + span], a "sphere" has diameter min(span) at offset + span / 2, a "plane" passes
+through offset and is solid behind `normal`.  The collider is the reference's SignedDistanceGrid (init_boundary,
+Projects/MGSP/mgsp_benchmark.cuh:257-266); "velocity" is its trans_vel.
+
 The reference only loads `.sdf` level sets (gmpm.cu:152, needs the absent Data submodule); here a model may also
 name a synthetic generator: "file": "box" (span in cells of the lattice sampler) or "sphere" (span = diameter),
 or a raw float32 xyz `.bin` cloud as used by mgsp.cu:11-17.
@@ -14,7 +22,7 @@ import os
 
 import numpy as np
 
-from . import samplers
+from . import levelset, samplers
 from ._capi import Config, FIXED_COROTATED, J_FLUID, NACC, SAND
 from .simulator import GmpmSimulator
 
@@ -38,6 +46,22 @@ def _positions(model, cfg, base_dir):
     if path.endswith(".npy"):
         return np.load(path).astype(np.float32).reshape(-1, 3)
     raise ValueError(f"unsupported model file {kind!r} (the reference's .sdf sampler is outside the hot path)")
+
+
+def _collider(sim, c, cfg, base_dir):
+    kind = c.get("file", "box")
+    offset = np.asarray(c.get("offset", [0, 0, 0]), dtype=np.float64)
+    span = np.asarray(c.get("span", [1, 1, 1]), dtype=np.float64)
+    if kind == "box":
+        sdf, grad = levelset.box(cfg, offset, offset + span)
+    elif kind == "sphere":
+        sdf, grad = levelset.sphere(cfg, offset + span / 2, float(span.min()) / 2)
+    elif kind == "plane":
+        sdf, grad = levelset.plane(cfg, offset, c.get("normal", [0, 1, 0]))
+    else:
+        sdf, grad = levelset.load(cfg, kind if os.path.isabs(kind) else os.path.join(base_dir, kind))
+    sim.set_collider(sdf, grad, type=c.get("type", "sticky"), friction=c.get("friction", 0.3), trans_vel=c.get("velocity", [0, 0, 0]),
+                     omega=c.get("omega", [0, 0, 0]), scale=c.get("scale", 1.0), dsdt=c.get("dsdt", 0.0))
 
 
 def parse_scene(path_or_dict, config=None, max_blocks=10000, **sim_kwargs):
@@ -69,4 +93,6 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, **sim_kwargs):
             sim.update_nacc_parameters(model["rho"], model["volume"], model["youngs_modulus"], model["poisson_ratio"], model["beta"], model["xi"], model=mid)
         elif c == "sand" and "youngs_modulus" in model:  # the reference leaves sand at its defaults (gmpm.cu:134-135)
             sim.update_sand_parameters(model["rho"], model["volume"], model["youngs_modulus"], model["poisson_ratio"], model=mid)
+    if "collider" in doc:
+        _collider(sim, doc["collider"], cfg, base)
     return sim

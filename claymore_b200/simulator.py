@@ -9,7 +9,9 @@ import ctypes as C
 import numpy as np
 
 from . import _capi
-from ._capi import CHANNELS, Config, SimDesc, SimStats, check, lib
+from ._capi import CHANNELS, SEPARATE, SLIP, STICKY, Collider, Config, SimDesc, SimStats, check, lib
+
+BOUNDARY_TYPES = {"sticky": STICKY, "slip": SLIP, "separate": SEPARATE}
 
 
 class GmpmSimulator:
@@ -116,6 +118,35 @@ class GmpmSimulator:
         mb, ev = C.c_int(0), C.c_int(0)
         check(self.L.cb200_sim_capacity(self.h, C.byref(mb), C.byref(ev)), "capacity")
         return mb.value, ev.value
+
+    # ---- signed-distance collider (SignedDistanceGrid, Projects/MGSP/boundary_condition.cuh:25-250) -------------------
+    def set_collider(self, sdf=None, grad=None, type="sticky", friction=0.3, trans=(0.0, 0.0, 0.0), trans_vel=(0.0, 0.0, 0.0),
+                     omega=(0.0, 0.0, 0.0), rot=None, scale=1.0, dsdt=0.0):
+        """One collision object acting on the grid update from the next sub-step on (synchronises).  sdf: (N, N, N) signed
+        distance on the N = 4G grid nodes, grad: (3, N, N, N) its gradient (see levelset); both None keep the field set before.
+        type: "sticky" / "slip" / "separate" or CB200_*; rot: 3x3 rotation (row i, column j = rot_mat(i, j)).  Defaults are
+        SignedDistanceGrid's (:38-49).  The collider is placed at the simulated time at the start of each sub-step."""
+        col = Collider()
+        col.type = BOUNDARY_TYPES[type] if isinstance(type, str) else int(type)
+        col.rot_mat[:] = [float(v) for v in np.asarray(np.eye(3) if rot is None else rot, dtype=np.float64).reshape(9)]
+        col.trans[:], col.trans_vel[:], col.omega[:] = [float(v) for v in trans], [float(v) for v in trans_vel], [float(v) for v in omega]
+        col.dsdt, col.scale, col.friction = dsdt, scale, friction
+        host = None
+        if sdf is not None:
+            n = 4 * self.cfg.grid_size
+            host = np.ascontiguousarray(np.concatenate([np.asarray(sdf, np.float32).reshape(1, -1), np.asarray(grad, np.float32).reshape(3, -1)]))
+            if host.shape != (4, n ** 3):
+                raise ValueError(f"level set must be {n}^3 nodes (distance) and 3 x {n}^3 (gradient)")
+        check(self.L.cb200_sim_set_collider(self.h, C.byref(col), host.ctypes.data_as(C.c_void_p) if host is not None else None), "set_collider")
+
+    def clear_collider(self):
+        check(self.L.cb200_sim_clear_collider(self.h), "clear_collider")
+
+    def sim_time(self):
+        """Simulated time since initial_setup (sum of the dt of every finished sub-step)."""
+        t = C.c_double(0.0)
+        check(self.L.cb200_sim_time(self.h, C.byref(t)), "sim_time")
+        return t.value
 
     # ---- observation --------------------------------------------------------------------------------
     def stats(self):

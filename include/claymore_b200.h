@@ -91,6 +91,24 @@ CB200_API int cb200_g2p2g(const cb200_config* cfg, float dt, float new_dt, int p
 /* update_grid_velocity_query_max  mgmpm_kernels.cuh:325-420, launched at gmpm_simulator.cuh:341.  max_vel: device float, max of |v|^2 (caller zeroes it) */
 CB200_API int cb200_update_grid_velocity_query_max(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, float* max_vel, void* stream);
 
+/* Signed-distance collision object: SignedDistanceGrid (Projects/MGSP/boundary_condition.cuh:25-250).
+ * sdf: DEVICE float[G^3 * 256], dense over the whole domain: one block per grid block, blocks row-major (x*G*G+y*G+z), each block
+ * 4 channels SoA (signed distance, gradient x, y, z) of 64 cells (cell = x*16+y*4+z): 1 KiB per grid block.
+ * rot_mat in vec3x3 storage (element (i, j) at 3*i+j); type: BoundaryT. */
+enum { CB200_STICKY = 0, CB200_SLIP = 1, CB200_SEPARATE = 2 };
+typedef struct cb200_collider {
+	const float* sdf;
+	float rot_mat[9];
+	float trans[3], trans_vel[3], omega[3];
+	float dsdt, scale, friction;
+	int type;
+} cb200_collider;
+
+/* update_grid_velocity_query_max<Grid, Partition, Boundary>  Projects/MGSP/mgmpm_kernels.cuh:323-399, launched at
+ * mgsp_benchmark.cuh:380-394: the grid update with a collider placed at `time` (the reference passes 0).  max_vel receives |v|^2,
+ * half of what that kernel reports (it adds every square twice). */
+CB200_API int cb200_update_grid_velocity_query_max_collider(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, float time, float* max_vel, void* stream);
+
 /* clear_grid  mgmpm_kernels.cuh:106-115 via GridBuffer::reset  grid_buffer.cuh:32-35 */
 CB200_API int cb200_clear_grid(int block_count, float* grid, void* stream);
 
@@ -197,6 +215,15 @@ CB200_API int cb200_sim_particle_state(cb200_sim* sim, int model, float* state_h
 /* copies for parity checks: active keys (int[3*ebc]) and grid blocks of grid[0] (float[256*nbc]) to HOST */
 CB200_API int cb200_sim_active_keys(cb200_sim* sim, int* keys_host, int capacity_blocks, int* n_out);
 CB200_API int cb200_sim_grid(cb200_sim* sim, float* grid_host, int capacity_blocks, int* n_out);
+/* One signed-distance collider acting on the grid update (init_boundary, mgsp_benchmark.cuh:257-266).  sdf_host: the four HOST
+ * float arrays of init_from_signed_distance_file (boundary_condition.cuh:297-320) back to back -- distance, gradient x, y, z, each
+ * dense row-major over the (4G)^3 grid nodes; NULL keeps the field uploaded before.  params->sdf is ignored: the simulator owns
+ * the device field (G^3 KiB).  The collider is placed at the simulated time at the start of each sub-step.  Both calls
+ * synchronise and re-capture the sub-step graphs; call them between sub-steps. */
+CB200_API int cb200_sim_set_collider(cb200_sim* sim, const cb200_collider* params, const float* sdf_host);
+CB200_API int cb200_sim_clear_collider(cb200_sim* sim);
+/* simulated time since initial_setup: the sum of the dt of every finished sub-step (synchronises) */
+CB200_API int cb200_sim_time(cb200_sim* sim, double* time);
 /* number of kernels this library launched on behalf of `sim` since creation */
 CB200_API long long cb200_sim_launch_count(cb200_sim* sim);
 /* per-kernel timing for the roofline: while enabled, sub-steps are issued as plain stream launches with a

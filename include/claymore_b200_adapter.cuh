@@ -32,8 +32,13 @@
 
 // Customisation point: how an entry point of the C ABI is reached.  Default: the linked symbol.  The test driver resolves
 // the library with dlopen and routes the calls through function pointers.
+// The collider overload of update_grid_velocity_query_max reaches cb200_update_grid_velocity_query_max_collider: a customised
+// CB200_ADAPTER_CALL that routes that entry too defines CB200_ADAPTER_COLLIDER (with the default call it is always there).
 #ifndef CB200_ADAPTER_CALL
 #define CB200_ADAPTER_CALL(name) ::name
+#ifndef CB200_ADAPTER_COLLIDER
+#define CB200_ADAPTER_COLLIDER 1
+#endif
 #endif
 
 namespace mn {
@@ -127,12 +132,42 @@ struct g2p2g_t {
 		return CB200_ADAPTER_CALL(cb200_g2p2g)(&c, dt.count(), new_dt.count(), (int) lc.dg.x, view(particle_buffer), view(next_particle_buffer), view(prev_partition), view(partition), view(grid), view(next_grid), s);
 	}
 };
-// update_grid_velocity_query_max  :325-326
+#ifdef CB200_ADAPTER_COLLIDER
+// the MGSP form with a collider (Projects/MGSP/mgmpm_kernels.cuh:323-324, launched at mgsp_benchmark.cuh:380-394): Boundary is
+// SignedDistanceGrid (boundary_condition.cuh:25-250), read member by member; its field is dense, so its base pointer is the
+// address of block (0, 0, 0).  The reference's kernel places the collider at time 0 (:363); so does this overload.
+template<typename Boundary>
+inline cb200_collider collider_of(Boundary& b) {
+	cb200_collider c {};
+	c.sdf = &b.ch(placeholder::_0, 0, 0, 0).val_1d(placeholder::_0, 0);
+	for(int i = 0; i < 3; ++i)
+		for(int j = 0; j < 3; ++j) c.rot_mat[3 * i + j] = b.rot_mat(i, j);
+	for(int d = 0; d < 3; ++d) {
+		c.trans[d] = b.trans[d];
+		c.trans_vel[d] = b.trans_vel[d];
+		c.omega[d] = b.omega[d];
+	}
+	c.dsdt = b.dsdt;
+	c.scale = b.scale;
+	c.friction = b.friction;
+	c.type = (int) b.type;
+	return c;
+}
+#endif
+// update_grid_velocity_query_max  :325-326; with a Boundary, the MGSP form
 struct update_grid_velocity_query_max_t {
 	int operator()(void* s, const LaunchConfig&, uint32_t block_count, GridBuffer grid, Partition<1> partition, Duration dt, float* max_vel) const {
 		const cb200_config c = config_of();
 		return CB200_ADAPTER_CALL(cb200_update_grid_velocity_query_max)(&c, (int) block_count, view(grid), view(partition), dt.count(), max_vel, s);
 	}
+#ifdef CB200_ADAPTER_COLLIDER
+	template<typename Boundary>
+	int operator()(void* s, const LaunchConfig&, uint32_t block_count, GridBuffer grid, Partition<1> partition, Duration dt, Boundary boundary, float* max_vel) const {
+		const cb200_config c = config_of();
+		const cb200_collider col = collider_of(boundary);
+		return CB200_ADAPTER_CALL(cb200_update_grid_velocity_query_max_collider)(&c, (int) block_count, view(grid), view(partition), dt.count(), &col, 0.f, max_vel, s);
+	}
+#endif
 };
 // clear_grid  :106-107, launched with {blocks, G_BLOCKVOLUME}
 struct clear_grid_t {
