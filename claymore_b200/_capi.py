@@ -75,6 +75,27 @@ class Collider(C.Structure):
                 ("dsdt", C.c_float), ("scale", C.c_float), ("friction", C.c_float), ("type", C.c_int)]
 
 
+CHECKPOINT_VERSION = 1          # CB200_CHECKPOINT_VERSION
+CHECKPOINT_HEADER_BYTES = 1024  # CB200_CHECKPOINT_HEADER_BYTES
+
+
+class CheckpointModel(C.Structure):
+    """cb200_checkpoint_model: one model's entry of a checkpoint's table of contents."""
+    _fields_ = [("material", C.c_int), ("channels", C.c_int), ("count", C.c_longlong), ("offset", C.c_ulonglong), ("bytes", C.c_ulonglong),
+                ("params", ParticleBuffer)]
+
+
+class CheckpointInfo(C.Structure):
+    """cb200_checkpoint_info: what cb200_checkpoint_inspect reads from a checkpoint's header."""
+    _fields_ = [("version", C.c_uint), ("n_models", C.c_int), ("bytes", C.c_ulonglong), ("cfg", Config), ("dt_default", C.c_float),
+                ("fps", C.c_int), ("mgsp_rank", C.c_int), ("mgsp_world", C.c_int), ("error", C.c_int),
+                ("dt", C.c_float), ("next_dt", C.c_float), ("step_time", C.c_float), ("frame_time", C.c_float), ("sim_time", C.c_double),
+                ("steps", C.c_longlong), ("frames", C.c_longlong),
+                ("particle_block_count", C.c_int), ("neighbor_block_count", C.c_int), ("exterior_block_count", C.c_int), ("max_blocks", C.c_int),
+                ("keys_offset", C.c_ulonglong), ("keys_bytes", C.c_ulonglong), ("grid_offset", C.c_ulonglong), ("grid_bytes", C.c_ulonglong),
+                ("models", CheckpointModel * 8)]
+
+
 def lib_path():
     return _LIB
 
@@ -148,6 +169,11 @@ _SIGNATURES = {
     "cb200_sim_mgsp_open_peers": [_P, _P],
     "cb200_sim_mgsp_set_peers": [_P, C.POINTER(_P), C.POINTER(_P)],
     "cb200_sim_mgsp_halo_counts": [_P, C.POINTER(_I), C.POINTER(_I)],
+    "cb200_checkpoint_inspect": [_P, C.c_size_t, C.POINTER(CheckpointInfo)],
+    "cb200_sim_checkpoint_begin": [_P, C.POINTER(C.c_size_t)],
+    "cb200_sim_checkpoint_end": [_P, C.POINTER(_P), C.POINTER(C.c_size_t)],
+    "cb200_sim_restore_models": [_P, _P, C.c_size_t],
+    "cb200_sim_restore": [_P, _P, C.c_size_t],
     "cb200_trim_pool": [],
     "cb200_test_svd3": [_I, _P, _P, _P, _P, _P],
     "cb200_test_stress": [_I, _I, ParticleBuffer, _I, _P, _P, _P, _P, _P, _P],

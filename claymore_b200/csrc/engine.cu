@@ -18,6 +18,7 @@
 #include <string>
 #include <vector>
 
+#include "checkpoint.cuh"
 #include "g2p2g.cuh"
 #include "grid.cuh"
 #include "init.cuh"
@@ -235,6 +236,25 @@ struct cb200_sim {
 	bool has_collider = false;
 	ColliderView collider {};
 	float* sdf = nullptr;
+	long long frames_done = 0;  // frames finished by cb200_sim_advance_frame (restored from a checkpoint)
+	// checkpoint (cb200_sim_checkpoint_begin / _end): device staging blob, per-model scans of the bucket sizes, pinned copy of the
+	// blob written on a stream of its own; allocated on first use, grown with the block capacity
+	unsigned char* ck_dev = nullptr;
+	size_t ck_dev_bytes = 0;
+	int* ck_base = nullptr;  // [kMaxModels][max_blocks + 1]
+	size_t ck_base_bytes = 0;
+	unsigned char* ck_host = nullptr;  // pinned
+	size_t ck_host_bytes = 0;
+	cudaStream_t ck_stream = nullptr;
+	cudaEvent_t ck_gathered = nullptr, ck_copied = nullptr;
+	bool ck_pending = false;  // a copy was queued and end has not collected it
+	bool ck_ready = false;    // ck_host holds a complete blob of ck_bytes
+	size_t ck_bytes = 0;
+	// cb200_sim_restore_models: the checkpoint's header and its state staged on the device, consumed by initial_setup
+	bool restore_pending = false;
+	cb200_checkpoint_info restore_info {};
+	float* restore_state[kMaxModels] = {};
+	unsigned char* restore_grid = nullptr;  // grid blocks, then keys
 };
 
 namespace {
@@ -608,6 +628,10 @@ void preload_kernels() {
 	preload(mgsp_clear_publish_kernel);
 	preload(grid_max_kernel<false>);
 	preload(grid_max_kernel<true>);
+	preload(snapshot_kernel);
+	preload(state_positions_kernel);
+	preload(state_to_bins_kernel);
+	preload(scatter_grid_kernel);
 	g2p2g_prepare_all();
 }
 int ensure_graph(cb200_sim* s, int R) {
@@ -669,6 +693,7 @@ int cb200_sim_reserve(cb200_sim* s, int new_max_blocks) {
 	if(new_max_blocks <= s->desc.max_blocks) return 0;
 	if(s->desc.mgsp_world > 1) return (int) cudaErrorNotSupported;  // the next grid / inbox are mapped into the peers (CUDA IPC)
 	CK(cudaStreamSynchronize(s->stream));
+	if(s->ck_pending) CK(cudaEventSynchronize(s->ck_copied));  // the next begin re-sizes the staging blob
 	const size_t ob = (size_t) s->desc.max_blocks, nb = (size_t) new_max_blocks;
 	for(int i = 0; i < 2; ++i) {
 		if(s->graph[i]) {
@@ -801,6 +826,15 @@ static int sim_create_impl(cb200_sim* s, const cb200_sim_desc* desc, void* strea
 int cb200_sim_destroy(cb200_sim* s) {
 	if(!s) return 0;
 	cudaStreamSynchronize(s->stream);
+	if(s->ck_stream) cudaStreamSynchronize(s->ck_stream);  // a checkpoint copy may still read the staging blob
+	g_pool.release(s->ck_dev);
+	g_pool.release(s->ck_base);
+	for(float* p : s->restore_state) g_pool.release(p);
+	g_pool.release(s->restore_grid);
+	if(s->ck_host) cudaFreeHost(s->ck_host);
+	if(s->ck_gathered) cudaEventDestroy(s->ck_gathered);
+	if(s->ck_copied) cudaEventDestroy(s->ck_copied);
+	if(s->ck_stream) cudaStreamDestroy(s->ck_stream);
 	for(auto& ev : s->prof_events) {
 		cudaEventDestroy(ev.first);
 		cudaEventDestroy(ev.second);
@@ -845,12 +879,9 @@ int cb200_sim_destroy(cb200_sim* s) {
 	return 0;
 }
 
-int cb200_sim_init_model(cb200_sim* s, int material, const float* positions_host, int n, const float* v0, int* model_id) {
-	if(!s || s->setup_done || material < 0 || material > 3 || n <= 0 || (int) s->models.size() >= kMaxModels) return (int) cudaErrorInvalidValue;
-	Model m;
-	m.material = material;
-	m.n = n;
-	for(int d = 0; d < 3; ++d) m.v0[d] = v0 ? v0[d] : 0.f;
+// the containers of one model of m.material and m.n particles (init_model and restore; the caller fills d_pos)
+static int alloc_model(cb200_sim* s, Model& m) {
+	const int material = m.material, n = m.n;
 	const size_t mb = (size_t) s->desc.max_blocks;
 	const size_t binf = material == CB200_J_FLUID ? 128 : 512;
 	// capacity rule of init_model (gmpm_simulator.cuh:173): n/32 bins + one partial bin per block
@@ -876,6 +907,16 @@ int cb200_sim_init_model(cb200_sim* s, int material, const float* positions_host
 		CK(cudaMemsetAsync(m.celloffs[i], 0, (mb + 1) * kBlockVol * sizeof(unsigned short), s->stream));
 	}
 	CK(pool_alloc(&m.d_pos, (size_t) n * 3 * sizeof(float)));
+	return 0;
+}
+
+int cb200_sim_init_model(cb200_sim* s, int material, const float* positions_host, int n, const float* v0, int* model_id) {
+	if(!s || s->setup_done || material < 0 || material > 3 || n <= 0 || (int) s->models.size() >= kMaxModels) return (int) cudaErrorInvalidValue;
+	Model m;
+	m.material = material;
+	m.n = n;
+	for(int d = 0; d < 3; ++d) m.v0[d] = v0 ? v0[d] : 0.f;
+	CK(alloc_model(s, m));
 	CK(cudaMemcpyAsync(m.d_pos, positions_host, (size_t) n * 3 * sizeof(float), cudaMemcpyHostToDevice, s->stream));
 	CK(cudaStreamSynchronize(s->stream));
 	if(model_id) *model_id = (int) s->models.size();
@@ -925,8 +966,18 @@ int cb200_sim_update_nacc_parameters(cb200_sim* s, int model, float rho, float v
 	return 0;
 }
 
-// initial_setup  gmpm_simulator.cuh:637-781 (counts are read back here: one-time cost)
-int cb200_sim_initial_setup(cb200_sim* s) {
+// What cb200_sim_restore puts in place of the rasterised start: the saved state, already on the device.
+struct RestoreSrc {
+	const cb200_checkpoint_info* info;
+	const float* state[kMaxModels];  // [count][channels] per model
+	const int* keys;                 // [nbc][3]
+	const float* grid;               // [nbc][256]
+};
+
+// initial_setup  gmpm_simulator.cuh:637-781 (counts are read back here: one-time cost).  With `rs` (restore) it differs in three
+// places: the bins get the saved channels, grid[0] gets the saved blocks (no MGSP halo reduction: they hold the full sums), and the
+// step state gets the saved clock.
+static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 	if(!s || s->setup_done || s->models.empty()) return (int) cudaErrorInvalidValue;
 	cudaStream_t st = s->stream;
 	const Cfg& cfg = s->cfg;
@@ -952,7 +1003,8 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 		a.in = m.bin_sizes;
 		a.out = m.pb[R].bin_offsets;
 		scan_kernel<<<1, 1024, 0, st>>>(a);
-		array_to_buffer_kernel<<<blocks_for(pbc, 1), 128, 0, st>>>(cfg, m.material, pbc, m.d_pos, view(m.pb[R]));
+		if(rs) state_to_bins_kernel<<<blocks_for(pbc, 1), 128, 0, st>>>(cfg, m.material, pbc, rs->state[&m - s->models.data()], view(m.pb[R]));
+		else array_to_buffer_kernel<<<blocks_for(pbc, 1), 128, 0, st>>>(cfg, m.material, pbc, m.d_pos, view(m.pb[R]));
 		s->launches += 5;
 	}
 	{
@@ -1002,13 +1054,30 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 	}
 	clear_grid_kernel<<<blocks_for((long long) nbc * 64, 256), 256, 0, st>>>(nbc, s->grid[0]);
 	++s->launches;
+	int* missing = s->d_scratch + 6;
+	if(rs) {  // the saved blocks by key; a key the rebuilt partition has no neighbour block for is counted, not written
+		const int saved = rs->info->neighbor_block_count;
+		CK(cudaMemsetAsync(missing, 0, sizeof(int), st));
+		scatter_grid_kernel<<<blocks_for(saved, 8), 256, 0, st>>>(cfg, saved, rs->keys, rs->grid, s->part[R].index_table, nbc, s->grid[0], missing);
+		++s->launches;
+	}
 	for(Model& m : s->models) {
-		rasterize_blocks_kernel<<<blocks_for(pbc, 1), 256, 0, st>>>(cfg, m.material, pbc, s->part[R].active_keys, s->part[R].index_table, view(m.pb[R]), s->grid[0], m.pb[R].mass, m.v0[0], m.v0[1], m.v0[2], err);
+		if(!rs) {
+			rasterize_blocks_kernel<<<blocks_for(pbc, 1), 256, 0, st>>>(cfg, m.material, pbc, s->part[R].active_keys, s->part[R].index_table, view(m.pb[R]), s->grid[0], m.pb[R].mass, m.v0[0], m.v0[1], m.v0[2], err);
+			++s->launches;
+		}
 		init_adv_bucket_kernel<<<blocks_for(pbc, 1), 128, 0, st>>>(cfg, pbc, m.pb[Rn].particle_bucket_sizes, m.pb[Rn].blockbuckets);
-		s->launches += 2;
+		++s->launches;
 	}
 	CK(cudaGetLastError());
-	if(s->desc.mgsp_world > 1) {  // the rasterised halo blocks are partial sums: reduce them (mgsp_benchmark.cuh:653-654, 723-776)
+	if(rs) {  // a blob that passed inspect but does not rebuild the saved partition (hand-edited): nothing to step
+		int miss = 0;
+		CK(cudaMemcpyAsync(&miss, missing, sizeof(int), cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+		const cb200_checkpoint_info& I = *rs->info;
+		if(miss || pbc != I.particle_block_count || nbc != I.neighbor_block_count || ebc != I.exterior_block_count) return (int) cudaErrorIllegalState;
+	}
+	if(s->desc.mgsp_world > 1 && !rs) {  // the rasterised halo blocks are partial sums: reduce them (mgsp_benchmark.cuh:653-654, 723-776)
 		mgsp_pack_send_kernel<<<grid_blocks(2), 256, 0, st>>>(cfg, mgsp_view(s), s->grid[0], s->part[R].index_table);
 		mgsp_wait_reduce_kernel<<<grid_blocks(2), 256, 0, st>>>(cfg, mgsp_view(s), s->grid[0], s->part[R].index_table, err);
 		s->launches += 2;
@@ -1026,9 +1095,22 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 	h.frame_time = s->desc.fps > 0 ? 1.f / (float) s->desc.fps : 0.f;
 	h.step_time = 0.f;
 	h.sim_time = 0.0;
+	if(rs) {
+		const cb200_checkpoint_info& I = *rs->info;
+		h.frame_time = I.frame_time;
+		h.step_time = I.step_time;
+		h.sim_time = I.sim_time;
+		h.dt = I.dt;
+		h.next_dt = I.next_dt;
+		h.steps = I.steps;
+		h.error |= I.error;
+		h.max_vel_sq = 0.f;
+		s->frames_done = I.frames;
+		CK(push_state(s));
+	}
 	float mv = 0.f;
 	for(const Model& m : s->models) mv = fmaxf(mv, sqrtf(m.v0[0] * m.v0[0] + m.v0[1] * m.v0[1] + m.v0[2] * m.v0[2]));
-	if(s->desc.mgsp_world > 1) {  // every rank must start from the same dt: max over the ranks' initial speeds
+	if(s->desc.mgsp_world > 1 && !rs) {  // every rank must start from the same dt: max over the ranks' initial speeds
 		h.max_vel_sq = mv * mv;
 		CK(push_state(s));
 		mgsp_allreduce_maxvel_kernel<<<1, 32, 0, st>>>(mgsp_view(s), &s->d_state->max_vel_sq);
@@ -1036,13 +1118,15 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 		CK(pull_state(s));
 		mv = sqrtf(s->h_state->max_vel_sq);
 	}
-	float dt = h.dt_default;
-	if(mv > 0.f) dt = fminf(dt, cfg.dx * cfg.cfl / mv);
-	if(h.frame_time > 0.f) dt = fminf(dt, h.frame_time);
-	h.dt = dt;
-	h.next_dt = dt;
-	h.max_vel_sq = 0.f;
-	CK(push_state(s));
+	if(!rs) {
+		float dt = h.dt_default;
+		if(mv > 0.f) dt = fminf(dt, cfg.dx * cfg.cfl / mv);
+		if(h.frame_time > 0.f) dt = fminf(dt, h.frame_time);
+		h.dt = dt;
+		h.next_dt = dt;
+		h.max_vel_sq = 0.f;
+		CK(push_state(s));
+	}
 	if(s->desc.mgsp_world > 1) {
 		// global max |v|^2 of the start grid (later sub-steps get it from the end-of-step exchange of the previous one)
 		if(s->has_collider) grid_max_kernel<true><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->collider);
@@ -1057,6 +1141,26 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 	}
 	s->setup_done = true;
 	return 0;
+}
+int cb200_sim_initial_setup(cb200_sim* s) {
+	if(!s || !s->restore_pending) return setup_impl(s, nullptr);
+	RestoreSrc rs {};
+	rs.info = &s->restore_info;
+	for(int m = 0; m < kMaxModels; ++m) rs.state[m] = s->restore_state[m];
+	rs.grid = reinterpret_cast<const float*>(s->restore_grid);
+	rs.keys = reinterpret_cast<const int*>(s->restore_grid + s->restore_info.grid_bytes);
+	int e = setup_impl(s, &rs);
+	if(!e) e = (int) cudaStreamSynchronize(s->stream);
+	if(!e) {  // the staged state is in the bins and the grid now
+		for(float*& p : s->restore_state) {
+			g_pool.release(p);
+			p = nullptr;
+		}
+		g_pool.release(s->restore_grid);
+		s->restore_grid = nullptr;
+		s->restore_pending = false;
+	}
+	return e;
 }
 
 static int set_frame_roll(cb200_sim* s, int on) {
@@ -1137,6 +1241,7 @@ int cb200_sim_advance_frame(cb200_sim* s, int* steps_taken) {
 		if(e) return e;
 		taken += batch;
 	}
+	++s->frames_done;
 	if(steps_taken) *steps_taken = taken;
 	return 0;
 }
@@ -1271,6 +1376,204 @@ int cb200_sim_time(cb200_sim* s, double* time) {
 	*time = s->h_state->sim_time;
 	return 0;
 }
+// ---- checkpoint / restore (format and kernels: checkpoint.cuh) ---------------------------------------------------------------
+int cb200_checkpoint_inspect(const void* blob, size_t bytes, cb200_checkpoint_info* info) { return ck_parse(blob, bytes, info); }
+
+}  // extern "C"
+namespace {
+size_t ck_capacity(const cb200_sim* s) {
+	int mats[kMaxModels];
+	long long counts[kMaxModels];
+	for(size_t m = 0; m < s->models.size(); ++m) {
+		mats[m] = s->models[m].material;
+		counts[m] = s->models[m].n;
+	}
+	return (size_t) ck_layout((int) s->models.size(), mats, counts, s->desc.max_blocks).total;
+}
+// grows a checkpoint buffer to `need` bytes (contents are not kept)
+template<typename T>
+int ck_grow(T*& p, size_t& have, size_t need) {
+	if(have >= need) return 0;
+	g_pool.release(p);
+	p = nullptr;
+	have = 0;
+	CK(pool_alloc(&p, need));
+	have = need;
+	return 0;
+}
+}  // namespace
+extern "C" {
+
+int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
+	if(!s || !s->setup_done) return (int) cudaErrorInvalidValue;
+	if(s->ck_pending) CK(cudaEventSynchronize(s->ck_copied));  // the pinned blob and the staging blob are re-used
+	s->ck_pending = s->ck_ready = false;
+	if(!s->ck_stream) {
+		CK(cudaStreamCreateWithFlags(&s->ck_stream, cudaStreamNonBlocking));
+		CK(cudaEventCreateWithFlags(&s->ck_gathered, cudaEventDisableTiming));
+		CK(cudaEventCreateWithFlags(&s->ck_copied, cudaEventDisableTiming));
+	}
+	const size_t cap = ck_capacity(s);
+	CK(ck_grow(s->ck_dev, s->ck_dev_bytes, cap));
+	CK(ck_grow(s->ck_base, s->ck_base_bytes, (size_t) kMaxModels * (s->desc.max_blocks + 1) * sizeof(int)));
+	if(s->ck_host_bytes < cap) {
+		if(s->ck_host) cudaFreeHost(s->ck_host);
+		s->ck_host = nullptr;
+		s->ck_host_bytes = 0;
+		CK(cudaMallocHost(&s->ck_host, cap));
+		s->ck_host_bytes = cap;
+	}
+	const int R = s->rollid, Rn = R ^ 1;
+	const int nm = (int) s->models.size();
+	cudaStream_t st = s->stream;
+	SnapshotArgs a {};
+	a.cfg = s->cfg;
+	a.state = s->d_state;
+	a.n_models = nm;
+	for(int m = 0; m < nm; ++m) {
+		const Model& md = s->models[m];
+		int* base = s->ck_base + (size_t) m * (s->desc.max_blocks + 1);
+		ScanArgs sc {};
+		sc.count = count_dev(&s->d_state->pbc);
+		sc.count_plus = 1;
+		sc.in = md.pb[Rn].particle_bucket_sizes;
+		sc.out = base;
+		scan_kernel<<<1, 1024, 0, st>>>(sc);
+		++s->launches;
+		a.material[m] = md.material;
+		a.cur[m] = view(md.pb[R]);
+		a.next[m] = view(md.pb[Rn]);
+		a.base[m] = base;
+	}
+	a.keys = s->part[R].active_keys;
+	a.prev_table = s->part[Rn].index_table;
+	a.grid = s->grid[0];
+	a.out = s->ck_dev;
+	snapshot_kernel<<<num_sms() * 8, kSnapThreads, 0, st>>>(a);
+	++s->launches;
+	CK(cudaGetLastError());
+	CK(cudaEventRecord(s->ck_gathered, st));
+	// the counts the layout follows from: the step state (pbc, nbc, clock), then each model's total, entry pbc of its scan
+	CK(pull_state(s));
+	const StepState& h = *s->h_state;
+	int totals[kMaxModels] = {};
+	for(int m = 0; m < nm; ++m) CK(cudaMemcpyAsync(&totals[m], s->ck_base + (size_t) m * (s->desc.max_blocks + 1) + h.pbc, sizeof(int), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	cb200_checkpoint_info I;
+	memset(&I, 0, sizeof(I));
+	int mats[kMaxModels];
+	long long counts[kMaxModels];
+	for(int m = 0; m < nm; ++m) {
+		mats[m] = s->models[m].material;
+		counts[m] = totals[m];
+	}
+	const CkLayout L = ck_layout(nm, mats, counts, h.nbc);
+	I.version = CB200_CHECKPOINT_VERSION;
+	I.n_models = nm;
+	I.bytes = L.total;
+	I.cfg = s->desc.cfg;
+	I.dt_default = s->desc.dt_default;
+	I.fps = s->desc.fps;
+	I.mgsp_rank = s->desc.mgsp_world > 1 ? s->desc.mgsp_rank : 0;
+	I.mgsp_world = s->desc.mgsp_world;
+	I.error = h.error;
+	I.dt = h.dt;
+	I.next_dt = h.next_dt;
+	I.step_time = h.step_time;
+	I.frame_time = h.frame_time;
+	I.sim_time = h.sim_time;
+	I.steps = h.steps;
+	I.frames = s->frames_done;
+	I.particle_block_count = h.pbc;
+	I.neighbor_block_count = h.nbc;
+	I.exterior_block_count = h.ebc;
+	I.max_blocks = s->desc.max_blocks;
+	I.keys_offset = L.keys_off;
+	I.keys_bytes = L.keys_bytes;
+	I.grid_offset = L.grid_off;
+	I.grid_bytes = L.grid_bytes;
+	for(int m = 0; m < nm; ++m) {
+		cb200_checkpoint_model& md = I.models[m];
+		md.material = mats[m];
+		md.channels = ck_channels(mats[m]);
+		md.count = counts[m];
+		md.offset = L.model_off[m];
+		md.bytes = L.model_bytes[m];
+		md.params = s->models[m].pb[0];
+		md.params.bins = nullptr;
+		md.params.cell_particle_counts = md.params.particle_bucket_sizes = md.params.cellbuckets = md.params.blockbuckets = md.params.bin_offsets = nullptr;
+	}
+	ck_write_header(s->ck_host, I);
+	// the data sections: behind the snapshot, on the copy stream, so that sub-steps enqueued from here on run alongside
+	CK(cudaStreamWaitEvent(s->ck_stream, s->ck_gathered, 0));
+	CK(cudaMemcpyAsync(s->ck_host + kCkHeader, s->ck_dev + kCkHeader, L.total - kCkHeader, cudaMemcpyDeviceToHost, s->ck_stream));
+	CK(cudaEventRecord(s->ck_copied, s->ck_stream));
+	s->ck_bytes = L.total;
+	s->ck_pending = true;
+	if(bytes) *bytes = L.total;
+	return 0;
+}
+
+int cb200_sim_checkpoint_end(cb200_sim* s, const void** blob, size_t* bytes) {
+	if(!s || (!s->ck_pending && !s->ck_ready)) return (int) cudaErrorInvalidValue;
+	if(s->ck_pending) {
+		CK(cudaEventSynchronize(s->ck_copied));
+		s->ck_pending = false;
+		s->ck_ready = true;
+	}
+	if(blob) *blob = s->ck_host;
+	if(bytes) *bytes = s->ck_bytes;
+	return 0;
+}
+
+int cb200_sim_restore_models(cb200_sim* s, const void* blob, size_t bytes) {
+	cb200_checkpoint_info I;
+	if(!s || s->setup_done || s->restore_pending || !s->models.empty() || ck_parse(blob, bytes, &I) != 0) return (int) cudaErrorInvalidValue;
+	const cb200_config& c = s->desc.cfg;
+	if(c.domain_bits != I.cfg.domain_bits || c.max_ppc != I.cfg.max_ppc || c.boundary != I.cfg.boundary || memcmp(&c.gravity, &I.cfg.gravity, sizeof(float)) != 0 ||
+	   memcmp(&c.cfl, &I.cfg.cfl, sizeof(float)) != 0 || memcmp(&s->desc.dt_default, &I.dt_default, sizeof(float)) != 0 || s->desc.fps != I.fps ||
+	   s->desc.mgsp_world != I.mgsp_world || (s->desc.mgsp_world > 1 ? s->desc.mgsp_rank : 0) != I.mgsp_rank)
+		return (int) cudaErrorInvalidValue;
+	if(s->desc.max_blocks < I.exterior_block_count) return (int) cudaErrorMemoryAllocation;
+	const unsigned char* src = static_cast<const unsigned char*>(blob);
+	cudaStream_t st = s->stream;
+	s->restore_info = I;
+	s->restore_pending = true;
+	for(int m = 0; m < I.n_models; ++m) {
+		const cb200_checkpoint_model& md = I.models[m];
+		Model model;
+		model.material = md.material;
+		model.n = (int) md.count;
+		CK(alloc_model(s, model));
+		for(int i = 0; i < 2; ++i) {  // the saved parameters, the containers of this simulator
+			cb200_particle_buffer& pb = model.pb[i];
+			cb200_particle_buffer p = md.params;
+			p.bins = pb.bins;
+			p.cell_particle_counts = pb.cell_particle_counts;
+			p.particle_bucket_sizes = pb.particle_bucket_sizes;
+			p.cellbuckets = pb.cellbuckets;
+			p.blockbuckets = pb.blockbuckets;
+			p.bin_offsets = pb.bin_offsets;
+			pb = p;
+		}
+		s->models.push_back(model);
+		CK(pool_alloc(&s->restore_state[m], md.bytes));
+		CK(cudaMemcpyAsync(s->restore_state[m], src + md.offset, md.bytes, cudaMemcpyHostToDevice, st));
+		state_positions_kernel<<<num_sms() * 4, 256, 0, st>>>(md.count, md.channels, s->restore_state[m], s->models.back().d_pos);
+		++s->launches;
+	}
+	CK(pool_alloc(&s->restore_grid, (size_t) I.grid_bytes + (size_t) I.keys_bytes));
+	CK(cudaMemcpyAsync(s->restore_grid, src + I.grid_offset, I.grid_bytes, cudaMemcpyHostToDevice, st));
+	CK(cudaMemcpyAsync(s->restore_grid + I.grid_bytes, src + I.keys_offset, I.keys_bytes, cudaMemcpyHostToDevice, st));
+	CK(cudaGetLastError());
+	return (int) cudaStreamSynchronize(st);
+}
+
+int cb200_sim_restore(cb200_sim* s, const void* blob, size_t bytes) {
+	CK(cb200_sim_restore_models(s, blob, bytes));
+	return cb200_sim_initial_setup(s);
+}
+
 int cb200_trim_pool(void) {
 	g_pool.trim();
 	return 0;

@@ -36,6 +36,7 @@ class GmpmSimulator:
         check(self.L.cb200_sim_create(C.byref(self.desc), self._stream, C.byref(self.h)), "cb200_sim_create")
         self.materials, self.counts = [], []
         self.cur_frame = 0
+        self.restored = False
 
     # ---- lifecycle -------------------------------------------------------------------------------
     def close(self):
@@ -89,9 +90,11 @@ class GmpmSimulator:
         return n.value
 
     def main_loop(self, on_frame=None):
-        """initial_setup + nframes frames (gmpm_simulator.cuh:303-591); on_frame(sim, frame) replaces the bgeo dump."""
-        self.initial_setup()
-        for f in range(1, self.nframes + 1):
+        """initial_setup + nframes frames (gmpm_simulator.cuh:303-591); on_frame(sim, frame) replaces the bgeo dump.
+        A restored simulator is set up already and runs only the frames after the ones its checkpoint had finished."""
+        if not self.restored:
+            self.initial_setup()
+        for f in range(self.cur_frame + 1, self.nframes + 1):
             self.advance_frame()
             if self.stats().error:
                 break
@@ -147,6 +150,56 @@ class GmpmSimulator:
         t = C.c_double(0.0)
         check(self.L.cb200_sim_time(self.h, C.byref(t)), "sim_time")
         return t.value
+
+    # ---- checkpoint / restore (format: include/claymore_b200.h, reader: claymore_b200.checkpoint) -------------------
+    def checkpoint_begin(self):
+        """Snapshot at the current sub-step boundary; returns the blob's size without waiting for its copy to the host, so
+        sub-steps issued before checkpoint_end overlap with it."""
+        n = C.c_size_t(0)
+        check(self.L.cb200_sim_checkpoint_begin(self.h, C.byref(n)), "checkpoint_begin")
+        return n.value
+
+    def checkpoint_end(self, path=None):
+        """Waits for the copy of the last checkpoint_begin.  Writes the blob to `path`, or returns a copy of it (uint8 array)."""
+        p, n = C.c_void_p(), C.c_size_t(0)
+        check(self.L.cb200_sim_checkpoint_end(self.h, C.byref(p), C.byref(n)), "checkpoint_end")
+        blob = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_ubyte)), shape=(n.value,))
+        if path is None:
+            return blob.copy()
+        with open(path, "wb") as f:
+            f.write(memoryview(blob))
+        return n.value
+
+    def save_checkpoint(self, path=None):
+        """checkpoint_begin + checkpoint_end: the whole state at this sub-step boundary to `path` (or returned as bytes)."""
+        self.checkpoint_begin()
+        return self.checkpoint_end(path)
+
+    @classmethod
+    def from_checkpoint(cls, path, **overrides):
+        """A simulator matching a checkpoint (config, dt_default, fps, MGSP rank / world; capacity defaults to the saved one),
+        not yet restored: set a collider or wire MGSP peers, then call restore(path)."""
+        from . import checkpoint
+        inf = checkpoint.inspect(path)[0]
+        c = inf.cfg
+        kw = dict(dt=inf.dt_default, fps=inf.fps, config=Config(c.domain_bits, c.max_ppc, c.boundary, c.gravity, c.cfl), max_blocks=inf.max_blocks,
+                  mgsp_rank=inf.mgsp_rank, mgsp_world=inf.mgsp_world)
+        kw.update(overrides)
+        return cls(**kw)
+
+    def restore(self, path_or_blob, setup=True):
+        """In place of init_model + initial_setup: the models, grid and clock of a checkpoint (file path or blob).
+        setup=False only registers the models and stages their state (in place of init_model); initial_setup() then restores.
+        MGSP ranks sharing a device in one process do that on every rank first, then run initial_setup concurrently."""
+        from . import checkpoint
+        inf, blob = checkpoint.inspect(path_or_blob)
+        data = np.ascontiguousarray(blob)   # one read of the file; the library copies it to the device
+        fn = self.L.cb200_sim_restore if setup else self.L.cb200_sim_restore_models
+        check(fn(self.h, data.ctypes.data_as(C.c_void_p), data.size), "restore")
+        self.materials = [m.material for m in inf.models[: inf.n_models]]
+        self.counts = [m.count for m in inf.models[: inf.n_models]]
+        self.cur_frame = inf.frames
+        self.restored = True
 
     # ---- observation --------------------------------------------------------------------------------
     def stats(self):

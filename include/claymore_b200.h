@@ -226,6 +226,76 @@ CB200_API int cb200_sim_clear_collider(cb200_sim* sim);
 CB200_API int cb200_sim_time(cb200_sim* sim, double* time);
 /* number of kernels this library launched on behalf of `sim` since creation */
 CB200_API long long cb200_sim_launch_count(cb200_sim* sim);
+
+/* ------------------------------------------------------------------------------------------------
+ * Checkpoint / restore of a running simulation at a sub-step boundary.  The checkpoint holds the physical state, not the
+ * device containers, so it restores into a simulator of any block capacity, graph mode or auto_grow setting.
+ *
+ * Blob layout (all little-endian; every offset and size is a 64-bit byte count from the start of the blob):
+ *   header, CB200_CHECKPOINT_HEADER_BYTES (1024) bytes:
+ *     0 char[8] "CB200CKP" | 8 u32 version | 12 u32 n_models (1..8) | 16 u64 bytes (whole blob)
+ *     24 cb200_config (i32 domain_bits, i32 max_ppc, i32 boundary, f32 gravity, f32 cfl)
+ *     44 f32 dt_default | 48 i32 fps | 52 i32 mgsp_rank | 56 i32 mgsp_world | 60 i32 error bits
+ *     64 f32 dt | 68 f32 next_dt | 72 f32 step_time | 76 f32 frame_time | 80 f64 sim_time | 88 i64 steps
+ *     96 i64 frames (finished by cb200_sim_advance_frame) | 104 i32 pbc | 108 i32 nbc | 112 i32 ebc | 116 i32 max_blocks at save
+ *     120 u64 keys_offset | 128 u64 keys_bytes | 136 u64 grid_offset | 144 u64 grid_bytes | 152..255 zero
+ *     256 + 96 m, m < 8: table of contents entry of model m (zero when m >= n_models):
+ *       0 i32 material | 4 i32 channels (4 / 12 / 13) | 8 i64 count | 16 u64 offset | 24 u64 bytes (= count * channels * 4)
+ *       32 sixteen 4-byte parameters in cb200_particle_buffer order, rho .. hardening_on
+ *   data sections (written 256-byte aligned, in this order; a reader must use the offsets):
+ *     per model: float state[count][channels], the layout of cb200_sim_particle_state
+ *     int32 keys[nbc][3]: the grid blocks of grid[0] (particle blocks first)
+ *     float grid[nbc][256]: mass and momentum the next sub-step's grid update starts from, layout of a grid block
+ * Particle rows are in partition order, then bucket order inside a block: two checkpoints of an unchanged simulator are
+ * byte-identical.  The collider field is not stored: set it before cb200_sim_restore. */
+#define CB200_CHECKPOINT_VERSION 1
+#define CB200_CHECKPOINT_HEADER_BYTES 1024
+typedef struct cb200_checkpoint_model {
+	int material;
+	int channels;
+	long long count;
+	unsigned long long offset, bytes;
+	cb200_particle_buffer params; /* pointers are null */
+} cb200_checkpoint_model;
+typedef struct cb200_checkpoint_info {
+	unsigned int version;
+	int n_models;
+	unsigned long long bytes;
+	cb200_config cfg;
+	float dt_default;
+	int fps, mgsp_rank, mgsp_world;
+	int error;
+	float dt, next_dt, step_time, frame_time;
+	double sim_time;
+	long long steps, frames;
+	int particle_block_count, neighbor_block_count, exterior_block_count, max_blocks;
+	unsigned long long keys_offset, keys_bytes, grid_offset, grid_bytes;
+	cb200_checkpoint_model models[8];
+} cb200_checkpoint_info;
+/* Host only, needs no device: validates a blob and fills *info.  cudaErrorInvalidValue for a bad magic or version, a blob shorter
+ * or longer than its header says, sections that overlap the header or each other or run past `bytes`, section sizes that disagree
+ * with count x channels or nbc, more than 8 (or no) models, a material out of range, counts that are not 0 < count < 2^31 and
+ * 0 < pbc <= nbc <= ebc, and keys outside the domain or repeated. */
+CB200_API int cb200_checkpoint_inspect(const void* blob, size_t bytes, cb200_checkpoint_info* info);
+/* Snapshot at the current sub-step boundary, enqueued on the simulator's stream; waits for the snapshot kernel (not for the sub-steps
+ * queued after it), then queues the copy into a pinned buffer the simulator owns on a stream of its own and returns.  *bytes: size
+ * of the blob.  Sub-steps enqueued afterwards overlap with the copy. */
+CB200_API int cb200_sim_checkpoint_begin(cb200_sim* sim, size_t* bytes);
+/* waits for the copy of the last begin; *blob_pinned stays valid until the next begin, reserve or destroy */
+CB200_API int cb200_sim_checkpoint_end(cb200_sim* sim, const void** blob_pinned, size_t* bytes);
+/* In place of init_model + initial_setup on a freshly created simulator (no models): rebuilds the partition, bins and buckets from the
+ * saved particles, the grid from the saved blocks and the step clock from the saved one.  cudaErrorInvalidValue (simulator unchanged)
+ * for a blob inspect rejects, a simulator that has models or is set up, or a cb200_config, dt_default, fps, mgsp_rank or mgsp_world
+ * that differs from the simulator's; cudaErrorMemoryAllocation (unchanged) when max_blocks is below the saved ebc.  A blob that
+ * passes inspect but whose particles or keys do not rebuild the saved partition returns cudaErrorIllegalState without writing out of
+ * bounds; such a simulator can only be destroyed.
+ * restore = restore_models + initial_setup.  restore_models takes the place of init_model: it checks the blob as above, registers
+ * the saved models and stages their state on the device (it allocates, so it synchronises the device); the next initial_setup
+ * restores instead of rasterising.  MGSP ranks that share a device in one process call restore_models on every rank, wire the
+ * peers, then run initial_setup concurrently, as after init_model.  The first checkpoint_begin allocates a pinned buffer: in that
+ * configuration take it while no rank has sub-steps in flight. */
+CB200_API int cb200_sim_restore_models(cb200_sim* sim, const void* blob_host, size_t bytes);
+CB200_API int cb200_sim_restore(cb200_sim* sim, const void* blob_host, size_t bytes);
 /* per-kernel timing for the roofline: while enabled, sub-steps are issued as plain stream launches with a
  * cudaEvent pair around every g2p2g launch; profile_read synchronises and returns the summed duration */
 CB200_API int cb200_sim_profile(cb200_sim* sim, int enable);

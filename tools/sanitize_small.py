@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Small driver for compute-sanitizer runs (memcheck / racecheck / synccheck) of the whole sub-step on an H100:
     compute-sanitizer --tool racecheck python tools/sanitize_small.py [scene] [steps]
-Scenes: small_cube (one model), two_models, mixed (fluid + sand + fixed-corotated in one partition)."""
+Scenes: small_cube (one model), two_models, mixed (fluid + sand + fixed-corotated in one partition), checkpoint (mixed: step,
+checkpoint, restore into a fresh simulator, step again)."""
 import os
 import sys
 
@@ -22,6 +23,14 @@ def main():
     sim = scenes.build_engine(scene, use_graph=False, auto_grow=False)
     sim.step(steps)
     sim.sync()
+    if name == "checkpoint":
+        from claymore_b200.simulator import GmpmSimulator
+        blob = sim.save_checkpoint()
+        sim.close()
+        sim = GmpmSimulator.from_checkpoint(blob, use_graph=False, auto_grow=False)
+        sim.restore(blob)
+        sim.step(steps)
+        sim.sync()
     st = sim.stats()
     print("SANITIZE_RUN", name, steps, scenes.n_particles(scene), st.particle_block_count, st.neighbor_block_count, st.exterior_block_count, "error", st.error)
     sim.close()
