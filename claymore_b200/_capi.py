@@ -75,6 +75,9 @@ class Collider(C.Structure):
                 ("dsdt", C.c_float), ("scale", C.c_float), ("friction", C.c_float), ("type", C.c_int)]
 
 
+OUTPUT_V, OUTPUT_J = 1, 2        # CB200_OUTPUT_V / CB200_OUTPUT_J: per-particle attributes of a frame's .bgeo files
+ERROR_OUTPUT_IO = 2000           # CB200_ERROR_OUTPUT_IO
+
 CHECKPOINT_VERSION = 1          # CB200_CHECKPOINT_VERSION
 CHECKPOINT_HEADER_BYTES = 1024  # CB200_CHECKPOINT_HEADER_BYTES
 
@@ -174,6 +177,10 @@ _SIGNATURES = {
     "cb200_sim_checkpoint_end": [_P, C.POINTER(_P), C.POINTER(C.c_size_t)],
     "cb200_sim_restore_models": [_P, _P, C.c_size_t],
     "cb200_sim_restore": [_P, _P, C.c_size_t],
+    "cb200_bgeo_header": [C.c_longlong, C.c_uint, _P, C.c_size_t, C.POINTER(C.c_size_t)],
+    "cb200_bgeo_trailer": [_P, C.c_size_t, C.POINTER(C.c_size_t)],
+    "cb200_sim_frame_output": [_P, C.POINTER(C.c_char_p), C.c_uint],
+    "cb200_sim_frame_output_wait": [_P, C.POINTER(_I)],
     "cb200_trim_pool": [],
     "cb200_test_svd3": [_I, _P, _P, _P, _P, _P],
     "cb200_test_stress": [_I, _I, ParticleBuffer, _I, _P, _P, _P, _P, _P, _P],

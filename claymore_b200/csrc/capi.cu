@@ -93,7 +93,7 @@ cudaError_t launch_g2p2g(int material, const G2P2GArgs& a, int block_hint, cudaS
 extern "C" {
 
 const char* cb200_version(void) { return "claymore_b200 0.1 (sm_90a)"; }
-const char* cb200_error_string(int err) { return cudaGetErrorString((cudaError_t) err); }
+const char* cb200_error_string(int err) { return err == CB200_ERROR_OUTPUT_IO ? "frame output: a file could not be opened or written" : cudaGetErrorString((cudaError_t) err); }
 
 int cb200_g2p2g(const cb200_config* c, float dt, float new_dt, int pbc, cb200_particle_buffer cur, cb200_particle_buffer next, cb200_partition prev_partition, cb200_partition partition, const float* grid, float* next_grid, void* stream) {
 	CB_CFG(c);

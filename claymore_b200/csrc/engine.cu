@@ -9,13 +9,20 @@
 //   * that sequence is captured once per roll parity into a CUDA graph and replayed;
 //   * every kernel runs on a persistent grid sized from the SM count and loops over device-read counts;
 //   * clears, marks, bucket compaction and the grid carry are fused as described in partition.cuh / grid.cuh.
-// Not built in this compiled library: file IO (the async .bgeo writer thread).  The JSON scene loader lives in
-// the Python host layer (claymore_b200/scene.py).
+//   * per-frame .bgeo output: the body of each file is gathered on the device, a writer thread the simulator owns writes the files
+//     while the next sub-steps run (the reference's IO thread, Library/MnSystem/IO/IO.h).
+// The JSON scene loader lives in the Python host layer (claymore_b200/scene.py).
+#include <fcntl.h>
+#include <unistd.h>
+
+#include <cerrno>
+#include <condition_variable>
 #include <cstdio>
 #include <cstring>
 #include <map>
 #include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "checkpoint.cuh"
@@ -23,6 +30,7 @@
 #include "grid.cuh"
 #include "init.cuh"
 #include "mgsp.cuh"
+#include "output.cuh"
 #include "partition.cuh"
 
 namespace cb200 {
@@ -255,6 +263,26 @@ struct cb200_sim {
 	cb200_checkpoint_info restore_info {};
 	float* restore_state[kMaxModels] = {};
 	unsigned char* restore_grid = nullptr;  // grid blocks, then keys
+	// frame output (cb200_sim_frame_output): device staging of the records, its pinned copy (written on a stream of its own), and the
+	// writer thread with its one job; allocated / started on first use.  `out_busy`: a frame is queued or being written
+	unsigned char* out_dev = nullptr;
+	size_t out_dev_bytes = 0;
+	unsigned char* out_host = nullptr;  // pinned
+	size_t out_host_bytes = 0;
+	cudaStream_t out_stream = nullptr;
+	cudaEvent_t out_copied = nullptr;
+	std::thread out_thread;
+	std::mutex out_mu;
+	std::condition_variable out_cv;
+	bool out_busy = false, out_quit = false;
+	struct OutputFile {
+		std::string path;
+		std::vector<unsigned char> header;
+		const unsigned char* body;
+		size_t body_bytes;
+	};
+	std::vector<OutputFile> out_files;
+	int out_errno = 0;  // first failure of a queued frame, until cb200_sim_frame_output_wait collects it
 };
 
 namespace {
@@ -632,6 +660,7 @@ void preload_kernels() {
 	preload(state_positions_kernel);
 	preload(state_to_bins_kernel);
 	preload(scatter_grid_kernel);
+	preload(output_kernel);
 	g2p2g_prepare_all();
 }
 int ensure_graph(cb200_sim* s, int R) {
@@ -673,6 +702,57 @@ int grow_array(cb200_sim* s, T*& p, size_t old_elems, size_t new_elems, int fill
 	p = q;
 	return 0;
 }
+
+// ---- frame output: the writer thread ------------------------------------------------------------------------------------------
+// One file: header, body, trailer.  Returns 0 or the errno of the failing open / write / close; a partially written file is removed.
+int write_bgeo(const cb200_sim::OutputFile& f) {
+	const int fd = open(f.path.c_str(), O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0644);
+	if(fd < 0) return errno;
+	auto put = [fd](const unsigned char* p, size_t n) {
+		while(n > 0) {
+			const ssize_t w = write(fd, p, std::min<size_t>(n, (size_t) 1 << 30));
+			if(w < 0) {
+				if(errno == EINTR) continue;
+				return errno;
+			}
+			p += w;
+			n -= (size_t) w;
+		}
+		return 0;
+	};
+	int e = put(f.header.data(), f.header.size());
+	if(!e) e = put(f.body, f.body_bytes);
+	if(!e) e = put(kBgeoTrailer, sizeof(kBgeoTrailer));
+	if(close(fd) != 0 && !e) e = errno;
+	if(e) unlink(f.path.c_str());
+	return e;
+}
+// Waits for the queued frame's copy, writes its files, records the first failure.  Ends when destroy asks it to and nothing is queued.
+void output_writer(cb200_sim* s) {
+	std::unique_lock<std::mutex> lk(s->out_mu);
+	for(;;) {
+		s->out_cv.wait(lk, [s] { return s->out_busy || s->out_quit; });
+		if(!s->out_busy) return;
+		std::vector<cb200_sim::OutputFile> files;
+		files.swap(s->out_files);
+		lk.unlock();
+		const bool copied = cudaEventSynchronize(s->out_copied) == cudaSuccess;  // (failed: nothing of this frame is written)
+		int e = copied ? 0 : EIO;
+		for(size_t i = 0; copied && i < files.size(); ++i) {
+			const int fe = write_bgeo(files[i]);
+			if(fe && !e) e = fe;
+		}
+		lk.lock();
+		if(e && !s->out_errno) s->out_errno = e;
+		s->out_busy = false;
+		s->out_cv.notify_all();
+	}
+}
+// blocks until no frame is queued or being written
+void output_idle(cb200_sim* s) {
+	std::unique_lock<std::mutex> lk(s->out_mu);
+	s->out_cv.wait(lk, [s] { return !s->out_busy; });
+}
 }  // namespace
 
 extern "C" {
@@ -694,6 +774,7 @@ int cb200_sim_reserve(cb200_sim* s, int new_max_blocks) {
 	if(s->desc.mgsp_world > 1) return (int) cudaErrorNotSupported;  // the next grid / inbox are mapped into the peers (CUDA IPC)
 	CK(cudaStreamSynchronize(s->stream));
 	if(s->ck_pending) CK(cudaEventSynchronize(s->ck_copied));  // the next begin re-sizes the staging blob
+	output_idle(s);
 	const size_t ob = (size_t) s->desc.max_blocks, nb = (size_t) new_max_blocks;
 	for(int i = 0; i < 2; ++i) {
 		if(s->graph[i]) {
@@ -826,6 +907,18 @@ static int sim_create_impl(cb200_sim* s, const cb200_sim_desc* desc, void* strea
 int cb200_sim_destroy(cb200_sim* s) {
 	if(!s) return 0;
 	cudaStreamSynchronize(s->stream);
+	if(s->out_thread.joinable()) {  // the queued frame is written, then the writer ends: no thread outlives the simulator
+		{
+			std::lock_guard<std::mutex> g(s->out_mu);
+			s->out_quit = true;
+		}
+		s->out_cv.notify_all();
+		s->out_thread.join();
+	}
+	g_pool.release(s->out_dev);
+	if(s->out_host) cudaFreeHost(s->out_host);
+	if(s->out_copied) cudaEventDestroy(s->out_copied);
+	if(s->out_stream) cudaStreamDestroy(s->out_stream);
 	if(s->ck_stream) cudaStreamSynchronize(s->ck_stream);  // a checkpoint copy may still read the staging blob
 	g_pool.release(s->ck_dev);
 	g_pool.release(s->ck_base);
@@ -1404,6 +1497,24 @@ int ck_grow(T*& p, size_t& have, size_t need) {
 }  // namespace
 extern "C" {
 
+// The row each particle block starts at in the checkpoint's order, per model: an exclusive scan of the bucket sizes of the current
+// partition into ck_base (entry pbc: the model's count), enqueued on the sim stream.  Shared by the checkpoint and the frame output,
+// which both wait for their gather before returning.
+static int enqueue_bucket_scans(cb200_sim* s) {
+	CK(ck_grow(s->ck_base, s->ck_base_bytes, (size_t) kMaxModels * (s->desc.max_blocks + 1) * sizeof(int)));
+	const int Rn = s->rollid ^ 1;
+	for(size_t m = 0; m < s->models.size(); ++m) {
+		ScanArgs sc {};
+		sc.count = count_dev(&s->d_state->pbc);
+		sc.count_plus = 1;
+		sc.in = s->models[m].pb[Rn].particle_bucket_sizes;
+		sc.out = s->ck_base + m * (s->desc.max_blocks + 1);
+		scan_kernel<<<1, 1024, 0, s->stream>>>(sc);
+		++s->launches;
+	}
+	return 0;
+}
+
 int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	if(!s || !s->setup_done) return (int) cudaErrorInvalidValue;
 	if(s->ck_pending) CK(cudaEventSynchronize(s->ck_copied));  // the pinned blob and the staging blob are re-used
@@ -1415,7 +1526,6 @@ int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	}
 	const size_t cap = ck_capacity(s);
 	CK(ck_grow(s->ck_dev, s->ck_dev_bytes, cap));
-	CK(ck_grow(s->ck_base, s->ck_base_bytes, (size_t) kMaxModels * (s->desc.max_blocks + 1) * sizeof(int)));
 	if(s->ck_host_bytes < cap) {
 		if(s->ck_host) cudaFreeHost(s->ck_host);
 		s->ck_host = nullptr;
@@ -1426,24 +1536,17 @@ int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	const int R = s->rollid, Rn = R ^ 1;
 	const int nm = (int) s->models.size();
 	cudaStream_t st = s->stream;
+	CK(enqueue_bucket_scans(s));
 	SnapshotArgs a {};
 	a.cfg = s->cfg;
 	a.state = s->d_state;
 	a.n_models = nm;
 	for(int m = 0; m < nm; ++m) {
 		const Model& md = s->models[m];
-		int* base = s->ck_base + (size_t) m * (s->desc.max_blocks + 1);
-		ScanArgs sc {};
-		sc.count = count_dev(&s->d_state->pbc);
-		sc.count_plus = 1;
-		sc.in = md.pb[Rn].particle_bucket_sizes;
-		sc.out = base;
-		scan_kernel<<<1, 1024, 0, st>>>(sc);
-		++s->launches;
 		a.material[m] = md.material;
 		a.cur[m] = view(md.pb[R]);
 		a.next[m] = view(md.pb[Rn]);
-		a.base[m] = base;
+		a.base[m] = s->ck_base + (size_t) m * (s->desc.max_blocks + 1);
 	}
 	a.keys = s->part[R].active_keys;
 	a.prev_table = s->part[Rn].index_table;
@@ -1529,6 +1632,7 @@ int cb200_sim_checkpoint_end(cb200_sim* s, const void** blob, size_t* bytes) {
 int cb200_sim_restore_models(cb200_sim* s, const void* blob, size_t bytes) {
 	cb200_checkpoint_info I;
 	if(!s || s->setup_done || s->restore_pending || !s->models.empty() || ck_parse(blob, bytes, &I) != 0) return (int) cudaErrorInvalidValue;
+	output_idle(s);
 	const cb200_config& c = s->desc.cfg;
 	if(c.domain_bits != I.cfg.domain_bits || c.max_ppc != I.cfg.max_ppc || c.boundary != I.cfg.boundary || memcmp(&c.gravity, &I.cfg.gravity, sizeof(float)) != 0 ||
 	   memcmp(&c.cfl, &I.cfg.cfl, sizeof(float)) != 0 || memcmp(&s->desc.dt_default, &I.dt_default, sizeof(float)) != 0 || s->desc.fps != I.fps ||
@@ -1572,6 +1676,112 @@ int cb200_sim_restore_models(cb200_sim* s, const void* blob, size_t bytes) {
 int cb200_sim_restore(cb200_sim* s, const void* blob, size_t bytes) {
 	CK(cb200_sim_restore_models(s, blob, bytes));
 	return cb200_sim_initial_setup(s);
+}
+
+// ---- per-frame .bgeo output (format and kernel: output.cuh) ---------------------------------------------------------------------
+int cb200_bgeo_header(long long points, unsigned attributes, void* out, size_t capacity, size_t* bytes) {
+	const std::vector<unsigned char> h = bgeo_header(points, attributes);
+	if(h.empty() || !out || capacity < h.size()) return (int) cudaErrorInvalidValue;
+	memcpy(out, h.data(), h.size());
+	if(bytes) *bytes = h.size();
+	return 0;
+}
+int cb200_bgeo_trailer(void* out, size_t capacity, size_t* bytes) {
+	if(!out || capacity < sizeof(kBgeoTrailer)) return (int) cudaErrorInvalidValue;
+	memcpy(out, kBgeoTrailer, sizeof(kBgeoTrailer));
+	if(bytes) *bytes = sizeof(kBgeoTrailer);
+	return 0;
+}
+
+// One frame in flight: the next call waits for the writer (back-pressure) before its gather re-uses the staging and pinned buffers.
+// A disk slower than the frames therefore slows the run down to the disk's pace instead of queueing frames in host memory without
+// bound.
+int cb200_sim_frame_output(cb200_sim* s, const char* const* paths, unsigned attributes) {
+	if(!s || !s->setup_done || !paths || (attributes & ~kOutAttrs)) return (int) cudaErrorInvalidValue;
+	const int nm = (int) s->models.size();
+	for(int m = 0; m < nm; ++m)
+		if(!paths[m]) return (int) cudaErrorInvalidValue;
+	output_idle(s);
+	{
+		std::lock_guard<std::mutex> g(s->out_mu);
+		if(s->out_errno) return CB200_ERROR_OUTPUT_IO;  // an earlier frame failed: report it before writing more
+	}
+	if(!s->out_stream) {
+		CK(cudaStreamCreateWithFlags(&s->out_stream, cudaStreamNonBlocking));
+		CK(cudaEventCreateWithFlags(&s->out_copied, cudaEventDisableTiming));
+	}
+	const int W = out_words(attributes);
+	OutputArgs a {};
+	size_t need = 0;
+	for(int m = 0; m < nm; ++m) {  // a section per model, sized for all its particles
+		a.off[m] = need;
+		a.cap[m] = s->models[m].n;
+		need += (size_t) s->models[m].n * W * sizeof(float);
+	}
+	CK(ck_grow(s->out_dev, s->out_dev_bytes, need));
+	if(s->out_host_bytes < need) {
+		if(s->out_host) cudaFreeHost(s->out_host);
+		s->out_host = nullptr;
+		s->out_host_bytes = 0;
+		CK(cudaMallocHost(&s->out_host, need));
+		s->out_host_bytes = need;
+	}
+	const int R = s->rollid, Rn = R ^ 1;
+	CK(enqueue_bucket_scans(s));
+	a.cfg = s->cfg;
+	a.state = s->d_state;
+	a.n_models = nm;
+	a.attrs = attributes;
+	for(int m = 0; m < nm; ++m) {
+		const Model& md = s->models[m];
+		a.material[m] = md.material;
+		a.cur[m] = view(md.pb[R]);
+		a.next[m] = view(md.pb[Rn]);
+		a.base[m] = s->ck_base + (size_t) m * (s->desc.max_blocks + 1);
+	}
+	a.keys = s->part[R].active_keys;
+	a.table = s->part[R].index_table;
+	a.prev_table = s->part[Rn].index_table;
+	a.grid = s->grid[0];
+	a.out = s->out_dev;
+	output_kernel<<<num_sms() * 8, kOutThreads, 0, s->stream>>>(a);
+	++s->launches;
+	CK(cudaGetLastError());
+	// the counts the headers need (each model's total, entry pbc of its scan): this is the only wait, and it ends with the gather
+	CK(pull_state(s));
+	int totals[kMaxModels] = {};
+	for(int m = 0; m < nm; ++m) CK(cudaMemcpyAsync(&totals[m], a.base[m] + s->h_state->pbc, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+	CK(cudaStreamSynchronize(s->stream));
+	std::vector<cb200_sim::OutputFile> files((size_t) nm);
+	for(int m = 0; m < nm; ++m) {
+		if(totals[m] < 0 || totals[m] > s->models[m].n) return (int) cudaErrorIllegalState;
+		files[m].path = paths[m];
+		files[m].header = bgeo_header(totals[m], attributes);
+		files[m].body = s->out_host + a.off[m];
+		files[m].body_bytes = (size_t) totals[m] * W * sizeof(float);
+		// the gather has finished (the host waited for it above): the copy needs no event to order it behind the kernel
+		if(files[m].body_bytes) CK(cudaMemcpyAsync(s->out_host + a.off[m], s->out_dev + a.off[m], files[m].body_bytes, cudaMemcpyDeviceToHost, s->out_stream));
+	}
+	CK(cudaEventRecord(s->out_copied, s->out_stream));
+	if(!s->out_thread.joinable()) s->out_thread = std::thread(output_writer, s);
+	{
+		std::lock_guard<std::mutex> g(s->out_mu);
+		s->out_files.swap(files);
+		s->out_busy = true;
+	}
+	s->out_cv.notify_all();
+	return 0;
+}
+
+int cb200_sim_frame_output_wait(cb200_sim* s, int* os_errno) {
+	if(os_errno) *os_errno = 0;
+	if(!s) return (int) cudaErrorInvalidValue;
+	output_idle(s);
+	std::lock_guard<std::mutex> g(s->out_mu);
+	if(!s->out_errno) return 0;
+	if(os_errno) *os_errno = s->out_errno;
+	s->out_errno = 0;
+	return CB200_ERROR_OUTPUT_IO;
 }
 
 int cb200_trim_pool(void) {

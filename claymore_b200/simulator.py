@@ -5,13 +5,17 @@ Mirrors the public interface of the reference's GmpmSimulator (Projects/GMPM/gmp
 All compute happens in libclaymore_b200.so; this class only marshals arguments.
 """
 import ctypes as C
+import errno
+import os
 
 import numpy as np
 
 from . import _capi
-from ._capi import CHANNELS, SEPARATE, SLIP, STICKY, Collider, Config, SimDesc, SimStats, check, lib
+from ._capi import (CHANNELS, ERROR_OUTPUT_IO, OUTPUT_J, OUTPUT_V, SEPARATE, SLIP, STICKY, Collider, Config, SimDesc, SimStats, check,
+                    lib)
 
 BOUNDARY_TYPES = {"sticky": STICKY, "slip": SLIP, "separate": SEPARATE}
+OUTPUT_ATTRIBUTES = {"v": OUTPUT_V, "J": OUTPUT_J}
 
 
 class GmpmSimulator:
@@ -37,6 +41,7 @@ class GmpmSimulator:
         self.materials, self.counts = [], []
         self.cur_frame = 0
         self.restored = False
+        self._output_paths = []   # files of the frame being written (for the error of wait_output)
 
     # ---- lifecycle -------------------------------------------------------------------------------
     def close(self):
@@ -89,8 +94,10 @@ class GmpmSimulator:
         self.cur_frame += 1
         return n.value
 
-    def main_loop(self, on_frame=None):
-        """initial_setup + nframes frames (gmpm_simulator.cuh:303-591); on_frame(sim, frame) replaces the bgeo dump.
+    def main_loop(self, on_frame=None, output=None, attributes=()):
+        """initial_setup + nframes frames (gmpm_simulator.cuh:303-591).  output: a directory that receives every finished frame
+        1..nframes as the reference's files (write_frame, `attributes` as there), written while the next frame runs; the loop waits
+        for the last files before it returns.  on_frame(sim, frame) is called after each frame.
         A restored simulator is set up already and runs only the frames after the ones its checkpoint had finished."""
         if not self.restored:
             self.initial_setup()
@@ -98,8 +105,12 @@ class GmpmSimulator:
             self.advance_frame()
             if self.stats().error:
                 break
+            if output is not None:
+                self.write_frame(output, f, attributes)
             if on_frame is not None:
                 on_frame(self, f)
+        if output is not None:
+            self.wait_output()
 
     def sync(self):
         check(self.L.cb200_sim_sync(self.h), "sync")
@@ -200,6 +211,42 @@ class GmpmSimulator:
         self.counts = [m.count for m in inf.models[: inf.n_models]]
         self.cur_frame = inf.frames
         self.restored = True
+
+    # ---- per-frame .bgeo output (output_model + write_partio; reader: claymore_b200.bgeo) --------------------------------------
+    def frame_paths(self, directory, frame):
+        """The reference's file names, model_id[i]_frame[f].bgeo; an MGSP rank adds itself: model_id[i]_rank[r]_frame[f].bgeo."""
+        rank = f"_rank[{self.mgsp_rank}]" if self.mgsp_world > 1 else ""
+        return [os.path.join(directory, f"model_id[{i}]{rank}_frame[{frame}].bgeo") for i in range(len(self.materials))]
+
+    def write_frame(self, directory, frame=None, attributes=()):
+        """One .bgeo file per model of the particles at this sub-step boundary, in `directory` (frame defaults to the current
+        frame).  attributes: any of "v" (velocity, VECTOR 3) and "J" (volume ratio, FLOAT 1).  Returns once the particles are
+        gathered; the files are written by the simulator's writer thread while later sub-steps run.  One frame is in flight: a
+        call while the previous frame is still being written waits for it.  Returns the paths."""
+        bits = 0
+        for a in attributes:
+            if a not in OUTPUT_ATTRIBUTES:
+                raise ValueError(f"unknown output attribute {a!r} (known: {', '.join(OUTPUT_ATTRIBUTES)})")
+            bits |= OUTPUT_ATTRIBUTES[a]
+        paths = self.frame_paths(directory, self.cur_frame if frame is None else frame)
+        arr = (C.c_char_p * len(paths))(*[os.fsencode(p) for p in paths])
+        err = self.L.cb200_sim_frame_output(self.h, arr, bits)
+        if err == ERROR_OUTPUT_IO:   # an earlier frame failed: raise its error (nothing of this frame was queued)
+            self.wait_output()
+        check(err, "frame_output")
+        self._output_paths = paths
+        return paths
+
+    def wait_output(self):
+        """Waits until the files of the last write_frame are written.  Raises OSError (with the path) when one failed."""
+        e = C.c_int(0)
+        err = self.L.cb200_sim_frame_output_wait(self.h, C.byref(e))
+        paths, self._output_paths = self._output_paths, []
+        if err == ERROR_OUTPUT_IO:
+            missing = [p for p in paths if not os.path.exists(p)]   # a file that failed is removed
+            path = missing[0] if missing else (paths[0] if paths else None)
+            raise OSError(e.value or errno.EIO, os.strerror(e.value or errno.EIO), path)
+        check(err, "frame_output_wait")
 
     # ---- observation --------------------------------------------------------------------------------
     def stats(self):

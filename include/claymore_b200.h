@@ -296,6 +296,33 @@ CB200_API int cb200_sim_checkpoint_end(cb200_sim* sim, const void** blob_pinned,
  * configuration take it while no rank has sub-steps in flight. */
 CB200_API int cb200_sim_restore_models(cb200_sim* sim, const void* blob_host, size_t bytes);
 CB200_API int cb200_sim_restore(cb200_sim* sim, const void* blob_host, size_t bytes);
+
+/* ------------------------------------------------------------------------------------------------
+ * Per-frame particle output (output_model, gmpm_simulator.cuh:594-634, and the IO thread of Library/MnSystem/IO/IO.h): one
+ * point-only BGEO V5 file per model, byte-identical to what partio's writer produces for the same points.  A point record is
+ * x y z 1.0, then v (VECTOR 3) if CB200_OUTPUT_V, then J (FLOAT 1) if CB200_OUTPUT_J, every word big-endian; after the records come
+ * the bytes 0x00 0xff.  Rows are in the checkpoint's order (partition order, then bucket order).  v is the G2P of grid[0]'s node
+ * velocities at the particle (MLS-MPM keeps no particle velocity); J is the fluid's J or det F.
+ * ---------------------------------------------------------------------------------------------- */
+#define CB200_OUTPUT_V 1u
+#define CB200_OUTPUT_J 2u
+/* returned when a file could not be opened or written; the errno comes with cb200_sim_frame_output_wait */
+#define CB200_ERROR_OUTPUT_IO 2000
+/* Host only: the header of a file of `points` points (0 <= points < 2^31) with `attributes`, and the 2-byte trailer.  *bytes gets
+ * the size; cudaErrorInvalidValue for a point count or attribute bits out of range, or a capacity below the size. */
+CB200_API int cb200_bgeo_header(long long points, unsigned attributes, void* out, size_t capacity, size_t* bytes);
+CB200_API int cb200_bgeo_trailer(void* out, size_t capacity, size_t* bytes);
+/* Writes the particles of every model at the current sub-step boundary to paths[m] (one path per model).  Runs the scans and the
+ * gather on the simulator's stream and waits for the gather only (the headers need the counts), queues the copy into a pinned
+ * buffer on a stream of its own and hands the files to a writer thread the simulator owns, then returns: sub-steps issued
+ * afterwards overlap with the copy and the writes.  One frame is in flight at a time: a call made while the previous frame's files
+ * are still being written waits for them first.  The staging and pinned buffers are allocated on first use and reused.
+ * cudaErrorInvalidValue (nothing queued, simulator usable) for a simulator not set up, a null path or unknown attribute bits;
+ * CB200_ERROR_OUTPUT_IO (nothing queued) while a failed write of an earlier frame has not been collected by frame_output_wait. */
+CB200_API int cb200_sim_frame_output(cb200_sim* sim, const char* const* paths, unsigned attributes);
+/* Waits until every queued file is written.  When an open or write failed, returns CB200_ERROR_OUTPUT_IO with its errno in
+ * *os_errno (nullable) and clears it; a partially written file is removed.  0 and *os_errno = 0 otherwise. */
+CB200_API int cb200_sim_frame_output_wait(cb200_sim* sim, int* os_errno);
 /* per-kernel timing for the roofline: while enabled, sub-steps are issued as plain stream launches with a
  * cudaEvent pair around every g2p2g launch; profile_read synchronises and returns the summed duration */
 CB200_API int cb200_sim_profile(cb200_sim* sim, int enable);

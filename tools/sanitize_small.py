@@ -2,7 +2,8 @@
 """Small driver for compute-sanitizer runs (memcheck / racecheck / synccheck) of the whole sub-step on an H100:
     compute-sanitizer --tool racecheck python tools/sanitize_small.py [scene] [steps]
 Scenes: small_cube (one model), two_models, mixed (fluid + sand + fixed-corotated in one partition), checkpoint (mixed: step,
-checkpoint, restore into a fresh simulator, step again)."""
+checkpoint, restore into a fresh simulator, step again), output (mixed: step, a frame of .bgeo files with v and J written while
+further sub-steps run)."""
 import os
 import sys
 
@@ -30,6 +31,13 @@ def main():
         sim = GmpmSimulator.from_checkpoint(blob, use_graph=False, auto_grow=False)
         sim.restore(blob)
         sim.step(steps)
+        sim.sync()
+    if name == "output":
+        import tempfile
+        with tempfile.TemporaryDirectory() as d:
+            sim.write_frame(d, 1, ("v", "J"))
+            sim.step(steps)
+            sim.wait_output()
         sim.sync()
     st = sim.stats()
     print("SANITIZE_RUN", name, steps, scenes.n_particles(scene), st.particle_block_count, st.neighbor_block_count, st.exterior_block_count, "error", st.error)
