@@ -251,13 +251,13 @@ int cb200_reset_table(const cb200_config* c, cb200_partition partition, void* st
 int cb200_activate_blocks(const cb200_config* c, int n, const float* positions, cb200_partition p, void* stream) {
 	CB_CFG(c);
 	if(n <= 0) return 0;
-	activate_blocks_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t) stream>>>(cfg, n, positions, p.index_table, p.active_keys, p.count, 0x7fffffff, nullptr);
+	activate_blocks_kernel<false><<<grid_for(n, 256), 256, 0, (cudaStream_t) stream>>>(cfg, n, positions, p.index_table, p.active_keys, p.count, 0x7fffffff, nullptr);
 	return (int) cudaGetLastError();
 }
 int cb200_build_particle_cell_buckets(const cb200_config* c, int n, const float* positions, cb200_particle_buffer pb, cb200_partition p, void* stream) {
 	CB_CFG(c);
 	if(n <= 0) return 0;
-	build_particle_cell_buckets_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t) stream>>>(cfg, n, positions, view(pb), p.index_table, nullptr);
+	build_particle_cell_buckets_kernel<false><<<grid_for(n, 256), 256, 0, (cudaStream_t) stream>>>(cfg, n, positions, view(pb), p.index_table, nullptr);
 	return (int) cudaGetLastError();
 }
 int cb200_array_to_buffer(const cb200_config* c, int block_count, const float* positions, cb200_particle_buffer pb, void* stream) {

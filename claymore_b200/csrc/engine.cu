@@ -638,8 +638,8 @@ void preload_kernels() {
 	preload(register_blocks_kernel);
 	preload(cell_bucket_to_block_kernel);
 	preload(compute_bin_capacity_kernel);
-	preload(activate_blocks_kernel);
-	preload(build_particle_cell_buckets_kernel);
+	preload(activate_blocks_kernel<true>);
+	preload(build_particle_cell_buckets_kernel<true>);
 	preload(array_to_buffer_kernel);
 	preload(rasterize_kernel);
 	preload(rasterize_blocks_kernel);
@@ -1081,14 +1081,14 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 	auto blocks_for = [](long long n, int per) { return (int) std::max<long long>(1, std::min<long long>((n + per - 1) / per, (long long) num_sms() * 16)); };
 
 	for(Model& m : s->models) {
-		activate_blocks_kernel<<<blocks_for(m.n, 256), 256, 0, st>>>(cfg, m.n, m.d_pos, s->part[Rn].index_table, s->part[Rn].active_keys, s->part[Rn].count, cap, err);
+		activate_blocks_kernel<true><<<blocks_for(m.n, 256), 256, 0, st>>>(cfg, m.n, m.d_pos, s->part[Rn].index_table, s->part[Rn].active_keys, s->part[Rn].count, cap, err);
 		++s->launches;
 	}
 	CK(cudaMemcpyAsync(&pbc, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToHost, st));
 	CK(cudaStreamSynchronize(st));
 	if(pbc > cap) return (int) cudaErrorMemoryAllocation;
 	for(Model& m : s->models) {
-		build_particle_cell_buckets_kernel<<<blocks_for(m.n, 256), 256, 0, st>>>(cfg, m.n, m.d_pos, view(m.pb[R]), s->part[Rn].index_table, err);
+		build_particle_cell_buckets_kernel<true><<<blocks_for(m.n, 256), 256, 0, st>>>(cfg, m.n, m.d_pos, view(m.pb[R]), s->part[Rn].index_table, err);
 		cell_bucket_to_block_kernel<<<blocks_for(pbc, 1), kBucketThreads, 0, st>>>(cfg, pbc, m.pb[R].cell_particle_counts, m.pb[R].cellbuckets, m.pb[R].particle_bucket_sizes, m.pb[R].blockbuckets, m.celloffs[Rn]);
 		compute_bin_capacity_kernel<<<blocks_for(pbc + 1, 256), 256, 0, st>>>(pbc + 1, m.pb[R].particle_bucket_sizes, m.bin_sizes);
 		ScanArgs a {};

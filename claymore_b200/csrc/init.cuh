@@ -7,19 +7,27 @@
 
 namespace cb200 {
 
+// Particle block of a bucket cell (cell index - 2).  The reference divides with C's truncation, so a particle less than 1.5 dx
+// from a low face (cell - 2 < 0) lands in block 0 although g2p2g's stencil offset and re-bucketing use floor semantics
+// (DESIGN.md section 3, quirk #8).  The step driver uses the floor (FLOOR = true): the block is negative, the particle is flagged
+// lost at set-up and never bucketed.  The kernel-level drop-in entries keep the reference's truncation.
+template<bool FLOOR> __device__ __forceinline__ int bucket_block(int c) { return FLOOR ? c >> 2 : c / 4; }
+
 // activate_blocks (mgmpm_kernels.cuh:21-34)
+template<bool FLOOR>
 __global__ void activate_blocks_kernel(Cfg cfg, int n, const float* pos, int* table, int* keys, int* count, int capacity, int* error) {
 	for(int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
-		const int x = (cell_index(cfg, pos[3 * p]) - 2) / 4, y = (cell_index(cfg, pos[3 * p + 1]) - 2) / 4, z = (cell_index(cfg, pos[3 * p + 2]) - 2) / 4;
+		const int x = bucket_block<FLOOR>(cell_index(cfg, pos[3 * p]) - 2), y = bucket_block<FLOOR>(cell_index(cfg, pos[3 * p + 1]) - 2), z = bucket_block<FLOOR>(cell_index(cfg, pos[3 * p + 2]) - 2);
 		partition_insert(cfg, table, keys, count, capacity, error, x, y, z);
 	}
 }
 
 // build_particle_cell_buckets (mgmpm_kernels.cuh:36-68)
+template<bool FLOOR>
 __global__ void build_particle_cell_buckets_kernel(Cfg cfg, int n, const float* pos, PBuf pb, const int* table, int* error) {
 	for(int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
 		const int cx = cell_index(cfg, pos[3 * p]) - 2, cy = cell_index(cfg, pos[3 * p + 1]) - 2, cz = cell_index(cfg, pos[3 * p + 2]) - 2;
-		const int bno = table_query(cfg, table, cx / 4, cy / 4, cz / 4);
+		const int bno = table_query(cfg, table, bucket_block<FLOOR>(cx), bucket_block<FLOOR>(cy), bucket_block<FLOOR>(cz));
 		if(bno < 0) {
 			if(error) atomicOr(error, kErrLostParticle);
 			continue;
@@ -144,9 +152,11 @@ __global__ void __launch_bounds__(256) rasterize_blocks_kernel(Cfg cfg, int mate
 		for(int i = threadIdx.x; i < 512; i += blockDim.x) {
 			const float m = arena[i];
 			if(m == 0.f) continue;
-			const int bno = s_bno[i >> 6];
+			const int lb = i >> 6, bno = s_bno[lb];
 			if(bno < 0) {
-				if(error) atomicOr(error, kErrLostParticle);
+				// a node beyond the top face (the stencil of a particle at cell index 4G - 1 or 4G) does not exist: its share is
+				// dropped, as g2p2g's flush drops it every sub-step.  A missing block inside the domain is a lost particle.
+				if(error && in_domain(cfg, kx + ((lb >> 2) & 1), ky + ((lb >> 1) & 1), kz + (lb & 1))) atomicOr(error, kErrLostParticle);
 				continue;
 			}
 			float* cell = grid + (size_t) bno * kGridBlockFloats + (i & 63);

@@ -639,6 +639,7 @@ void orc_rasterize(const orc_config* cfg, int n, const float* pos, float* grid, 
 					const float W = w[0][i] * w[1][j] * w[2][k];
 					const float wm = mass * W;
 					const int blockno = part_query(cfg, &part, g[0] >> 2, g[1] >> 2, g[2] >> 2);
+					if(blockno < 0) continue; /* node beyond the top face: no block (the reference indexes out of bounds) */
 					float* blk = grid + (long) blockno * 256;
 					const int c = (g[0] & 3) * 16 + (g[1] & 3) * 4 + (g[2] & 3);
 					blk[c] += wm;
