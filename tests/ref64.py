@@ -414,9 +414,7 @@ def compare(ref, keys, grid, states, kappa, stress_allow, f_allow, margin=1e-4, 
     ``keys``/``grid`` its keyed grid after the sub-step, ``states`` its particle_state rows per model.
     bound = kappa[q] * 2^-24 * M (+ stress_allow[model] * the stress column of the node, + f_allow[model] for F / logJp).
     Particles within ``margin`` of a return-mapping branch are left out of the particle check and counted."""
-    from scipy.spatial import cKDTree
     rep = dict(mass=0.0, momentum=0.0, pos=0.0, F=0.0, near_branch=0, worst={})
-    rg = Grid(ref["keys"], np.concatenate([ref["grid"], ref["mag"], ref["stress"]], 1))
     keys = np.asarray(keys, np.int64)
     grid = np.asarray(grid, np.float64)
     # every block of the reference's P2G must exist; blocks the reference never touched must be zero
@@ -425,11 +423,7 @@ def compare(ref, keys, grid, states, kappa, stress_allow, f_allow, margin=1e-4, 
     touched = ref["grid"][:, 0].max(1) > 0
     missing = np.setdiff1d(rh[touched], eh)
     assert len(missing) == 0, f"{len(missing)} grid blocks with mass missing from the implementation's grid"
-    cells = np.stack(np.meshgrid(np.arange(4), np.arange(4), np.arange(4), indexing="ij"), -1).reshape(64, 3)
-    nodes = keys[:, None, :] * 4 + cells[None]
-    r, _ = rg.gather(nodes)                                  # [nb, 64, 12]
-    r = r.transpose(0, 2, 1)
-    val, mag, st = r[:, :4], r[:, 4:8], r[:, 8:12]
+    val, mag, st = ref_at(ref, keys)
     err = np.abs(grid - val)
     bm = kappa["mass"] * EPS32 * mag[:, 0]
     bmv = kappa["momentum"] * EPS32 * mag[:, 1:] + stress_allow * st[:, 1:]
@@ -440,7 +434,24 @@ def compare(ref, keys, grid, states, kappa, stress_allow, f_allow, margin=1e-4, 
     if rep["momentum"] > 1 or rep["mass"] > 1:
         i = np.unravel_index(np.argmax(np.nan_to_num(rmv, nan=np.inf)), rmv.shape)
         rep["worst"]["momentum"] = (tuple(int(k) for k in keys[i[0]]), int(i[2]), float(grid[i[0], 1 + i[1], i[2]]), float(val[i[0], 1 + i[1], i[2]]), float(bmv[i]))
-    for m, (res, se) in enumerate(zip(ref["models"], states)):
+    compare_particles(ref["models"], states, kappa, f_allow, margin, match_tol, rep)
+    return rep
+
+
+def ref_at(ref, keys):
+    """The reference's (value, magnitude, stress column) [nb, 4, 64] at the blocks ``keys`` (0 where it touched nothing)."""
+    rg = Grid(ref["keys"], np.concatenate([ref["grid"], ref["mag"], ref["stress"]], 1))
+    cells = np.stack(np.meshgrid(np.arange(4), np.arange(4), np.arange(4), indexing="ij"), -1).reshape(64, 3)
+    nodes = np.asarray(keys, np.int64)[:, None, :] * 4 + cells[None]
+    r, _ = rg.gather(nodes)                                  # [nb, 64, 12]
+    r = r.transpose(0, 2, 1)
+    return r[:, :4], r[:, 4:8], r[:, 8:12]
+
+
+def compare_particles(ref_models, states, kappa, f_allow, margin, match_tol, rep):
+    """compare()'s per-particle rules: ``states[m]`` against ``ref_models[m]`` (lost particles left out), worst ratios into rep."""
+    from scipy.spatial import cKDTree
+    for m, (res, se) in enumerate(zip(ref_models, states)):
         keep = ~res["lost"]
         rs = res["state"][keep]
         assert len(se) == len(rs), f"model {m}: {len(se)} particles, reference keeps {len(rs)}"
@@ -459,4 +470,3 @@ def compare(ref, keys, grid, states, kappa, stress_allow, f_allow, margin=1e-4, 
             with np.errstate(divide="ignore", invalid="ignore"):
                 rf = np.where(ef > 0, ef / (kappa["F"] * EPS32 * fm + f_allow[m]), 0.0)
             rep["F"] = max(rep["F"], float(rf[~near].max(initial=0)))
-    return rep
