@@ -99,6 +99,19 @@ class CheckpointInfo(C.Structure):
                 ("models", CheckpointModel * 8)]
 
 
+SDF_RANDOM, SDF_LATTICE = 0, 1   # CB200_SDF_RANDOM / CB200_SDF_LATTICE
+
+
+class SdfHeader(C.Structure):
+    """cb200_sdf_header: an SDFGen level set's first two lines (SampleGenerator::LoadSDF, PoissonDisk/SampleGenerator.h:68-93)."""
+    _fields_ = [("ni", C.c_int), ("nj", C.c_int), ("nk", C.c_int), ("min", C.c_float * 3), ("h", C.c_float)]
+
+
+class SdfSampling(C.Structure):
+    """cb200_sdf_sampling: how a level set becomes particles (mode, placement, density, Philox key)."""
+    _fields_ = [("mode", C.c_int), ("ppc", C.c_int), ("offset", C.c_double * 3), ("span", C.c_double * 3), ("seed", C.c_ulonglong)]
+
+
 def lib_path():
     return _LIB
 
@@ -182,6 +195,9 @@ _SIGNATURES = {
     "cb200_sim_frame_output": [_P, C.POINTER(C.c_char_p), C.c_uint],
     "cb200_sim_frame_output_wait": [_P, C.POINTER(_I)],
     "cb200_trim_pool": [],
+    "cb200_sdf_parse": [C.c_char_p, C.c_size_t, C.POINTER(SdfHeader), _P, C.c_size_t],
+    "cb200_sample_sdf": [_CFG, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.c_longlong, C.POINTER(C.c_longlong), _P],
+    "cb200_sim_init_model_sdf": [_P, _I, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.POINTER(_I), C.POINTER(_I)],
     "cb200_test_svd3": [_I, _P, _P, _P, _P, _P],
     "cb200_test_stress": [_I, _I, ParticleBuffer, _I, _P, _P, _P, _P, _P, _P],
     "cb200_sim_profile": [_P, _I],

@@ -32,6 +32,7 @@
 #include "mgsp.cuh"
 #include "output.cuh"
 #include "partition.cuh"
+#include "sdf.cuh"
 
 namespace cb200 {
 int num_sms();
@@ -1786,6 +1787,149 @@ int cb200_sim_frame_output_wait(cb200_sim* s, int* os_errno) {
 
 int cb200_trim_pool(void) {
 	g_pool.trim();
+	return 0;
+}
+
+// ---- particle models from level sets (format, plan and kernels: sdf.cuh) -------------------------------------------------------------
+}  // extern "C"
+namespace {
+// One sampling run: phi on the device, the valid-cell list (random mode) and the tile offsets of the last count, all from the pool.
+// count() runs the passes up to the particle count; write() fills `out` (device) in candidate / lattice-point order.
+struct SdfRun {
+	SdfPlan P {};
+	cudaStream_t st = nullptr;
+	float* phi = nullptr;
+	int* list = nullptr;
+	long long* tile_off = nullptr;
+	unsigned* done = nullptr;
+	SdfScan scan {};
+	int tiles = 0;
+	long long count = 0;
+	SdfRandom rnd {};
+	SdfLattice lat {};
+	~SdfRun() {
+		g_pool.release(phi);
+		g_pool.release(list);
+		g_pool.release(tile_off);
+		g_pool.release(done);
+	}
+	// the count kernel over n_items: scan / tiles describe the launch, *total the kept items
+	template<class G>
+	int count_pass(const G& g, long long n_items, long long* total) {
+		*total = 0;
+		if(n_items <= 0) return 0;
+		g_pool.release(tile_off);
+		tile_off = nullptr;
+		// at most 64 Ki tiles, so the last CTA's scan stays short
+		const long long per_round = kSdfThreads, min_rounds = (n_items + 65536LL * per_round - 1) / (65536LL * per_round);
+		scan.n_items = n_items;
+		scan.rounds = (int) std::max<long long>(8, min_rounds);
+		tiles = (int) ((n_items + per_round * scan.rounds - 1) / (per_round * scan.rounds));
+		CK(pool_alloc(&tile_off, (size_t) (tiles + 1) * sizeof(long long)));
+		scan.tile_off = tile_off;
+		scan.done = done;
+		CK(cudaMemsetAsync(done, 0, sizeof(unsigned), st));
+		sdf_count_kernel<G><<<tiles, kSdfThreads, 0, st>>>(g, scan);
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(total, tile_off + tiles, sizeof(long long), cudaMemcpyDeviceToHost, st));
+		return (int) cudaStreamSynchronize(st);
+	}
+	template<class G>
+	int write_pass(const G& g) {
+		if(!tiles) return 0;
+		sdf_write_kernel<G><<<tiles, kSdfThreads, 0, st>>>(g, scan);
+		return (int) cudaGetLastError();
+	}
+	int run_count(const cb200_config& cfg, const cb200_sdf_header& hdr, const float* phi_host, const cb200_sdf_sampling& smp) {
+		if(!phi_host) return (int) cudaErrorInvalidValue;
+		CK(sdf_plan(cfg, hdr, smp, P));
+		const size_t nodes = (size_t) hdr.ni * hdr.nj * hdr.nk;
+		CK(pool_alloc(&phi, nodes * sizeof(float)));
+		CK(pool_alloc(&done, sizeof(unsigned)));
+		CK(cudaMemcpyAsync(phi, phi_host, nodes * sizeof(float), cudaMemcpyHostToDevice, st));
+		const SdfField f {phi, hdr.ni, hdr.nj};
+		if(P.mode == CB200_SDF_LATTICE) {
+			lat.f = f;
+			lat.nk = hdr.nk;
+			lat.k = P.k;
+			for(int d = 0; d < 3; ++d) {
+				lat.lo[d] = P.lo[d];
+				lat.ext[d] = P.ext[d];
+				lat.off[d] = P.offset[d];
+			}
+			lat.dx = P.dx;
+			lat.c = P.c;
+			return count_pass(lat, P.lattice_items, &count);
+		}
+		SdfClassify cls {f, nullptr};
+		long long n_valid = 0;
+		CK(count_pass(cls, (long long) (hdr.ni - 1) * (hdr.nj - 1) * (hdr.nk - 1), &n_valid));
+		if(!n_valid) return 0;
+		CK(pool_alloc(&list, (size_t) n_valid * sizeof(int)));
+		cls.list = list;
+		CK(write_pass(cls));
+		const double cand = std::floor((double) n_valid * P.spc);
+		if(!(cand < 0x1p62)) return (int) cudaErrorInvalidValue;
+		rnd.f = f;
+		rnd.list = list;
+		rnd.n_valid = n_valid;
+		rnd.spc = P.spc;
+		rnd.c = P.c;
+		for(int d = 0; d < 3; ++d) rnd.off[d] = P.offset[d];
+		rnd.key = make_uint2((unsigned) smp.seed, (unsigned) (smp.seed >> 32));
+		return count_pass(rnd, (long long) cand, &count);
+	}
+	int run_write(float* out) {
+		if(P.mode == CB200_SDF_LATTICE) {
+			lat.out = out;
+			return write_pass(lat);
+		}
+		rnd.out = out;
+		return write_pass(rnd);
+	}
+};
+}  // namespace
+extern "C" {
+
+int cb200_sdf_parse(const char* text, size_t bytes, cb200_sdf_header* header, float* phi, size_t capacity) {
+	return sdf_parse(text, bytes, header, phi, capacity);
+}
+
+int cb200_sample_sdf(const cb200_config* cfg, const cb200_sdf_header* header, const float* phi_host, const cb200_sdf_sampling* sampling,
+                     float* pos_host, long long capacity, long long* n_out, void* stream) {
+	if(!cfg || !cfg_valid(*cfg) || !header || !sampling || !n_out) return (int) cudaErrorInvalidValue;
+	SdfRun r;
+	r.st = (cudaStream_t) stream;
+	CK(r.run_count(*cfg, *header, phi_host, *sampling));
+	*n_out = r.count;
+	if(!pos_host || !r.count) return 0;
+	if(capacity < r.count) return (int) cudaErrorInvalidValue;
+	float* staging = nullptr;
+	CK(pool_alloc(&staging, (size_t) r.count * 3 * sizeof(float)));
+	int e = r.run_write(staging);
+	if(!e) e = (int) cudaMemcpyAsync(pos_host, staging, (size_t) r.count * 3 * sizeof(float), cudaMemcpyDeviceToHost, r.st);
+	if(!e) e = (int) cudaStreamSynchronize(r.st);
+	g_pool.release(staging);
+	return e;
+}
+
+int cb200_sim_init_model_sdf(cb200_sim* s, int material, const cb200_sdf_header* header, const float* phi_host, const cb200_sdf_sampling* sampling,
+                             const float* v0, int* model_id, int* n_out) {
+	if(!s || s->setup_done || material < 0 || material > 3 || (int) s->models.size() >= kMaxModels || !header || !sampling) return (int) cudaErrorInvalidValue;
+	SdfRun r;
+	r.st = s->stream;
+	CK(r.run_count(s->desc.cfg, *header, phi_host, *sampling));
+	if(r.count <= 0 || r.count >= (1LL << 31)) return (int) cudaErrorInvalidValue;
+	Model m;
+	m.material = material;
+	m.n = (int) r.count;
+	for(int d = 0; d < 3; ++d) m.v0[d] = v0 ? v0[d] : 0.f;
+	CK(alloc_model(s, m));
+	CK(r.run_write(m.d_pos));
+	CK(cudaStreamSynchronize(s->stream));
+	if(model_id) *model_id = (int) s->models.size();
+	if(n_out) *n_out = m.n;
+	s->models.push_back(m);
 	return 0;
 }
 

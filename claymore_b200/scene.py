@@ -13,20 +13,24 @@ A "box" collider spans [offset, offset + span], a "sphere" has diameter min(span
 through offset and is solid behind `normal`.  The collider is the reference's SignedDistanceGrid (init_boundary,
 Projects/MGSP/mgsp_benchmark.cuh:257-266); "velocity" is its trans_vel.
 
-The reference only loads `.sdf` level sets (gmpm.cu:152, needs the absent Data submodule); here a model may also
-name a synthetic generator: "file": "box" (span in cells of the lattice sampler) or "sphere" (span = diameter),
-or a raw float32 xyz `.bin` cloud as used by mgsp.cu:11-17.
+The reference only loads `.sdf` level sets (gmpm.cu:152-159).  Here "file": "<name>.sdf" is sampled on the device by
+GmpmSimulator.init_model_sdf with the optional keys "sampler" ("random", the default, or "lattice"), "ppc" (particles per
+simulation cell, default 8: the reference's MODEL_PPC, settings.h:51) and "seed" (default 0); the level set is fitted into
+[offset, offset + span] with one scale for all axes, and a node box outside the domain rejects the scene before any device work
+(claymore_b200.sdf).  A model may also name a synthetic generator: "file": "box" (span in cells of the lattice sampler) or
+"sphere" (span = diameter), or a raw float32 xyz `.bin` cloud as used by mgsp.cu:11-17.
 """
 import json
 import os
 
 import numpy as np
 
-from . import levelset, samplers
+from . import levelset, samplers, sdf
 from ._capi import Config, FIXED_COROTATED, J_FLUID, NACC, SAND
 from .simulator import GmpmSimulator
 
 CONSTITUTIVE = {"jfluid": J_FLUID, "fixed_corotated": FIXED_COROTATED, "sand": SAND, "nacc": NACC}
+PARTICLE_TYPES = ("particles", "particle")   # the reference's scene.json says "particle"; gmpm.cu:96-165 does not read the key
 
 
 def _positions(model, cfg, base_dir):
@@ -45,7 +49,25 @@ def _positions(model, cfg, base_dir):
         return np.fromfile(path, dtype=np.float32).reshape(-1, 3)
     if path.endswith(".npy"):
         return np.load(path).astype(np.float32).reshape(-1, 3)
-    raise ValueError(f"unsupported model file {kind!r} (the reference's .sdf sampler is outside the hot path)")
+    raise ValueError(f"unsupported model file {kind!r} (known: box, sphere, *.sdf, *.bin, *.npy)")
+
+
+def _model_path(model, base_dir):
+    kind = model.get("file", "box")
+    return kind if os.path.isabs(kind) else os.path.join(base_dir, kind)
+
+
+def _level_sets(models, base_dir):
+    """Reads every `.sdf` model's level set and checks its node box: {model index: LevelSet}, before any device work."""
+    out = {}
+    for i, model in enumerate(models):
+        if str(model.get("file", "box")).endswith(".sdf"):
+            ls = sdf.read(_model_path(model, base_dir))
+            sdf.check_box(ls, model.get("offset", [0, 0, 0]), model.get("span", [1, 1, 1]), what=f"model {i} ({model['file']})")
+            sdf.sampling(model.get("offset", [0, 0, 0]), model.get("span", [1, 1, 1]), model.get("ppc", 8), model.get("sampler", "random"),
+                         model.get("seed", 0))
+            out[i] = ls
+    return out
 
 
 def _collider(sim, c, cfg, base_dir):
@@ -75,7 +97,7 @@ def _check_resume(doc, cfg, resume):
         raise ValueError(f"checkpoint {resume}: config {inf['cfg']} differs from the scene's {want}")
     if inf["dt_default"] != f32(s.get("default_dt", GmpmSimulator.DEFAULT_DT)) or inf["fps"] != s.get("fps", GmpmSimulator.DEFAULT_FPS):
         raise ValueError(f"checkpoint {resume}: default_dt / fps {inf['dt_default']} / {inf['fps']} differ from the scene's simulation section")
-    mats = [CONSTITUTIVE.get(m.get("constitutive")) for m in doc.get("models", []) if m.get("type", "particles") == "particles"]
+    mats = [CONSTITUTIVE.get(m.get("constitutive")) for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
     if [m["material"] for m in inf["models"]] != mats:
         raise ValueError(f"checkpoint {resume}: its models are not the scene's")
     return inf
@@ -102,16 +124,21 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
             _collider(sim, doc["collider"], cfg, base)
         sim.restore(resume)
         return sim
+    models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
+    for model in models:
+        if model.get("constitutive") not in CONSTITUTIVE:
+            raise ValueError(f"unknown constitutive model {model.get('constitutive')!r}")
+    level_sets = _level_sets(models, base)
     sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                         frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max_blocks, **sim_kwargs)
-    for model in doc.get("models", []):
-        if model.get("type", "particles") != "particles":
-            continue
+    for i, model in enumerate(models):
         c = model["constitutive"]
-        if c not in CONSTITUTIVE:
-            raise ValueError(f"unknown constitutive model {c!r}")
-        pos = _positions(model, cfg, base)
-        mid = sim.init_model(CONSTITUTIVE[c], pos, model.get("velocity", [0, 0, 0]))
+        v0 = model.get("velocity", [0, 0, 0])
+        if i in level_sets:
+            mid = sim.init_model_sdf(CONSTITUTIVE[c], level_sets[i], model.get("offset", [0, 0, 0]), model.get("span", [1, 1, 1]), v0,
+                                     ppc=model.get("ppc", 8), mode=model.get("sampler", "random"), seed=model.get("seed", 0))
+        else:
+            mid = sim.init_model(CONSTITUTIVE[c], _positions(model, cfg, base), v0)
         # material parameters exactly as gmpm.cu:108-150 forwards them
         if c == "jfluid":
             sim.update_j_fluid_parameters(model["rho"], model["volume"], model["bulk_modulus"], model["gamma"], model["viscosity"], model=mid)

@@ -65,6 +65,21 @@ class GmpmSimulator:
         self.counts.append(len(pos))
         return mid.value
 
+    def init_model_sdf(self, material, ls, offset, span, v0=(0.0, 0.0, 0.0), ppc=8, mode="random", seed=0):
+        """init_model from a level set (claymore_b200.sdf.LevelSet): the particles are counted, the model allocated and the positions
+        written on the device, with no host copy of them.  The node box must lie inside the domain (ValueError otherwise)."""
+        from . import sdf
+        sdf.check_box(ls, offset, span)
+        smp = sdf.sampling(offset, span, ppc, mode, seed)
+        phi = np.ascontiguousarray(ls.phi, dtype=np.float32)
+        v = np.ascontiguousarray(v0, dtype=np.float32)
+        mid, n = C.c_int(-1), C.c_int(0)
+        check(self.L.cb200_sim_init_model_sdf(self.h, material, C.byref(ls.header), phi.ctypes.data_as(C.c_void_p), C.byref(smp),
+                                              v.ctypes.data_as(C.c_void_p), C.byref(mid), C.byref(n)), "init_model_sdf")
+        self.materials.append(material)
+        self.counts.append(n.value)
+        return mid.value
+
     def update_fr_parameters(self, rho, vol, ym, pr, model=-1):
         check(self.L.cb200_sim_update_fr_parameters(self.h, self._m(model), rho, vol, ym, pr), "update_fr_parameters")
 

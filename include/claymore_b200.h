@@ -350,6 +350,52 @@ CB200_API int cb200_sim_mgsp_set_peers(cb200_sim* sim, void* const* inbox_ptrs_b
 CB200_API int cb200_sim_mgsp_halo_counts(cb200_sim* sim, int* shared_blocks_by_rank, int* halo_particle_blocks);
 
 /* ------------------------------------------------------------------------------------------------
+ * Particle models sampled from a level set (the reference's read_sdf, Library/MnSystem/IO/ParticleIO.hpp:65-97, and
+ * SampleGenerator::LoadSDF / GenerateUniformSamples, Library/MnSystem/IO/PoissonDisk/SampleGenerator.h:68-93,149-177; gmpm.cu:152-159
+ * builds every model so).  The file is SDFGen text: `ni nj nk`, `min_x min_y min_z`, `h`, then ni nj nk values with i fastest
+ * (phi[i + ni (j + nj k)]).  The origin is metadata only.  Placement: one scale for all axes, c = h min_d span_d / ((n_d - 1) h);
+ * node q (index units) lands at offset + q c, and the node box [offset, offset + (n - 1) c] must lie inside [0, 1]^3.
+ *   CB200_SDF_RANDOM   the reference's sampler with DESIGN §2.7's S1-S4 fixed: valid cells (a negative node) in ascending id
+ *                      i + (ni-1)(j + (nj-1) k); spc = ppc (c / dx)^3; valid cell v holds candidates floor(v spc) <= j <
+ *                      floor((v + 1) spc); candidate j draws Philox4x32-10 at counter (j lo, j hi, 0, 0), key (seed lo, seed hi), and
+ *                      u_d = (r_d >> 8) 2^-24 from the first three words; q = cell + u is kept when the trilinear phi (double,
+ *                      fetchGridTrilinear's corners and order) is negative.  Expected density: ppc particles per simulation cell.
+ *   CB200_SDF_LATTICE  ppc = k^3 (k = 1..4) lattice points per simulation cell, (cell + (m - (k-1)/2) / k) dx, cells row-major with x
+ *                      slowest, kept where q = (x - offset) / c lies in [0, n - 1] and phi(q) < 0 (samplers.uniform_box's order
+ *                      and bits for k = 2).
+ * Positions are offset + q c in double rounded to float32, in candidate (lattice point) order.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct cb200_sdf_header {
+	int ni, nj, nk;  /* nodes per axis */
+	float min[3];    /* SDFGen's origin (not used for placement) */
+	float h;         /* node spacing */
+} cb200_sdf_header;
+#define CB200_SDF_RANDOM 0
+#define CB200_SDF_LATTICE 1
+typedef struct cb200_sdf_sampling {
+	int mode;                /* CB200_SDF_RANDOM / CB200_SDF_LATTICE */
+	int ppc;                 /* particles per simulation cell (lattice: 1, 8, 27 or 64) */
+	double offset[3];        /* world position of node 0 */
+	double span[3];          /* the box the level set is fitted into (the smallest ratio decides) */
+	unsigned long long seed; /* random: Philox key */
+} cb200_sdf_sampling;
+/* Host only.  Parses `bytes` of text with strtof, so values are bitwise those of LoadSDF's `>>`.  phi (nullable): receives the
+ * ni nj nk values when capacity allows.  cudaErrorInvalidValue for a dimension below 2 or ni nj nk >= 2^31, an h that is not finite
+ * and positive, a value that is not a finite number, too few or too many values, or a capacity below ni nj nk. */
+CB200_API int cb200_sdf_parse(const char* text, size_t bytes, cb200_sdf_header* header, float* phi, size_t capacity);
+/* Samples on the current device (phi_host: ni nj nk floats) and returns the particle count in *n_out; with pos_host (nullable)
+ * and capacity >= the count (in particles) the positions are copied there.  Synchronises `stream`.  cudaErrorInvalidValue for a
+ * bad config, header, mode or ppc, a span that is not positive, a node box outside the domain, or a capacity below the count
+ * (*n_out still set). */
+CB200_API int cb200_sample_sdf(const cb200_config* cfg, const cb200_sdf_header* header, const float* phi_host, const cb200_sdf_sampling* sampling,
+                               float* pos_host, long long capacity, long long* n_out, void* stream);
+/* init_model from a level set: counts, allocates the model, then writes the positions straight into its device array.
+ * cudaErrorInvalidValue, simulator unchanged, for a bad material, mode or ppc, a span that is not positive, a node box outside
+ * the domain, a count of 0 or >= 2^31, a simulator that is set up or has 8 models.  *n_out (nullable): the particle count. */
+CB200_API int cb200_sim_init_model_sdf(cb200_sim* sim, int material, const cb200_sdf_header* header, const float* phi_host,
+                                       const cb200_sdf_sampling* sampling, const float* v0, int* model_id, int* n_out);
+
+/* ------------------------------------------------------------------------------------------------
  * Test-only hooks (used by tests/, not part of the drop-in surface): the device 3x3 SVD and constitutive models of g2p2g on
  * caller-supplied DEVICE vectors, against math::svd (Library/MnBase/Math/Matrix/svd.cuh:28-1124) and compute_stress<M>
  * (Projects/GMPM/constitutive_models.cuh:36-335).  F: float[9n] column-major; mode 0 = the path g2p2g takes, 1 = FIXED_COROTATED via SVD.
