@@ -100,6 +100,7 @@ class CheckpointInfo(C.Structure):
 
 
 SDF_RANDOM, SDF_LATTICE = 0, 1   # CB200_SDF_RANDOM / CB200_SDF_LATTICE
+EMIT_EMPTY_CELLS = 1             # CB200_EMIT_EMPTY_CELLS: add only particles whose cell held none before the call
 
 
 class SdfHeader(C.Structure):
@@ -198,6 +199,8 @@ _SIGNATURES = {
     "cb200_sdf_parse": [C.c_char_p, C.c_size_t, C.POINTER(SdfHeader), _P, C.c_size_t],
     "cb200_sample_sdf": [_CFG, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.c_longlong, C.POINTER(C.c_longlong), _P],
     "cb200_sim_init_model_sdf": [_P, _I, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.POINTER(_I), C.POINTER(_I)],
+    "cb200_sim_add_particles": [_P, _I, _P, _I, _P, C.c_uint, C.POINTER(_I)],
+    "cb200_sim_add_particles_sdf": [_P, _I, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.c_uint, C.POINTER(_I)],
     "cb200_test_svd3": [_I, _P, _P, _P, _P, _P],
     "cb200_test_stress": [_I, _I, ParticleBuffer, _I, _P, _P, _P, _P, _P, _P],
     "cb200_sim_profile": [_P, _I],

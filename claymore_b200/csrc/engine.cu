@@ -16,6 +16,7 @@
 #include <unistd.h>
 
 #include <cerrno>
+#include <cmath>
 #include <condition_variable>
 #include <cstdio>
 #include <cstring>
@@ -26,6 +27,7 @@
 #include <vector>
 
 #include "checkpoint.cuh"
+#include "emit.cuh"
 #include "g2p2g.cuh"
 #include "grid.cuh"
 #include "init.cuh"
@@ -1065,7 +1067,8 @@ struct RestoreSrc {
 	const cb200_checkpoint_info* info;
 	const float* state[kMaxModels];  // [count][channels] per model
 	const int* keys;                 // [nbc][3]
-	const float* grid;               // [nbc][256]
+	const float* grid;               // [grid_count][256]
+	int grid_count;                  // saved blocks: the checkpoint's nbc; an emission's old nbc, a subset of the rebuilt partition's
 };
 
 // initial_setup  gmpm_simulator.cuh:637-781 (counts are read back here: one-time cost).  With `rs` (restore) it differs in three
@@ -1150,7 +1153,7 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 	++s->launches;
 	int* missing = s->d_scratch + 6;
 	if(rs) {  // the saved blocks by key; a key the rebuilt partition has no neighbour block for is counted, not written
-		const int saved = rs->info->neighbor_block_count;
+		const int saved = rs->grid_count;
 		CK(cudaMemsetAsync(missing, 0, sizeof(int), st));
 		scatter_grid_kernel<<<blocks_for(saved, 8), 256, 0, st>>>(cfg, saved, rs->keys, rs->grid, s->part[R].index_table, nbc, s->grid[0], missing);
 		++s->launches;
@@ -1243,6 +1246,7 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 	for(int m = 0; m < kMaxModels; ++m) rs.state[m] = s->restore_state[m];
 	rs.grid = reinterpret_cast<const float*>(s->restore_grid);
 	rs.keys = reinterpret_cast<const int*>(s->restore_grid + s->restore_info.grid_bytes);
+	rs.grid_count = s->restore_info.neighbor_block_count;
 	int e = setup_impl(s, &rs);
 	if(!e) e = (int) cudaStreamSynchronize(s->stream);
 	if(!e) {  // the staged state is in the bins and the grid now
@@ -1516,6 +1520,32 @@ static int enqueue_bucket_scans(cb200_sim* s) {
 	return 0;
 }
 
+// The snapshot gather of the current state into `out` (a blob of ck_capacity bytes, header left to the caller), behind the bucket
+// scans, on the sim stream.  Shared by the checkpoint and the emission, which rebuilds the simulator from it.
+static int enqueue_snapshot(cb200_sim* s, unsigned char* out) {
+	const int R = s->rollid, Rn = R ^ 1;
+	const int nm = (int) s->models.size();
+	CK(enqueue_bucket_scans(s));
+	SnapshotArgs a {};
+	a.cfg = s->cfg;
+	a.state = s->d_state;
+	a.n_models = nm;
+	for(int m = 0; m < nm; ++m) {
+		const Model& md = s->models[m];
+		a.material[m] = md.material;
+		a.cur[m] = view(md.pb[R]);
+		a.next[m] = view(md.pb[Rn]);
+		a.base[m] = s->ck_base + (size_t) m * (s->desc.max_blocks + 1);
+	}
+	a.keys = s->part[R].active_keys;
+	a.prev_table = s->part[Rn].index_table;
+	a.grid = s->grid[0];
+	a.out = out;
+	snapshot_kernel<<<num_sms() * 8, kSnapThreads, 0, s->stream>>>(a);
+	++s->launches;
+	return (int) cudaGetLastError();
+}
+
 int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	if(!s || !s->setup_done) return (int) cudaErrorInvalidValue;
 	if(s->ck_pending) CK(cudaEventSynchronize(s->ck_copied));  // the pinned blob and the staging blob are re-used
@@ -1534,30 +1564,11 @@ int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 		CK(cudaMallocHost(&s->ck_host, cap));
 		s->ck_host_bytes = cap;
 	}
-	const int R = s->rollid, Rn = R ^ 1;
+	CK(enqueue_snapshot(s, s->ck_dev));
+	CK(cudaEventRecord(s->ck_gathered, s->stream));
+	// the counts the layout follows from: the step state (pbc, nbc, clock), then each model's total, entry pbc of its scan
 	const int nm = (int) s->models.size();
 	cudaStream_t st = s->stream;
-	CK(enqueue_bucket_scans(s));
-	SnapshotArgs a {};
-	a.cfg = s->cfg;
-	a.state = s->d_state;
-	a.n_models = nm;
-	for(int m = 0; m < nm; ++m) {
-		const Model& md = s->models[m];
-		a.material[m] = md.material;
-		a.cur[m] = view(md.pb[R]);
-		a.next[m] = view(md.pb[Rn]);
-		a.base[m] = s->ck_base + (size_t) m * (s->desc.max_blocks + 1);
-	}
-	a.keys = s->part[R].active_keys;
-	a.prev_table = s->part[Rn].index_table;
-	a.grid = s->grid[0];
-	a.out = s->ck_dev;
-	snapshot_kernel<<<num_sms() * 8, kSnapThreads, 0, st>>>(a);
-	++s->launches;
-	CK(cudaGetLastError());
-	CK(cudaEventRecord(s->ck_gathered, st));
-	// the counts the layout follows from: the step state (pbc, nbc, clock), then each model's total, entry pbc of its scan
 	CK(pull_state(s));
 	const StepState& h = *s->h_state;
 	int totals[kMaxModels] = {};
@@ -1931,6 +1942,251 @@ int cb200_sim_init_model_sdf(cb200_sim* s, int material, const cb200_sdf_header*
 	if(n_out) *n_out = m.n;
 	s->models.push_back(m);
 	return 0;
+}
+
+// ---- adding particles at a sub-step boundary (kernels: emit.cuh) ----------------------------------------------------------------------
+}  // extern "C"
+namespace {
+// every buffer one call allocates; what the commit swaps out of the model (its old bins and positions) lands here and goes back too
+struct EmitBuffers {
+	float* cand = nullptr;  // [n][3] candidates
+	int* keep = nullptr;    // [n]
+	int* offs = nullptr;    // [n + 1] exclusive scan of keep
+	float* kept = nullptr;  // [k][3] kept candidates, in candidate order
+	int* word = nullptr;    // [0] scratch partition count, [1] kEmit* bits
+	int* table = nullptr;   // scratch partition of the union: table, keys
+	int* keys = nullptr;
+	int* cells = nullptr;   // [union pbc][64] new particles per cell
+	unsigned char* blob = nullptr;  // the gathered state, checkpoint layout
+	float* rows = nullptr;  // the model's rows with the new ones appended
+	float* bins[2] = {nullptr, nullptr};
+	float* pos = nullptr;
+	~EmitBuffers() {
+		for(void* p : {(void*) cand, (void*) keep, (void*) offs, (void*) kept, (void*) word, (void*) table, (void*) keys, (void*) cells, (void*) blob, (void*) rows,
+		               (void*) bins[0], (void*) bins[1], (void*) pos})
+			g_pool.release(p);
+	}
+};
+
+int emit_precheck(cb200_sim* s, int model, unsigned flags, const float* v0) {
+	if(!s) return (int) cudaErrorInvalidValue;
+	if(s->desc.mgsp_world > 1) return (int) cudaErrorNotSupported;  // a rank's rebuild would have to be agreed with its peers
+	if(!s->setup_done || model < 0 || model >= (int) s->models.size() || (flags & ~CB200_EMIT_EMPTY_CELLS)) return (int) cudaErrorInvalidValue;
+	if(v0 && !(std::isfinite(v0[0]) && std::isfinite(v0[1]) && std::isfinite(v0[2]))) return (int) cudaErrorInvalidValue;  // NaN momentum, or dt = 0
+	return 0;
+}
+
+inline int launch_items(long long n, int per) { return (int) std::max<long long>(1, std::min<long long>((n + per - 1) / per, (long long) num_sms() * 16)); }
+
+// The shared path of both entries, with the n candidates in eb.cand.  Everything up to the commit reads the live state and writes
+// scratch only, so a rejection leaves the simulator as it was.
+int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, unsigned flags, int* n_added) {
+	cudaStream_t st = s->stream;
+	const Cfg& cfg = s->cfg;
+	const int nm = (int) s->models.size();
+	const float v[3] = {v0 ? v0[0] : 0.f, v0 ? v0[1] : 0.f, v0 ? v0[2] : 0.f};
+	// (1) finite, inside the domain, the empty-cell filter: against the current partition's buckets
+	CK(pool_alloc(&eb.keep, (size_t) n * sizeof(int)));
+	CK(pool_alloc(&eb.offs, ((size_t) n + 1) * sizeof(int)));
+	CK(pool_alloc(&eb.word, 4 * sizeof(int)));
+	CK(cudaMemsetAsync(eb.word, 0, 4 * sizeof(int), st));
+	EmitCells occ {};
+	{
+		const int R = s->rollid, Rn = R ^ 1;
+		occ.cfg = cfg;
+		occ.table = s->part[R].index_table;
+		occ.pbc = &s->d_state->pbc;
+		occ.n_models = nm;
+		for(int m = 0; m < nm; ++m) {
+			occ.offs[m] = s->models[m].celloffs[Rn];
+			occ.sizes[m] = s->models[m].pb[Rn].particle_bucket_sizes;
+		}
+	}
+	emit_filter_kernel<<<launch_items(n, 256), 256, 0, st>>>(occ, n, eb.cand, (flags & CB200_EMIT_EMPTY_CELLS) ? 1 : 0, eb.keep, eb.word + 1);
+	ScanArgs sc {};
+	sc.count = count_imm(n);
+	sc.count_plus = 1;
+	sc.in = eb.keep;
+	sc.out = eb.offs;
+	scan_kernel<<<1, 1024, 0, st>>>(sc);
+	s->launches += 2;
+	CK(cudaGetLastError());
+	int k = 0, bad = 0;
+	CK(cudaMemcpyAsync(&k, eb.offs + n, sizeof(int), cudaMemcpyDeviceToHost, st));
+	CK(cudaMemcpyAsync(&bad, eb.word + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	if(bad) return (int) cudaErrorInvalidValue;
+	if(k == 0) return 0;
+	CK(pool_alloc(&eb.kept, (size_t) k * 3 * sizeof(float)));
+	emit_compact_kernel<<<launch_items(n, 256), 256, 0, st>>>(n, eb.cand, eb.keep, eb.offs, eb.kept);
+	++s->launches;
+	// (2) the union's partition on a scratch table: the current particle blocks first, then the candidates' blocks, then the neighbour
+	// and exterior registrations of initial_setup.  Its capacity holds every block they can register, so the counts are exact.
+	CK(pull_state(s));
+	const StepState h0 = *s->h_state;
+	const int cap_s = (int) std::min<long long>((long long) s->table_entries, 27LL * ((long long) h0.pbc + k));
+	CK(pool_alloc(&eb.table, s->table_entries * sizeof(int)));
+	CK(pool_alloc(&eb.keys, ((size_t) cap_s + 1) * 3 * sizeof(int)));
+	CK(cudaMemsetAsync(eb.table, 0xff, s->table_entries * sizeof(int), st));
+	emit_insert_keys_kernel<<<launch_items(h0.pbc, 256), 256, 0, st>>>(cfg, h0.pbc, s->part[s->rollid].active_keys, eb.table, eb.keys, eb.word, cap_s);
+	activate_blocks_kernel<true><<<launch_items(k, 256), 256, 0, st>>>(cfg, k, eb.kept, eb.table, eb.keys, eb.word, cap_s, nullptr);
+	s->launches += 2;
+	int cnt[3] = {0, 0, 0};  // the union's pbc, nbc, ebc
+	CK(cudaMemcpyAsync(&cnt[0], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	RegisterArgs ra {};
+	ra.cfg = cfg;
+	ra.block_count = count_imm(cnt[0]);
+	ra.table = eb.table;
+	ra.keys = eb.keys;
+	ra.count = eb.word;
+	ra.capacity = cap_s;
+	ra.lo = 0;
+	ra.span = 2;
+	register_blocks_kernel<<<launch_items((long long) cnt[0] * 8, 128), 128, 0, st>>>(ra);
+	CK(cudaMemcpyAsync(&cnt[1], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
+	ra.lo = -1;
+	ra.span = 3;
+	register_blocks_kernel<<<launch_items((long long) cnt[0] * 27, 128), 128, 0, st>>>(ra);
+	CK(cudaMemcpyAsync(&cnt[2], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
+	// (3) no cell above max_ppc, existing and new particles together
+	CK(pool_alloc(&eb.cells, (size_t) cnt[0] * kBlockVol * sizeof(int)));
+	CK(cudaMemsetAsync(eb.cells, 0, (size_t) cnt[0] * kBlockVol * sizeof(int), st));
+	emit_count_kernel<<<launch_items(k, 256), 256, 0, st>>>(cfg, k, eb.kept, eb.table, eb.cells);
+	emit_overflow_kernel<<<launch_items(k, 256), 256, 0, st>>>(occ, k, eb.kept, eb.table, eb.cells, eb.word + 1);
+	s->launches += 4;
+	CK(cudaGetLastError());
+	CK(cudaMemcpyAsync(&bad, eb.word + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	if(bad) return (int) cudaErrorInvalidValue;
+	if((long long) s->models[model].n + k > 0x7fffffffLL) return (int) cudaErrorInvalidValue;  // n bounds the model's live count
+	// (4) capacity: the union's exterior blocks must fit (auto_grow: grow to 4/3 of them, after everything else that can fail)
+	int new_mb = s->desc.max_blocks;
+	if(cnt[2] > new_mb) {
+		if(!s->desc.auto_grow) return (int) cudaErrorMemoryAllocation;
+		new_mb = (int) (((long long) cnt[2] * 4 + 2) / 3);
+	}
+	// (5) gather the current state (checkpoint layout) and allocate what the commit swaps in: nothing live is written yet
+	CK(pool_alloc(&eb.blob, ck_capacity(s)));
+	CK(enqueue_snapshot(s, eb.blob));
+	int mats[kMaxModels];
+	long long counts[kMaxModels];
+	int totals[kMaxModels] = {};
+	for(int m = 0; m < nm; ++m) {
+		mats[m] = s->models[m].material;
+		CK(cudaMemcpyAsync(&totals[m], s->ck_base + (size_t) m * (s->desc.max_blocks + 1) + h0.pbc, sizeof(int), cudaMemcpyDeviceToHost, st));
+	}
+	CK(cudaStreamSynchronize(st));
+	for(int m = 0; m < nm; ++m) {
+		if(totals[m] < 0 || totals[m] > s->models[m].n) return (int) cudaErrorIllegalState;
+		counts[m] = totals[m];
+	}
+	const CkLayout L = ck_layout(nm, mats, counts, h0.nbc);
+	Model& md = s->models[model];
+	const int C = ck_channels(md.material);
+	const long long n_union = counts[model] + k;
+	const long long new_bins = n_union / kBinCap + new_mb;  // alloc_model's rule
+	const size_t binf = md.material == CB200_J_FLUID ? 128 : 512;
+	CK(pool_alloc(&eb.rows, (size_t) n_union * C * sizeof(float)));
+	CK(pool_alloc(&eb.pos, (size_t) n_union * 3 * sizeof(float)));
+	if(new_bins > md.bin_capacity)
+		for(int i = 0; i < 2; ++i) CK(pool_alloc(&eb.bins[i], (size_t) new_bins * binf * sizeof(float)));
+	if(L.model_bytes[model]) CK(cudaMemcpyAsync(eb.rows, eb.blob + L.model_off[model], L.model_bytes[model], cudaMemcpyDeviceToDevice, st));
+	emit_rows_kernel<<<launch_items(k, 256), 256, 0, st>>>(md.material, k, eb.kept, eb.rows + (size_t) counts[model] * C);
+	++s->launches;
+	CK(cudaGetLastError());
+	CK(cudaStreamSynchronize(st));
+	// the last step that can reject: cb200_sim_reserve (an out-of-memory failure there leaves a valid simulator, part-grown)
+	if(new_mb > s->desc.max_blocks) CK(cb200_sim_reserve(s, new_mb));
+	// (6) commit: initial_setup's restore path over the union, then the new particles' mass and momentum added to grid[0]
+	for(int i = 0; i < 2; ++i) {
+		if(s->graph[i]) cudaGraphExecDestroy(s->graph[i]);
+		s->graph[i] = nullptr;
+	}
+	if(eb.bins[0] && new_bins > md.bin_capacity) {  // (reserve may have grown the bins past the new count's rule already)
+		for(int i = 0; i < 2; ++i) std::swap(md.pb[i].bins, eb.bins[i]);
+		md.bin_capacity = new_bins;
+	}
+	std::swap(md.d_pos, eb.pos);
+	RestoreSrc rs {};
+	for(int m = 0; m < nm; ++m) {
+		Model& mm = s->models[m];
+		mm.n = (int) (m == model ? n_union : counts[m]);
+		rs.state[m] = m == model ? eb.rows : reinterpret_cast<const float*>(eb.blob + L.model_off[m]);
+		state_positions_kernel<<<num_sms() * 4, 256, 0, st>>>(mm.n, ck_channels(mm.material), rs.state[m], mm.d_pos);
+		++s->launches;
+	}
+	rs.keys = reinterpret_cast<const int*>(eb.blob + L.keys_off);
+	rs.grid = reinterpret_cast<const float*>(eb.blob + L.grid_off);
+	rs.grid_count = h0.nbc;
+	{  // setup_impl starts from an empty partition (roll Rn) and zero cell counts / bucket sizes in the buffers it buckets into (roll R)
+		const int R = s->rollid, Rn = R ^ 1;
+		const size_t mb = (size_t) s->desc.max_blocks;
+		CK(cudaMemsetAsync(s->part[Rn].index_table, 0xff, s->table_entries * sizeof(int), st));
+		CK(cudaMemsetAsync(s->part[Rn].count, 0, sizeof(int), st));
+		for(Model& mm : s->models) {
+			CK(cudaMemsetAsync(mm.pb[R].cell_particle_counts, 0, (mb + 1) * kBlockVol * sizeof(int), st));
+			CK(cudaMemsetAsync(mm.pb[R].particle_bucket_sizes, 0, (mb + 2) * sizeof(int), st));
+		}
+	}
+	// the clock stays; dt and next_dt follow initial_setup's rule for v0
+	cb200_checkpoint_info I;
+	memset(&I, 0, sizeof(I));
+	I.particle_block_count = cnt[0];
+	I.neighbor_block_count = cnt[1];
+	I.exterior_block_count = cnt[2];
+	I.error = h0.error;
+	I.step_time = h0.step_time;
+	I.frame_time = h0.frame_time;
+	I.sim_time = h0.sim_time;
+	I.steps = h0.steps;
+	I.frames = s->frames_done;
+	float dt = h0.dt;
+	const float mv = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+	if(mv > 0.f) dt = fminf(dt, cfg.dx * cfg.cfl / mv);
+	I.dt = I.next_dt = dt;
+	rs.info = &I;
+	s->setup_done = false;
+	CK(setup_impl(s, &rs));
+	// every stencil node of a new particle inside the domain lies in a neighbour block of its particle block; nodes past the top face
+	// are dropped, as rasterize_blocks_kernel drops them
+	rasterize_kernel<<<launch_items(k, 256), 256, 0, st>>>(cfg, k, eb.kept, s->grid[0], s->part[s->rollid].index_table, md.pb[0].mass, v[0], v[1], v[2], nullptr);
+	++s->launches;
+	CK(cudaGetLastError());
+	CK(cudaStreamSynchronize(st));
+	if(n_added) *n_added = k;
+	return 0;
+}
+}  // namespace
+extern "C" {
+
+int cb200_sim_add_particles(cb200_sim* s, int model, const float* positions_host, int n, const float* v0, unsigned flags, int* n_added) {
+	if(n_added) *n_added = 0;
+	CK(emit_precheck(s, model, flags, v0));
+	if(n < 0 || (n > 0 && !positions_host)) return (int) cudaErrorInvalidValue;
+	if(n == 0) return 0;
+	CK(cudaStreamSynchronize(s->stream));
+	EmitBuffers eb;
+	CK(pool_alloc(&eb.cand, (size_t) n * 3 * sizeof(float)));
+	CK(cudaMemcpyAsync(eb.cand, positions_host, (size_t) n * 3 * sizeof(float), cudaMemcpyHostToDevice, s->stream));
+	return emit_impl(s, model, eb, n, v0, flags, n_added);
+}
+
+int cb200_sim_add_particles_sdf(cb200_sim* s, int model, const cb200_sdf_header* header, const float* phi_host, const cb200_sdf_sampling* sampling,
+                                const float* v0, unsigned flags, int* n_added) {
+	if(n_added) *n_added = 0;
+	CK(emit_precheck(s, model, flags, v0));
+	if(!header || !sampling) return (int) cudaErrorInvalidValue;
+	CK(cudaStreamSynchronize(s->stream));
+	SdfRun r;
+	r.st = s->stream;
+	CK(r.run_count(s->desc.cfg, *header, phi_host, *sampling));
+	if(r.count >= (1LL << 31)) return (int) cudaErrorInvalidValue;
+	if(r.count == 0) return 0;
+	EmitBuffers eb;
+	CK(pool_alloc(&eb.cand, (size_t) r.count * 3 * sizeof(float)));
+	CK(r.run_write(eb.cand));
+	return emit_impl(s, model, eb, (int) r.count, v0, flags, n_added);
 }
 
 // ---- MGSP peer wiring ------------------------------------------------------------------------------------------

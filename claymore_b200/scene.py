@@ -19,6 +19,14 @@ simulation cell, default 8: the reference's MODEL_PPC, settings.h:51) and "seed"
 [offset, offset + span] with one scale for all axes, and a node box outside the domain rejects the scene before any device work
 (claymore_b200.sdf).  A model may also name a synthetic generator: "file": "box" (span in cells of the lattice sampler) or
 "sphere" (span = diameter), or a raw float32 xyz `.bin` cloud as used by mgsp.cu:11-17.
+
+A model may be a source: "emit": {"start": 2, "every": 1, "until": <frames>, "fill": "all"|"empty"} (defaults as shown; "until"
+defaults to the scene's frame count).  At the start of frames start, start + every, ... <= until, before the frame's sub-steps, the
+model's own shape (its file / offset / span, or its `.sdf` level set with its sampler and ppc; random mode with seed seed + frame) is
+sampled again and added with the model's "velocity" (GmpmSimulator.add_particles).  "fill": "empty" adds only particles whose cell
+holds no particle, so a repeating source refills only the cells its material has left.  Frame 1 starts from the model's initial
+particles; a resumed run emits exactly the frames an uninterrupted run emits after the checkpoint's frame.  Bad "emit" keys or
+values, or "emit" in MGSP mode, raise ValueError before any device work.
 """
 import json
 import os
@@ -86,6 +94,77 @@ def _collider(sim, c, cfg, base_dir):
                      omega=c.get("omega", [0, 0, 0]), scale=c.get("scale", 1.0), dsdt=c.get("dsdt", 0.0))
 
 
+EMIT_KEYS = ("start", "every", "until", "fill")
+EMIT_FILLS = ("all", "empty")
+
+
+def _emit_spec(model, i, frames):
+    """The validated "emit" entry of scene model i (None without one): {"start", "every", "until", "fill"}."""
+    e = model.get("emit")
+    if e is None:
+        return None
+    if not isinstance(e, dict):
+        raise ValueError(f"model {i}: \"emit\" must be an object with keys {', '.join(EMIT_KEYS)}")
+    unknown = sorted(set(e) - set(EMIT_KEYS))
+    if unknown:
+        raise ValueError(f"model {i}: unknown \"emit\" keys {unknown} (known: {', '.join(EMIT_KEYS)})")
+    spec = {"start": e.get("start", 2), "every": e.get("every", 1), "until": e.get("until"), "fill": e.get("fill", "all")}
+    if spec["until"] is None:   # the last frame; a scene shorter than `start` then has no emission
+        spec["until"] = max(frames, spec["start"]) if isinstance(spec["start"], int) else frames
+    for k in ("start", "every", "until"):
+        if isinstance(spec[k], bool) or not isinstance(spec[k], int):
+            raise ValueError(f"model {i}: \"emit\".{k} must be an integer, not {spec[k]!r}")
+    if spec["every"] < 1:
+        raise ValueError(f"model {i}: \"emit\".every must be at least 1, not {spec['every']}")
+    if spec["start"] < 2:
+        raise ValueError(f"model {i}: \"emit\".start must be at least 2 (frame 1 starts from the initial particles), not {spec['start']}")
+    if spec["until"] < spec["start"]:
+        raise ValueError(f"model {i}: \"emit\".until ({spec['until']}) must not precede start ({spec['start']})")
+    if spec["fill"] not in EMIT_FILLS:
+        raise ValueError(f"model {i}: unknown \"emit\".fill {spec['fill']!r} (known: {', '.join(EMIT_FILLS)})")
+    return spec
+
+
+def emit_schedule(doc, after=0):
+    """{scene model index: [(frame, seed), ...]}: the emissions of every source model at frames > `after` (a resumed run's checkpoint
+    frame), with the seed its random-mode sampling uses.  Validates every "emit" entry (ValueError)."""
+    frames = doc.get("simulation", {}).get("frames", GmpmSimulator.DEFAULT_FRAMES)
+    models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
+    out = {}
+    for i, model in enumerate(models):
+        spec = _emit_spec(model, i, frames)
+        if spec is not None:
+            seed = model.get("seed", 0)
+            out[i] = [(f, seed + f) for f in range(spec["start"], min(spec["until"], frames) + 1, spec["every"]) if f > after]
+    return out
+
+
+def _emitters(doc, cfg, base, level_sets):
+    """main_loop's per-frame emitters of the scene's source models (every source file is read here, before any device work)."""
+    frames = doc.get("simulation", {}).get("frames", GmpmSimulator.DEFAULT_FRAMES)
+    models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
+    out = []
+    for i, frames_seeds in emit_schedule(doc).items():
+        model = models[i]
+        todo = dict(frames_seeds)
+        v0, fill = model.get("velocity", [0, 0, 0]), _emit_spec(model, i, frames)["fill"]
+        offset, span = model.get("offset", [0, 0, 0]), model.get("span", [1, 1, 1])
+        if i in level_sets:
+            ls, ppc, mode = level_sets[i], model.get("ppc", 8), model.get("sampler", "random")
+
+            def emit(s, f, i=i, ls=ls, ppc=ppc, mode=mode, todo=todo, v0=v0, fill=fill, offset=offset, span=span):
+                if f in todo:
+                    s.add_particles_sdf(i, ls, offset, span, v0, ppc=ppc, mode=mode, seed=todo[f], fill=fill)
+        else:
+            pos = _positions(model, cfg, base)
+
+            def emit(s, f, i=i, pos=pos, todo=todo, v0=v0, fill=fill):
+                if f in todo:
+                    s.add_particles(i, pos, v0, fill=fill)
+        out.append(emit)
+    return out
+
+
 def _check_resume(doc, cfg, resume):
     """The checkpoint `resume` must belong to this document: same config, default dt, fps and constitutive models."""
     from . import checkpoint
@@ -116,19 +195,24 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
         base = os.path.dirname(os.path.abspath(path_or_dict))
     cfg = config if config is not None else Config()
     s = doc.get("simulation", {})
+    if emit_schedule(doc) and sim_kwargs.get("mgsp_world", 1) > 1:
+        raise ValueError("\"emit\" is not supported in MGSP mode")
+    models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
     if resume is not None:
         inf = _check_resume(doc, cfg, resume)
+        emitters = _emitters(doc, cfg, base, _level_sets(models, base))
         sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                             frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max(max_blocks, inf["max_blocks"]), **sim_kwargs)
         if "collider" in doc:
             _collider(sim, doc["collider"], cfg, base)
         sim.restore(resume)
+        sim.emitters = emitters
         return sim
-    models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
     for model in models:
         if model.get("constitutive") not in CONSTITUTIVE:
             raise ValueError(f"unknown constitutive model {model.get('constitutive')!r}")
     level_sets = _level_sets(models, base)
+    emitters = _emitters(doc, cfg, base, level_sets)
     sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                         frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max_blocks, **sim_kwargs)
     for i, model in enumerate(models):
@@ -150,4 +234,5 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
             sim.update_sand_parameters(model["rho"], model["volume"], model["youngs_modulus"], model["poisson_ratio"], model=mid)
     if "collider" in doc:
         _collider(sim, doc["collider"], cfg, base)
+    sim.emitters = emitters
     return sim

@@ -41,6 +41,7 @@ class GmpmSimulator:
         self.materials, self.counts = [], []
         self.cur_frame = 0
         self.restored = False
+        self.emitters = []   # fn(sim, frame): called by main_loop at the start of each frame, before its sub-steps
         self._output_paths = []   # files of the frame being written (for the error of wait_output)
 
     # ---- lifecycle -------------------------------------------------------------------------------
@@ -80,6 +81,49 @@ class GmpmSimulator:
         self.counts.append(n.value)
         return mid.value
 
+    # ---- sources: particles added to a set-up simulator at the current sub-step boundary (synchronises) -------------------
+    EMIT_FILL = {"all": 0, "empty": _capi.EMIT_EMPTY_CELLS}
+
+    def _fill(self, fill):
+        if fill not in self.EMIT_FILL:
+            raise ValueError(f"unknown fill {fill!r} (known: {', '.join(self.EMIT_FILL)})")
+        return self.EMIT_FILL[fill]
+
+    @staticmethod
+    def _v0(v0):
+        v = np.ascontiguousarray(v0, dtype=np.float32)
+        if v.shape != (3,):
+            raise ValueError(f"v0 must have 3 components, not shape {v.shape}")
+        return v
+
+    def add_particles(self, model, positions, v0=(0.0, 0.0, 0.0), fill="all"):
+        """Appends particles to `model`, all with velocity v0 (the model starts them from F = I, as init_model).  fill="empty" keeps
+        only positions whose cell held no particle of any model before the call.  Returns the count added.  The clock is kept;
+        dt becomes min(dt, dx cfl / |v0|).  counts[model] grows by the count added; every model's library-side count becomes its
+        live count, so counts stays an upper bound for sizing buffers, as it is once particles are lost."""
+        flags = self._fill(fill)
+        pos = np.ascontiguousarray(positions, dtype=np.float32).reshape(-1, 3)
+        v = self._v0(v0)
+        n = C.c_int(0)
+        check(self.L.cb200_sim_add_particles(self.h, model, pos.ctypes.data_as(C.c_void_p), len(pos), v.ctypes.data_as(C.c_void_p), flags, C.byref(n)),
+              "add_particles")
+        self.counts[model] += n.value
+        return n.value
+
+    def add_particles_sdf(self, model, ls, offset, span, v0=(0.0, 0.0, 0.0), ppc=8, mode="random", seed=0, fill="all"):
+        """add_particles with the positions sampled on the device from a level set, as init_model_sdf samples them."""
+        from . import sdf
+        flags = self._fill(fill)
+        v = self._v0(v0)
+        sdf.check_box(ls, offset, span)
+        smp = sdf.sampling(offset, span, ppc, mode, seed)
+        phi = np.ascontiguousarray(ls.phi, dtype=np.float32)
+        n = C.c_int(0)
+        check(self.L.cb200_sim_add_particles_sdf(self.h, model, C.byref(ls.header), phi.ctypes.data_as(C.c_void_p), C.byref(smp),
+                                                 v.ctypes.data_as(C.c_void_p), flags, C.byref(n)), "add_particles_sdf")
+        self.counts[model] += n.value
+        return n.value
+
     def update_fr_parameters(self, rho, vol, ym, pr, model=-1):
         check(self.L.cb200_sim_update_fr_parameters(self.h, self._m(model), rho, vol, ym, pr), "update_fr_parameters")
 
@@ -112,11 +156,14 @@ class GmpmSimulator:
     def main_loop(self, on_frame=None, output=None, attributes=()):
         """initial_setup + nframes frames (gmpm_simulator.cuh:303-591).  output: a directory that receives every finished frame
         1..nframes as the reference's files (write_frame, `attributes` as there), written while the next frame runs; the loop waits
-        for the last files before it returns.  on_frame(sim, frame) is called after each frame.
+        for the last files before it returns.  on_frame(sim, frame) is called after each frame; every emitter (sim, frame) at the
+        start of the frame, before its sub-steps (after the previous frame's files were queued).
         A restored simulator is set up already and runs only the frames after the ones its checkpoint had finished."""
         if not self.restored:
             self.initial_setup()
         for f in range(self.cur_frame + 1, self.nframes + 1):
+            for emit in self.emitters:
+                emit(self, f)
             self.advance_frame()
             if self.stats().error:
                 break

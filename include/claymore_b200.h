@@ -396,6 +396,45 @@ CB200_API int cb200_sim_init_model_sdf(cb200_sim* sim, int material, const cb200
                                        const cb200_sdf_sampling* sampling, const float* v0, int* model_id, int* n_out);
 
 /* ------------------------------------------------------------------------------------------------
+ * Adding particles to a running simulation (sources: inlets, pouring, an object dropped later).  Both entries share one path and
+ * differ only in where the candidate positions come from.  The call synchronises and acts at the current sub-step boundary.
+ *   Rejections, all before anything changes (a checkpoint taken after one is byte-identical to one taken before it):
+ *     cudaErrorNotSupported    MGSP mode (as cb200_sim_reserve);
+ *     cudaErrorInvalidValue    a simulator that is not set up, an unknown model, unknown flag bits, a v0 that is not finite, a bad
+ *                              .sdf header, mode or ppc (as cb200_sim_init_model_sdf), a candidate that is not finite or whose bucket block (cell_index - 2,
+ *                              floor, per axis) lies outside the domain, a cell that would hold more than max_ppc particles
+ *                              (existing ones of every model plus the new ones), or more than 2^31 - 1 particles in the model;
+ *     cudaErrorMemoryAllocation  the union's exterior blocks exceed the block capacity and auto_grow is off (with auto_grow the
+ *                              capacity grows, through cb200_sim_reserve, to 4/3 of them: the last step before the commit, so an
+ *                              out-of-memory failure of that growth may leave the capacity grown, as cb200_sim_reserve does).
+ *   n = 0, or a filter that keeps nothing, is a successful no-op.
+ *   A device error after the commit has begun (out of memory while re-capturing the sub-step graphs, a failing launch) leaves a
+ *   simulator that cannot step: destroy it, or restore a checkpoint into a new one.
+ *   After the call, at the same boundary:
+ *     - every existing particle of every model keeps all its channels bitwise (as a multiset of rows);
+ *     - a new row holds the candidate's position bitwise and the model's start state: F = I (J_FLUID: J = 1), logJp = LOG_JP_0;
+ *     - the partition's particle / neighbour / exterior keys are the ones initial_setup builds for the union of the positions;
+ *     - grid[0] holds, cell by cell, its value before the call plus the rasterisation of the new particles (mass pb.mass, momentum
+ *       mass * v0, the quadratic B-spline); blocks new to the partition hold only the new contribution;
+ *     - steps, sim_time, step_time, frame_time and the frames finished are kept; dt and next_dt become min(dt, dx cfl / |v0|),
+ *       initial_setup's float expression, so an emission right after initial_setup starts from the dt of a set-up over the union;
+ *     - the model's bins grow to n / 32 + max_blocks; the sub-step graphs are re-captured;
+ *     - every model's particle count becomes its live count: a model that lost particles before the call (kErrLostParticle,
+ *       kErrCellOverflow) no longer counts them, as cb200_sim_retrieve and a checkpoint already did not.
+ *   A checkpoint_begin copy or a frame_output frame in flight still delivers the state from before the call.
+ * ---------------------------------------------------------------------------------------------- */
+#define CB200_EMIT_EMPTY_CELLS 1u   /* keep only particles whose cell holds no particle of any model before the call */
+/* Appends particles to `model` at the current sub-step boundary.  positions_host: HOST float[3n]; v0: one velocity for all of them
+ * (nullable = 0).  *n_added (nullable): rows actually appended (n, or fewer with CB200_EMIT_EMPTY_CELLS).
+ * CB200_EMIT_EMPTY_CELLS: a candidate's cell is cell_index(x) per axis (the cell the buckets are built by); the candidate is dropped,
+ * not rejected, when any model held a particle in that cell before the call.  Candidates of one call that share a cell are all
+ * kept, so emitting the same region twice at one boundary adds nothing the second time. */
+CB200_API int cb200_sim_add_particles(cb200_sim* sim, int model, const float* positions_host, int n, const float* v0, unsigned flags, int* n_added);
+/* The same with positions sampled on the device from a level set, as cb200_sim_init_model_sdf samples them (no host copy). */
+CB200_API int cb200_sim_add_particles_sdf(cb200_sim* sim, int model, const cb200_sdf_header* header, const float* phi_host,
+                                          const cb200_sdf_sampling* sampling, const float* v0, unsigned flags, int* n_added);
+
+/* ------------------------------------------------------------------------------------------------
  * Test-only hooks (used by tests/, not part of the drop-in surface): the device 3x3 SVD and constitutive models of g2p2g on
  * caller-supplied DEVICE vectors, against math::svd (Library/MnBase/Math/Matrix/svd.cuh:28-1124) and compute_stress<M>
  * (Projects/GMPM/constitutive_models.cuh:36-335).  F: float[9n] column-major; mode 0 = the path g2p2g takes, 1 = FIXED_COROTATED via SVD.
