@@ -17,7 +17,9 @@ Conventions the engine keeps (DESIGN.md section 3, quirks):
 * #6 the fluid's J is clamped at 0.1; #7 FIXED_COROTATED stores the trial F;
 * #9 a node whose FP32 mass is subnormal holds no mass for the grid update (the reference flushes subnormals to zero);
 * a cell takes at most max_ppc particles at re-bucketing; the rest leave the next partition (``cell_overflow``);
-* nodes outside the domain do not exist: what a particle would add there is dropped.
+* nodes outside the domain do not exist: what a particle would add there is dropped;
+* a signed-distance collider (DESIGN.md section 2.4, C1-C6) acts after the wall mask and gravity on the nodes with mass
+  (collider_resolve); nodes near one of its discontinuities, and what reads them, are left out of the checks and counted.
 
 Every output comes with a magnitude M such that an FP32 implementation of the same operations differs from the float64
 value by at most a small multiple of 2^-24 * M.  The tests fix that multiple (kappa) per quantity.
@@ -179,11 +181,14 @@ def compute_dt(cfg, max_vsq, dt_default, time_left=np.inf):
     return min(dt, time_left)
 
 
-def grid_update(cfg, keys, grid, dt):
+def grid_update(cfg, keys, grid, dt, collider=None, t=0.0):
     """v = mv / m, wall mask on both faces (key < boundary or key >= G - boundary), then gravity, on the nodes whose mass
     is at least FLT_MIN (a subnormal FP32 mass is no mass: the reference flushes subnormals to zero); other nodes keep
-    their momentum channels as they are (0 where nothing was added).
-    Returns (vel[nb,3,64], magnitude[nb,3,64], max |v|^2 over the nodes with mass, NaN -> +inf)."""
+    their momentum channels as they are (0 where nothing was added).  With ``collider`` = (col, sdf, grad) the nodes with
+    mass then resolve against it, placed at time ``t`` (collider_resolve), and the max is |v|^2 after the collider (C2).
+    Returns (vel[nb,3,64], magnitude[nb,3,64], max |v|^2 over the nodes with mass, NaN -> +inf), and with a collider a
+    fourth item: dict(near[nb,64], branch[nb,64], margin[nb,64], vo[nb,3,64], mx_lo, mx_hi, mx_err), the max over every
+    choice of the near nodes' branches lying in [mx_lo, mx_hi], and each other node's |v|^2 within kappa 2^-24 mx_err."""
     keys = np.asarray(keys, np.int64)
     grid = np.asarray(grid, np.float64)
     G, bc = 1 << (cfg.domain_bits - 2), cfg.boundary
@@ -197,9 +202,307 @@ def grid_update(cfg, keys, grid, dt):
     gdt = float(np.float32(cfg.gravity)) * dt
     v[:, 1] += np.where(has, gdt, 0.0)
     mag[:, 1] += np.where(has, abs(gdt), 0.0)
+    info = None
+    if collider is not None:
+        col, sdf, grad = collider
+        nb = len(keys)
+        info = dict(near=np.zeros((nb, 64), bool), branch=np.full((nb, 64), "", dtype=object), margin=np.full((nb, 64), np.inf),
+                    vo=np.zeros((nb, 3, 64)))
+        b, c = np.nonzero(has)
+        nodes = keys[b] * 4 + _CELLS[c]
+        r = collider_resolve(cfg, col, sdf, grad, t, nodes, v[b, :, c], mag[b, :, c])
+        v[b, :, c], mag[b, :, c] = r["v"], r["mag"]
+        for f in ("near", "branch", "margin"):
+            info[f][b, c] = r[f]
+        info["vo"][b, :, c] = r["vo"]
+        lo, hi = np.zeros((nb, 64)), np.zeros((nb, 64))
+        lo[b, c], hi[b, c] = r["vsq_lo"], r["vsq_hi"]
+        info["mx_lo"] = float(np.nan_to_num(lo, nan=np.inf).max(initial=0.0))
+        info["mx_hi"] = float(np.nan_to_num(hi, nan=np.inf).max(initial=0.0))
+        # E of each resolved node's |v|^2 (sum 2 |v_d| E_d, first order): at a box's edge it can exceed |v|^2 by far
+        info["mx_err"] = float(np.where(r["near"], 0.0, (2 * np.abs(r["v"]) * r["mag"]).sum(1)).max(initial=0.0))
     vsq = np.where(has, (v ** 2).sum(1), 0.0)
     vsq = np.where(np.isnan(vsq), np.inf, vsq)
-    return v, mag, float(vsq.max()) if vsq.size else 0.0
+    mx = float(vsq.max()) if vsq.size else 0.0
+    return (v, mag, mx) if info is None else (v, mag, mx, info)
+
+
+# ---- signed-distance collider (DESIGN.md section 2.4, oracle/collider_oracle.c) ----------------------------------------
+# Every FP32 quantity of the collider is carried as (value, E): its float64 value and an error magnitude E such that the FP32
+# value differs from it by at most a small multiple of 2^-24 * E (first order).  Rules, for exact float32 inputs (E = 0):
+#   a + b: Ea + Eb + rnd(a + b);  a * b: Ea |b| + |a| Eb + rnd(a b);  a / b: Ea / |b| + |a| Eb / b^2 + rnd(a / b);
+#   sqrt(a): Ea / (2 sqrt a) + rnd(sqrt a);  rnd(r) = |r| unless r is a float32 value (then the operation is exact);
+#   sin / cos of an angle a: SINCOS_ULPS |value| + |cos / sin| Ea (the device's sinf / cosf are within a few ulp);
+#   trilinear phi (distance or a gradient component) at the material-space point x: sum_c (E_w,c |f_c| + 2 w_c |f_c|) over
+#   the 8 corners, plus its sensitivity to the rounding of x, sum_d |d phi / d x_d| E_x,d with |d phi / d x_d| the largest
+#   one-sided slope of the cell and of its two neighbours along d (the 1/dx amplification at a box's edges);
+#   normalisation: |dn| <= 2 |dn_raw| / |n_raw|, plus the roundings of the sqrt and the division;
+#   friction: v += v / len * (vn f) as the products and sums it is, with |vn f| / len taken at most 1 (the slide side at the
+#   stick switch, where both sides are 0).
+# Exact zeros and exact copies (STICKY's v = 0, the identity frame of a static collider) carry E = 0, so a node of a static
+# collider on the lattice is not near the wall band edge it sits on.
+# Discontinuities: the hit test (sd <= 0), the wall band (x < lo, x >= hi), the top guard (node gc + 1 >= 4G) and the exact
+# zero-normal test.  A node whose distance to one of them is within NEAR x 2^-24 x its own E is "near": its branch may differ
+# in FP32, it leaves the checks and is counted.  The approach / separate switch (vn = 0) and the stick / slide switch
+# (-vn f = len) are continuous; within NEAR x their error, E is the larger of the two sides'.
+STICKY, SLIP, SEPARATE = 0, 1, 2
+NEAR = 16.0
+SINCOS_ULPS = 4.0
+_CELLS = np.stack(np.meshgrid(np.arange(4), np.arange(4), np.arange(4), indexing="ij"), -1).reshape(64, 3)
+
+
+def _rnd(r):
+    r = np.asarray(r, np.float64)
+    with np.errstate(over="ignore", invalid="ignore"):
+        return np.where(np.float32(r).astype(np.float64) == r, 0.0, np.abs(r))
+
+
+def _add(a, b):
+    v = a[0] + b[0]
+    return v, a[1] + b[1] + _rnd(v)
+
+
+def _sub(a, b):
+    v = a[0] - b[0]
+    return v, a[1] + b[1] + _rnd(v)
+
+
+def _mul(a, b):
+    v = a[0] * b[0]
+    return v, a[1] * np.abs(b[0]) + np.abs(a[0]) * b[1] + _rnd(v)
+
+
+def _div(a, b):
+    v = a[0] / b[0]
+    return v, a[1] / np.abs(b[0]) + np.abs(a[0]) * b[1] / b[0] ** 2 + _rnd(v)
+
+
+def _exact(x):
+    x = np.asarray(x, np.float64)
+    return x, np.zeros_like(x)
+
+
+def _dot3(a, b, i, j):
+    """sum_k a[i(k)] * b[j(k)], k = 0, 1, 2 left to right (a, b: (value, E) with the components on the last axis)."""
+    s = None
+    for k in range(3):
+        p = _mul((a[0][..., i(k)], a[1][..., i(k)]), (b[0][..., j(k)], b[1][..., j(k)]))
+        s = p if s is None else _add(s, p)
+    return s
+
+
+def collider_params(c):
+    """The collider's float32 parameters as float64 values: a cb200_collider / orc_collider struct or a dict with its fields."""
+    get = (lambda k: c[k]) if isinstance(c, dict) else (lambda k: getattr(c, k))
+    f = lambda x: np.asarray(np.asarray(x, np.float32), np.float64)   # noqa: E731
+    return dict(rot_mat=f(list(get("rot_mat"))).reshape(9), trans=f(list(get("trans"))), trans_vel=f(list(get("trans_vel"))),
+                omega=f(list(get("omega"))), dsdt=float(f(get("dsdt"))), scale=float(f(get("scale"))), friction=float(f(get("friction"))),
+                type=int(get("type")))
+
+
+def collider_frame(col, t):
+    """The collider's frame at the float32 time t: rot (9, storage (i, j) at 3i + j) = Rz(w_z t) Ry(w_y t) Rx(w_x t) rot_mat in
+    storage order (collider_mat_mul multiplies the new axis rotation from the left), b = trans + trans_vel t,
+    s_inv = 1 / (1 + dsdt t); each as (value, E)."""
+    col = collider_params(col)
+    t = float(np.float32(t))
+    cur = _exact(col["rot_mat"])
+    for d in range(3):
+        a = _mul(_exact(col["omega"][d]), _exact(t))
+        c, s = np.cos(a[0]), np.sin(a[0])
+        ec, es = SINCOS_ULPS * abs(c) + abs(s) * a[1], SINCOS_ULPS * abs(s) + abs(c) * a[1]
+        if a[0] == 0.0:
+            c, s, ec, es = 1.0, 0.0, 0.0, 0.0                     # sinf(0) = 0, cosf(0) = 1 exactly
+        r, er = np.zeros(9), np.zeros(9)
+        one = [0, 4, 8][d]
+        r[one] = 1.0
+        ci, si, mi = {0: ((4, 8), 7, 5), 1: ((0, 8), 2, 6), 2: ((0, 4), 3, 1)}[d]
+        r[list(ci)], er[list(ci)] = c, ec
+        r[si], er[si] = s, es
+        r[mi], er[mi] = -s, es
+        # c[3j + i] = a[i] b[3j] + a[3 + i] b[3j + 1] + a[6 + i] b[3j + 2], a = the previous frame, b = the axis rotation
+        nv, ne = np.zeros(9), np.zeros(9)
+        for j in range(3):
+            for i in range(3):
+                v = _dot3(cur, (r, er), lambda k, i=i: 3 * k + i, lambda k, j=j: 3 * j + k)
+                nv[3 * j + i], ne[3 * j + i] = v
+        cur = (nv, ne)
+    b = _add(_exact(col["trans"]), _mul(_exact(col["trans_vel"]), _exact(t)))
+    s_inv = _div(_exact(1.0), _add(_exact(1.0), _mul(_exact(col["dsdt"]), _exact(t))))
+    return dict(rot=cur, b=b, s_inv=s_inv, t=t, col=col)
+
+
+def _trilinear(f, gc, w, ew, N):
+    """phi at the 8 corners gc + {0, 1}^3 of the dense field f[(N, N, N)] with weights w[n, 3, 2] (errors ew), and its E
+    without the position sensitivity."""
+    val, err = 0.0, 0.0
+    for i in range(2):
+        for j in range(2):
+            for k in range(2):
+                fc = f[np.minimum(gc[:, 0] + i, N - 1), np.minimum(gc[:, 1] + j, N - 1), np.minimum(gc[:, 2] + k, N - 1)].astype(np.float64)
+                wc = w[:, 0, i] * w[:, 1, j] * w[:, 2, k]
+                ewc = ew[:, 0, i] * w[:, 1, j] * w[:, 2, k] + w[:, 0, i] * ew[:, 1, j] * w[:, 2, k] + w[:, 0, i] * w[:, 1, j] * ew[:, 2, k]
+                val = val + wc * fc
+                err = err + ewc * np.abs(fc) + 2 * wc * np.abs(fc)
+    return val, err
+
+
+def _slope(f, gc, w, N, dx):
+    """[n, 3]: the largest |d phi / d x_d| of the trilinear interpolant over the cell gc and its two neighbours along d."""
+    out = np.zeros((len(gc), 3))
+    for d in range(3):
+        o1, o2 = [e for e in range(3) if e != d]
+        for shift in (-1, 0, 1):
+            s = 0.0
+            for i in range(2):
+                for j in range(2):
+                    idx_lo, idx_hi = [None] * 3, [None] * 3
+                    idx_lo[o1] = idx_hi[o1] = np.clip(gc[:, o1] + i, 0, N - 1)
+                    idx_lo[o2] = idx_hi[o2] = np.clip(gc[:, o2] + j, 0, N - 1)
+                    idx_lo[d] = np.clip(gc[:, d] + shift, 0, N - 1)
+                    idx_hi[d] = np.clip(gc[:, d] + shift + 1, 0, N - 1)
+                    s = s + w[:, o1, i] * w[:, o2, j] * (f[tuple(idx_hi)].astype(np.float64) - f[tuple(idx_lo)])
+            out[:, d] = np.maximum(out[:, d], np.abs(s) / dx)
+    return out
+
+
+def collider_resolve(cfg, col, sdf, grad, t, nodes, v, vmag):
+    """detect_and_resolve_collision of the velocities v[n, 3] (magnitudes vmag[n, 3]) at the grid nodes nodes[n, 3], the
+    collider col (collider_params) placed at the float32 time t, its level set the dense sdf[(N, N, N)], grad[(3, N, N, N)]
+    read by node index.  Returns dict(v, mag (E of each component), vo (the object velocity), hit, branch (label), margin
+    (distance to the nearest discontinuity in units of 2^-24 E), near, vsq_lo, vsq_hi (|v|^2 over both sides of a near
+    node's branch))."""
+    f = collider_frame(col, t)
+    col = f["col"]
+    nodes = np.asarray(nodes, np.int64).reshape(-1, 3)
+    n = len(nodes)
+    G = 1 << (cfg.domain_bits - 2)
+    N, bc = 4 * G, cfg.boundary
+    dx = 1.0 / (1 << cfg.domain_bits)
+    vin = (np.asarray(v, np.float64).reshape(n, 3), np.asarray(vmag, np.float64).reshape(n, 3))
+    R = f["rot"]
+    Rb = (np.broadcast_to(R[0], (n, 9)), np.broadcast_to(R[1], (n, 9)))
+    # material-space point: x = R (node dx - b) s_inv scale + trans
+    xm = _sub(_exact(nodes * dx), (np.broadcast_to(f["b"][0], (n, 3)), np.broadcast_to(f["b"][1], (n, 3))))
+    x0 = _mul(xm, f["s_inv"])
+    y = [_dot3(Rb, x0, lambda k, d=d: 3 * d + k, lambda k: k) for d in range(3)]
+    y = (np.stack([a[0] for a in y], -1), np.stack([a[1] for a in y], -1))
+    x = _add(_mul(y, _exact(col["scale"])), _exact(col["trans"]))
+    tol = EPS32 * NEAR
+    # query: wall band, top guard, trilinear distance and gradient
+    lo, hi = float(bc) * dx * 4.0, float(G - bc) * 4.0 * dx
+    band = np.any((x[0] < lo) | (x[0] >= hi), axis=1)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        m_band = np.min(np.minimum(np.abs(x[0] - lo), np.abs(x[0] - hi)) / (EPS32 * x[1]), axis=1)
+    gc = np.clip(np.floor(x[0] / dx), 0, N - 1).astype(np.int64)
+    top = ~band & np.any(gc + 1 >= N, axis=1)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        m_top = np.min(np.abs(x[0] - (N - 1) * dx) / (EPS32 * x[1]), axis=1)
+    gcs = np.minimum(gc, N - 2)
+    dl = x[0] - gcs * dx
+    w = np.stack([1.0 - dl / dx, dl / dx], -1)                                 # [n, 3, 2]
+    ew = np.stack([_rnd(1.0 - dl / dx), _rnd(dl / dx)], -1)                    # the rounding of 1 - dl / dx (dl / dx is exact)
+    sd, esd = _trilinear(sdf, gcs, w, ew, N)
+    esd = esd + (_slope(sdf, gcs, w, N, dx) * x[1]).sum(1)                     # the sensitivity to the rounding of x
+    nr, enr = np.zeros((n, 3)), np.zeros((n, 3))
+    for d in range(3):
+        nr[:, d], enr[:, d] = _trilinear(grad[d], gcs, w, ew, N)
+        enr[:, d] += (_slope(grad[d], gcs, w, N, dx) * x[1]).sum(1)
+    hit = ~band & ~top & (sd <= 0)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        m_hit = np.abs(sd) / (EPS32 * esd)
+    nn = (nr ** 2).sum(1)
+    ln = np.sqrt(nn)
+    zero = nn == 0
+    enr_len = np.sqrt((enr ** 2).sum(1))
+    with np.errstate(divide="ignore", invalid="ignore"):
+        m_zero = np.where(zero, np.where(enr_len > 0, 0.0, np.inf), ln / (EPS32 * enr_len))
+        on = np.where(zero[:, None], 0.0, nr / np.where(zero, 1.0, ln)[:, None])
+        eon = np.where(zero[:, None], 0.0, (2 * enr_len / np.where(zero, 1.0, ln))[:, None] + 3 * np.abs(on))
+    # object velocity: omega x xm + xm dsdt / scale + R^T (omega (all-plus) r + trans_vel) scale + trans_vel, r = x - trans
+    wv = _exact(np.broadcast_to(col["omega"], (n, 3)))
+    cross = [_sub(_mul((wv[0][:, a], wv[1][:, a]), (xm[0][:, b], xm[1][:, b])), _mul((wv[0][:, b], wv[1][:, b]), (xm[0][:, a], xm[1][:, a])))
+             for a, b in ((1, 2), (2, 0), (0, 1))]
+    vo = (np.stack([c[0] for c in cross], -1), np.stack([c[1] for c in cross], -1))
+    ds = _div(_exact(col["dsdt"]), _exact(col["scale"]))
+    vo = _add(vo, _mul(xm, ds))
+    r = _sub(x, _exact(col["trans"]))
+    tv = _exact(np.broadcast_to(col["trans_vel"], (n, 3)))
+    mv = [_add(_add(_mul((wv[0][:, a], wv[1][:, a]), (r[0][:, b], r[1][:, b])), _mul((wv[0][:, b], wv[1][:, b]), (r[0][:, a], r[1][:, a]))),
+               (tv[0][:, d], tv[1][:, d])) for d, (a, b) in enumerate(((1, 2), (2, 0), (0, 1)))]
+    mv = (np.stack([m[0] for m in mv], -1), np.stack([m[1] for m in mv], -1))
+    rot_t = [_dot3(Rb, mv, lambda k, d=d: d + 3 * k, lambda k: k) for d in range(3)]
+    rot_t = (np.stack([a[0] for a in rot_t], -1), np.stack([a[1] for a in rot_t], -1))
+    vo = _add(vo, _add(_mul(rot_t, _exact(col["scale"])), tv))
+    # resolve
+    vr = _sub(vin, vo)
+    typ, fr = col["type"], col["friction"]
+    out_v, out_e = vin[0].copy(), vin[1].copy()
+    branch = np.where(band, "band", np.where(top, "top", "miss")).astype(object)
+    margin = np.where(band | top, np.minimum(m_band, m_top), np.minimum(np.minimum(m_band, m_top), m_hit))
+    zero_alt = np.zeros(n, bool)
+    res_v, res_e = vo[0].copy(), vo[1].copy()                               # STICKY: v = 0 + vo
+    if typ == STICKY:
+        lab = np.full(n, "sticky", dtype=object)
+    else:
+        nv = [_dot3(Rb, (on, eon), lambda k, d=d: d + 3 * k, lambda k: k) for d in range(3)]
+        nvec = (np.stack([a[0] for a in nv], -1), np.stack([a[1] for a in nv], -1))
+        vn = _dot3(nvec, vr, lambda k: k, lambda k: k)
+        proj = _sub(vr, _mul(nvec, (vn[0][:, None], vn[1][:, None])))
+        fric = (fr > 0) if typ == SLIP else (fr != 0)
+        ln2 = (proj[0] ** 2).sum(1)
+        plen = np.sqrt(ln2)
+        eplen = np.where(plen > 0, (np.abs(proj[0]) * proj[1]).sum(1) / np.where(plen > 0, plen, 1.0), np.sqrt((proj[1] ** 2).sum(1))) + _rnd(plen)
+        vnf = _mul(vn, _exact(fr))
+        with np.errstate(divide="ignore", invalid="ignore"):
+            q = np.minimum(np.abs(vnf[0]) / plen, 1.0)
+            q = np.where(plen > 0, q, 1.0)
+            unit = proj[0] / np.where(plen > 0, plen, 1.0)[:, None]
+        slide_v = proj[0] + unit * vnf[0][:, None]
+        slide_e = proj[1] * (1 + q)[:, None] + np.abs(unit) * (vnf[1] + q * eplen)[:, None] + _rnd(slide_v)
+        stick = -vnf[0] >= plen
+        with np.errstate(divide="ignore", invalid="ignore"):
+            near_stick = np.abs(plen + vnf[0]) <= tol * (eplen + vnf[1])
+            near_vn = np.abs(vn[0]) <= tol * vn[1]
+        approach = vn[0] < 0
+        use_fric = fric & approach
+        fv = np.where(use_fric[:, None], np.where(stick[:, None], 0.0, slide_v), proj[0])
+        fe = np.where(use_fric[:, None], np.where(stick[:, None] & ~near_stick[:, None], 0.0, slide_e), proj[1])
+        fe = np.where((fric & near_vn)[:, None], np.maximum(fe, np.maximum(slide_e, proj[1])), fe)
+        if typ == SLIP:
+            sv, se = fv, fe
+            lab = np.where(use_fric, np.where(stick, "slip_stick", "slip_friction"), "slip").astype(object)
+        else:
+            sv = np.where(approach[:, None], fv, vr[0])
+            se = np.where(approach[:, None], fe, vr[1])
+            se = np.where(near_vn[:, None], np.maximum(se, np.maximum(fe, vr[1])), se)
+            lab = np.where(approach, "separate_approach", "separate_separate").astype(object)
+        res_v, res_e = _add((sv, se), vo)
+        # zero normal (C5): SEPARATE gives 0 (it returns before the object velocity is added back); SLIP's projection on n = 0
+        # leaves v - vo as it is, and adding vo back gives v up to the two roundings the general path already carries
+        if typ == SEPARATE:
+            res_v = np.where(zero[:, None], 0.0, res_v)
+            res_e = np.where(zero[:, None], 0.0, res_e)
+        lab = np.where(zero, "zero_normal", lab)
+        margin = np.where(hit, np.minimum(margin, m_zero), margin)
+        zero_alt = hit & (np.nan_to_num(m_zero, nan=np.inf) <= NEAR)
+    out_v = np.where(hit[:, None], res_v, out_v)
+    out_e = np.where(hit[:, None], res_e, out_e)
+    branch = np.where(hit, lab, branch)
+    margin = np.nan_to_num(margin, nan=np.inf)            # 0 / 0: an exact quantity on the discontinuity, decided alike
+    near = margin <= NEAR
+    # |v|^2 over both sides of a near node: hit <-> no hit, and for a near zero normal any unit normal
+    vsq = (out_v ** 2).sum(1)
+    alt_hit = (res_v ** 2).sum(1)
+    alt_miss = (vin[0] ** 2).sum(1)
+    lo_sq = np.where(near, np.minimum(alt_hit, alt_miss), vsq)
+    hi_sq = np.where(near, np.maximum(alt_hit, alt_miss), vsq)
+    if typ != STICKY:
+        span = (1 + abs(fr)) * np.sqrt((vr[0] ** 2).sum(1))
+        ovo = np.sqrt((vo[0] ** 2).sum(1))
+        lo_sq = np.where(zero_alt, np.minimum(lo_sq, np.maximum(ovo - span, 0.0) ** 2), lo_sq)
+        hi_sq = np.where(zero_alt, np.maximum(hi_sq, (ovo + span) ** 2), hi_sq)
+    return dict(v=out_v, mag=out_e, vo=vo[0], hit=hit, branch=branch, margin=margin, near=near, vsq_lo=lo_sq, vsq_hi=hi_sq)
 
 
 # ---- constitutive models (exact float64) -------------------------------------------------------------------------------
@@ -315,19 +618,22 @@ def stress_nacc(p, F, log_jp):
 
 
 # ---- g2p2g -------------------------------------------------------------------------------------------------------------
-def g2p2g(cfg, models, vkeys, vel, vmag, dt, new_dt):
+def g2p2g(cfg, models, vkeys, vel, vmag, dt, new_dt, near=None):
     """One G2P -> constitutive update -> P2G over all models.
 
     models: [dict(material, params, state[n,C])]; (vkeys, vel, vmag): grid_update's node velocities and their magnitudes.
     Returns dict(models=[dict(state, pos_mag, f_mag, margin, dropped, lost)], keys, grid[nb,4,64], mag[nb,4,64], stress[nb,4,64]):
     ``mag`` is the per-node magnitude sum M_c of the P2G; ``stress`` sums each particle's stress magnitude (its scale
     (2 mu + lambda) vol |F|^2, for the fluid bulk (gamma + 1) J^-gamma vol J) times its weight and |x_i - x_p| new_dt D^-1,
-    the unit in which the tests allow a constitutive model's own error."""
+    the unit in which the tests allow a constitutive model's own error.
+    ``near`` [nb, 64] (grid_update's collider info): a particle whose G2P stencil reads a near node is ``tainted``, and so is
+    every cell its P2G writes (``taint`` [nb, 64] counts the tainted particles writing a cell)."""
     dx_inv = float(1 << cfg.domain_bits)
     dx = 1.0 / dx_inv
     dinv = 4.0 * dx_inv * dx_inv
-    vg = Grid(vkeys, np.concatenate([vel, vmag], 1))
-    acc = Accumulator(12)
+    near = np.zeros((len(vkeys), 64), bool) if near is None else np.asarray(near, bool)
+    vg = Grid(vkeys, np.concatenate([vel, vmag, near[:, None, :].astype(np.float64)], 1))
+    acc = Accumulator(13)
     out = []
     for m in models:
         mat, p = m["material"], m["params"]
@@ -337,7 +643,8 @@ def g2p2g(cfg, models, vkeys, vel, vmag, dt, new_dt):
         base, _, W, _, xixp, off = stencil(pos, dx_inv)
         nodes = base[:, None, :] + off[None]
         nv, _ = vg.gather(nodes)
-        vi, vim = nv[..., :3], nv[..., 3:]
+        vi, vim = nv[..., :3], nv[..., 3:6]
+        tainted = np.any(nv[..., 6] > 0, axis=1)
         v = np.einsum("nk,nkc->nc", W, vi)
         vm = np.einsum("nk,nkc->nc", W, vim)
         A = np.einsum("nk,nkc,nkd->ncd", W, vi, xixp)
@@ -397,21 +704,27 @@ def g2p2g(cfg, models, vkeys, vel, vmag, dt, new_dt):
         vals = np.concatenate([
             (mass * W2)[..., None], W2[..., None] * mom,
             (mass * (W2 + sens))[..., None], W2[..., None] * tm + sens[..., None] * tm_s,
-            (W2 * smag)[..., None].repeat(4, -1) * np.array([0, 1, 1, 1.0])], -1)
+            (W2 * smag)[..., None].repeat(4, -1) * np.array([0, 1, 1, 1.0]),
+            np.broadcast_to(tainted[:, None, None], W2.shape + (1,)).astype(np.float64)], -1)
         acc.add(nodes2, vals, in_domain_nodes(cfg, nodes2) & ~dropped[:, None])
         res.update(state=new, pos_mag=pos_mag, f_mag=f_mag, dropped=dropped, lost=lost, stress_scale=scale,
-                   v=v, v_mag=vm, cell=nbase - 1)
+                   v=v, v_mag=vm, cell=nbase - 1, tainted=tainted)
         out.append(res)
     keys, g = acc.result()
-    return dict(models=out, keys=keys, grid=g[:, :4], mag=g[:, 4:8], stress=g[:, 8:12])
+    return dict(models=out, keys=keys, grid=g[:, :4], mag=g[:, 4:8], stress=g[:, 8:12], taint=g[:, 12])
 
 
-def substep(cfg, models, keys, grid, dt, dt_default, time_left=np.inf):
-    """The whole sub-step: grid update at dt, new_dt from its max, g2p2g with (dt, new_dt)."""
-    vel, vmag, mx = grid_update(cfg, keys, grid, dt)
+def substep(cfg, models, keys, grid, dt, dt_default, time_left=np.inf, collider=None, t=0.0):
+    """The whole sub-step: grid update at dt (with ``collider`` = (col, sdf, grad) placed at the float32 time t), new_dt
+    from its max, g2p2g with (dt, new_dt).  ``dt_range`` = (new_dt of mx_hi, new_dt of mx_lo): the new dt over every branch
+    choice of the collider's near nodes; ``collider_info`` is grid_update's."""
+    u = grid_update(cfg, keys, grid, dt, collider, t)
+    vel, vmag, mx = u[:3]
+    info = u[3] if collider is not None else dict(near=None, mx_lo=mx, mx_hi=mx, mx_err=0.0)
     new_dt = compute_dt(cfg, mx, dt_default, time_left)
-    r = g2p2g(cfg, models, keys, vel, vmag, dt, new_dt)
-    r.update(max_vsq=mx, new_dt=new_dt, vel=vel, vel_mag=vmag)
+    r = g2p2g(cfg, models, keys, vel, vmag, dt, new_dt, info["near"])
+    r.update(max_vsq=mx, new_dt=new_dt, vel=vel, vel_mag=vmag, collider_info=info,
+             dt_range=(compute_dt(cfg, info["mx_hi"], dt_default, time_left), compute_dt(cfg, info["mx_lo"], dt_default, time_left)))
     return r
 
 
@@ -436,7 +749,7 @@ def compare(ref, keys, grid, states, kappa, stress_allow, f_allow, margin=1e-4, 
     Particles within ``margin`` of a return-mapping branch are left out of the particle check and counted.  With
     ``max_ppc``, a new cell that ref64 gives more than max_ppc particles must hold exactly max_ppc of them (cell_overflow);
     the grid includes every particle's P2G either way."""
-    rep = dict(mass=0.0, momentum=0.0, pos=0.0, F=0.0, near_branch=0, worst={})
+    rep = dict(mass=0.0, momentum=0.0, pos=0.0, F=0.0, near_branch=0, worst={}, tainted_cells=0, tainted_particles=0)
     keys = np.asarray(keys, np.int64)
     grid = np.asarray(grid, np.float64)
     # every block of the reference's P2G must exist; blocks the reference never touched must be zero
@@ -447,6 +760,11 @@ def compare(ref, keys, grid, states, kappa, stress_allow, f_allow, margin=1e-4, 
     assert len(missing) == 0, f"{len(missing)} grid blocks with mass missing from the implementation's grid"
     val, mag, st = ref_at(ref, keys)
     err = np.abs(grid - val)
+    if "taint" in ref:   # cells written by a particle that read a collider node near a discontinuity
+        taint, _ = Grid(ref["keys"], ref["taint"][:, None, :]).gather(np.asarray(keys, np.int64)[:, None, :] * 4 + _CELLS[None])
+        bad = taint[..., 0] > 0
+        rep["tainted_cells"] = int(bad.sum())
+        err = np.where(bad[:, None, :], 0.0, err)
     bm = kappa["mass"] * EPS32 * mag[:, 0]
     bmv = kappa["momentum"] * EPS32 * mag[:, 1:] + stress_allow * st[:, 1:]
     with np.errstate(divide="ignore", invalid="ignore"):
@@ -496,7 +814,9 @@ def compare_particles(ref_models, states, kappa, f_allow, margin, match_tol, rep
             _, cnt = np.unique(held, return_counts=True)
             assert len(cnt) == n_over and np.all(cnt == max_ppc), f"model {m}: overflowing cells hold {sorted(cnt.tolist())}, want {n_over} x {max_ppc}"
         rs = rs[idx]
-        rp = np.abs(se[:, :3] - rs[:, :3]) / (kappa["pos"] * EPS32 * res["pos_mag"][keep][idx])
+        tainted = res["tainted"][keep][idx] if "tainted" in res else np.zeros(len(idx), bool)
+        rep["tainted_particles"] = rep.get("tainted_particles", 0) + int(tainted.sum())
+        rp = np.where(tainted[:, None], 0.0, np.abs(se[:, :3] - rs[:, :3]) / (kappa["pos"] * EPS32 * res["pos_mag"][keep][idx]))
         rep["pos"] = max(rep["pos"], float(rp.max()))
         if rs.shape[1] > 3:
             near = res["margin"][keep][idx] < margin
@@ -505,4 +825,4 @@ def compare_particles(ref_models, states, kappa, f_allow, margin, match_tol, rep
             ef = np.abs(se[:, 3:] - rs[:, 3:])
             with np.errstate(divide="ignore", invalid="ignore"):
                 rf = np.where(ef > 0, ef / (kappa["F"] * EPS32 * fm + f_allow[m]), 0.0)
-            rep["F"] = max(rep["F"], float(rf[~near].max(initial=0)))
+            rep["F"] = max(rep["F"], float(rf[~near & ~tainted].max(initial=0)))

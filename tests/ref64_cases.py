@@ -1,7 +1,9 @@
 """The scene matrix of the float64-reference tests (test_ref64_cpu.py, test_gpu_ref64.py) and its builders.
 
-A case is dict(domain_bits, models=[dict(material, pos, v0, rho, vol, args)], dt, steps, cfl, max_ppc, gravity): ``args``
-are the material setter's arguments after (rho, vol); ``steps`` the sub-steps k at which one sub-step is checked.
+A case is dict(domain_bits, models=[dict(material, pos, v0, rho, vol, args)], dt, steps, cfl, max_ppc, gravity, boundary): ``args``
+are the material setter's arguments after (rho, vol); ``steps`` the sub-steps k at which one sub-step is checked.  A case with
+a ``collider`` = dict(field=(kind, *args), type, friction, rot_mat, trans, trans_vel, omega, dsdt, scale) has a signed-distance
+collider (collider_field, collider_struct; the other keys default to SignedDistanceGrid's).
 """
 import numpy as np
 
@@ -27,8 +29,8 @@ def box(dx, lo, hi):
     return samplers.uniform_box(dx, lo, hi)
 
 
-def _case(domain_bits, models, steps, dt=1e-4, cfl=0.5, max_ppc=128, gravity=-9.8, **kw):
-    return dict(domain_bits=domain_bits, models=models, steps=steps, dt=dt, cfl=cfl, max_ppc=max_ppc, gravity=gravity, **kw)
+def _case(domain_bits, models, steps, dt=1e-4, cfl=0.5, max_ppc=128, gravity=-9.8, boundary=2, **kw):
+    return dict(domain_bits=domain_bits, models=models, steps=steps, dt=dt, cfl=cfl, max_ppc=max_ppc, gravity=gravity, boundary=boundary, **kw)
 
 
 def _cube(material, domain_bits=6, lo=20, hi=32, v0=(0.3, -1.0, 0.2), **kw):
@@ -36,7 +38,7 @@ def _cube(material, domain_bits=6, lo=20, hi=32, v0=(0.3, -1.0, 0.2), **kw):
     return _case(domain_bits, [model(material, box(dx, (lo,) * 3, (hi,) * 3), v0, dx)], **kw)
 
 
-def _walls(material):
+def _walls(material, boundary=2):
     """A 4^3-cell cube pressed into each of the six wall bands and one into a corner (64^3 grid, bands: cells < 8, >= 56)."""
     dx = 1.0 / 64
     ms = []
@@ -48,7 +50,7 @@ def _walls(material):
             v0[axis] = v
             ms.append(model(material, box(dx, a, b), v0, dx))
     ms.append(model(material, box(dx, (3, 3, 3), (7, 7, 7)), (-1.0, -1.0, -1.0), dx))
-    return _case(6, ms, [0, 3])
+    return _case(6, ms, [0, 3], boundary=boundary)
 
 
 def _multi_model():
@@ -265,12 +267,20 @@ def states_from_bins(bins, offsets, sizes, block_count, material):
 
 
 def config(case):
-    return Config(domain_bits=case["domain_bits"], max_ppc=case["max_ppc"], cfl=case["cfl"], gravity=case.get("gravity", -9.8))
+    return Config(domain_bits=case["domain_bits"], max_ppc=case["max_ppc"], cfl=case["cfl"], gravity=case.get("gravity", -9.8),
+                  boundary=case.get("boundary", 2))
 
 
 def build_oracle(ob, case, max_blocks=6000):
-    cfg = ob.make_config(domain_bits=case["domain_bits"], max_ppc=case["max_ppc"], cfl=case["cfl"], gravity=case.get("gravity", -9.8))
-    sim = ob.OracleSim(cfg, case["dt"], max_blocks)
+    cfg = ob.make_config(domain_bits=case["domain_bits"], max_ppc=case["max_ppc"], cfl=case["cfl"], gravity=case.get("gravity", -9.8),
+                         boundary=case.get("boundary", 2))
+    if case.get("collider"):
+        import collider_oracle_binding as cob
+        sim = cob.ColliderOracleSim(cfg, case["dt"], max_blocks)
+        sdf, grad = collider_field(case)
+        sim.set_collider(collider_struct(cob.Collider(), case["collider"]), sdf, grad)
+    else:
+        sim = ob.OracleSim(cfg, case["dt"], max_blocks)
     sim.frame = np.float32(1.0 / case["fps"]) if case.get("fps") else None
     for m in case["models"]:
         mid = sim.init_model(m["material"], m["pos"], m["v0"])
@@ -285,5 +295,127 @@ def build_engine(case, use_graph=True, max_blocks=6000):
     for m in case["models"]:
         mid = sim.init_model(m["material"], m["pos"], m["v0"])
         getattr(sim, SETTER[m["material"]])(m["rho"], m["vol"], *m["args"], model=mid)
+    if case.get("collider"):
+        sdf, grad = collider_field(case)
+        p = collider_spec(case["collider"])
+        sim.set_collider(sdf, grad, type=p["type"], friction=p["friction"], trans=p["trans"], trans_vel=p["trans_vel"], omega=p["omega"],
+                         rot=np.asarray(p["rot_mat"]).reshape(3, 3), scale=p["scale"], dsdt=p["dsdt"])
     sim.initial_setup()
     return sim
+
+
+# ---- the collider of a case -------------------------------------------------------------------------------------------
+def collider_spec(c):
+    """A case's collider parameters with SignedDistanceGrid's defaults (identity rot_mat, no motion, scale 1)."""
+    return dict(type=c["type"], friction=c.get("friction", 0.3), rot_mat=tuple(np.asarray(c.get("rot_mat", np.eye(3)), np.float64).reshape(9)),
+                trans=tuple(c.get("trans", (0.0, 0.0, 0.0))), trans_vel=tuple(c.get("trans_vel", (0.0, 0.0, 0.0))),
+                omega=tuple(c.get("omega", (0.0, 0.0, 0.0))), dsdt=c.get("dsdt", 0.0), scale=c.get("scale", 1.0))
+
+
+def collider_struct(col, c):
+    """Fill a cb200_collider / orc_collider ctypes struct (its sdf pointer left alone) from a case's collider."""
+    p = collider_spec(c)
+    col.rot_mat[:] = [float(v) for v in p["rot_mat"]]
+    col.trans[:], col.trans_vel[:], col.omega[:] = [float(v) for v in p["trans"]], [float(v) for v in p["trans_vel"]], [float(v) for v in p["omega"]]
+    col.dsdt, col.scale, col.friction, col.type = float(p["dsdt"]), float(p["scale"]), float(p["friction"]), int(p["type"])
+    return col
+
+
+_FIELDS = {}
+
+
+def make_field(domain_bits, field, boundary=2):
+    """(sdf (N, N, N), grad (3, N, N, N)) float32 of a field spec: ("box", lo, hi), ("sphere", centre, radius),
+    ("plane", point, normal), ("zero_slab", y_top): sdf -1 at y <= y_top and +1 above, gradient 0 everywhere (quirk C5);
+    ("solid",): sdf -1 and gradient (0, 1, 0) everywhere."""
+    from claymore_b200 import levelset
+    key = (domain_bits, repr(field))
+    if key not in _FIELDS:
+        cfg = Config(domain_bits=domain_bits, boundary=boundary)
+        kind = field[0]
+        N = 4 << (domain_bits - 2)
+        if kind in ("box", "sphere", "plane"):
+            out = getattr(levelset, kind)(cfg, *field[1:])
+        elif kind == "zero_slab":
+            y = np.arange(N) / float(1 << domain_bits)
+            sdf = np.broadcast_to(np.where(y <= field[1], -1.0, 1.0)[None, :, None], (N, N, N)).astype(np.float32)
+            out = (np.ascontiguousarray(sdf), np.zeros((3, N, N, N), np.float32))
+        elif kind == "solid":
+            grad = np.zeros((3, N, N, N), np.float32)
+            grad[1] = 1.0
+            out = (-np.ones((N, N, N), np.float32), grad)
+        else:
+            raise ValueError(kind)
+        _FIELDS.clear()   # one field at a time: 4 MiB at 64^3, 256 MiB at 256^3
+        _FIELDS[key] = out
+    return _FIELDS[key]
+
+
+def collider_field(case):
+    return make_field(case["domain_bits"], case["collider"]["field"])
+
+
+def ref_collider(case):
+    """The (col, sdf, grad) argument of ref64.grid_update / substep for a case (None without a collider)."""
+    if not case.get("collider"):
+        return None
+    sdf, grad = collider_field(case)
+    return ref64.collider_params(collider_spec(case["collider"])), sdf, grad
+
+
+STICKY, SLIP, SEPARATE = ref64.STICKY, ref64.SLIP, ref64.SEPARATE
+FLOOR = ("box", (0.15, 0.15, 0.15), (0.85, 0.305, 0.85))   # a floor whose top (0.305) is not on a node (19.52 dx)
+
+
+def _on_floor(material, typ, friction=0.3, steps=(0, 12, 30), **kw):
+    """An 8 x 6 x 8-cell block falling at 6 m/s onto FLOOR: its stencils reach the floor's nodes (y <= 19 dx) at sub-step ~12."""
+    dx = 1.0 / 64
+    return _case(6, [model(material, box(dx, (26, 21, 26), (34, 27, 34)), (0.3, -6.0, 0.2), dx)], list(steps), dt=2e-4,
+                 collider=dict(field=FLOOR, type=typ, friction=friction), **kw)
+
+
+def _paddle(world_rot=(0.4, -0.3, 0.25), steps=(0, 3, 6)):
+    """A box paddle through a resting fluid block with every motion at once: a non-identity rot_mat, trans, trans_vel, all three
+    omega components, scale and dsdt; SLIP with friction 0.3.  The paddle moves at ~3 m/s, so the nodes it resolves set the max
+    and dt is CFL-bound: cfl 0.05 keeps that dt (~2.5e-4) within the fluid's own stable step."""
+    dx = 1.0 / 64
+    return _case(6, [model(J_FLUID, box(dx, (18, 18, 18), (34, 34, 34)), (0.0, 0.0, 0.0), dx)], list(steps), dt=1e-3, cfl=0.05,
+                 collider=dict(field=("box", (0.36, 0.30, 0.37), (0.43, 0.50, 0.44)), type=SLIP, friction=0.3, rot_mat=_rot(*world_rot),
+                               trans=(0.40, 0.40, 0.40), trans_vel=(3.0, 0.5, -1.0), omega=(0.5, -0.7, 1.1), scale=1.1, dsdt=0.3))
+
+
+def _thin_top():
+    """boundary = 0: a block moving up into a sticky half-space y > 0.95 (nodes 61 .. 63); node 63 is solid, but its cell's
+    +1 node (64 = 4G) does not exist, so the top guard (C6) leaves it alone."""
+    dx = 1.0 / 64
+    return _case(6, [model(FIXED_COROTATED, box(dx, (26, 57, 26), (34, 63, 34)), (0.2, 1.0, -0.1), dx)], [0, 2], boundary=0, gravity=0.0,
+                 collider=dict(field=("plane", (0.5, 0.95, 0.5), (0.0, -1.0, 0.0)), type=STICKY, friction=0.0))
+
+
+COLLIDER_CASES = {
+    "floor_fc_sticky": _on_floor(FIXED_COROTATED, STICKY),
+    "floor_fc_slip": _on_floor(FIXED_COROTATED, SLIP),
+    "floor_fc_separate": _on_floor(FIXED_COROTATED, SEPARATE),
+    "floor_fluid_slip": _on_floor(J_FLUID, SLIP),
+    "floor_sand_sticky": dict(_on_floor(SAND, STICKY), max_near_branch=1.0),   # F = I at sub-step 0: the cone tip
+    "floor_nacc_separate": _on_floor(NACC, SEPARATE),
+    # frictionless SEPARATE on a sphere: normals in every direction
+    "sphere_separate": _case(6, [model(FIXED_COROTATED, box(1.0 / 64, (26, 22, 26), (38, 28, 38)), (0.0, -2.0, 0.0), 1.0 / 64)], [0, 10],
+                             collider=dict(field=("sphere", (0.5, 0.25, 0.5), 0.09), type=SEPARATE, friction=0.0)),
+    "paddle_combined": _paddle(),
+    # quirk C5: a slab of sdf -1 with a zero gradient; SLIP leaves the velocity as it is, SEPARATE stops it
+    "zero_grad_slip": _case(6, [model(FIXED_COROTATED, box(1.0 / 64, (26, 18, 26), (34, 26, 34)), (0.3, -1.0, 0.2), 1.0 / 64)], [0, 3],
+                            collider=dict(field=("zero_slab", 0.305), type=SLIP, friction=0.3)),
+    "zero_grad_separate": _case(6, [model(FIXED_COROTATED, box(1.0 / 64, (26, 18, 26), (34, 26, 34)), (0.3, -1.0, 0.2), 1.0 / 64)], [0, 3],
+                                collider=dict(field=("zero_slab", 0.305), type=SEPARATE, friction=0.3)),
+    "thin_top_boundary0": _thin_top(),
+    # quirk C1: a field that is solid everywhere; the wall-band nodes keep the update without the collider
+    "walls_solid": dict(_walls(FIXED_COROTATED), collider=dict(field=("solid",), type=STICKY)),
+    # a moving floor at the frame end: fps = 390 makes sub-step 25 end the frame with new_dt = 0.64 dt
+    "moving_floor_frame_end": dict(_floor(FIXED_COROTATED, [24, 25, 26]), fps=390,
+                                   collider=dict(field=("box", (0.15, 0.05, 0.15), (0.85, 0.2, 0.85)), type=SLIP, friction=0.3,
+                                                 trans_vel=(0.2, 0.05, 0.0))),
+    # the wall thickness without a collider
+    "walls_boundary1": _walls(FIXED_COROTATED, boundary=1),
+    "fc_cube_boundary0": _cube(FIXED_COROTATED, steps=[0, 3], boundary=0),
+}

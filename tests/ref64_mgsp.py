@@ -90,32 +90,38 @@ def _union_models(per_rank, n_models):
             out.append(None)
             continue
         u = {}
-        for f in ("state", "pos_mag", "f_mag", "margin", "branch", "dropped", "lost"):
+        for f in ("state", "pos_mag", "f_mag", "margin", "branch", "dropped", "lost", "tainted"):
             u[f] = np.concatenate([g[f] for g in got])
         out.append(u)
     return out
 
 
-def substep(cfg, ranks, dt, dt_default, time_left=np.inf, n_models=None):
+def substep(cfg, ranks, dt, dt_default, time_left=np.inf, n_models=None, collider=None, t=0.0):
     """The reference sub-step of all ranks: every rank's grid update and g2p2g on its own view (fresh copies filled), the
     next grid summed key-wise over the ranks (magnitudes and stress columns likewise), new_dt from the max over the ranks'
-    maxima.  Returns a dict ref64.compare-like (keys, grid, mag, stress, models per scene model, new_dt) plus owners
+    maxima.  ``collider`` = (col, sdf, grad) acts in every rank's grid update at the float32 time t (ref64.grid_update); the
+    engine's ranks agree on a max their next-max predictor computed at the end of the previous sub-step, at the time this
+    grid update sees.  Returns a dict ref64.compare-like (keys, grid, mag, stress, models per scene model, new_dt) plus owners
     (contributing ranks per cell), pre_keys (every rank's key hashes before the sub-step), fresh_in (copies filled), and per
     rank its models' results (per_rank: [(scene model, result)]) and its P2G (partials: (keys, grid))."""
     views, fresh_in = _fill_fresh(ranks)
-    ups = [ref64.grid_update(cfg, r["keys"], v, dt) for r, v in zip(ranks, views)]
+    ups = [ref64.grid_update(cfg, r["keys"], v, dt, collider, t) for r, v in zip(ranks, views)]
     mx = max((u[2] for u in ups), default=0.0)
     new_dt = ref64.compute_dt(cfg, mx, dt_default, time_left)
+    infos = [u[3] if collider is not None else dict(near=None, mx_lo=u[2], mx_hi=u[2], mx_err=0.0) for u in ups]
+    mx_lo, mx_hi = max((i["mx_lo"] for i in infos), default=0.0), max((i["mx_hi"] for i in infos), default=0.0)
+    mx_err = max((i["mx_err"] for i in infos), default=0.0)
     if n_models is None:
         n_models = 1 + max((m["model"] for r in ranks for m in r["models"]), default=-1)
     parts, per_rank = [], []
-    for r, (vel, vmag, _) in zip(ranks, ups):
-        res = ref64.g2p2g(cfg, r["models"], r["keys"], vel, vmag, dt, new_dt)
-        parts.append((res["keys"], np.concatenate([res["grid"], res["mag"], res["stress"]], 1)))
+    for r, u, info in zip(ranks, ups, infos):
+        res = ref64.g2p2g(cfg, r["models"], r["keys"], u[0], u[1], dt, new_dt, info["near"])
+        parts.append((res["keys"], np.concatenate([res["grid"], res["mag"], res["stress"], res["taint"][:, None]], 1)))
         per_rank.append([(m["model"], mr) for m, mr in zip(r["models"], res["models"])])
-    keys, s, owners = _sum_keyed(parts, 12)
-    return dict(keys=keys, grid=s[:, :4], mag=s[:, 4:8], stress=s[:, 8:12], owners=owners, models=_union_models(per_rank, n_models),
-                new_dt=new_dt, max_vsq=mx, fresh_in=fresh_in, per_rank=per_rank, partials=[(k, d[:, :4]) for k, d in parts], pre_keys=[set(key_hash(np.asarray(r["keys"], np.int64).reshape(-1, 3)).tolist()) for r in ranks])
+    keys, s, owners = _sum_keyed(parts, 13)
+    return dict(keys=keys, grid=s[:, :4], mag=s[:, 4:8], stress=s[:, 8:12], taint=s[:, 12], owners=owners, models=_union_models(per_rank, n_models),
+                new_dt=new_dt, max_vsq=mx, near=sum(int(i["near"].sum()) for i in infos if i["near"] is not None),
+                mx_hi=mx_hi, mx_lo=mx_lo, mx_err=mx_err, dt_range=(ref64.compute_dt(cfg, mx_hi, dt_default, time_left), ref64.compute_dt(cfg, mx_lo, dt_default, time_left)), fresh_in=fresh_in, per_rank=per_rank, partials=[(k, d[:, :4]) for k, d in parts], pre_keys=[set(key_hash(np.asarray(r["keys"], np.int64).reshape(-1, 3)).tolist()) for r in ranks])
 
 
 def rasterize(cfg, ranks_models):
@@ -162,7 +168,7 @@ def compare(cfg, ref, after, kappa, stress_allow, f_allow, margin=1e-4, match_to
     non-zero copy and no particle of that rank reads the block at its next G2P; anything else raises AssertionError naming the
     block.  Also: every block the reference touches has a non-fresh copy somewhere.
     Returns dict(mass, momentum, pos, F, near_branch, worst, fresh, max_owners, shared)."""
-    rep = dict(mass=0.0, momentum=0.0, pos=0.0, F=0.0, near_branch=0, worst={}, fresh=0, max_owners=0, shared=0)
+    rep = dict(mass=0.0, momentum=0.0, pos=0.0, F=0.0, near_branch=0, worst={}, fresh=0, max_owners=0, shared=0, tainted_cells=0)
     hs = [key_hash(np.asarray(a["keys"], np.int64).reshape(-1, 3)) for a in after]
     nonzero = [np.abs(np.asarray(a["grid"], np.float64)).reshape(len(h), -1).max(1, initial=0) > 0 for a, h in zip(after, hs)]
     holders = {}
@@ -195,7 +201,13 @@ def compare(cfg, ref, after, kappa, stress_allow, f_allow, margin=1e-4, match_to
             fresh[b] = True
         rep["fresh"] += int(fresh.sum())
         good |= set(h[~fresh].tolist())
-        err = np.abs(grid - val)[~fresh]
+        err = np.abs(grid - val)
+        if "taint" in ref:   # cells written by a particle that read a collider node near a discontinuity (ref64.g2p2g)
+            taint, _ = ref64.Grid(ref["keys"], ref["taint"][:, None, :]).gather(keys[:, None, :] * 4 + _CELLS[None])
+            bad = (taint[..., 0] > 0) & ~fresh[:, None]
+            rep["tainted_cells"] += int(bad.sum())
+            err = np.where(bad[:, None, :], 0.0, err)
+        err = err[~fresh]
         bm = kappa["mass"] * EPS32 * mag[~fresh, 0]
         bmv = kappa["momentum"] * EPS32 * mag[~fresh, 1:] + stress_allow * st[~fresh, 1:]
         with np.errstate(divide="ignore", invalid="ignore"):

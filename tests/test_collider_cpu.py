@@ -101,6 +101,8 @@ MOTIONS = {
     "scale": dict(scale=1.15),
     "dsdt": dict(dsdt=0.6),
     "rot_mat": dict(rot=_rot(0.3, -0.2, 0.5)),
+    # every motion at once except omega (with omega != 0 the fixed cross product, C3, departs from the reference)
+    "combined": dict(rot=_rot(0.3, -0.2, 0.5), trans=(0.03, -0.02, 0.01), trans_vel=(0.4, -0.3, 0.2), scale=1.15, dsdt=0.6),
 }
 
 
