@@ -19,6 +19,8 @@ constexpr char kCkMagic[8] = {'C', 'B', '2', '0', '0', 'C', 'K', 'P'};
 static_assert(256 + kMaxModels * kCkTocEntry <= kCkHeader, "checkpoint table of contents must fit the header");
 
 __host__ __device__ inline int ck_channels(int material) { return material == CB200_J_FLUID ? 4 : (material == CB200_FIXED_COROTATED ? 12 : 13); }
+// floats of one bin of kBinCap particles (J_FLUID: 4 channels, the others: 16)
+inline size_t bin_floats(int material) { return material == CB200_J_FLUID ? 128 : 512; }
 __host__ __device__ inline unsigned long long ck_align(unsigned long long x) { return (x + kCkAlign - 1) & ~(unsigned long long) (kCkAlign - 1); }
 
 // Section offsets of the blob the snapshot writes, from the particle counts and nbc: the host writer of the header evaluates it

@@ -172,6 +172,24 @@ struct Model {
 	float* h_out = nullptr;
 	size_t out_floats = 0;
 };
+// capacity rule of init_model (gmpm_simulator.cuh:173): n/32 bins + one partial bin per block
+inline long long bin_rows(long long n, long long max_blocks) { return n / kBinCap + max_blocks; }
+
+// counters and maxima the driver's kernels hand to each other within a sub-step (or a set-up, a retrieve)
+struct DeviceScratch {
+	int new_pbc;         // particle blocks of the rebuilt partition (summary_kernel)
+	int new_nbc;         // neighbour blocks, snapshotted by the last CTA of their registration; MGSP: the exchange's key count
+	int retrieve_count;  // particles written by retrieve_kernel
+	float local_max;     // MGSP: this rank's max |v|^2 of the new grid
+	float global_max;    // MGSP: the max over the ranks
+	float mgsp_grid_max; // MGSP: the grid update's max |v|^2, never read (the exchange agreed on the max already)
+	int missing;         // saved grid blocks scatter_grid_kernel found no block for
+};
+// MGSP: the last-CTA counters and the exchange epochs (MgspView::done / ::epochs)
+struct MgspCounters {
+	int done[4];
+	int epochs[3];
+};
 
 void default_material(const cb200_config& cfg, int material, cb200_particle_buffer& pb) {
 	// defaults of ParticleBuffer<M>, reference Projects/GMPM/particle_buffer.cuh:141-264
@@ -207,7 +225,7 @@ struct cb200_sim {
 	float* grid[2] = {nullptr, nullptr};
 	int* tile_sums = nullptr;     // [tiles + 1][kScanComps] of summary_kernel / rebuild_kernel
 	int* block_totals = nullptr;  // [kMaxModels][max_blocks] particles per old block
-	int* d_scratch = nullptr;  // [0] new_pbc, [1] new_nbc snapshot, [2] parcount
+	DeviceScratch* scr = nullptr;
 	std::vector<Model> models;
 	int rollid = 0;
 	long long launches = 0;
@@ -224,8 +242,7 @@ struct cb200_sim {
 	bool peers_ready = false;
 	int* peer_bno = nullptr;                 // [world][max_blocks]
 	float* grid1_peer[kMaxRanks] = {};       // every rank's next grid mapped here (fused remote halo reduction)
-	int* mgsp_done = nullptr;    // [4] last-CTA counters
-	int* mgsp_epochs = nullptr;  // [3]
+	MgspCounters* mgsp_sync = nullptr;
 	// per-kernel timing (cudaEvent pairs around the g2p2g launches; stream mode only)
 	bool profiling = false;
 	std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;
@@ -289,31 +306,105 @@ struct cb200_sim {
 };
 
 namespace {
-int alloc_partition(cb200_sim* s, cb200_partition& p) {
-	const size_t mb = (size_t) s->desc.max_blocks;
-	CK(pool_alloc(&p.count, sizeof(int)));
-	CK(pool_alloc(&p.index_table, s->table_entries * sizeof(int)));
-	CK(pool_alloc(&p.active_keys, (mb + 1) * 3 * sizeof(int)));
-	CK(pool_alloc(&p.halo_count, sizeof(int)));
-	CK(pool_alloc(&p.halo_marks, mb + 1));
-	CK(pool_alloc(&p.overlap_marks, (mb + 1) * sizeof(int)));
-	p.halo_blocks = nullptr;
-	CK(cudaMemsetAsync(p.count, 0, sizeof(int), s->stream));
-	CK(cudaMemsetAsync(p.index_table, 0xff, s->table_entries * sizeof(int), s->stream));
-	CK(cudaMemsetAsync(p.active_keys, 0, (mb + 1) * 3 * sizeof(int), s->stream));
-	CK(cudaMemsetAsync(p.halo_count, 0, sizeof(int), s->stream));
-	CK(cudaMemsetAsync(p.halo_marks, 0, mb + 1, s->stream));
-	CK(cudaMemsetAsync(p.overlap_marks, 0, (mb + 1) * sizeof(int), s->stream));
+// ---- the device arrays of each owner (a model, a partition, the simulator), listed once -------------------------------------------
+// An entry is the pointer an array lives in, its bytes at the capacity the list was made for, and the byte every element starts as.
+// Allocation, growth, the emission's reset and release all walk these lists.  A list holds pointers into its owner: it is made from
+// the owner at the call and used there, never kept.
+constexpr int kNoFill = -1;  // the contents are left as allocated: every element is written before it is read
+struct DevArray {
+	void** p;
+	size_t bytes;
+	int fill;
+};
+using DevArrays = std::vector<DevArray>;
+template<typename T>
+DevArray dev_array(T*& p, size_t count, int fill) { return {reinterpret_cast<void**>(&p), count * sizeof(T), fill}; }
+
+// one roll's particle buffer at block capacity mb, with `rows` bins
+void buffer_arrays(DevArrays& a, const cb200_sim* s, const Model& m, cb200_particle_buffer& pb, size_t mb, long long rows) {
+	const size_t ppb = (size_t) s->cfg.ppb;
+	a.push_back(dev_array(pb.bins, (size_t) rows * bin_floats(m.material), kNoFill));
+	a.push_back(dev_array(pb.cell_particle_counts, (mb + 1) * kBlockVol, 0));
+	a.push_back(dev_array(pb.particle_bucket_sizes, mb + 2, 0));
+	a.push_back(dev_array(pb.cellbuckets, (mb + 1) * ppb, kNoFill));
+	a.push_back(dev_array(pb.blockbuckets, (mb + 1) * ppb, kNoFill));
+	a.push_back(dev_array(pb.bin_offsets, mb + 2, 0));
+}
+// a model: both rolls' buffers, the bin sizes, both rolls' cell offsets and the m.n start positions (the caller fills those)
+DevArrays model_arrays(const cb200_sim* s, Model& m, size_t mb, long long rows) {
+	DevArrays a;
+	for(cb200_particle_buffer& pb : m.pb) buffer_arrays(a, s, m, pb, mb, rows);
+	a.push_back(dev_array(m.bin_sizes, mb + 2, 0));
+	for(unsigned short*& offs : m.celloffs) a.push_back(dev_array(offs, (mb + 1) * kBlockVol, 0));
+	a.push_back(dev_array(m.d_pos, (size_t) m.n * 3, kNoFill));
+	return a;
+}
+// a partition, empty (halo_blocks stays null: the fused MGSP path collects no halo block list)
+DevArrays partition_arrays(const cb200_sim* s, cb200_partition& p, size_t mb) {
+	return {dev_array(p.count, 1, 0),
+	        dev_array(p.index_table, s->table_entries, 0xff),
+	        dev_array(p.active_keys, (mb + 1) * 3, 0),
+	        dev_array(p.halo_count, 1, 0),
+	        dev_array(p.halo_marks, mb + 1, 0),
+	        dev_array(p.overlap_marks, mb + 1, 0)};
+}
+// the simulator's own: step state, scratch, both grids and the rebuild's scratch (produced and consumed inside a sub-step)
+DevArrays sim_arrays(cb200_sim* s, size_t mb) {
+	const size_t tiles = (mb + kRebuildTile - 1) / kRebuildTile + 1;
+	return {dev_array(s->d_state, 1, 0),
+	        dev_array(s->scr, 1, 0),
+	        dev_array(s->grid[0], (mb + 1) * kGridBlockFloats, 0),
+	        dev_array(s->grid[1], (mb + 1) * kGridBlockFloats, 0),
+	        dev_array(s->tile_sums, tiles * kScanComps, kNoFill),
+	        dev_array(s->block_totals, (size_t) kMaxModels * mb, kNoFill)};
+}
+
+int fill_arrays(cb200_sim* s, const DevArrays& a) {
+	for(const DevArray& d : a)
+		if(d.fill != kNoFill) CK(cudaMemsetAsync(*d.p, d.fill, d.bytes, s->stream));
 	return 0;
 }
-void free_partition(cb200_partition& p) {
-	g_pool.release(p.count);
-	g_pool.release(p.index_table);
-	g_pool.release(p.active_keys);
-	g_pool.release(p.halo_count);
-	g_pool.release(p.halo_marks);
-	g_pool.release(p.overlap_marks);
+int alloc_arrays(cb200_sim* s, const DevArrays& a) {
+	for(const DevArray& d : a) CK(g_pool.alloc(d.p, d.bytes));
+	return fill_arrays(s, a);
 }
+void free_arrays(const DevArrays& a) {
+	for(const DevArray& d : a) g_pool.release(*d.p);
+}
+// Grows the arrays of `from` to their sizes in `to`, the same list at a larger capacity: allocate the larger array, copy the live
+// prefix, fill the tail by the array's rule, release the old one.  One array at a time, so the peak is the footprint plus the
+// largest array; a failure leaves every array valid, those already moved merely larger.
+int grow_arrays(cb200_sim* s, const DevArrays& from, const DevArrays& to) {
+	for(size_t i = 0; i < to.size(); ++i) {
+		const DevArray& d = to[i];
+		const size_t old_bytes = from[i].bytes;
+		if(d.bytes <= old_bytes) continue;
+		void* q = nullptr;
+		CK(g_pool.alloc(&q, d.bytes));
+		int e = (int) cudaMemcpyAsync(q, *d.p, old_bytes, cudaMemcpyDeviceToDevice, s->stream);
+		if(!e && d.fill != kNoFill) e = (int) cudaMemsetAsync((unsigned char*) q + old_bytes, d.fill, d.bytes - old_bytes, s->stream);
+		if(!e) e = (int) cudaStreamSynchronize(s->stream);
+		if(e) {
+			g_pool.release(q);
+			return e;
+		}
+		g_pool.release(*d.p);
+		*d.p = q;
+	}
+	return 0;
+}
+
+// the material parameters of `from` (every field from rho on), the containers of `to`
+void copy_params(cb200_particle_buffer& to, const cb200_particle_buffer& from) {
+	memcpy(&to.rho, &from.rho, sizeof(to) - offsetof(cb200_particle_buffer, rho));
+}
+void drop_graphs(cb200_sim* s) {
+	for(cudaGraphExec_t& g : s->graph) {
+		if(g) cudaGraphExecDestroy(g);
+		g = nullptr;
+	}
+}
+
 inline int grid_blocks(int per_sm) { return num_sms() * per_sm; }
 
 int pull_state(cb200_sim* s) {
@@ -371,7 +462,7 @@ int enqueue_grid_update(cb200_sim* s, int R) {
 	if(s->desc.mgsp_world > 1) {
 		// the global max |v|^2 was agreed on at the end of the previous sub-step (it rides on the key exchange) and the next grid
 		// was cleared there as well, before the peers were told they may reduce into it
-		gu.max_vel = reinterpret_cast<float*>(s->d_scratch + 5);
+		gu.max_vel = &s->scr->mgsp_grid_max;
 		gu.clear_grid = nullptr;
 	}
 	gu.n_clear = (int) s->models.size();
@@ -428,7 +519,7 @@ int enqueue_rebuild(cb200_sim* s, int R) {
 		a.stale_table = s->part[Rn].index_table;
 		a.stale_keys = s->part[Rn].active_keys;
 		a.stale_count = s->part[Rn].count;
-		a.new_pbc = s->d_scratch + 0;
+		a.new_pbc = &s->scr->new_pbc;
 		summary_kernel<<<tiles, kSummaryThreads, 0, st>>>(a);
 		++s->launches;
 	}
@@ -457,7 +548,7 @@ int enqueue_rebuild(cb200_sim* s, int R) {
 	{
 		RegisterArgs a {};
 		a.cfg = s->cfg;
-		a.block_count = count_dev(s->d_scratch + 0);
+		a.block_count = count_dev(&s->scr->new_pbc);
 		a.table = s->part[Rn].index_table;
 		a.keys = s->part[Rn].active_keys;
 		a.count = s->part[Rn].count;
@@ -466,7 +557,7 @@ int enqueue_rebuild(cb200_sim* s, int R) {
 		a.lo = 0;
 		a.span = 2;
 		a.done_counter = &s->d_state->done_counter;  // the last CTA snapshots the neighbour count
-		a.snapshot_out = s->d_scratch + 1;
+		a.snapshot_out = &s->scr->new_nbc;
 		register_blocks_kernel<<<grid_blocks(4), 128, 0, st>>>(a);
 		++s->launches;
 	}
@@ -485,8 +576,7 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 	const int Rn = R ^ 1;
 	cudaStream_t st = s->stream;
 	const bool mgsp = s->desc.mgsp_world > 1;
-	float* local_max = reinterpret_cast<float*>(s->d_scratch + 3);
-	float* global_max = reinterpret_cast<float*>(s->d_scratch + 4);
+	DeviceScratch* scr = s->scr;
 	{
 		CarryArgs a {};
 		if(mgsp) {  // behind the wait for the peers' "reductions landed" flags; resets the tagging state of the new partition on the way
@@ -497,13 +587,13 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 			a.overlap_marks = s->part[Rn].overlap_marks;
 		}
 		a.cfg = s->cfg;
-		a.new_count = s->d_scratch + 1;
+		a.new_count = &scr->new_nbc;
 		a.new_keys = s->part[Rn].active_keys;
 		a.old_table = s->part[R].index_table;
 		a.state = s->d_state;
 		a.old_grid = s->grid[1];
 		a.new_grid = s->grid[0];
-		a.next_max_vel = mgsp ? local_max : nullptr;
+		a.next_max_vel = mgsp ? &scr->local_max : nullptr;
 		if(mgsp && s->has_collider) {  // the predicted max must be the one the next grid update finds
 			a.col = s->collider;
 			carry_grid_kernel<true><<<grid_blocks(4), 256, 0, st>>>(a);
@@ -513,23 +603,23 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 		++s->launches;
 	}
 	if(mgsp) {
-		mgsp_clear_publish_kernel<<<grid_blocks(2), 256, 0, st>>>(mgsp_view(s), s->part[Rn].active_keys, s->d_scratch + 1, local_max, s->grid[1]);
+		mgsp_clear_publish_kernel<<<grid_blocks(2), 256, 0, st>>>(mgsp_view(s), s->part[Rn].active_keys, &scr->new_nbc, &scr->local_max, s->grid[1]);
 		++s->launches;
 	}
 	FinalizeArgs fin {};
 	fin.cfg = s->cfg;
 	fin.state = s->d_state;
-	fin.new_pbc = s->d_scratch + 0;
-	fin.new_nbc = s->d_scratch + 1;
+	fin.new_pbc = &scr->new_pbc;
+	fin.new_nbc = &scr->new_nbc;
 	fin.new_count = s->part[Rn].count;
 	fin.max_blocks = s->desc.max_blocks;
 	fin.n_models = (int) s->models.size();
 	for(size_t m = 0; m < s->models.size(); ++m) fin.bin_capacity[m] = s->models[m].bin_capacity;
-	fin.next_max_vel = mgsp ? global_max : nullptr;
+	fin.next_max_vel = mgsp ? &scr->global_max : nullptr;
 	{
 		RegisterArgs a {};
 		a.cfg = s->cfg;
-		a.block_count = count_dev(s->d_scratch + 0);
+		a.block_count = count_dev(&scr->new_pbc);
 		a.table = s->part[Rn].index_table;
 		a.keys = s->part[Rn].active_keys;
 		a.count = s->part[Rn].count;
@@ -547,7 +637,7 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 	}
 	mark_phase(s, 9);
 	if(mgsp) {
-		mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(s->cfg, mgsp_view(s), s->part[Rn].index_table, s->part[Rn].overlap_marks, s->d_scratch + 1, local_max, global_max, 1, fin);
+		mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(s->cfg, mgsp_view(s), s->part[Rn].index_table, s->part[Rn].overlap_marks, &scr->new_nbc, &scr->local_max, &scr->global_max, 1, fin);
 		++s->launches;
 		mark_phase(s, 8);
 	}
@@ -564,8 +654,8 @@ MgspView mgsp_view(cb200_sim* s) {
 	v.overlap_keys = s->peer_overlap_keys;
 	v.overlap_count = s->peer_overlap_count;
 	v.peer_bno = s->peer_bno;
-	v.done = s->mgsp_done;
-	v.epochs = s->mgsp_epochs;
+	v.done = s->mgsp_sync->done;
+	v.epochs = s->mgsp_sync->epochs;
 	return v;
 }
 
@@ -686,26 +776,6 @@ int ensure_graph(cb200_sim* s, int R) {
 }  // namespace
 
 namespace {
-// Grows one block-indexed device array: allocate the larger one, copy the live prefix, initialise the tail the way
-// cb200_sim_create / cb200_sim_init_model initialised it, release the old one.  One array at a time, so the peak is the
-// footprint plus the largest array.
-template<typename T>
-int grow_array(cb200_sim* s, T*& p, size_t old_elems, size_t new_elems, int fill_byte) {
-	T* q = nullptr;
-	CK(pool_alloc(&q, new_elems * sizeof(T)));
-	int e = 0;
-	if(p && old_elems) e = (int) cudaMemcpyAsync(q, p, old_elems * sizeof(T), cudaMemcpyDeviceToDevice, s->stream);
-	if(!e && new_elems > old_elems) e = (int) cudaMemsetAsync(q + old_elems, fill_byte, (new_elems - old_elems) * sizeof(T), s->stream);
-	if(!e) e = (int) cudaStreamSynchronize(s->stream);
-	if(e) {
-		g_pool.release(q);
-		return e;
-	}
-	g_pool.release(p);
-	p = q;
-	return 0;
-}
-
 // ---- frame output: the writer thread ------------------------------------------------------------------------------------------
 // One file: header, body, trailer.  Returns 0 or the errno of the failing open / write / close; a partially written file is removed.
 int write_bgeo(const cb200_sim::OutputFile& f) {
@@ -779,42 +849,13 @@ int cb200_sim_reserve(cb200_sim* s, int new_max_blocks) {
 	if(s->ck_pending) CK(cudaEventSynchronize(s->ck_copied));  // the next begin re-sizes the staging blob
 	output_idle(s);
 	const size_t ob = (size_t) s->desc.max_blocks, nb = (size_t) new_max_blocks;
-	for(int i = 0; i < 2; ++i) {
-		if(s->graph[i]) {
-			cudaGraphExecDestroy(s->graph[i]);
-			s->graph[i] = nullptr;
-		}
-		cb200_partition& p = s->part[i];
-		CK(grow_array(s, p.active_keys, (ob + 1) * 3, (nb + 1) * 3, 0));
-		CK(grow_array(s, p.halo_marks, ob + 1, nb + 1, 0));
-		CK(grow_array(s, p.overlap_marks, ob + 1, nb + 1, 0));
-		CK(grow_array(s, s->grid[i], (ob + 1) * kGridBlockFloats, (nb + 1) * kGridBlockFloats, 0));
-	}
-	{  // scratch of the rebuild: produced and consumed inside a sub-step, nothing to keep
-		g_pool.release(s->tile_sums);
-		g_pool.release(s->block_totals);
-		s->tile_sums = nullptr;
-		s->block_totals = nullptr;
-		const size_t tiles = (nb + kRebuildTile - 1) / kRebuildTile + 1;
-		CK(pool_alloc(&s->tile_sums, tiles * kScanComps * sizeof(int)));
-		CK(pool_alloc(&s->block_totals, (size_t) kMaxModels * nb * sizeof(int)));
-	}
-	const size_t ppb = (size_t) s->cfg.ppb;
+	drop_graphs(s);
+	for(cb200_partition& p : s->part) CK(grow_arrays(s, partition_arrays(s, p, ob), partition_arrays(s, p, nb)));
+	CK(grow_arrays(s, sim_arrays(s, ob), sim_arrays(s, nb)));
 	for(Model& m : s->models) {
-		const size_t binf = m.material == CB200_J_FLUID ? 128 : 512;
-		const long long new_bins = (long long) m.n / kBinCap + (long long) nb;
-		for(int i = 0; i < 2; ++i) {
-			cb200_particle_buffer& pb = m.pb[i];
-			CK(grow_array(s, pb.bins, (size_t) m.bin_capacity * binf, (size_t) new_bins * binf, 0));
-			CK(grow_array(s, pb.cell_particle_counts, (ob + 1) * kBlockVol, (nb + 1) * kBlockVol, 0));
-			CK(grow_array(s, pb.particle_bucket_sizes, ob + 2, nb + 2, 0));
-			CK(grow_array(s, pb.cellbuckets, (ob + 1) * ppb, (nb + 1) * ppb, 0));
-			CK(grow_array(s, pb.blockbuckets, (ob + 1) * ppb, (nb + 1) * ppb, 0));
-			CK(grow_array(s, pb.bin_offsets, ob + 2, nb + 2, 0));
-		}
-		CK(grow_array(s, m.bin_sizes, ob + 2, nb + 2, 0));
-		for(int i = 0; i < 2; ++i) CK(grow_array(s, m.celloffs[i], (ob + 1) * kBlockVol, (nb + 1) * kBlockVol, 0));
-		m.bin_capacity = new_bins;
+		const long long rows = std::max(m.bin_capacity, bin_rows(m.n, (long long) nb));
+		CK(grow_arrays(s, model_arrays(s, m, ob, m.bin_capacity), model_arrays(s, m, nb, rows)));
+		m.bin_capacity = rows;
 	}
 	s->desc.max_blocks = new_max_blocks;
 	++s->grow_events;
@@ -869,23 +910,10 @@ static int sim_create_impl(cb200_sim* s, const cb200_sim_desc* desc, void* strea
 	}
 	s->table_entries = (size_t) s->cfg.gsize * s->cfg.gsize * s->cfg.gsize;
 	const size_t mb = (size_t) desc->max_blocks;
-	CK(pool_alloc(&s->d_state, sizeof(StepState)));
-	CK(cudaMemsetAsync(s->d_state, 0, sizeof(StepState), s->stream));
 	CK(g_pinned.get(&s->h_state));
 	memset(s->h_state, 0, sizeof(StepState));
-	for(int i = 0; i < 2; ++i) {
-		int e = alloc_partition(s, s->part[i]);
-		if(e) return e;
-		CK(pool_alloc(&s->grid[i], (mb + 1) * kGridBlockFloats * sizeof(float)));
-		CK(cudaMemsetAsync(s->grid[i], 0, (mb + 1) * kGridBlockFloats * sizeof(float), s->stream));
-	}
-	{
-		const size_t tiles = (mb + kRebuildTile - 1) / kRebuildTile + 1;
-		CK(pool_alloc(&s->tile_sums, tiles * kScanComps * sizeof(int)));
-		CK(pool_alloc(&s->block_totals, (size_t) kMaxModels * mb * sizeof(int)));
-	}
-	CK(pool_alloc(&s->d_scratch, 16 * sizeof(int)));
-	CK(cudaMemsetAsync(s->d_scratch, 0, 16 * sizeof(int), s->stream));
+	CK(alloc_arrays(s, sim_arrays(s, mb)));
+	for(cb200_partition& p : s->part) CK(alloc_arrays(s, partition_arrays(s, p, mb)));
 	if(s->desc.mgsp_world > 1) {
 		if(s->desc.mgsp_world > kMaxRanks || s->desc.mgsp_rank < 0 || s->desc.mgsp_rank >= s->desc.mgsp_world) return (int) cudaErrorInvalidValue;
 		if(s->desc.mgsp_halo_cap <= 0) s->desc.mgsp_halo_cap = desc->max_blocks / 2;
@@ -899,9 +927,8 @@ static int sim_create_impl(cb200_sim* s, const cb200_sim_desc* desc, void* strea
 		s->grid1_peer[s->desc.mgsp_rank] = s->grid[1];
 		CK(pool_alloc(&s->peer_bno, (size_t) s->desc.mgsp_world * mb * sizeof(int)));
 		CK(cudaMemsetAsync(s->peer_bno, 0xff, (size_t) s->desc.mgsp_world * mb * sizeof(int), s->stream));
-		CK(pool_alloc(&s->mgsp_done, 16 * sizeof(int)));
-		CK(cudaMemsetAsync(s->mgsp_done, 0, 16 * sizeof(int), s->stream));
-		s->mgsp_epochs = s->mgsp_done + 4;
+		CK(pool_alloc(&s->mgsp_sync, sizeof(MgspCounters)));
+		CK(cudaMemsetAsync(s->mgsp_sync, 0, sizeof(MgspCounters), s->stream));
 		CK(cudaStreamSynchronize(s->stream));
 	}
 	return 0;
@@ -935,37 +962,21 @@ int cb200_sim_destroy(cb200_sim* s) {
 		cudaEventDestroy(ev.first);
 		cudaEventDestroy(ev.second);
 	}
-	for(int i = 0; i < 2; ++i) {
-		if(s->graph[i]) cudaGraphExecDestroy(s->graph[i]);
-		free_partition(s->part[i]);
-		g_pool.release(s->grid[i]);
-	}
+	drop_graphs(s);
+	const size_t mb = (size_t) s->desc.max_blocks;
+	for(cb200_partition& p : s->part) free_arrays(partition_arrays(s, p, mb));
 	for(Model& m : s->models) {
-		for(int i = 0; i < 2; ++i) {
-			g_pool.release(m.pb[i].bins);
-			g_pool.release(m.pb[i].cell_particle_counts);
-			g_pool.release(m.pb[i].particle_bucket_sizes);
-			g_pool.release(m.pb[i].cellbuckets);
-			g_pool.release(m.pb[i].blockbuckets);
-			g_pool.release(m.pb[i].bin_offsets);
-		}
-		g_pool.release(m.d_pos);
-		g_pool.release(m.bin_sizes);
-		g_pool.release(m.celloffs[0]);
-		g_pool.release(m.celloffs[1]);
+		free_arrays(model_arrays(s, m, mb, m.bin_capacity));
 		g_pool.release(m.d_out);
 		cudaFreeHost(m.h_out);
 	}
-	g_pool.release(s->tile_sums);
-	g_pool.release(s->block_totals);
-	g_pool.release(s->d_scratch);
-	g_pool.release(s->d_state);
+	free_arrays(sim_arrays(s, mb));
 	g_pool.release(s->peer_overlap_keys);
 	g_pool.release(s->peer_overlap_count);
 	// peer mappings stay open (IpcCache): the exporting rank pools the buffer, the next simulator maps the same handle
 	g_pool.release(s->peer_bno);
 	g_pool.release(s->inbox_local);
-	g_pool.release(s->mgsp_done);
+	g_pool.release(s->mgsp_sync);
 	g_pool.release(s->sdf);
 	g_pinned.put(s->h_state);
 	g_pinned.put(s->h_poll);
@@ -977,33 +988,13 @@ int cb200_sim_destroy(cb200_sim* s) {
 
 // the containers of one model of m.material and m.n particles (init_model and restore; the caller fills d_pos)
 static int alloc_model(cb200_sim* s, Model& m) {
-	const int material = m.material, n = m.n;
-	const size_t mb = (size_t) s->desc.max_blocks;
-	const size_t binf = material == CB200_J_FLUID ? 128 : 512;
-	// capacity rule of init_model (gmpm_simulator.cuh:173): n/32 bins + one partial bin per block
-	m.bin_capacity = (long long) n / kBinCap + (long long) mb;
-	for(int i = 0; i < 2; ++i) {
-		cb200_particle_buffer& pb = m.pb[i];
+	const long long mb = s->desc.max_blocks;
+	m.bin_capacity = bin_rows(m.n, mb);
+	for(cb200_particle_buffer& pb : m.pb) {
 		memset(&pb, 0, sizeof(pb));
-		default_material(s->desc.cfg, material, pb);
-		CK(pool_alloc(&pb.bins, (size_t) m.bin_capacity * binf * sizeof(float)));
-		CK(pool_alloc(&pb.cell_particle_counts, (mb + 1) * kBlockVol * sizeof(int)));
-		CK(pool_alloc(&pb.particle_bucket_sizes, (mb + 2) * sizeof(int)));
-		CK(pool_alloc(&pb.cellbuckets, (mb + 1) * (size_t) s->cfg.ppb * sizeof(int)));
-		CK(pool_alloc(&pb.blockbuckets, (mb + 1) * (size_t) s->cfg.ppb * sizeof(int)));
-		CK(pool_alloc(&pb.bin_offsets, (mb + 2) * sizeof(int)));
-		CK(cudaMemsetAsync(pb.cell_particle_counts, 0, (mb + 1) * kBlockVol * sizeof(int), s->stream));
-		CK(cudaMemsetAsync(pb.particle_bucket_sizes, 0, (mb + 2) * sizeof(int), s->stream));
-		CK(cudaMemsetAsync(pb.bin_offsets, 0, (mb + 2) * sizeof(int), s->stream));
+		default_material(s->desc.cfg, m.material, pb);
 	}
-	CK(pool_alloc(&m.bin_sizes, (mb + 2) * sizeof(int)));
-	CK(cudaMemsetAsync(m.bin_sizes, 0, (mb + 2) * sizeof(int), s->stream));
-	for(int i = 0; i < 2; ++i) {
-		CK(pool_alloc(&m.celloffs[i], (mb + 1) * kBlockVol * sizeof(unsigned short)));
-		CK(cudaMemsetAsync(m.celloffs[i], 0, (mb + 1) * kBlockVol * sizeof(unsigned short), s->stream));
-	}
-	CK(pool_alloc(&m.d_pos, (size_t) n * 3 * sizeof(float)));
-	return 0;
+	return alloc_arrays(s, model_arrays(s, m, (size_t) mb, m.bin_capacity));
 }
 
 int cb200_sim_init_model(cb200_sim* s, int material, const float* positions_host, int n, const float* v0, int* model_id) {
@@ -1082,26 +1073,25 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 	const int cap = s->desc.max_blocks;
 	int* err = &s->d_state->error;
 	int pbc = 0, nbc = 0, ebc = 0;
-	auto blocks_for = [](long long n, int per) { return (int) std::max<long long>(1, std::min<long long>((n + per - 1) / per, (long long) num_sms() * 16)); };
 
 	for(Model& m : s->models) {
-		activate_blocks_kernel<true><<<blocks_for(m.n, 256), 256, 0, st>>>(cfg, m.n, m.d_pos, s->part[Rn].index_table, s->part[Rn].active_keys, s->part[Rn].count, cap, err);
+		activate_blocks_kernel<true><<<grid_for(m.n, 256, 16), 256, 0, st>>>(cfg, m.n, m.d_pos, s->part[Rn].index_table, s->part[Rn].active_keys, s->part[Rn].count, cap, err);
 		++s->launches;
 	}
 	CK(cudaMemcpyAsync(&pbc, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToHost, st));
 	CK(cudaStreamSynchronize(st));
 	if(pbc > cap) return (int) cudaErrorMemoryAllocation;
 	for(Model& m : s->models) {
-		build_particle_cell_buckets_kernel<true><<<blocks_for(m.n, 256), 256, 0, st>>>(cfg, m.n, m.d_pos, view(m.pb[R]), s->part[Rn].index_table, err);
-		cell_bucket_to_block_kernel<<<blocks_for(pbc, 1), kBucketThreads, 0, st>>>(cfg, pbc, m.pb[R].cell_particle_counts, m.pb[R].cellbuckets, m.pb[R].particle_bucket_sizes, m.pb[R].blockbuckets, m.celloffs[Rn]);
-		compute_bin_capacity_kernel<<<blocks_for(pbc + 1, 256), 256, 0, st>>>(pbc + 1, m.pb[R].particle_bucket_sizes, m.bin_sizes);
+		build_particle_cell_buckets_kernel<true><<<grid_for(m.n, 256, 16), 256, 0, st>>>(cfg, m.n, m.d_pos, view(m.pb[R]), s->part[Rn].index_table, err);
+		cell_bucket_to_block_kernel<<<grid_for(pbc, 1, 16), kBucketThreads, 0, st>>>(cfg, pbc, m.pb[R].cell_particle_counts, m.pb[R].cellbuckets, m.pb[R].particle_bucket_sizes, m.pb[R].blockbuckets, m.celloffs[Rn]);
+		compute_bin_capacity_kernel<<<grid_for(pbc + 1, 256, 16), 256, 0, st>>>(pbc + 1, m.pb[R].particle_bucket_sizes, m.bin_sizes);
 		ScanArgs a {};
 		a.count = count_imm(pbc + 1);
 		a.in = m.bin_sizes;
 		a.out = m.pb[R].bin_offsets;
 		scan_kernel<<<1, 1024, 0, st>>>(a);
-		if(rs) state_to_bins_kernel<<<blocks_for(pbc, 1), 128, 0, st>>>(cfg, m.material, pbc, rs->state[&m - s->models.data()], view(m.pb[R]));
-		else array_to_buffer_kernel<<<blocks_for(pbc, 1), 128, 0, st>>>(cfg, m.material, pbc, m.d_pos, view(m.pb[R]));
+		if(rs) state_to_bins_kernel<<<grid_for(pbc, 1, 16), 128, 0, st>>>(cfg, m.material, pbc, rs->state[&m - s->models.data()], view(m.pb[R]));
+		else array_to_buffer_kernel<<<grid_for(pbc, 1, 16), 128, 0, st>>>(cfg, m.material, pbc, m.d_pos, view(m.pb[R]));
 		s->launches += 5;
 	}
 	{
@@ -1115,24 +1105,25 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 		a.error = err;
 		a.lo = 0;
 		a.span = 2;
-		register_blocks_kernel<<<blocks_for((long long) pbc * 8, 128), 128, 0, st>>>(a);
+		register_blocks_kernel<<<grid_for((long long) pbc * 8, 128, 16), 128, 0, st>>>(a);
 		CK(cudaMemcpyAsync(&nbc, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToHost, st));
 		CK(cudaStreamSynchronize(st));
 		if(s->desc.mgsp_world > 1) {  // halo_tagging of the initial partition (mgsp_benchmark.cuh:633), with the kernels of the sub-step
 			if(!s->peers_ready) return (int) cudaErrorNotReady;
 			const MgspView v = mgsp_view(s);
-			float* local_max = reinterpret_cast<float*>(s->d_scratch + 3);
-			CK(cudaMemcpyAsync(s->d_scratch + 1, &nbc, sizeof(int), cudaMemcpyHostToDevice, st));  // key count of the exchange
-			CK(cudaMemsetAsync(s->d_scratch + 3, 0, 2 * sizeof(int), st));
-			mgsp_tag_reset_kernel<<<grid_blocks(1), 256, 0, st>>>(v, s->part[Rn].overlap_marks, s->d_scratch + 1);
+			DeviceScratch* scr = s->scr;
+			CK(cudaMemcpyAsync(&scr->new_nbc, &nbc, sizeof(int), cudaMemcpyHostToDevice, st));  // key count of the exchange
+			CK(cudaMemsetAsync(&scr->local_max, 0, sizeof(float), st));
+			CK(cudaMemsetAsync(&scr->global_max, 0, sizeof(float), st));
+			mgsp_tag_reset_kernel<<<grid_blocks(1), 256, 0, st>>>(v, s->part[Rn].overlap_marks, &scr->new_nbc);
 			// the next grid is still all zero from cb200_sim_create: the clear changes nothing, and the flag still goes out behind it
-			mgsp_clear_publish_kernel<<<grid_blocks(2), 256, 0, st>>>(v, s->part[Rn].active_keys, s->d_scratch + 1, local_max, s->grid[1]);
-			mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(cfg, v, s->part[Rn].index_table, s->part[Rn].overlap_marks, s->d_scratch + 1, local_max, reinterpret_cast<float*>(s->d_scratch + 4), 0, FinalizeArgs {});
+			mgsp_clear_publish_kernel<<<grid_blocks(2), 256, 0, st>>>(v, s->part[Rn].active_keys, &scr->new_nbc, &scr->local_max, s->grid[1]);
+			mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(cfg, v, s->part[Rn].index_table, s->part[Rn].overlap_marks, &scr->new_nbc, &scr->local_max, &scr->global_max, 0, FinalizeArgs {});
 			s->launches += 3;
 		}
 		a.lo = -1;
 		a.span = 3;
-		register_blocks_kernel<<<blocks_for((long long) pbc * 27, 128), 128, 0, st>>>(a);
+		register_blocks_kernel<<<grid_for((long long) pbc * 27, 128, 16), 128, 0, st>>>(a);
 		CK(cudaMemcpyAsync(&ebc, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToHost, st));
 		CK(cudaStreamSynchronize(st));
 		s->launches += 2;
@@ -1149,21 +1140,21 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 		CK(cudaMemcpyAsync(m.pb[Rn].bin_offsets, m.pb[R].bin_offsets, (size_t) (pbc + 1) * sizeof(int), cudaMemcpyDeviceToDevice, st));
 		CK(cudaMemcpyAsync(m.pb[Rn].particle_bucket_sizes, m.pb[R].particle_bucket_sizes, (size_t) pbc * sizeof(int), cudaMemcpyDeviceToDevice, st));
 	}
-	clear_grid_kernel<<<blocks_for((long long) nbc * 64, 256), 256, 0, st>>>(nbc, s->grid[0]);
+	clear_grid_kernel<<<grid_for((long long) nbc * 64, 256, 16), 256, 0, st>>>(nbc, s->grid[0]);
 	++s->launches;
-	int* missing = s->d_scratch + 6;
+	int* missing = &s->scr->missing;
 	if(rs) {  // the saved blocks by key; a key the rebuilt partition has no neighbour block for is counted, not written
 		const int saved = rs->grid_count;
 		CK(cudaMemsetAsync(missing, 0, sizeof(int), st));
-		scatter_grid_kernel<<<blocks_for(saved, 8), 256, 0, st>>>(cfg, saved, rs->keys, rs->grid, s->part[R].index_table, nbc, s->grid[0], missing);
+		scatter_grid_kernel<<<grid_for(saved, 8, 16), 256, 0, st>>>(cfg, saved, rs->keys, rs->grid, s->part[R].index_table, nbc, s->grid[0], missing);
 		++s->launches;
 	}
 	for(Model& m : s->models) {
 		if(!rs) {
-			rasterize_blocks_kernel<<<blocks_for(pbc, 1), 256, 0, st>>>(cfg, m.material, pbc, s->part[R].active_keys, s->part[R].index_table, view(m.pb[R]), s->grid[0], m.pb[R].mass, m.v0[0], m.v0[1], m.v0[2], err);
+			rasterize_blocks_kernel<<<grid_for(pbc, 1, 16), 256, 0, st>>>(cfg, m.material, pbc, s->part[R].active_keys, s->part[R].index_table, view(m.pb[R]), s->grid[0], m.pb[R].mass, m.v0[0], m.v0[1], m.v0[2], err);
 			++s->launches;
 		}
-		init_adv_bucket_kernel<<<blocks_for(pbc, 1), 128, 0, st>>>(cfg, pbc, m.pb[Rn].particle_bucket_sizes, m.pb[Rn].blockbuckets);
+		init_adv_bucket_kernel<<<grid_for(pbc, 1, 16), 128, 0, st>>>(cfg, pbc, m.pb[Rn].particle_bucket_sizes, m.pb[Rn].blockbuckets);
 		++s->launches;
 	}
 	CK(cudaGetLastError());
@@ -1383,13 +1374,14 @@ static int retrieve_impl(cb200_sim* s, int model, float* host, int nch, int* n_o
 	}
 	if(!host && !m.h_out) CK(cudaMallocHost(&m.h_out, m.out_floats * sizeof(float)));
 	float* dst = host ? host : m.h_out;  // caller memory (fast when it is pinned) or the simulator's pinned mirror
-	CK(cudaMemsetAsync(s->d_scratch + 2, 0, sizeof(int), s->stream));
-	retrieve_kernel<<<num_sms() * 8, 128, 0, s->stream>>>(s->cfg, m.material, count_dev(&s->d_state->pbc), s->part[R].active_keys, s->part[Rn].index_table, view(m.pb[R]), view(m.pb[Rn]), m.d_out, nch, s->d_scratch + 2);
+	int* parcount = &s->scr->retrieve_count;
+	CK(cudaMemsetAsync(parcount, 0, sizeof(int), s->stream));
+	retrieve_kernel<<<num_sms() * 8, 128, 0, s->stream>>>(s->cfg, m.material, count_dev(&s->d_state->pbc), s->part[R].active_keys, s->part[Rn].index_table, view(m.pb[R]), view(m.pb[Rn]), m.d_out, nch, parcount);
 	++s->launches;
 	// the count is only known on the device: copy the full staging buffer behind the kernel, read the count with it
 	CK(cudaMemcpyAsync(dst, m.d_out, need * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
 	int n = 0;
-	CK(cudaMemcpyAsync(&n, s->d_scratch + 2, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+	CK(cudaMemcpyAsync(&n, parcount, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
 	CK(cudaStreamSynchronize(s->stream));
 	if(n > m.n) n = m.n;
 	if(pinned_out) *pinned_out = m.h_out;
@@ -1401,8 +1393,7 @@ int cb200_sim_retrieve(cb200_sim* s, int model, float* positions_host, int* n_ou
 int cb200_sim_retrieve_pinned(cb200_sim* s, int model, const float** positions_pinned, int* n_out) { return retrieve_impl(s, model, nullptr, 3, n_out, positions_pinned); }
 int cb200_sim_particle_state(cb200_sim* s, int model, float* state_host, int* n_out) {
 	if(!s || model < 0 || model >= (int) s->models.size()) return (int) cudaErrorInvalidValue;
-	const int mat = s->models[model].material;
-	return retrieve_impl(s, model, state_host, mat == CB200_J_FLUID ? 4 : (mat == CB200_FIXED_COROTATED ? 12 : 13), n_out, nullptr);
+	return retrieve_impl(s, model, state_host, ck_channels(s->models[model].material), n_out, nullptr);
 }
 
 int cb200_sim_active_keys(cb200_sim* s, int* keys_host, int capacity_blocks, int* n_out) {
@@ -1426,10 +1417,7 @@ long long cb200_sim_launch_count(cb200_sim* s) { return s ? s->launches : 0; }
 // The sub-step graphs hold the grid-update and carry launches of the collider state they were captured with: drop them and,
 // once set up, instantiate both roll parities again right away (never later, while an MGSP peer may be waiting on this rank).
 static int recapture(cb200_sim* s) {
-	for(int i = 0; i < 2; ++i) {
-		if(s->graph[i]) cudaGraphExecDestroy(s->graph[i]);
-		s->graph[i] = nullptr;
-	}
+	drop_graphs(s);
 	if(s->setup_done && s->desc.use_graph) {
 		CK(ensure_graph(s, 0));
 		CK(ensure_graph(s, 1));
@@ -1479,14 +1467,16 @@ int cb200_checkpoint_inspect(const void* blob, size_t bytes, cb200_checkpoint_in
 
 }  // extern "C"
 namespace {
-size_t ck_capacity(const cb200_sim* s) {
+// the checkpoint layout of the simulator's models with counts[m] particles each and nbc grid blocks
+CkLayout models_layout(const cb200_sim* s, const long long* counts, long long nbc) {
 	int mats[kMaxModels];
+	for(size_t m = 0; m < s->models.size(); ++m) mats[m] = s->models[m].material;
+	return ck_layout((int) s->models.size(), mats, counts, nbc);
+}
+size_t ck_capacity(const cb200_sim* s) {
 	long long counts[kMaxModels];
-	for(size_t m = 0; m < s->models.size(); ++m) {
-		mats[m] = s->models[m].material;
-		counts[m] = s->models[m].n;
-	}
-	return (size_t) ck_layout((int) s->models.size(), mats, counts, s->desc.max_blocks).total;
+	for(size_t m = 0; m < s->models.size(); ++m) counts[m] = s->models[m].n;
+	return (size_t) models_layout(s, counts, s->desc.max_blocks).total;
 }
 // grows a checkpoint buffer to `need` bytes (contents are not kept)
 template<typename T>
@@ -1497,6 +1487,30 @@ int ck_grow(T*& p, size_t& have, size_t need) {
 	have = 0;
 	CK(pool_alloc(&p, need));
 	have = need;
+	return 0;
+}
+// the same for a pinned host buffer
+int pinned_grow(unsigned char*& p, size_t& have, size_t need) {
+	if(have >= need) return 0;
+	if(p) cudaFreeHost(p);
+	p = nullptr;
+	have = 0;
+	CK(cudaMallocHost(&p, need));
+	have = need;
+	return 0;
+}
+// model m's row of ck_base: the exclusive scan of its bucket sizes, entry pbc its particle count
+int* ck_row(const cb200_sim* s, int m) { return s->ck_base + (size_t) m * (s->desc.max_blocks + 1); }
+// every model's particle count, entry pbc of its scan, once the bucket scans have run (synchronises)
+int read_totals(cb200_sim* s, int pbc, long long* counts) {
+	const int nm = (int) s->models.size();
+	int totals[kMaxModels] = {};
+	for(int m = 0; m < nm; ++m) CK(cudaMemcpyAsync(&totals[m], ck_row(s, m) + pbc, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+	CK(cudaStreamSynchronize(s->stream));
+	for(int m = 0; m < nm; ++m) {
+		if(totals[m] < 0 || totals[m] > s->models[m].n) return (int) cudaErrorIllegalState;
+		counts[m] = totals[m];
+	}
 	return 0;
 }
 }  // namespace
@@ -1513,7 +1527,7 @@ static int enqueue_bucket_scans(cb200_sim* s) {
 		sc.count = count_dev(&s->d_state->pbc);
 		sc.count_plus = 1;
 		sc.in = s->models[m].pb[Rn].particle_bucket_sizes;
-		sc.out = s->ck_base + m * (s->desc.max_blocks + 1);
+		sc.out = ck_row(s, (int) m);
 		scan_kernel<<<1, 1024, 0, s->stream>>>(sc);
 		++s->launches;
 	}
@@ -1535,7 +1549,7 @@ static int enqueue_snapshot(cb200_sim* s, unsigned char* out) {
 		a.material[m] = md.material;
 		a.cur[m] = view(md.pb[R]);
 		a.next[m] = view(md.pb[Rn]);
-		a.base[m] = s->ck_base + (size_t) m * (s->desc.max_blocks + 1);
+		a.base[m] = ck_row(s, m);
 	}
 	a.keys = s->part[R].active_keys;
 	a.prev_table = s->part[Rn].index_table;
@@ -1557,32 +1571,18 @@ int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	}
 	const size_t cap = ck_capacity(s);
 	CK(ck_grow(s->ck_dev, s->ck_dev_bytes, cap));
-	if(s->ck_host_bytes < cap) {
-		if(s->ck_host) cudaFreeHost(s->ck_host);
-		s->ck_host = nullptr;
-		s->ck_host_bytes = 0;
-		CK(cudaMallocHost(&s->ck_host, cap));
-		s->ck_host_bytes = cap;
-	}
+	CK(pinned_grow(s->ck_host, s->ck_host_bytes, cap));
 	CK(enqueue_snapshot(s, s->ck_dev));
 	CK(cudaEventRecord(s->ck_gathered, s->stream));
-	// the counts the layout follows from: the step state (pbc, nbc, clock), then each model's total, entry pbc of its scan
+	// the counts the layout follows from: the step state (pbc, nbc, clock), then each model's total
 	const int nm = (int) s->models.size();
-	cudaStream_t st = s->stream;
 	CK(pull_state(s));
 	const StepState& h = *s->h_state;
-	int totals[kMaxModels] = {};
-	for(int m = 0; m < nm; ++m) CK(cudaMemcpyAsync(&totals[m], s->ck_base + (size_t) m * (s->desc.max_blocks + 1) + h.pbc, sizeof(int), cudaMemcpyDeviceToHost, st));
-	CK(cudaStreamSynchronize(st));
+	long long counts[kMaxModels];
+	CK(read_totals(s, h.pbc, counts));
+	const CkLayout L = models_layout(s, counts, h.nbc);
 	cb200_checkpoint_info I;
 	memset(&I, 0, sizeof(I));
-	int mats[kMaxModels];
-	long long counts[kMaxModels];
-	for(int m = 0; m < nm; ++m) {
-		mats[m] = s->models[m].material;
-		counts[m] = totals[m];
-	}
-	const CkLayout L = ck_layout(nm, mats, counts, h.nbc);
 	I.version = CB200_CHECKPOINT_VERSION;
 	I.n_models = nm;
 	I.bytes = L.total;
@@ -1609,14 +1609,12 @@ int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	I.grid_bytes = L.grid_bytes;
 	for(int m = 0; m < nm; ++m) {
 		cb200_checkpoint_model& md = I.models[m];
-		md.material = mats[m];
-		md.channels = ck_channels(mats[m]);
+		md.material = s->models[m].material;
+		md.channels = ck_channels(md.material);
 		md.count = counts[m];
 		md.offset = L.model_off[m];
 		md.bytes = L.model_bytes[m];
-		md.params = s->models[m].pb[0];
-		md.params.bins = nullptr;
-		md.params.cell_particle_counts = md.params.particle_bucket_sizes = md.params.cellbuckets = md.params.blockbuckets = md.params.bin_offsets = nullptr;
+		md.params = s->models[m].pb[0];  // (ck_write_header writes the parameters only)
 	}
 	ck_write_header(s->ck_host, I);
 	// the data sections: behind the snapshot, on the copy stream, so that sub-steps enqueued from here on run alongside
@@ -1661,17 +1659,7 @@ int cb200_sim_restore_models(cb200_sim* s, const void* blob, size_t bytes) {
 		model.material = md.material;
 		model.n = (int) md.count;
 		CK(alloc_model(s, model));
-		for(int i = 0; i < 2; ++i) {  // the saved parameters, the containers of this simulator
-			cb200_particle_buffer& pb = model.pb[i];
-			cb200_particle_buffer p = md.params;
-			p.bins = pb.bins;
-			p.cell_particle_counts = pb.cell_particle_counts;
-			p.particle_bucket_sizes = pb.particle_bucket_sizes;
-			p.cellbuckets = pb.cellbuckets;
-			p.blockbuckets = pb.blockbuckets;
-			p.bin_offsets = pb.bin_offsets;
-			pb = p;
-		}
+		for(cb200_particle_buffer& pb : model.pb) copy_params(pb, md.params);
 		s->models.push_back(model);
 		CK(pool_alloc(&s->restore_state[m], md.bytes));
 		CK(cudaMemcpyAsync(s->restore_state[m], src + md.offset, md.bytes, cudaMemcpyHostToDevice, st));
@@ -1731,13 +1719,7 @@ int cb200_sim_frame_output(cb200_sim* s, const char* const* paths, unsigned attr
 		need += (size_t) s->models[m].n * W * sizeof(float);
 	}
 	CK(ck_grow(s->out_dev, s->out_dev_bytes, need));
-	if(s->out_host_bytes < need) {
-		if(s->out_host) cudaFreeHost(s->out_host);
-		s->out_host = nullptr;
-		s->out_host_bytes = 0;
-		CK(cudaMallocHost(&s->out_host, need));
-		s->out_host_bytes = need;
-	}
+	CK(pinned_grow(s->out_host, s->out_host_bytes, need));
 	const int R = s->rollid, Rn = R ^ 1;
 	CK(enqueue_bucket_scans(s));
 	a.cfg = s->cfg;
@@ -1749,7 +1731,7 @@ int cb200_sim_frame_output(cb200_sim* s, const char* const* paths, unsigned attr
 		a.material[m] = md.material;
 		a.cur[m] = view(md.pb[R]);
 		a.next[m] = view(md.pb[Rn]);
-		a.base[m] = s->ck_base + (size_t) m * (s->desc.max_blocks + 1);
+		a.base[m] = ck_row(s, m);
 	}
 	a.keys = s->part[R].active_keys;
 	a.table = s->part[R].index_table;
@@ -1759,14 +1741,12 @@ int cb200_sim_frame_output(cb200_sim* s, const char* const* paths, unsigned attr
 	output_kernel<<<num_sms() * 8, kOutThreads, 0, s->stream>>>(a);
 	++s->launches;
 	CK(cudaGetLastError());
-	// the counts the headers need (each model's total, entry pbc of its scan): this is the only wait, and it ends with the gather
+	// the counts the headers need (each model's total): this is the only wait, and it ends with the gather
 	CK(pull_state(s));
-	int totals[kMaxModels] = {};
-	for(int m = 0; m < nm; ++m) CK(cudaMemcpyAsync(&totals[m], a.base[m] + s->h_state->pbc, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-	CK(cudaStreamSynchronize(s->stream));
+	long long totals[kMaxModels];
+	CK(read_totals(s, s->h_state->pbc, totals));
 	std::vector<cb200_sim::OutputFile> files((size_t) nm);
 	for(int m = 0; m < nm; ++m) {
-		if(totals[m] < 0 || totals[m] > s->models[m].n) return (int) cudaErrorIllegalState;
 		files[m].path = paths[m];
 		files[m].header = bgeo_header(totals[m], attributes);
 		files[m].body = s->out_host + a.off[m];
@@ -1976,8 +1956,6 @@ int emit_precheck(cb200_sim* s, int model, unsigned flags, const float* v0) {
 	return 0;
 }
 
-inline int launch_items(long long n, int per) { return (int) std::max<long long>(1, std::min<long long>((n + per - 1) / per, (long long) num_sms() * 16)); }
-
 // The shared path of both entries, with the n candidates in eb.cand.  Everything up to the commit reads the live state and writes
 // scratch only, so a rejection leaves the simulator as it was.
 int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, unsigned flags, int* n_added) {
@@ -2002,7 +1980,7 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 			occ.sizes[m] = s->models[m].pb[Rn].particle_bucket_sizes;
 		}
 	}
-	emit_filter_kernel<<<launch_items(n, 256), 256, 0, st>>>(occ, n, eb.cand, (flags & CB200_EMIT_EMPTY_CELLS) ? 1 : 0, eb.keep, eb.word + 1);
+	emit_filter_kernel<<<grid_for(n, 256, 16), 256, 0, st>>>(occ, n, eb.cand, (flags & CB200_EMIT_EMPTY_CELLS) ? 1 : 0, eb.keep, eb.word + 1);
 	ScanArgs sc {};
 	sc.count = count_imm(n);
 	sc.count_plus = 1;
@@ -2018,7 +1996,7 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	if(bad) return (int) cudaErrorInvalidValue;
 	if(k == 0) return 0;
 	CK(pool_alloc(&eb.kept, (size_t) k * 3 * sizeof(float)));
-	emit_compact_kernel<<<launch_items(n, 256), 256, 0, st>>>(n, eb.cand, eb.keep, eb.offs, eb.kept);
+	emit_compact_kernel<<<grid_for(n, 256, 16), 256, 0, st>>>(n, eb.cand, eb.keep, eb.offs, eb.kept);
 	++s->launches;
 	// (2) the union's partition on a scratch table: the current particle blocks first, then the candidates' blocks, then the neighbour
 	// and exterior registrations of initial_setup.  Its capacity holds every block they can register, so the counts are exact.
@@ -2028,8 +2006,8 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	CK(pool_alloc(&eb.table, s->table_entries * sizeof(int)));
 	CK(pool_alloc(&eb.keys, ((size_t) cap_s + 1) * 3 * sizeof(int)));
 	CK(cudaMemsetAsync(eb.table, 0xff, s->table_entries * sizeof(int), st));
-	emit_insert_keys_kernel<<<launch_items(h0.pbc, 256), 256, 0, st>>>(cfg, h0.pbc, s->part[s->rollid].active_keys, eb.table, eb.keys, eb.word, cap_s);
-	activate_blocks_kernel<true><<<launch_items(k, 256), 256, 0, st>>>(cfg, k, eb.kept, eb.table, eb.keys, eb.word, cap_s, nullptr);
+	emit_insert_keys_kernel<<<grid_for(h0.pbc, 256, 16), 256, 0, st>>>(cfg, h0.pbc, s->part[s->rollid].active_keys, eb.table, eb.keys, eb.word, cap_s);
+	activate_blocks_kernel<true><<<grid_for(k, 256, 16), 256, 0, st>>>(cfg, k, eb.kept, eb.table, eb.keys, eb.word, cap_s, nullptr);
 	s->launches += 2;
 	int cnt[3] = {0, 0, 0};  // the union's pbc, nbc, ebc
 	CK(cudaMemcpyAsync(&cnt[0], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2043,17 +2021,17 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	ra.capacity = cap_s;
 	ra.lo = 0;
 	ra.span = 2;
-	register_blocks_kernel<<<launch_items((long long) cnt[0] * 8, 128), 128, 0, st>>>(ra);
+	register_blocks_kernel<<<grid_for((long long) cnt[0] * 8, 128, 16), 128, 0, st>>>(ra);
 	CK(cudaMemcpyAsync(&cnt[1], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
 	ra.lo = -1;
 	ra.span = 3;
-	register_blocks_kernel<<<launch_items((long long) cnt[0] * 27, 128), 128, 0, st>>>(ra);
+	register_blocks_kernel<<<grid_for((long long) cnt[0] * 27, 128, 16), 128, 0, st>>>(ra);
 	CK(cudaMemcpyAsync(&cnt[2], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
 	// (3) no cell above max_ppc, existing and new particles together
 	CK(pool_alloc(&eb.cells, (size_t) cnt[0] * kBlockVol * sizeof(int)));
 	CK(cudaMemsetAsync(eb.cells, 0, (size_t) cnt[0] * kBlockVol * sizeof(int), st));
-	emit_count_kernel<<<launch_items(k, 256), 256, 0, st>>>(cfg, k, eb.kept, eb.table, eb.cells);
-	emit_overflow_kernel<<<launch_items(k, 256), 256, 0, st>>>(occ, k, eb.kept, eb.table, eb.cells, eb.word + 1);
+	emit_count_kernel<<<grid_for(k, 256, 16), 256, 0, st>>>(cfg, k, eb.kept, eb.table, eb.cells);
+	emit_overflow_kernel<<<grid_for(k, 256, 16), 256, 0, st>>>(occ, k, eb.kept, eb.table, eb.cells, eb.word + 1);
 	s->launches += 4;
 	CK(cudaGetLastError());
 	CK(cudaMemcpyAsync(&bad, eb.word + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2069,40 +2047,26 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	// (5) gather the current state (checkpoint layout) and allocate what the commit swaps in: nothing live is written yet
 	CK(pool_alloc(&eb.blob, ck_capacity(s)));
 	CK(enqueue_snapshot(s, eb.blob));
-	int mats[kMaxModels];
 	long long counts[kMaxModels];
-	int totals[kMaxModels] = {};
-	for(int m = 0; m < nm; ++m) {
-		mats[m] = s->models[m].material;
-		CK(cudaMemcpyAsync(&totals[m], s->ck_base + (size_t) m * (s->desc.max_blocks + 1) + h0.pbc, sizeof(int), cudaMemcpyDeviceToHost, st));
-	}
-	CK(cudaStreamSynchronize(st));
-	for(int m = 0; m < nm; ++m) {
-		if(totals[m] < 0 || totals[m] > s->models[m].n) return (int) cudaErrorIllegalState;
-		counts[m] = totals[m];
-	}
-	const CkLayout L = ck_layout(nm, mats, counts, h0.nbc);
+	CK(read_totals(s, h0.pbc, counts));
+	const CkLayout L = models_layout(s, counts, h0.nbc);
 	Model& md = s->models[model];
 	const int C = ck_channels(md.material);
 	const long long n_union = counts[model] + k;
-	const long long new_bins = n_union / kBinCap + new_mb;  // alloc_model's rule
-	const size_t binf = md.material == CB200_J_FLUID ? 128 : 512;
+	const long long new_bins = bin_rows(n_union, new_mb);
 	CK(pool_alloc(&eb.rows, (size_t) n_union * C * sizeof(float)));
 	CK(pool_alloc(&eb.pos, (size_t) n_union * 3 * sizeof(float)));
 	if(new_bins > md.bin_capacity)
-		for(int i = 0; i < 2; ++i) CK(pool_alloc(&eb.bins[i], (size_t) new_bins * binf * sizeof(float)));
+		for(float*& bins : eb.bins) CK(pool_alloc(&bins, (size_t) new_bins * bin_floats(md.material) * sizeof(float)));
 	if(L.model_bytes[model]) CK(cudaMemcpyAsync(eb.rows, eb.blob + L.model_off[model], L.model_bytes[model], cudaMemcpyDeviceToDevice, st));
-	emit_rows_kernel<<<launch_items(k, 256), 256, 0, st>>>(md.material, k, eb.kept, eb.rows + (size_t) counts[model] * C);
+	emit_rows_kernel<<<grid_for(k, 256, 16), 256, 0, st>>>(md.material, k, eb.kept, eb.rows + (size_t) counts[model] * C);
 	++s->launches;
 	CK(cudaGetLastError());
 	CK(cudaStreamSynchronize(st));
 	// the last step that can reject: cb200_sim_reserve (an out-of-memory failure there leaves a valid simulator, part-grown)
 	if(new_mb > s->desc.max_blocks) CK(cb200_sim_reserve(s, new_mb));
 	// (6) commit: initial_setup's restore path over the union, then the new particles' mass and momentum added to grid[0]
-	for(int i = 0; i < 2; ++i) {
-		if(s->graph[i]) cudaGraphExecDestroy(s->graph[i]);
-		s->graph[i] = nullptr;
-	}
+	drop_graphs(s);
 	if(eb.bins[0] && new_bins > md.bin_capacity) {  // (reserve may have grown the bins past the new count's rule already)
 		for(int i = 0; i < 2; ++i) std::swap(md.pb[i].bins, eb.bins[i]);
 		md.bin_capacity = new_bins;
@@ -2119,14 +2083,15 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	rs.keys = reinterpret_cast<const int*>(eb.blob + L.keys_off);
 	rs.grid = reinterpret_cast<const float*>(eb.blob + L.grid_off);
 	rs.grid_count = h0.nbc;
-	{  // setup_impl starts from an empty partition (roll Rn) and zero cell counts / bucket sizes in the buffers it buckets into (roll R)
+	{  // setup_impl starts from an empty partition (roll Rn) and zero cell counts / bucket sizes in the buffers it buckets into (roll R):
+		// both as allocation leaves them
 		const int R = s->rollid, Rn = R ^ 1;
 		const size_t mb = (size_t) s->desc.max_blocks;
-		CK(cudaMemsetAsync(s->part[Rn].index_table, 0xff, s->table_entries * sizeof(int), st));
-		CK(cudaMemsetAsync(s->part[Rn].count, 0, sizeof(int), st));
+		CK(fill_arrays(s, partition_arrays(s, s->part[Rn], mb)));
 		for(Model& mm : s->models) {
-			CK(cudaMemsetAsync(mm.pb[R].cell_particle_counts, 0, (mb + 1) * kBlockVol * sizeof(int), st));
-			CK(cudaMemsetAsync(mm.pb[R].particle_bucket_sizes, 0, (mb + 2) * sizeof(int), st));
+			DevArrays a;
+			buffer_arrays(a, s, mm, mm.pb[R], mb, mm.bin_capacity);
+			CK(fill_arrays(s, a));
 		}
 	}
 	// the clock stays; dt and next_dt follow initial_setup's rule for v0
@@ -2150,7 +2115,7 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	CK(setup_impl(s, &rs));
 	// every stencil node of a new particle inside the domain lies in a neighbour block of its particle block; nodes past the top face
 	// are dropped, as rasterize_blocks_kernel drops them
-	rasterize_kernel<<<launch_items(k, 256), 256, 0, st>>>(cfg, k, eb.kept, s->grid[0], s->part[s->rollid].index_table, md.pb[0].mass, v[0], v[1], v[2], nullptr);
+	rasterize_kernel<<<grid_for(k, 256, 16), 256, 0, st>>>(cfg, k, eb.kept, s->grid[0], s->part[s->rollid].index_table, md.pb[0].mass, v[0], v[1], v[2], nullptr);
 	++s->launches;
 	CK(cudaGetLastError());
 	CK(cudaStreamSynchronize(st));
