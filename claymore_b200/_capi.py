@@ -203,6 +203,7 @@ _SIGNATURES = {
     "cb200_sim_add_particles_sdf": [_P, _I, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.c_uint, C.POINTER(_I)],
     "cb200_test_svd3": [_I, _P, _P, _P, _P, _P],
     "cb200_test_stress": [_I, _I, ParticleBuffer, _I, _P, _P, _P, _P, _P, _P],
+    "cb200_test_warp_flatten": [_CFG, _I, _P, _P, _P, _P, _P, _P],
     "cb200_sim_profile": [_P, _I],
     "cb200_sim_profile_read": [_P, C.POINTER(C.c_double), C.POINTER(_I)],
     "cb200_sim_profile_phases": [_P, C.POINTER(C.c_double)],

@@ -361,6 +361,12 @@ int cb200_test_stress(int material, int mode, cb200_particle_buffer params, int 
 	test_stress_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t) stream>>>(material, mode, mat_of(params), n, F_in, log_jp_in, F_out, PF_out, log_jp_out);
 	return (int) cudaGetLastError();
 }
+int cb200_test_warp_flatten(const cb200_config* c, int block_count, const int* cell_particle_counts, const int* cellbuckets, int* particle_bucket_sizes, int* buckets, unsigned short* cell_offsets, void* stream) {
+	CB_CFG(c);
+	if(block_count <= 0) return 0;
+	warp_flatten_kernel<<<(block_count + 7) / 8, 256, 0, (cudaStream_t) stream>>>(cfg, block_count, cell_particle_counts, cellbuckets, particle_bucket_sizes, buckets, cell_offsets);
+	return (int) cudaGetLastError();
+}
 // ParticleBuffer<M> defaults (particle_buffer.cuh:141-264) as the step driver sets them (engine.cu)
 void cb200_default_material(const cb200_config* cfg, int material, cb200_particle_buffer* out);
 }

@@ -406,6 +406,9 @@ void drop_graphs(cb200_sim* s) {
 }
 
 inline int grid_blocks(int per_sm) { return num_sms() * per_sm; }
+// A registration thread walks its (block, offset) pairs one after the other, each a key read and then a table CAS that waits for L2:
+// the launch is bound by how many threads walk at once, so it fills every thread slot of the SMs (16 x 128; the kernel takes 32 registers)
+constexpr int kRegisterCtasPerSm = 16;
 
 int pull_state(cb200_sim* s) {
 	CK(cudaMemcpyAsync(s->h_state, s->d_state, sizeof(StepState), cudaMemcpyDeviceToHost, s->stream));
@@ -542,7 +545,7 @@ int enqueue_rebuild(cb200_sim* s, int R) {
 			a.bin_offsets[m] = s->models[m].pb[R].bin_offsets;
 			a.dst_offs[m] = s->models[m].celloffs[R];
 		}
-		rebuild_kernel<<<tiles, kRebuildThreads, 0, st>>>(a);
+		rebuild_kernel<<<tiles * kRebuildSplit, kRebuildThreads, 0, st>>>(a);
 		++s->launches;
 	}
 	{
@@ -558,7 +561,7 @@ int enqueue_rebuild(cb200_sim* s, int R) {
 		a.span = 2;
 		a.done_counter = &s->d_state->done_counter;  // the last CTA snapshots the neighbour count
 		a.snapshot_out = &s->scr->new_nbc;
-		register_blocks_kernel<<<grid_blocks(4), 128, 0, st>>>(a);
+		register_blocks_kernel<<<grid_blocks(kRegisterCtasPerSm), 128, 0, st>>>(a);
 		++s->launches;
 	}
 	return (int) cudaGetLastError();
@@ -632,7 +635,7 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 			a.do_finalize = 1;
 			a.fin = fin;
 		}
-		register_blocks_kernel<<<grid_blocks(4), 128, 0, st>>>(a);
+		register_blocks_kernel<<<grid_blocks(kRegisterCtasPerSm), 128, 0, st>>>(a);
 		++s->launches;
 	}
 	mark_phase(s, 9);

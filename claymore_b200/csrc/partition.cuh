@@ -9,6 +9,7 @@ namespace cb200 {
 __device__ __forceinline__ int partition_insert(const Cfg& cfg, int* table, int* keys, int* count, int capacity, int* error, int x, int y, int z) {
 	if(!in_domain(cfg, x, y, z)) return -1;
 	int* slot = table + table_offset(cfg, x, y, z);
+	if(*(volatile int*) slot != -1) return -1;  // taken already (most probes of a registration are): a load where the CAS would fail
 	if(atomicCAS(slot, -1, 0) == -1) {
 		const int idx = atomicAdd(count, 1);
 		if(idx >= capacity) {
@@ -163,7 +164,9 @@ __global__ void __launch_bounds__(kBucketThreads) cell_bucket_to_block_kernel(Cf
 // ------------------------------------------------------------------------------------------------
 constexpr int kRebuildTile = 64;        // old blocks per CTA
 constexpr int kSummaryThreads = 256;    // 8 warps x 8 blocks (eight independent row loads in flight per warp)
-constexpr int kRebuildThreads = 1024;   // 32 warps x 2 blocks: a marked block costs a dozen dependent gather rounds
+constexpr int kRebuildThreads = 256;    // 8 warps x 2 blocks: a CTA compacts a quarter of a tile (and repeats the tile's 64-thread scan)
+constexpr int kRebuildSplit = 4;        // CTAs per tile.  Every CTA costs about the same, so the launch ends with the SMs draining their last round of
+                                        // CTAs: sixteen blocks per CTA make that round an eighth of the launch where 64 blocks made it a third
 constexpr int kScanComps = kMaxModels + 1;  // component 0: marked blocks, 1 + m: bins of model m
 
 struct SummaryArgs {
@@ -198,16 +201,19 @@ __global__ void __launch_bounds__(kSummaryThreads) summary_kernel(const SummaryA
 	}
 	const int tile = blockIdx.x, b0 = tile * kRebuildTile;
 	if(tile < n_tiles) {
-		// warp w sums the cell counts of its blocks (one coalesced 256-byte row per block and model)
+		// warp w sums the cell counts of its blocks (one coalesced 256-byte row per block and model; a model's rows are all
+		// requested before the first is summed)
+		for(int m = 0; m < nm; ++m) {
+			int2 c[PER_WARP];
 #pragma unroll
-		for(int j = 0; j < PER_WARP; ++j) {
-			const int t = warp * PER_WARP + j, b = b0 + t;
-			for(int m = 0; m < nm; ++m) {
-				int tot = 0;
-				if(b < ebc) {
-					const int2 c = reinterpret_cast<const int2*>(a.cell_counts[m] + (size_t) b * kBlockVol)[lane];
-					tot = __reduce_add_sync(0xffffffffu, c.x + c.y);
-				}
+			for(int j = 0; j < PER_WARP; ++j) {
+				const int b = b0 + warp * PER_WARP + j;
+				c[j] = b < ebc ? __ldg(reinterpret_cast<const int2*>(a.cell_counts[m] + (size_t) b * kBlockVol) + lane) : make_int2(0, 0);
+			}
+#pragma unroll
+			for(int j = 0; j < PER_WARP; ++j) {
+				const int t = warp * PER_WARP + j, b = b0 + t;
+				const int tot = __reduce_add_sync(0xffffffffu, c[j].x + c[j].y);
 				if(lane == 0) {
 					s_tot[m][t] = tot;
 					if(b < ebc) a.block_totals[(size_t) m * a.max_blocks + b] = tot;
@@ -244,43 +250,61 @@ __global__ void __launch_bounds__(kSummaryThreads) summary_kernel(const SummaryA
 	if(!s_last) return;
 	__threadfence();
 	if(tid == 0) a.state->done_counter = 0;
-	// CTA-wide scan per component: thread i owns the tiles [i K, (i + 1) K)
+	// CTA-wide scan, thread i owns the tiles [i K, (i + 1) K): the components of a tile are read together, so a walk over the
+	// tiles costs one round trip per tile and not one per tile and component
 	{
-		__shared__ int s_wsum[kSummaryThreads / 32];
+		__shared__ int s_wsum[kScanComps][kSummaryThreads / 32];
 		const int K = (n_tiles + kSummaryThreads - 1) / kSummaryThreads;
-		for(int c = 0; c < nc; ++c) {
-			volatile int* col = a.tile_sums + c;
-			int sum = 0;
-			for(int k = 0; k < K; ++k) {
-				const int t = tid * K + k;
-				if(t < n_tiles) sum += col[(size_t) t * kScanComps];
+		volatile int* sums = a.tile_sums;
+		int sum[kScanComps], run[kScanComps];
+#pragma unroll
+		for(int c = 0; c < kScanComps; ++c) sum[c] = 0;
+		for(int k = 0; k < K; ++k) {
+			const int t = tid * K + k;
+			if(t < n_tiles) {
+#pragma unroll
+				for(int c = 0; c < kScanComps; ++c)
+					if(c < nc) sum[c] += sums[(size_t) t * kScanComps + c];
 			}
-			int inc = sum;
+		}
+#pragma unroll
+		for(int c = 0; c < kScanComps; ++c) {
+			int inc = sum[c];
 #pragma unroll
 			for(int o = 1; o < 32; o <<= 1) {
 				const int u = __shfl_up_sync(0xffffffffu, inc, o);
 				if(lane >= o) inc += u;
 			}
-			if(lane == 31) s_wsum[warp] = inc;
-			__syncthreads();
+			if(lane == 31) s_wsum[c][warp] = inc;
+			run[c] = inc - sum[c];  // exclusive inside the warp
+		}
+		__syncthreads();
+#pragma unroll
+		for(int c = 0; c < kScanComps; ++c) {
 			int base = 0, total = 0;
 #pragma unroll
 			for(int w = 0; w < kSummaryThreads / 32; ++w) {
-				const int v = s_wsum[w];
+				const int v = s_wsum[c][w];
 				if(w < warp) base += v;
 				total += v;
 			}
-			int run = base + inc - sum;  // exclusive prefix of this thread's first tile
-			for(int k = 0; k < K; ++k) {
-				const int t = tid * K + k;
-				if(t < n_tiles) {
-					const int v = col[(size_t) t * kScanComps];
-					col[(size_t) t * kScanComps] = run;
-					run += v;
-				}
+			run[c] += base;  // exclusive prefix of this thread's first tile
+			if(tid == 0 && c < nc) sums[(size_t) n_tiles * kScanComps + c] = total;  // grand total behind the last tile
+		}
+		for(int k = 0; k < K; ++k) {
+			const int t = tid * K + k;
+			if(t < n_tiles) {
+				int v[kScanComps];
+#pragma unroll
+				for(int c = 0; c < kScanComps; ++c)
+					if(c < nc) v[c] = sums[(size_t) t * kScanComps + c];
+#pragma unroll
+				for(int c = 0; c < kScanComps; ++c)
+					if(c < nc) {
+						sums[(size_t) t * kScanComps + c] = run[c];
+						run[c] += v[c];
+					}
 			}
-			if(tid == 0) col[(size_t) n_tiles * kScanComps] = total;  // grand total behind the last tile
-			__syncthreads();
 		}
 	}
 	__syncthreads();
@@ -297,12 +321,15 @@ __global__ void __launch_bounds__(kSummaryThreads) summary_kernel(const SummaryA
 	}
 }
 
-// one WARP per old block: the 64 cell counts are prefix-summed with shuffles, a tag finds its cell by a 6-step binary
-// search over the lane-distributed prefix (shuffles, no shared memory, no block barrier), so the eight warps of a CTA
-// stream independent blocks and hide each other's latency.
-__device__ __forceinline__ int warp_flatten_block(const Cfg& cfg, const int* __restrict__ cell_counts_blk, const int* __restrict__ cellbuckets_blk, int* __restrict__ dst, unsigned short* __restrict__ offs) {
+// one WARP per old block, no search: the block's tags are walked in the order they lie in `cellbuckets` (cell-major rows of
+// max_ppc slots), eight slots of four cells per step, and the bucket is those tags with the empty slots left out.  A lane
+// therefore knows its destination from its cell's count and exclusive prefix alone (one shuffle each from the lane that scanned
+// the cell): every load of a step is one 32-byte sector per cell, independent of every other load, kBatch steps are in flight
+// per warp before the first is consumed, and the valid tags of a step land in one contiguous run of the bucket.
+// Cells holding more than eight tags take further passes over the slots [8 g, 8 g + 8); the order inside a cell is its slot order.
+constexpr int kFlattenBatch = 8;
+__device__ __forceinline__ int warp_flatten_block(const Cfg& cfg, const int2 c, const int* __restrict__ cellbuckets_blk, int* __restrict__ dst, unsigned short* __restrict__ offs) {
 	const int lane = threadIdx.x & 31;
-	const int2 c = reinterpret_cast<const int2*>(cell_counts_blk)[lane];
 	const int pair = c.x + c.y;
 	int inc = pair;
 #pragma unroll
@@ -314,24 +341,40 @@ __device__ __forceinline__ int warp_flatten_block(const Cfg& cfg, const int* __r
 	const int p_odd = p_even + c.x;      // exclusive prefix of cell 2*lane + 1
 	const int total = __shfl_sync(0xffffffffu, inc, 31);
 	if(offs) reinterpret_cast<ushort2*>(offs)[lane] = make_ushort2((unsigned short) p_even, (unsigned short) p_odd);  // cell starts inside the bucket
-#pragma unroll 2
-	for(int i0 = 0; i0 < total; i0 += 32) {
-		const int i = i0 + lane;
-		// largest lane L with p_even(L) <= i
-		int L = 0;
+	// prefix << 8 | count: a prefix is below 64 * 128 and a count at most 128
+	const int meta_even = (p_even << 8) | c.x, meta_odd = (p_odd << 8) | c.y;
+	const int max_count = __reduce_max_sync(0xffffffffu, max(c.x, c.y));
+	const int sub = lane >> 3, slot0 = lane & 7;  // the step's cell 4 k + sub, the slot inside the group of eight
+	for(int g8 = 0; g8 < max_count; g8 += 8) {
+		const int slot = g8 + slot0;
+#pragma unroll 1
+		for(int k0 = 0; k0 < kBlockVol / 4; k0 += kFlattenBatch) {
+			int tag[kFlattenBatch], at[kFlattenBatch];
 #pragma unroll
-		for(int s = 16; s > 0; s >>= 1) {
-			const int probe = __shfl_sync(0xffffffffu, p_even, (L + s) & 31);
-			if(probe <= i) L += s;
+			for(int u = 0; u < kFlattenBatch; ++u) {
+				const int cell = 4 * (k0 + u) + sub;
+				const int me = __shfl_sync(0xffffffffu, meta_even, cell >> 1);
+				const int mo = __shfl_sync(0xffffffffu, meta_odd, cell >> 1);
+				const int meta = (cell & 1) ? mo : me;
+				at[u] = slot < (meta & 0xff) ? (meta >> 8) + slot : -1;
+				if(at[u] >= 0) tag[u] = __ldg(cellbuckets_blk + (cell << cfg.ppc_shift) + slot);
+			}
+#pragma unroll
+			for(int u = 0; u < kFlattenBatch; ++u)
+				if(at[u] >= 0) dst[at[u]] = tag[u];
 		}
-		const int pe = __shfl_sync(0xffffffffu, p_even, L);
-		const int po = __shfl_sync(0xffffffffu, p_odd, L);
-		const bool odd = po <= i;
-		const int cell = 2 * L + (odd ? 1 : 0);
-		const int off = i - (odd ? po : pe);
-		if(i < total) dst[i] = cellbuckets_blk[(cell << cfg.ppc_shift) + off];
 	}
 	return total;
+}
+
+// the flatten above on its own, one warp per block in place (no renumbering): what the tests hold against cell_bucket_to_block_kernel
+__global__ void __launch_bounds__(256) warp_flatten_kernel(Cfg cfg, int block_count, const int* cell_particle_counts, const int* cellbuckets, int* particle_bucket_sizes, int* buckets, unsigned short* cell_offsets) {
+	const int lane = threadIdx.x & 31;
+	for(int b = blockIdx.x * 8 + (threadIdx.x >> 5); b < block_count; b += gridDim.x * 8) {
+		const int2 c = reinterpret_cast<const int2*>(cell_particle_counts + (size_t) b * kBlockVol)[lane];
+		const int total = warp_flatten_block(cfg, c, cellbuckets + ((size_t) b << cfg.ppb_shift), buckets + ((size_t) b << cfg.ppb_shift), cell_offsets + (size_t) b * kBlockVol);
+		if(lane == 0) particle_bucket_sizes[b] = total;
+	}
 }
 
 struct RebuildArgs {
@@ -351,8 +394,8 @@ struct RebuildArgs {
 	int* bin_offsets[kMaxModels];        // cur buffers: exclusive scan of the bin demand
 	unsigned short* dst_offs[kMaxModels];  // cur buffers (new numbering): start of every cell inside the cell-major block bucket
 };
-__global__ void __launch_bounds__(kRebuildThreads, 2) rebuild_kernel(const RebuildArgs a) {  // 2 CTAs/SM: the gather rounds of a marked block are latency bound
-	constexpr int PER_WARP = kRebuildTile / (kRebuildThreads / 32);
+__global__ void __launch_bounds__(kRebuildThreads, 5) rebuild_kernel(const RebuildArgs a) {
+	constexpr int PER_WARP = kRebuildTile / kRebuildSplit / (kRebuildThreads / 32);
 	static_assert(kRebuildTile == 64, "the tile scan below is written for two warps");
 	__shared__ int s_tot[kMaxModels][kRebuildTile];
 	__shared__ int s_pre[kScanComps][kRebuildTile];  // exclusive prefix inside a 32-block half
@@ -361,8 +404,9 @@ __global__ void __launch_bounds__(kRebuildThreads, 2) rebuild_kernel(const Rebui
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const int nm = a.n_models, nc = nm + 1;
 	const int ebc = a.state->ebc;
-	const int tile = blockIdx.x, b0 = tile * kRebuildTile;
-	if(b0 >= ebc) return;
+	const int tile = blockIdx.x / kRebuildSplit, b0 = tile * kRebuildTile;
+	const int t0 = (blockIdx.x % kRebuildSplit) * (kRebuildTile / kRebuildSplit) + warp * PER_WARP;  // this warp's first block of the tile
+	if(b0 + t0 - warp * PER_WARP >= ebc) return;
 	if(tid < kRebuildTile) {  // thread t = block b0 + t
 		const int b = b0 + tid;
 		int any = 0;
@@ -384,14 +428,29 @@ __global__ void __launch_bounds__(kRebuildThreads, 2) rebuild_kernel(const Rebui
 		}
 	}
 	__syncthreads();
-	// ---- compaction: warp per marked old block
+	// ---- compaction: warp per marked old block.  The (block, model) pairs of a warp are walked in order, and the cell counts of
+	// the next pair that holds particles are requested before the current one is flattened.
+	const int* tp = a.tile_sums + (size_t) tile * kScanComps;
+	auto count_row = [&](int j, int m) {
+		const int t = t0 + j;
+		return __ldg(reinterpret_cast<const int2*>(a.cell_counts[m] + (size_t) (b0 + t) * kBlockVol) + lane);
+	};
+	// the first pair at or behind (j, m) with particles (blocks past ebc hold none)
+	auto advance = [&](int& j, int& m) {
+		while(j < PER_WARP && s_tot[m][t0 + j] == 0) {
+			if(++m == nm) m = 0, ++j;
+		}
+	};
+	int nj = 0, nmod = 0;
+	advance(nj, nmod);
+	int2 next_row = make_int2(0, 0);
+	if(nj < PER_WARP) next_row = count_row(nj, nmod);
 	for(int j = 0; j < PER_WARP; ++j) {
-		const int t = warp * PER_WARP + j, b = b0 + t;
+		const int t = t0 + j, b = b0 + t;
 		if(b >= ebc) break;
 		int any = 0;
 		for(int m = 0; m < nm; ++m) any |= s_tot[m][t];
 		if(!any) continue;
-		const int* tp = a.tile_sums + (size_t) tile * kScanComps;
 		const int nb = tp[0] + s_pre[0][t] + (t >= 32 ? s_half[0] : 0);
 		if(lane == 0) {
 			const int x = a.old_keys[3 * b], y = a.old_keys[3 * b + 1], z = a.old_keys[3 * b + 2];
@@ -401,15 +460,15 @@ __global__ void __launch_bounds__(kRebuildThreads, 2) rebuild_kernel(const Rebui
 			a.new_table[table_offset(cfg, x, y, z)] = nb;
 		}
 		for(int m = 0; m < nm; ++m) {
-			if(s_tot[m][t] == 0) {  // nothing to flatten
-				if(lane == 0) {
-					a.dst_sizes[m][nb] = 0;
-					a.bin_offsets[m][nb] = tp[1 + m] + s_pre[1 + m][t] + (t >= 32 ? s_half[1 + m] : 0);
-				}
-				continue;
+			int total = 0;
+			if(s_tot[m][t] != 0) {  // (j, m) is the pair whose counts were requested
+				const int2 row = next_row;
+				if(++nmod == nm) nmod = 0, ++nj;
+				advance(nj, nmod);
+				if(nj < PER_WARP) next_row = count_row(nj, nmod);
+				total = warp_flatten_block(cfg, row, a.cellbuckets[m] + ((size_t) b << cfg.ppb_shift), a.dst_buckets[m] + ((size_t) nb << cfg.ppb_shift),
+				                           a.dst_offs[m] ? a.dst_offs[m] + (size_t) nb * kBlockVol : nullptr);
 			}
-			const int total = warp_flatten_block(cfg, a.cell_counts[m] + (size_t) b * kBlockVol, a.cellbuckets[m] + ((size_t) b << cfg.ppb_shift), a.dst_buckets[m] + ((size_t) nb << cfg.ppb_shift),
-			                                     a.dst_offs[m] ? a.dst_offs[m] + (size_t) nb * kBlockVol : nullptr);
 			if(lane == 0) {
 				a.dst_sizes[m][nb] = total;
 				a.bin_offsets[m][nb] = tp[1 + m] + s_pre[1 + m][t] + (t >= 32 ? s_half[1 + m] : 0);

@@ -441,6 +441,9 @@ CB200_API int cb200_sim_add_particles_sdf(cb200_sim* sim, int model, const cb200
  * ---------------------------------------------------------------------------------------------- */
 CB200_API int cb200_test_svd3(int n, const float* F, float* U, float* S, float* V, void* stream);
 CB200_API int cb200_test_stress(int material, int mode, cb200_particle_buffer params, int n, const float* F_in, const float* log_jp_in, float* F_out, float* PF_out, float* log_jp_out, void* stream);
+/* The step driver's bucket flatten (the rebuild's warp-per-block copy) on caller-supplied DEVICE containers of `block_count` blocks, in place
+ * of cb200_cell_bucket_to_block: sizes are SET (not added to), and cell_offsets[64 * block_count] receives every cell's start in its bucket. */
+CB200_API int cb200_test_warp_flatten(const cb200_config* cfg, int block_count, const int* cell_particle_counts, const int* cellbuckets, int* particle_bucket_sizes, int* buckets, unsigned short* cell_offsets, void* stream);
 /* ParticleBuffer<M> default parameters (particle_buffer.cuh:141-264) for `material` on the grid of `cfg` (pointers zero) */
 CB200_API void cb200_default_material(const cb200_config* cfg, int material, cb200_particle_buffer* out);
 
