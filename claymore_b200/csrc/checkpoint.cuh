@@ -1,11 +1,13 @@
 // checkpoint.cuh -- portable checkpoint of a running simulation (layout: include/claymore_b200.h, "Checkpoint / restore").
 //   * the one parser of the blob format (host only: cb200_checkpoint_inspect and cb200_sim_restore share it) and its writer;
+//   * the row gather every particle read-out shares, and its state rows (retrieve, particle_state);
 //   * the snapshot gather: every model's particles and the keyed grid blocks of grid[0] packed into a device staging blob in
 //     partition order, in one launch behind a scan of the per-block particle counts;
 //   * the restore kernels: saved state into the bins (array_to_buffer's traversal) and a keyed scatter of the saved grid blocks.
 #pragma once
 #include <algorithm>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -209,65 +211,108 @@ inline int ck_parse(const void* blob, size_t bytes, cb200_checkpoint_info* out) 
 	return 0;
 }
 
-// ---- device: snapshot -------------------------------------------------------------------------------------------------
-constexpr int kSnapThreads = 256;
-struct SnapshotArgs {
-	Cfg cfg;
-	const StepState* state;
+// ---- device: the row gather ---------------------------------------------------------------------------------------------------
+// Every read-out of particles (snapshot, frame output, retrieve / particle_state) walks the current partition's buckets with one
+// routine, so all of them emit rows in one order: particle blocks in partition order, then bucket order inside a block.
+constexpr int kGatherThreads = 256;
+
+// where the particles of every model are read from
+struct GatherSrc {
 	int n_models;
 	int material[kMaxModels];
 	PBuf cur[kMaxModels];          // the bins the particles live in
 	PBuf next[kMaxModels];         // the buckets of the current partition: advection tags into `cur`
 	const int* base[kMaxModels];   // [pbc + 1]: exclusive scan of next.particle_bucket_sizes (entry pbc: the model's count)
+	int cap[kMaxModels];           // rows the model's section of the destination holds (its particle count)
 	const int* keys;               // current partition
 	const int* prev_table;         // the partition the tags point into
-	const float* grid;             // grid[0]
-	unsigned char* out;            // staging blob (the header is written by the host)
 };
 
-// One particle block of one model: each warp takes 32 rows, gathers them through the tags into a shared tile (one row per lane,
-// the source reads coalesced along the bin lanes) and writes the tile's 32*C floats as one contiguous run.
-template<int C>
-__device__ __forceinline__ void snapshot_block(const Cfg& cfg, const PBuf cur, const PBuf nx, const int* __restrict__ base, const int* __restrict__ prev_table, int b, int kx, int ky, int kz, float* out, float* tile) {
-	constexpr int S = C | 1;  // odd row stride: the lanes' row writes fall on distinct banks
+// f(std::integral_constant<int, C>) with the material's channel count C as a compile-time value
+template<class F>
+__device__ __forceinline__ void with_channels(int material, F&& f) {
+	switch(material) {
+	case CB200_J_FLUID: f(std::integral_constant<int, 4>()); break;
+	case CB200_FIXED_COROTATED: f(std::integral_constant<int, 12>()); break;
+	default: f(std::integral_constant<int, 13>()); break;
+	}
+}
+
+// A state row: the first W of the C channels of a particle (the snapshot and particle_state: W = C, retrieve: W = 3)
+template<int C_, int W>
+struct StateRow {
+	static constexpr int C = C_;
+	__device__ __forceinline__ int words() const { return W; }
+	__device__ __forceinline__ void operator()(float* rec, const float* __restrict__ src) const {
+#pragma unroll
+		for(int c = 0; c < W; ++c) rec[c] = src ? __ldg(src + c * 32) : 0.f;
+	}
+};
+
+// One particle block b of model m: each warp takes 32 rows, resolves each tag to its slot in the bins (one row per lane, the source
+// reads coalesced along the bin lanes), has `row` fill the lane's row of a shared tile, and writes the tile's 32 rows of
+// row.words() words to `out` as one contiguous run, rows below the model's cap only.  `row` gets src == nullptr for a tag without a
+// source block: the partition lost that particle (error bit set by the sub-step) and its row is zeros.
+template<class Row, class T>
+__device__ __forceinline__ void gather_block(const Cfg& cfg, const GatherSrc& g, int m, int b, int kx, int ky, int kz, T* out, T* tile, const Row& row) {
+	const int W = row.words(), S = W | 1;  // odd row stride: the lanes' row writes fall on distinct banks
+	constexpr int binf = Row::C == 4 ? 128 : 512;
+	const PBuf cur = g.cur[m], nx = g.next[m];
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int cnt = nx.particle_bucket_sizes[b];
-	const long long row0 = base[b];
-	const int binf = C == 4 ? 128 : 512;
-	for(int c0 = warp * 32; c0 < cnt; c0 += kSnapThreads) {
+	const long long row0 = g.base[m][b];
+	for(int c0 = warp * 32; c0 < cnt; c0 += kGatherThreads) {
 		const int i = c0 + lane;
 		if(i < cnt) {
 			const int tag = __ldg(nx.blockbuckets + ((size_t) b << cfg.ppb_shift) + i);
 			const int dir = tag >> cfg.ppb_shift, sp = tag & (cfg.ppb - 1);
-			const int sno = table_query(cfg, prev_table, kx + dir / 9 - 1, ky + (dir / 3) % 3 - 1, kz + dir % 3 - 1);
-			if(sno >= 0) {
-				const float* src = cur.bins + ((size_t) __ldg(cur.bin_offsets + sno) + (sp >> 5)) * binf + (sp & 31);
-#pragma unroll
-				for(int c = 0; c < C; ++c) tile[lane * S + c] = __ldg(src + c * 32);
-			} else {  // a tag without a source block: the partition lost this particle (error bit set by the sub-step)
-#pragma unroll
-				for(int c = 0; c < C; ++c) tile[lane * S + c] = 0.f;
-			}
+			const int sno = table_query(cfg, g.prev_table, kx + dir / 9 - 1, ky + (dir / 3) % 3 - 1, kz + dir % 3 - 1);
+			row(tile + lane * S, sno >= 0 ? cur.bins + ((size_t) __ldg(cur.bin_offsets + sno) + (sp >> 5)) * binf + (sp & 31) : nullptr);
 		}
 		__syncwarp();
-		const int rows = min(32, cnt - c0);
-		float* dst = out + (size_t) (row0 + c0) * C;
-		for(int j = lane; j < rows * C; j += 32) dst[j] = tile[(j / C) * S + j % C];
+		const int rows = min(min(32, cnt - c0), g.cap[m] - (int) (row0 + c0));
+		T* dst = out + (size_t) (row0 + c0) * W;
+		for(int j = lane; j < rows * W; j += 32) dst[j] = tile[(j / W) * S + j % W];
 		__syncwarp();
 	}
 }
 
+// One model's state rows, the first 3 channels of each (positions) or all of them, for retrieve and particle_state
+template<bool kPositions>
+__global__ void __launch_bounds__(kGatherThreads) state_rows_kernel(const Cfg cfg, const StepState* state, const GatherSrc g, int m, float* out) {
+	__shared__ float s_tile[kGatherThreads / 32][32 * (kPositions ? 3 : 13)];
+	const int pbc = state->pbc;
+	float* tile = s_tile[threadIdx.x >> 5];
+	for(int u = blockIdx.x; u < pbc; u += gridDim.x) {
+		const int kx = g.keys[3 * u], ky = g.keys[3 * u + 1], kz = g.keys[3 * u + 2];
+		with_channels(g.material[m], [&](auto c) {
+			constexpr int C = decltype(c)::value;
+			gather_block(cfg, g, m, u, kx, ky, kz, out, tile, StateRow<C, kPositions ? 3 : C>());
+		});
+	}
+}
+
+// ---- device: snapshot -------------------------------------------------------------------------------------------------
+struct SnapshotArgs {
+	Cfg cfg;
+	const StepState* state;
+	GatherSrc src;
+	const float* grid;             // grid[0]
+	unsigned char* out;            // staging blob (the header is written by the host)
+};
+
 // One launch: units [0, pbc) are particle blocks (all models of the block), units [pbc, pbc + ceil(nbc / 8)) eight grid blocks each
 // (a warp per block: its key and its 1 KiB as float4).
-__global__ void __launch_bounds__(kSnapThreads) snapshot_kernel(const SnapshotArgs a) {
-	__shared__ float s_tile[kSnapThreads / 32][32 * 13];
+__global__ void __launch_bounds__(kGatherThreads) snapshot_kernel(const SnapshotArgs a) {
+	__shared__ float s_tile[kGatherThreads / 32][32 * 13];
 	__shared__ unsigned long long s_off[kMaxModels + 2];
+	const GatherSrc& g = a.src;
 	const int pbc = a.state->pbc, nbc = a.state->nbc;
 	if(threadIdx.x == 0) {  // ck_layout's walk, one section at a time (no local arrays)
 		unsigned long long o = kCkHeader;
-		for(int m = 0; m < a.n_models; ++m) {
+		for(int m = 0; m < g.n_models; ++m) {
 			s_off[m] = o;
-			o = ck_align(o + (unsigned long long) a.base[m][pbc] * ck_channels(a.material[m]) * sizeof(float));
+			o = ck_align(o + (unsigned long long) g.base[m][pbc] * ck_channels(g.material[m]) * sizeof(float));
 		}
 		s_off[kMaxModels] = o;
 		s_off[kMaxModels + 1] = ck_align(o + (unsigned long long) nbc * 3 * sizeof(int));
@@ -278,20 +323,19 @@ __global__ void __launch_bounds__(kSnapThreads) snapshot_kernel(const SnapshotAr
 	const int units = pbc + (nbc + 7) / 8;
 	for(int u = blockIdx.x; u < units; u += gridDim.x) {
 		if(u < pbc) {
-			const int kx = a.keys[3 * u], ky = a.keys[3 * u + 1], kz = a.keys[3 * u + 2];
-			for(int m = 0; m < a.n_models; ++m) {
+			const int kx = g.keys[3 * u], ky = g.keys[3 * u + 1], kz = g.keys[3 * u + 2];
+			for(int m = 0; m < g.n_models; ++m) {
 				float* out = reinterpret_cast<float*>(a.out + s_off[m]);
-				switch(a.material[m]) {
-				case CB200_J_FLUID: snapshot_block<4>(a.cfg, a.cur[m], a.next[m], a.base[m], a.prev_table, u, kx, ky, kz, out, tile); break;
-				case CB200_FIXED_COROTATED: snapshot_block<12>(a.cfg, a.cur[m], a.next[m], a.base[m], a.prev_table, u, kx, ky, kz, out, tile); break;
-				default: snapshot_block<13>(a.cfg, a.cur[m], a.next[m], a.base[m], a.prev_table, u, kx, ky, kz, out, tile); break;
-				}
+				with_channels(g.material[m], [&](auto c) {
+					constexpr int C = decltype(c)::value;
+					gather_block(a.cfg, g, m, u, kx, ky, kz, out, tile, StateRow<C, C>());
+				});
 			}
 		} else {
 			const int b = (u - pbc) * 8 + warp;
 			if(b < nbc) {
 				int* keys = reinterpret_cast<int*>(a.out + s_off[kMaxModels]);
-				if(lane < 3) keys[3 * b + lane] = a.keys[3 * b + lane];
+				if(lane < 3) keys[3 * b + lane] = g.keys[3 * b + lane];
 				const float4* s = reinterpret_cast<const float4*>(a.grid + (size_t) b * kGridBlockFloats);
 				float4* d = reinterpret_cast<float4*>(a.out + s_off[kMaxModels + 1]) + (size_t) b * (kGridBlockFloats / 4);
 				d[lane] = s[lane];

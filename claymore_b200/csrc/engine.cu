@@ -158,6 +158,57 @@ PinnedStates g_pinned;
 template<typename T>
 cudaError_t pool_alloc(T** p, size_t bytes) { return g_pool.alloc(reinterpret_cast<void**>(p), bytes); }
 
+// Where a read-out lands before the host has it: a device buffer from the pool and its pinned host mirror, grown on demand (contents
+// are not kept) and reused; with open_stream(), a stream of its own for the device->host copy and the event that marks the copy done.
+// `pending`: a copy was queued on that stream and nobody has waited for it yet.
+struct Staging {
+	unsigned char* dev = nullptr;
+	unsigned char* host = nullptr;  // pinned
+	size_t dev_bytes = 0, host_bytes = 0;
+	cudaStream_t stream = nullptr;
+	cudaEvent_t copied = nullptr;
+	bool pending = false;
+
+	// at least `bytes` on the device and, with `mirror`, in the pinned mirror (a copy into caller memory needs none)
+	int grow(size_t bytes, bool mirror) {
+		if(dev_bytes < bytes) {
+			g_pool.release(dev);
+			dev = nullptr;
+			dev_bytes = 0;
+			CK(pool_alloc(&dev, bytes));
+			dev_bytes = bytes;
+		}
+		if(mirror && host_bytes < bytes) {
+			if(host) cudaFreeHost(host);
+			host = nullptr;
+			host_bytes = 0;
+			CK(cudaMallocHost(&host, bytes));
+			host_bytes = bytes;
+		}
+		return 0;
+	}
+	int open_stream() {
+		if(stream) return 0;
+		CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+		return (int) cudaEventCreateWithFlags(&copied, cudaEventDisableTiming);
+	}
+	int wait() {
+		if(!pending) return 0;
+		CK(cudaEventSynchronize(copied));
+		pending = false;
+		return 0;
+	}
+	// after every copy on the stream has finished
+	void release() {
+		if(stream) cudaStreamSynchronize(stream);
+		g_pool.release(dev);
+		if(host) cudaFreeHost(host);
+		if(copied) cudaEventDestroy(copied);
+		if(stream) cudaStreamDestroy(stream);
+		*this = Staging {};
+	}
+};
+
 struct Model {
 	int material = 0;
 	cb200_particle_buffer pb[2];
@@ -167,10 +218,7 @@ struct Model {
 	float v0[3] = {0, 0, 0};
 	int* bin_sizes = nullptr;
 	unsigned short* celloffs[2] = {nullptr, nullptr};  // per buffer: start of every cell inside the (cell-major) block bucket, [blocks][64]
-	// output staging (retrieve): device buffer + pinned host mirror, grown on demand, reused across frames
-	float* d_out = nullptr;
-	float* h_out = nullptr;
-	size_t out_floats = 0;
+	Staging out;  // retrieve and particle_state
 };
 // capacity rule of init_model (gmpm_simulator.cuh:173): n/32 bins + one partial bin per block
 inline long long bin_rows(long long n, long long max_blocks) { return n / kBinCap + max_blocks; }
@@ -179,11 +227,11 @@ inline long long bin_rows(long long n, long long max_blocks) { return n / kBinCa
 struct DeviceScratch {
 	int new_pbc;         // particle blocks of the rebuilt partition (summary_kernel)
 	int new_nbc;         // neighbour blocks, snapshotted by the last CTA of their registration; MGSP: the exchange's key count
-	int retrieve_count;  // particles written by retrieve_kernel
 	float local_max;     // MGSP: this rank's max |v|^2 of the new grid
 	float global_max;    // MGSP: the max over the ranks
 	float mgsp_grid_max; // MGSP: the grid update's max |v|^2, never read (the exchange agreed on the max already)
 	int missing;         // saved grid blocks scatter_grid_kernel found no block for
+	int model_count[kMaxModels];  // each model's particle count, from its last bucket scan (enqueue_bucket_scan)
 };
 // MGSP: the last-CTA counters and the exchange epochs (MgspView::done / ::epochs)
 struct MgspCounters {
@@ -265,32 +313,19 @@ struct cb200_sim {
 	ColliderView collider {};
 	float* sdf = nullptr;
 	long long frames_done = 0;  // frames finished by cb200_sim_advance_frame (restored from a checkpoint)
-	// checkpoint (cb200_sim_checkpoint_begin / _end): device staging blob, per-model scans of the bucket sizes, pinned copy of the
-	// blob written on a stream of its own; allocated on first use, grown with the block capacity
-	unsigned char* ck_dev = nullptr;
-	size_t ck_dev_bytes = 0;
-	int* ck_base = nullptr;  // [kMaxModels][max_blocks + 1]
-	size_t ck_base_bytes = 0;
-	unsigned char* ck_host = nullptr;  // pinned
-	size_t ck_host_bytes = 0;
-	cudaStream_t ck_stream = nullptr;
-	cudaEvent_t ck_gathered = nullptr, ck_copied = nullptr;
-	bool ck_pending = false;  // a copy was queued and end has not collected it
-	bool ck_ready = false;    // ck_host holds a complete blob of ck_bytes
-	size_t ck_bytes = 0;
+	// the rows each particle block starts at in every read-out, per model: the scans of the bucket sizes, [kMaxModels][max_blocks + 1]
+	int* ck_base = nullptr;
+	// checkpoint (cb200_sim_checkpoint_begin / _end): the blob, copied to the host on the staging's own stream
+	Staging ck;
+	size_t ck_bytes = 0;  // bytes of the blob the last begin queued (0: none)
 	// cb200_sim_restore_models: the checkpoint's header and its state staged on the device, consumed by initial_setup
 	bool restore_pending = false;
 	cb200_checkpoint_info restore_info {};
 	float* restore_state[kMaxModels] = {};
 	unsigned char* restore_grid = nullptr;  // grid blocks, then keys
-	// frame output (cb200_sim_frame_output): device staging of the records, its pinned copy (written on a stream of its own), and the
-	// writer thread with its one job; allocated / started on first use.  `out_busy`: a frame is queued or being written
-	unsigned char* out_dev = nullptr;
-	size_t out_dev_bytes = 0;
-	unsigned char* out_host = nullptr;  // pinned
-	size_t out_host_bytes = 0;
-	cudaStream_t out_stream = nullptr;
-	cudaEvent_t out_copied = nullptr;
+	// frame output (cb200_sim_frame_output): the records, copied to the host on the staging's own stream, and the writer thread with
+	// its one job, which waits for that copy; started on first use.  `out_busy`: a frame is queued or being written
+	Staging out;
 	std::thread out_thread;
 	std::mutex out_mu;
 	std::condition_variable out_cv;
@@ -348,7 +383,8 @@ DevArrays partition_arrays(const cb200_sim* s, cb200_partition& p, size_t mb) {
 	        dev_array(p.halo_marks, mb + 1, 0),
 	        dev_array(p.overlap_marks, mb + 1, 0)};
 }
-// the simulator's own: step state, scratch, both grids and the rebuild's scratch (produced and consumed inside a sub-step)
+// the simulator's own: step state, scratch, both grids, the rebuild's scratch (produced and consumed inside a sub-step) and the
+// read-outs' scans (produced and consumed inside a read-out)
 DevArrays sim_arrays(cb200_sim* s, size_t mb) {
 	const size_t tiles = (mb + kRebuildTile - 1) / kRebuildTile + 1;
 	return {dev_array(s->d_state, 1, 0),
@@ -356,7 +392,8 @@ DevArrays sim_arrays(cb200_sim* s, size_t mb) {
 	        dev_array(s->grid[0], (mb + 1) * kGridBlockFloats, 0),
 	        dev_array(s->grid[1], (mb + 1) * kGridBlockFloats, 0),
 	        dev_array(s->tile_sums, tiles * kScanComps, kNoFill),
-	        dev_array(s->block_totals, (size_t) kMaxModels * mb, kNoFill)};
+	        dev_array(s->block_totals, (size_t) kMaxModels * mb, kNoFill),
+	        dev_array(s->ck_base, (size_t) kMaxModels * (mb + 1), kNoFill)};
 }
 
 int fill_arrays(cb200_sim* s, const DevArrays& a) {
@@ -740,7 +777,6 @@ void preload_kernels() {
 	preload(rasterize_kernel);
 	preload(rasterize_blocks_kernel);
 	preload(init_adv_bucket_kernel);
-	preload(retrieve_kernel);
 	preload(collect_halo_blockids_kernel);
 	preload(mgsp_allreduce_maxvel_kernel);
 	preload(mgsp_pack_send_kernel);
@@ -757,6 +793,8 @@ void preload_kernels() {
 	preload(state_to_bins_kernel);
 	preload(scatter_grid_kernel);
 	preload(output_kernel);
+	preload(state_rows_kernel<true>);
+	preload(state_rows_kernel<false>);
 	g2p2g_prepare_all();
 }
 int ensure_graph(cb200_sim* s, int R) {
@@ -812,7 +850,7 @@ void output_writer(cb200_sim* s) {
 		std::vector<cb200_sim::OutputFile> files;
 		files.swap(s->out_files);
 		lk.unlock();
-		const bool copied = cudaEventSynchronize(s->out_copied) == cudaSuccess;  // (failed: nothing of this frame is written)
+		const bool copied = cudaEventSynchronize(s->out.copied) == cudaSuccess;  // (failed: nothing of this frame is written)
 		int e = copied ? 0 : EIO;
 		for(size_t i = 0; copied && i < files.size(); ++i) {
 			const int fe = write_bgeo(files[i]);
@@ -849,7 +887,7 @@ int cb200_sim_reserve(cb200_sim* s, int new_max_blocks) {
 	if(new_max_blocks <= s->desc.max_blocks) return 0;
 	if(s->desc.mgsp_world > 1) return (int) cudaErrorNotSupported;  // the next grid / inbox are mapped into the peers (CUDA IPC)
 	CK(cudaStreamSynchronize(s->stream));
-	if(s->ck_pending) CK(cudaEventSynchronize(s->ck_copied));  // the next begin re-sizes the staging blob
+	CK(s->ck.wait());  // the next begin re-sizes the staging blob
 	output_idle(s);
 	const size_t ob = (size_t) s->desc.max_blocks, nb = (size_t) new_max_blocks;
 	drop_graphs(s);
@@ -948,19 +986,10 @@ int cb200_sim_destroy(cb200_sim* s) {
 		s->out_cv.notify_all();
 		s->out_thread.join();
 	}
-	g_pool.release(s->out_dev);
-	if(s->out_host) cudaFreeHost(s->out_host);
-	if(s->out_copied) cudaEventDestroy(s->out_copied);
-	if(s->out_stream) cudaStreamDestroy(s->out_stream);
-	if(s->ck_stream) cudaStreamSynchronize(s->ck_stream);  // a checkpoint copy may still read the staging blob
-	g_pool.release(s->ck_dev);
-	g_pool.release(s->ck_base);
+	s->out.release();
+	s->ck.release();  // (a checkpoint copy may still read the staging blob: release waits for it)
 	for(float* p : s->restore_state) g_pool.release(p);
 	g_pool.release(s->restore_grid);
-	if(s->ck_host) cudaFreeHost(s->ck_host);
-	if(s->ck_gathered) cudaEventDestroy(s->ck_gathered);
-	if(s->ck_copied) cudaEventDestroy(s->ck_copied);
-	if(s->ck_stream) cudaStreamDestroy(s->ck_stream);
 	for(auto& ev : s->prof_events) {
 		cudaEventDestroy(ev.first);
 		cudaEventDestroy(ev.second);
@@ -970,8 +999,7 @@ int cb200_sim_destroy(cb200_sim* s) {
 	for(cb200_partition& p : s->part) free_arrays(partition_arrays(s, p, mb));
 	for(Model& m : s->models) {
 		free_arrays(model_arrays(s, m, mb, m.bin_capacity));
-		g_pool.release(m.d_out);
-		cudaFreeHost(m.h_out);
+		m.out.release();
 	}
 	free_arrays(sim_arrays(s, mb));
 	g_pool.release(s->peer_overlap_keys);
@@ -1360,45 +1388,6 @@ int cb200_sim_stats_get(cb200_sim* s, cb200_sim_stats* out) {
 	return 0;
 }
 
-// output_model (gmpm_simulator.cuh:594-634): particles -> flat array -> host.  The staging buffers persist (the reference borrows
-// and re-allocates per frame) and the device->host copy lands in pinned memory; `host` == nullptr returns the pinned mirror itself.
-static int retrieve_impl(cb200_sim* s, int model, float* host, int nch, int* n_out, const float** pinned_out) {
-	if(!s || !s->setup_done || model < 0 || model >= (int) s->models.size()) return (int) cudaErrorInvalidValue;
-	Model& m = s->models[model];
-	const int R = s->rollid, Rn = R ^ 1;
-	const size_t need = (size_t) m.n * nch;
-	if(m.out_floats < need) {
-		g_pool.release(m.d_out);
-		cudaFreeHost(m.h_out);
-		m.d_out = nullptr;
-		m.h_out = nullptr;
-		CK(pool_alloc(&m.d_out, need * sizeof(float)));
-		m.out_floats = need;
-	}
-	if(!host && !m.h_out) CK(cudaMallocHost(&m.h_out, m.out_floats * sizeof(float)));
-	float* dst = host ? host : m.h_out;  // caller memory (fast when it is pinned) or the simulator's pinned mirror
-	int* parcount = &s->scr->retrieve_count;
-	CK(cudaMemsetAsync(parcount, 0, sizeof(int), s->stream));
-	retrieve_kernel<<<num_sms() * 8, 128, 0, s->stream>>>(s->cfg, m.material, count_dev(&s->d_state->pbc), s->part[R].active_keys, s->part[Rn].index_table, view(m.pb[R]), view(m.pb[Rn]), m.d_out, nch, parcount);
-	++s->launches;
-	// the count is only known on the device: copy the full staging buffer behind the kernel, read the count with it
-	CK(cudaMemcpyAsync(dst, m.d_out, need * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
-	int n = 0;
-	CK(cudaMemcpyAsync(&n, parcount, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-	CK(cudaStreamSynchronize(s->stream));
-	if(n > m.n) n = m.n;
-	if(pinned_out) *pinned_out = m.h_out;
-	if(n_out) *n_out = n;
-	return 0;
-}
-int cb200_sim_retrieve(cb200_sim* s, int model, float* positions_host, int* n_out) { return retrieve_impl(s, model, positions_host, 3, n_out, nullptr); }
-// zero-copy variant: *positions_pinned points at the simulator's pinned staging buffer (valid until the next retrieve of that model)
-int cb200_sim_retrieve_pinned(cb200_sim* s, int model, const float** positions_pinned, int* n_out) { return retrieve_impl(s, model, nullptr, 3, n_out, positions_pinned); }
-int cb200_sim_particle_state(cb200_sim* s, int model, float* state_host, int* n_out) {
-	if(!s || model < 0 || model >= (int) s->models.size()) return (int) cudaErrorInvalidValue;
-	return retrieve_impl(s, model, state_host, ck_channels(s->models[model].material), n_out, nullptr);
-}
-
 int cb200_sim_active_keys(cb200_sim* s, int* keys_host, int capacity_blocks, int* n_out) {
 	if(!s || !s->setup_done) return (int) cudaErrorInvalidValue;
 	CK(pull_state(s));
@@ -1481,34 +1470,45 @@ size_t ck_capacity(const cb200_sim* s) {
 	for(size_t m = 0; m < s->models.size(); ++m) counts[m] = s->models[m].n;
 	return (size_t) models_layout(s, counts, s->desc.max_blocks).total;
 }
-// grows a checkpoint buffer to `need` bytes (contents are not kept)
-template<typename T>
-int ck_grow(T*& p, size_t& have, size_t need) {
-	if(have >= need) return 0;
-	g_pool.release(p);
-	p = nullptr;
-	have = 0;
-	CK(pool_alloc(&p, need));
-	have = need;
-	return 0;
-}
-// the same for a pinned host buffer
-int pinned_grow(unsigned char*& p, size_t& have, size_t need) {
-	if(have >= need) return 0;
-	if(p) cudaFreeHost(p);
-	p = nullptr;
-	have = 0;
-	CK(cudaMallocHost(&p, need));
-	have = need;
-	return 0;
-}
 // model m's row of ck_base: the exclusive scan of its bucket sizes, entry pbc its particle count
 int* ck_row(const cb200_sim* s, int m) { return s->ck_base + (size_t) m * (s->desc.max_blocks + 1); }
-// every model's particle count, entry pbc of its scan, once the bucket scans have run (synchronises)
-int read_totals(cb200_sim* s, int pbc, long long* counts) {
+
+// The row each particle block of model m starts at in every read-out: an exclusive scan of the bucket sizes of the current
+// partition into ck_row (entry pbc and model_count[m]: the model's count), enqueued on the sim stream
+int enqueue_bucket_scan(cb200_sim* s, int m) {
+	ScanArgs sc {};
+	sc.count = count_dev(&s->d_state->pbc);
+	sc.count_plus = 1;
+	sc.in = s->models[m].pb[s->rollid ^ 1].particle_bucket_sizes;
+	sc.out = ck_row(s, m);
+	sc.total_out = &s->scr->model_count[m];
+	scan_kernel<<<1, 1024, 0, s->stream>>>(sc);
+	++s->launches;
+	return (int) cudaGetLastError();
+}
+// the current state's particles as the gathers read them, every model's rows placed by its bucket scan
+GatherSrc gather_src(const cb200_sim* s) {
+	const int R = s->rollid, Rn = R ^ 1;
+	GatherSrc g {};
+	g.n_models = (int) s->models.size();
+	for(int m = 0; m < g.n_models; ++m) {
+		const Model& md = s->models[m];
+		g.material[m] = md.material;
+		g.cur[m] = view(md.pb[R]);
+		g.next[m] = view(md.pb[Rn]);
+		g.base[m] = ck_row(s, m);
+		g.cap[m] = md.n;
+	}
+	g.keys = s->part[R].active_keys;
+	g.prev_table = s->part[Rn].index_table;
+	return g;
+}
+
+// every model's particle count from the bucket scans queued before (synchronises)
+int read_totals(cb200_sim* s, long long* counts) {
 	const int nm = (int) s->models.size();
 	int totals[kMaxModels] = {};
-	for(int m = 0; m < nm; ++m) CK(cudaMemcpyAsync(&totals[m], ck_row(s, m) + pbc, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+	CK(cudaMemcpyAsync(totals, s->scr->model_count, nm * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
 	CK(cudaStreamSynchronize(s->stream));
 	for(int m = 0; m < nm; ++m) {
 		if(totals[m] < 0 || totals[m] > s->models[m].n) return (int) cudaErrorIllegalState;
@@ -1516,73 +1516,71 @@ int read_totals(cb200_sim* s, int pbc, long long* counts) {
 	}
 	return 0;
 }
+
+// A read-out of every model (the checkpoint's and the emission's snapshot_kernel, the frame's output_kernel): the bucket scans and the
+// gather `kernel` over `a` (its cfg, state and src filled in here) on the sim stream, then the step state and every model's count.
+// The host has waited for the gather when this returns, so a copy of its staging queued on another stream needs no event behind it.
+template<class Args>
+int read_out(cb200_sim* s, void (*kernel)(Args), Args a, long long* counts) {
+	for(int m = 0; m < (int) s->models.size(); ++m) CK(enqueue_bucket_scan(s, m));
+	a.cfg = s->cfg;
+	a.state = s->d_state;
+	a.src = gather_src(s);
+	kernel<<<num_sms() * 8, kGatherThreads, 0, s->stream>>>(a);
+	++s->launches;
+	CK(cudaGetLastError());
+	CK(pull_state(s));
+	return read_totals(s, counts);
+}
+
+// output_model (gmpm_simulator.cuh:594-634): one model's rows -> host, in the order of the checkpoint's section of that model.  The
+// staging persists (the reference borrows and re-allocates per frame) and the device->host copy lands in pinned memory; `host` ==
+// nullptr returns the pinned mirror itself.
+int retrieve_impl(cb200_sim* s, int model, float* host, bool positions, int* n_out, const float** pinned_out) {
+	if(!s || !s->setup_done || model < 0 || model >= (int) s->models.size()) return (int) cudaErrorInvalidValue;
+	Model& m = s->models[model];
+	const size_t bytes = (size_t) m.n * (positions ? 3 : ck_channels(m.material)) * sizeof(float);
+	CK(m.out.grow(bytes, !host));
+	CK(enqueue_bucket_scan(s, model));
+	float* out = reinterpret_cast<float*>(m.out.dev);
+	if(positions)
+		state_rows_kernel<true><<<num_sms() * 8, kGatherThreads, 0, s->stream>>>(s->cfg, s->d_state, gather_src(s), model, out);
+	else
+		state_rows_kernel<false><<<num_sms() * 8, kGatherThreads, 0, s->stream>>>(s->cfg, s->d_state, gather_src(s), model, out);
+	++s->launches;
+	CK(cudaGetLastError());
+	// the count is only known on the device: copy the full staging buffer behind the kernel, read the count with it
+	CK(cudaMemcpyAsync(host ? (void*) host : m.out.host, m.out.dev, bytes, cudaMemcpyDeviceToHost, s->stream));
+	int n = 0;
+	CK(cudaMemcpyAsync(&n, &s->scr->model_count[model], sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+	CK(cudaStreamSynchronize(s->stream));
+	if(n > m.n) n = m.n;
+	if(pinned_out) *pinned_out = reinterpret_cast<const float*>(m.out.host);
+	if(n_out) *n_out = n;
+	return 0;
+}
 }  // namespace
 extern "C" {
 
-// The row each particle block starts at in the checkpoint's order, per model: an exclusive scan of the bucket sizes of the current
-// partition into ck_base (entry pbc: the model's count), enqueued on the sim stream.  Shared by the checkpoint and the frame output,
-// which both wait for their gather before returning.
-static int enqueue_bucket_scans(cb200_sim* s) {
-	CK(ck_grow(s->ck_base, s->ck_base_bytes, (size_t) kMaxModels * (s->desc.max_blocks + 1) * sizeof(int)));
-	const int Rn = s->rollid ^ 1;
-	for(size_t m = 0; m < s->models.size(); ++m) {
-		ScanArgs sc {};
-		sc.count = count_dev(&s->d_state->pbc);
-		sc.count_plus = 1;
-		sc.in = s->models[m].pb[Rn].particle_bucket_sizes;
-		sc.out = ck_row(s, (int) m);
-		scan_kernel<<<1, 1024, 0, s->stream>>>(sc);
-		++s->launches;
-	}
-	return 0;
-}
-
-// The snapshot gather of the current state into `out` (a blob of ck_capacity bytes, header left to the caller), behind the bucket
-// scans, on the sim stream.  Shared by the checkpoint and the emission, which rebuilds the simulator from it.
-static int enqueue_snapshot(cb200_sim* s, unsigned char* out) {
-	const int R = s->rollid, Rn = R ^ 1;
-	const int nm = (int) s->models.size();
-	CK(enqueue_bucket_scans(s));
-	SnapshotArgs a {};
-	a.cfg = s->cfg;
-	a.state = s->d_state;
-	a.n_models = nm;
-	for(int m = 0; m < nm; ++m) {
-		const Model& md = s->models[m];
-		a.material[m] = md.material;
-		a.cur[m] = view(md.pb[R]);
-		a.next[m] = view(md.pb[Rn]);
-		a.base[m] = ck_row(s, m);
-	}
-	a.keys = s->part[R].active_keys;
-	a.prev_table = s->part[Rn].index_table;
-	a.grid = s->grid[0];
-	a.out = out;
-	snapshot_kernel<<<num_sms() * 8, kSnapThreads, 0, s->stream>>>(a);
-	++s->launches;
-	return (int) cudaGetLastError();
-}
+int cb200_sim_retrieve(cb200_sim* s, int model, float* positions_host, int* n_out) { return retrieve_impl(s, model, positions_host, true, n_out, nullptr); }
+// zero-copy variant: *positions_pinned points at the simulator's pinned staging buffer (valid until the next retrieve of that model)
+int cb200_sim_retrieve_pinned(cb200_sim* s, int model, const float** positions_pinned, int* n_out) { return retrieve_impl(s, model, nullptr, true, n_out, positions_pinned); }
+int cb200_sim_particle_state(cb200_sim* s, int model, float* state_host, int* n_out) { return retrieve_impl(s, model, state_host, false, n_out, nullptr); }
 
 int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	if(!s || !s->setup_done) return (int) cudaErrorInvalidValue;
-	if(s->ck_pending) CK(cudaEventSynchronize(s->ck_copied));  // the pinned blob and the staging blob are re-used
-	s->ck_pending = s->ck_ready = false;
-	if(!s->ck_stream) {
-		CK(cudaStreamCreateWithFlags(&s->ck_stream, cudaStreamNonBlocking));
-		CK(cudaEventCreateWithFlags(&s->ck_gathered, cudaEventDisableTiming));
-		CK(cudaEventCreateWithFlags(&s->ck_copied, cudaEventDisableTiming));
-	}
-	const size_t cap = ck_capacity(s);
-	CK(ck_grow(s->ck_dev, s->ck_dev_bytes, cap));
-	CK(pinned_grow(s->ck_host, s->ck_host_bytes, cap));
-	CK(enqueue_snapshot(s, s->ck_dev));
-	CK(cudaEventRecord(s->ck_gathered, s->stream));
+	CK(s->ck.wait());  // the pinned blob and the staging blob are re-used
+	s->ck_bytes = 0;
+	CK(s->ck.open_stream());
+	CK(s->ck.grow(ck_capacity(s), true));
 	// the counts the layout follows from: the step state (pbc, nbc, clock), then each model's total
-	const int nm = (int) s->models.size();
-	CK(pull_state(s));
-	const StepState& h = *s->h_state;
+	SnapshotArgs a {};
+	a.grid = s->grid[0];
+	a.out = s->ck.dev;
 	long long counts[kMaxModels];
-	CK(read_totals(s, h.pbc, counts));
+	CK(read_out(s, snapshot_kernel, a, counts));
+	const int nm = (int) s->models.size();
+	const StepState& h = *s->h_state;
 	const CkLayout L = models_layout(s, counts, h.nbc);
 	cb200_checkpoint_info I;
 	memset(&I, 0, sizeof(I));
@@ -1619,25 +1617,20 @@ int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 		md.bytes = L.model_bytes[m];
 		md.params = s->models[m].pb[0];  // (ck_write_header writes the parameters only)
 	}
-	ck_write_header(s->ck_host, I);
-	// the data sections: behind the snapshot, on the copy stream, so that sub-steps enqueued from here on run alongside
-	CK(cudaStreamWaitEvent(s->ck_stream, s->ck_gathered, 0));
-	CK(cudaMemcpyAsync(s->ck_host + kCkHeader, s->ck_dev + kCkHeader, L.total - kCkHeader, cudaMemcpyDeviceToHost, s->ck_stream));
-	CK(cudaEventRecord(s->ck_copied, s->ck_stream));
+	ck_write_header(s->ck.host, I);
+	// the data sections: on the copy stream (the snapshot has finished), so that sub-steps enqueued from here on run alongside
+	CK(cudaMemcpyAsync(s->ck.host + kCkHeader, s->ck.dev + kCkHeader, L.total - kCkHeader, cudaMemcpyDeviceToHost, s->ck.stream));
+	CK(cudaEventRecord(s->ck.copied, s->ck.stream));
+	s->ck.pending = true;
 	s->ck_bytes = L.total;
-	s->ck_pending = true;
 	if(bytes) *bytes = L.total;
 	return 0;
 }
 
 int cb200_sim_checkpoint_end(cb200_sim* s, const void** blob, size_t* bytes) {
-	if(!s || (!s->ck_pending && !s->ck_ready)) return (int) cudaErrorInvalidValue;
-	if(s->ck_pending) {
-		CK(cudaEventSynchronize(s->ck_copied));
-		s->ck_pending = false;
-		s->ck_ready = true;
-	}
-	if(blob) *blob = s->ck_host;
+	if(!s || !s->ck_bytes) return (int) cudaErrorInvalidValue;
+	CK(s->ck.wait());
+	if(blob) *blob = s->ck.host;
 	if(bytes) *bytes = s->ck_bytes;
 	return 0;
 }
@@ -1709,55 +1702,31 @@ int cb200_sim_frame_output(cb200_sim* s, const char* const* paths, unsigned attr
 		std::lock_guard<std::mutex> g(s->out_mu);
 		if(s->out_errno) return CB200_ERROR_OUTPUT_IO;  // an earlier frame failed: report it before writing more
 	}
-	if(!s->out_stream) {
-		CK(cudaStreamCreateWithFlags(&s->out_stream, cudaStreamNonBlocking));
-		CK(cudaEventCreateWithFlags(&s->out_copied, cudaEventDisableTiming));
-	}
+	CK(s->out.open_stream());
 	const int W = out_words(attributes);
 	OutputArgs a {};
 	size_t need = 0;
 	for(int m = 0; m < nm; ++m) {  // a section per model, sized for all its particles
 		a.off[m] = need;
-		a.cap[m] = s->models[m].n;
 		need += (size_t) s->models[m].n * W * sizeof(float);
 	}
-	CK(ck_grow(s->out_dev, s->out_dev_bytes, need));
-	CK(pinned_grow(s->out_host, s->out_host_bytes, need));
-	const int R = s->rollid, Rn = R ^ 1;
-	CK(enqueue_bucket_scans(s));
-	a.cfg = s->cfg;
-	a.state = s->d_state;
-	a.n_models = nm;
+	CK(s->out.grow(need, true));
 	a.attrs = attributes;
-	for(int m = 0; m < nm; ++m) {
-		const Model& md = s->models[m];
-		a.material[m] = md.material;
-		a.cur[m] = view(md.pb[R]);
-		a.next[m] = view(md.pb[Rn]);
-		a.base[m] = ck_row(s, m);
-	}
-	a.keys = s->part[R].active_keys;
-	a.table = s->part[R].index_table;
-	a.prev_table = s->part[Rn].index_table;
+	a.table = s->part[s->rollid].index_table;
 	a.grid = s->grid[0];
-	a.out = s->out_dev;
-	output_kernel<<<num_sms() * 8, kOutThreads, 0, s->stream>>>(a);
-	++s->launches;
-	CK(cudaGetLastError());
+	a.out = s->out.dev;
 	// the counts the headers need (each model's total): this is the only wait, and it ends with the gather
-	CK(pull_state(s));
 	long long totals[kMaxModels];
-	CK(read_totals(s, s->h_state->pbc, totals));
+	CK(read_out(s, output_kernel, a, totals));
 	std::vector<cb200_sim::OutputFile> files((size_t) nm);
 	for(int m = 0; m < nm; ++m) {
 		files[m].path = paths[m];
 		files[m].header = bgeo_header(totals[m], attributes);
-		files[m].body = s->out_host + a.off[m];
+		files[m].body = s->out.host + a.off[m];
 		files[m].body_bytes = (size_t) totals[m] * W * sizeof(float);
-		// the gather has finished (the host waited for it above): the copy needs no event to order it behind the kernel
-		if(files[m].body_bytes) CK(cudaMemcpyAsync(s->out_host + a.off[m], s->out_dev + a.off[m], files[m].body_bytes, cudaMemcpyDeviceToHost, s->out_stream));
+		if(files[m].body_bytes) CK(cudaMemcpyAsync(s->out.host + a.off[m], s->out.dev + a.off[m], files[m].body_bytes, cudaMemcpyDeviceToHost, s->out.stream));
 	}
-	CK(cudaEventRecord(s->out_copied, s->out_stream));
+	CK(cudaEventRecord(s->out.copied, s->out.stream));
 	if(!s->out_thread.joinable()) s->out_thread = std::thread(output_writer, s);
 	{
 		std::lock_guard<std::mutex> g(s->out_mu);
@@ -2049,9 +2018,11 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	}
 	// (5) gather the current state (checkpoint layout) and allocate what the commit swaps in: nothing live is written yet
 	CK(pool_alloc(&eb.blob, ck_capacity(s)));
-	CK(enqueue_snapshot(s, eb.blob));
+	SnapshotArgs sa {};
+	sa.grid = s->grid[0];
+	sa.out = eb.blob;
 	long long counts[kMaxModels];
-	CK(read_totals(s, h0.pbc, counts));
+	CK(read_out(s, snapshot_kernel, sa, counts));
 	const CkLayout L = models_layout(s, counts, h0.nbc);
 	Model& md = s->models[model];
 	const int C = ck_channels(md.material);

@@ -206,11 +206,14 @@ CB200_API int cb200_sim_reserve(cb200_sim* sim, int new_max_blocks);
 CB200_API int cb200_sim_check_capacity(cb200_sim* sim, int* grown);
 CB200_API int cb200_sim_capacity(cb200_sim* sim, int* max_blocks, int* grow_events);
 CB200_API int cb200_sim_stats_get(cb200_sim* sim, cb200_sim_stats* out); /* synchronises */
-/* output_model  gmpm_simulator.cuh:594-634: positions to HOST float[3*n]; returns count in *n_out */
+/* output_model  gmpm_simulator.cuh:594-634: positions to HOST float[3*n]; returns count in *n_out.  Rows in the order of a
+ * checkpoint of the same state (partition order, then bucket order), bit for bit the first three columns of its state rows
+ * and of cb200_sim_particle_state; two calls on an unchanged simulator return the same bytes */
 CB200_API int cb200_sim_retrieve(cb200_sim* sim, int model, float* positions_host, int* n_out);
 /* same, zero-copy: *positions_pinned is the simulator's pinned staging buffer, valid until the next retrieve of that model */
 CB200_API int cb200_sim_retrieve_pinned(cb200_sim* sim, int model, const float** positions_pinned, int* n_out);
-/* full particle state (all channels, [n][channels]) to HOST, same traversal as retrieve */
+/* full particle state (all channels, [n][channels]) to HOST: byte for byte the model's section of a checkpoint of the same
+ * state (a particle the partition lost is a row of zeros in both) */
 CB200_API int cb200_sim_particle_state(cb200_sim* sim, int model, float* state_host, int* n_out);
 /* copies for parity checks: active keys (int[3*ebc]) and grid blocks of grid[0] (float[256*nbc]) to HOST */
 CB200_API int cb200_sim_active_keys(cb200_sim* sim, int* keys_host, int capacity_blocks, int* n_out);
