@@ -263,7 +263,7 @@ int cb200_build_particle_cell_buckets(const cb200_config* c, int n, const float*
 int cb200_array_to_buffer(const cb200_config* c, int block_count, const float* positions, cb200_particle_buffer pb, void* stream) {
 	CB_CFG(c);
 	if(block_count <= 0) return 0;
-	array_to_buffer_kernel<<<grid_for(block_count, 1, 16), 128, 0, (cudaStream_t) stream>>>(cfg, pb.material, block_count, positions, view(pb));
+	array_to_buffer_kernel<<<grid_for(block_count, 1, 16), 128, 0, (cudaStream_t) stream>>>(cfg, pb.material, block_count, positions, nullptr, view(pb));
 	return (int) cudaGetLastError();
 }
 int cb200_rasterize(const cb200_config* c, int n, const float* positions, float* grid, cb200_partition p, float mass, const float* v0, void* stream) {

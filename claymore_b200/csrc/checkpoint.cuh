@@ -3,7 +3,8 @@
 //   * the row gather every particle read-out shares, and its state rows (retrieve, particle_state);
 //   * the snapshot gather: every model's particles and the keyed grid blocks of grid[0] packed into a device staging blob in
 //     partition order, in one launch behind a scan of the per-block particle counts;
-//   * the restore kernels: saved state into the bins (array_to_buffer's traversal) and a keyed scatter of the saved grid blocks.
+//   * the restore kernels: the positions of a saved state and a keyed scatter of the saved grid blocks (array_to_buffer_kernel,
+//     init.cuh, puts the saved rows into the bins).
 #pragma once
 #include <algorithm>
 #include <cstring>
@@ -20,9 +21,6 @@ constexpr size_t kCkAlign = 256;
 constexpr char kCkMagic[8] = {'C', 'B', '2', '0', '0', 'C', 'K', 'P'};
 static_assert(256 + kMaxModels * kCkTocEntry <= kCkHeader, "checkpoint table of contents must fit the header");
 
-__host__ __device__ inline int ck_channels(int material) { return material == CB200_J_FLUID ? 4 : (material == CB200_FIXED_COROTATED ? 12 : 13); }
-// floats of one bin of kBinCap particles (J_FLUID: 4 channels, the others: 16)
-inline size_t bin_floats(int material) { return material == CB200_J_FLUID ? 128 : 512; }
 __host__ __device__ inline unsigned long long ck_align(unsigned long long x) { return (x + kCkAlign - 1) & ~(unsigned long long) (kCkAlign - 1); }
 
 // Section offsets of the blob the snapshot writes, from the particle counts and nbc: the host writer of the header evaluates it
@@ -267,7 +265,7 @@ __device__ __forceinline__ void gather_block(const Cfg& cfg, const GatherSrc& g,
 			const int tag = __ldg(nx.blockbuckets + ((size_t) b << cfg.ppb_shift) + i);
 			const int dir = tag >> cfg.ppb_shift, sp = tag & (cfg.ppb - 1);
 			const int sno = table_query(cfg, g.prev_table, kx + dir / 9 - 1, ky + (dir / 3) % 3 - 1, kz + dir % 3 - 1);
-			row(tile + lane * S, sno >= 0 ? cur.bins + ((size_t) __ldg(cur.bin_offsets + sno) + (sp >> 5)) * binf + (sp & 31) : nullptr);
+			row(tile + lane * S, sno >= 0 ? bin_slot(cur.bins, __ldg(cur.bin_offsets + sno), sp, binf) : nullptr);
 		}
 		__syncwarp();
 		const int rows = min(min(32, cnt - c0), g.cap[m] - (int) (row0 + c0));
@@ -350,21 +348,6 @@ __global__ void __launch_bounds__(kGatherThreads) snapshot_kernel(const Snapshot
 __global__ void state_positions_kernel(long long n, int channels, const float* state, float* pos) {
 	for(long long p = blockIdx.x * (long long) blockDim.x + threadIdx.x; p < n; p += (long long) gridDim.x * blockDim.x)
 		for(int d = 0; d < 3; ++d) pos[3 * p + d] = state[p * channels + d];
-}
-
-// array_to_buffer's traversal (init.cuh), writing every saved channel of particle `pid` instead of the identity state
-__global__ void state_to_bins_kernel(Cfg cfg, int material, int block_count, const float* state, PBuf pb) {
-	const int binf = material == CB200_J_FLUID ? 128 : 512;
-	const int C = ck_channels(material);
-	for(int b = blockIdx.x; b < block_count; b += gridDim.x) {
-		const int n = pb.particle_bucket_sizes[b];
-		const int* bucket = pb.blockbuckets + ((size_t) b << cfg.ppb_shift);
-		for(int i = threadIdx.x; i < n; i += blockDim.x) {
-			const float* row = state + (size_t) bucket[i] * C;
-			float* bin = pb.bins + ((size_t) pb.bin_offsets[b] + (i >> 5)) * binf + (i & 31);
-			for(int c = 0; c < C; ++c) bin[c * 32] = row[c];
-		}
-	}
 }
 
 // keyed grid scatter: warp per saved block, table query, float4 copy.  A saved key without a block among the first `nbc` of the

@@ -119,6 +119,33 @@ struct StepState {
 enum : int { kErrBlockCapacity = 1, kErrBinCapacity = 2, kErrLostParticle = 4, kErrCellOverflow = 8, kErrHaloMap = 16 };
 
 // ------------------------------------------------------------------------------------------------
+// particle channels and bins
+// ------------------------------------------------------------------------------------------------
+// channels of a particle: the position, then J (J_FLUID) or F (9, row-major), then logJp (SAND, NACC)
+__host__ __device__ inline int ck_channels(int material) { return material == CB200_J_FLUID ? 4 : (material == CB200_FIXED_COROTATED ? 12 : 13); }
+// floats of one bin of kBinCap particles (J_FLUID: 4 channels, the others: 16)
+__host__ __device__ constexpr int bin_floats(int material) { return material == CB200_J_FLUID ? 128 : 512; }
+// particle i of the bucket whose bins start at bin `first`: its channel c is at [c * kBinCap]
+template<class T>
+__device__ __forceinline__ T* bin_slot(T* bins, int first, int i, int binf) { return bins + ((size_t) first + (i >> 5)) * binf + (i & 31); }
+
+// The start state of a particle at x (array_to_buffer, mgmpm_kernels.cuh:221-323), channel c to out[c * stride]: the position, then
+// J = 1 or F = I, then logJp = ParticleBuffer<M>::LOG_JP_0 (particle_buffer.cuh:207, 241)
+__device__ __forceinline__ void start_state(int material, const float* x, float* out, int stride) {
+	out[0] = x[0];
+	out[stride] = x[1];
+	out[2 * stride] = x[2];
+	if(material == CB200_J_FLUID) {
+		out[3 * stride] = 1.f;
+		return;
+	}
+#pragma unroll
+	for(int d = 0; d < 9; ++d) out[(3 + d) * stride] = (d % 4 == 0) ? 1.f : 0.f;
+	if(material == CB200_SAND) out[12 * stride] = 0.f;
+	if(material == CB200_NACC) out[12 * stride] = -0.01f;
+}
+
+// ------------------------------------------------------------------------------------------------
 // index helpers
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool in_domain(const Cfg& c, int x, int y, int z) { return ((unsigned) x < (unsigned) c.gsize) & ((unsigned) y < (unsigned) c.gsize) & ((unsigned) z < (unsigned) c.gsize); }

@@ -1,7 +1,7 @@
 // emit.cuh -- adding particles to a set-up simulator at a sub-step boundary (cb200_sim_add_particles*, include/claymore_b200.h).
 //   * the checks of the candidates and the empty-cell filter, read against the current partition's cell offsets;
 //   * the union's block counts and per-cell counts, built on a scratch table so that nothing live is touched before the commit;
-//   * the state rows of the new particles, in the checkpoint's layout, so the commit is the restore path of initial_setup.
+//   * the state rows of the new particles, in the checkpoint's layout, so the commit is initial_setup over saved rows.
 // One-time work per call, thread per candidate.
 #pragma once
 #include "checkpoint.cuh"
@@ -92,22 +92,10 @@ __global__ void emit_overflow_kernel(EmitCells c, int n, const float* pos, const
 	}
 }
 
-// the state rows of new particles (checkpoint channels): the position, then array_to_buffer's start state
+// the state rows of new particles (checkpoint channels): their start state
 __global__ void emit_rows_kernel(int material, int n, const float* pos, float* rows) {
 	const int C = ck_channels(material);
-	for(int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
-		float* r = rows + (size_t) p * C;
-		r[0] = pos[3 * p];
-		r[1] = pos[3 * p + 1];
-		r[2] = pos[3 * p + 2];
-		if(material == CB200_J_FLUID) {
-			r[3] = 1.f;
-			continue;
-		}
-		for(int d = 0; d < 9; ++d) r[3 + d] = (d % 4 == 0) ? 1.f : 0.f;
-		if(material == CB200_SAND) r[12] = 0.f;     // ParticleBuffer<SAND>::LOG_JP_0
-		if(material == CB200_NACC) r[12] = -0.01f;  // ParticleBuffer<NACC>::LOG_JP_0
-	}
+	for(int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) start_state(material, pos + 3 * p, rows + (size_t) p * C, 1);
 }
 
 }  // namespace cb200

@@ -239,6 +239,69 @@ struct MgspCounters {
 	int epochs[3];
 };
 
+// the simulation clock: what a checkpoint saves of StepState (+ the frames cb200_sim_advance_frame finished) and a start sets
+struct Clock {
+	float dt, next_dt, step_time, frame_time;
+	double sim_time;
+	long long steps, frames;
+	int error;
+};
+Clock clock_of(const StepState& h, long long frames) { return Clock {h.dt, h.next_dt, h.step_time, h.frame_time, h.sim_time, h.steps, frames, h.error}; }
+void set_clock(StepState& h, long long& frames, const Clock& c) {
+	h.dt = c.dt;
+	h.next_dt = c.next_dt;
+	h.step_time = c.step_time;
+	h.frame_time = c.frame_time;
+	h.sim_time = c.sim_time;
+	h.steps = c.steps;
+	h.error |= c.error;
+	frames = c.frames;
+}
+// min(dt, dx·cfl/mv), dt for mv = 0: initial_setup's dt rule (gmpm_simulator.cuh:305-315) for the start and for an emission, whose dt
+// is held to a set-up's bitwise
+float cfl_dt(const Cfg& cfg, float dt, float mv) { return mv > 0.f ? fminf(dt, cfg.dx * cfg.cfl / mv) : dt; }
+
+struct BlockCounts {
+	int pbc, nbc, ebc;
+};
+// What a start (initial_setup) is made of.  Each part may be absent, and then set-up makes it itself.
+struct StartSrc {
+	const float* rows[kMaxModels] = {};  // per model, [n][channels] state rows; absent: the start state at d_pos
+	const float* grid = nullptr;         // [grid_count][256] saved grid blocks with their keys [grid_count][3]; absent: rasterise the bins
+	const int* keys = nullptr;
+	int grid_count = 0;                  // a checkpoint's nbc; an emission's old nbc, a subset of the rebuilt partition's
+	const Clock* clock = nullptr;        // absent: the fresh clock of desc and the models' v0
+	const BlockCounts* expect = nullptr; // the block counts the rebuild must reproduce; absent: no check
+};
+
+// cb200_sim_restore_models: the checkpoint's state, clock and block counts, staged on the device until initial_setup consumes them
+struct RestoreStaging {
+	bool pending = false;
+	Clock clock {};
+	BlockCounts counts {};
+	float* rows[kMaxModels] = {};
+	unsigned char* grid = nullptr;  // grid blocks, then keys
+	size_t grid_bytes = 0;
+
+	StartSrc start() const {
+		StartSrc s;
+		if(!pending) return s;
+		for(int m = 0; m < kMaxModels; ++m) s.rows[m] = rows[m];
+		s.grid = reinterpret_cast<const float*>(grid);
+		s.keys = reinterpret_cast<const int*>(grid + grid_bytes);
+		s.grid_count = counts.nbc;
+		s.clock = &clock;
+		s.expect = &counts;
+		return s;
+	}
+	// after every read of the staged buffers has finished
+	void release() {
+		for(float* p : rows) g_pool.release(p);
+		g_pool.release(grid);
+		*this = RestoreStaging {};
+	}
+};
+
 void default_material(const cb200_config& cfg, int material, cb200_particle_buffer& pb) {
 	// defaults of ParticleBuffer<M>, reference Projects/GMPM/particle_buffer.cuh:141-264
 	const float cells = (float) (1u << cfg.domain_bits);
@@ -318,11 +381,7 @@ struct cb200_sim {
 	// checkpoint (cb200_sim_checkpoint_begin / _end): the blob, copied to the host on the staging's own stream
 	Staging ck;
 	size_t ck_bytes = 0;  // bytes of the blob the last begin queued (0: none)
-	// cb200_sim_restore_models: the checkpoint's header and its state staged on the device, consumed by initial_setup
-	bool restore_pending = false;
-	cb200_checkpoint_info restore_info {};
-	float* restore_state[kMaxModels] = {};
-	unsigned char* restore_grid = nullptr;  // grid blocks, then keys
+	RestoreStaging restore;
 	// frame output (cb200_sim_frame_output): the records, copied to the host on the staging's own stream, and the writer thread with
 	// its one job, which waits for that copy; started on first use.  `out_busy`: a frame is queued or being written
 	Staging out;
@@ -440,6 +499,35 @@ void drop_graphs(cb200_sim* s) {
 		if(g) cudaGraphExecDestroy(g);
 		g = nullptr;
 	}
+}
+
+// A new model of `material`, n particles and the default parameters (init_model, init_model_sdf, restore): its containers, then
+// fill(m) enqueues the n start positions into m.d_pos on the sim stream.  Appended once they are there; a failure releases it.
+template<class Fill>
+int add_model(cb200_sim* s, int material, int n, const float* v0, int* model_id, Fill&& fill) {
+	if(material < 0 || material > 3 || n <= 0 || (int) s->models.size() >= kMaxModels) return (int) cudaErrorInvalidValue;
+	Model m;
+	m.material = material;
+	m.n = n;
+	for(int d = 0; d < 3; ++d) m.v0[d] = v0 ? v0[d] : 0.f;
+	const long long mb = s->desc.max_blocks;
+	m.bin_capacity = bin_rows(n, mb);
+	for(cb200_particle_buffer& pb : m.pb) {
+		memset(&pb, 0, sizeof(pb));
+		default_material(s->desc.cfg, material, pb);
+	}
+	const DevArrays a = model_arrays(s, m, (size_t) mb, m.bin_capacity);
+	int e = alloc_arrays(s, a);
+	if(!e) e = fill(m);
+	if(!e) e = (int) cudaStreamSynchronize(s->stream);
+	if(e) {
+		cudaStreamSynchronize(s->stream);
+		free_arrays(a);
+		return e;
+	}
+	if(model_id) *model_id = (int) s->models.size();
+	s->models.push_back(m);
+	return 0;
 }
 
 inline int grid_blocks(int per_sm) { return num_sms() * per_sm; }
@@ -790,7 +878,6 @@ void preload_kernels() {
 	preload(grid_max_kernel<true>);
 	preload(snapshot_kernel);
 	preload(state_positions_kernel);
-	preload(state_to_bins_kernel);
 	preload(scatter_grid_kernel);
 	preload(output_kernel);
 	preload(state_rows_kernel<true>);
@@ -988,8 +1075,7 @@ int cb200_sim_destroy(cb200_sim* s) {
 	}
 	s->out.release();
 	s->ck.release();  // (a checkpoint copy may still read the staging blob: release waits for it)
-	for(float* p : s->restore_state) g_pool.release(p);
-	g_pool.release(s->restore_grid);
+	s->restore.release();
 	for(auto& ev : s->prof_events) {
 		cudaEventDestroy(ev.first);
 		cudaEventDestroy(ev.second);
@@ -1017,29 +1103,11 @@ int cb200_sim_destroy(cb200_sim* s) {
 	return 0;
 }
 
-// the containers of one model of m.material and m.n particles (init_model and restore; the caller fills d_pos)
-static int alloc_model(cb200_sim* s, Model& m) {
-	const long long mb = s->desc.max_blocks;
-	m.bin_capacity = bin_rows(m.n, mb);
-	for(cb200_particle_buffer& pb : m.pb) {
-		memset(&pb, 0, sizeof(pb));
-		default_material(s->desc.cfg, m.material, pb);
-	}
-	return alloc_arrays(s, model_arrays(s, m, (size_t) mb, m.bin_capacity));
-}
-
 int cb200_sim_init_model(cb200_sim* s, int material, const float* positions_host, int n, const float* v0, int* model_id) {
-	if(!s || s->setup_done || material < 0 || material > 3 || n <= 0 || (int) s->models.size() >= kMaxModels) return (int) cudaErrorInvalidValue;
-	Model m;
-	m.material = material;
-	m.n = n;
-	for(int d = 0; d < 3; ++d) m.v0[d] = v0 ? v0[d] : 0.f;
-	CK(alloc_model(s, m));
-	CK(cudaMemcpyAsync(m.d_pos, positions_host, (size_t) n * 3 * sizeof(float), cudaMemcpyHostToDevice, s->stream));
-	CK(cudaStreamSynchronize(s->stream));
-	if(model_id) *model_id = (int) s->models.size();
-	s->models.push_back(m);
-	return 0;
+	if(!s || s->setup_done) return (int) cudaErrorInvalidValue;
+	return add_model(s, material, n, v0, model_id, [&](Model& m) {
+		return (int) cudaMemcpyAsync(m.d_pos, positions_host, (size_t) n * 3 * sizeof(float), cudaMemcpyHostToDevice, s->stream);
+	});
 }
 
 static int set_elastic(cb200_sim* s, int model, int material, float rho, float vol, float ym, float pr) {
@@ -1084,36 +1152,55 @@ int cb200_sim_update_nacc_parameters(cb200_sim* s, int model, float rho, float v
 	return 0;
 }
 
-// What cb200_sim_restore puts in place of the rasterised start: the saved state, already on the device.
-struct RestoreSrc {
-	const cb200_checkpoint_info* info;
-	const float* state[kMaxModels];  // [count][channels] per model
-	const int* keys;                 // [nbc][3]
-	const float* grid;               // [grid_count][256]
-	int grid_count;                  // saved blocks: the checkpoint's nbc; an emission's old nbc, a subset of the rebuilt partition's
-};
+// register_blocks_kernel over the (lo, span) ring of the first pbc blocks of partition p; returns p's new block count in *out
+// (synchronises).  initial_setup's neighbour (0, 2) and exterior (-1, 3) registrations.
+static int register_ring(cb200_sim* s, Part p, int capacity, int* error, int pbc, int lo, int span, int* out) {
+	RegisterArgs a {};
+	a.cfg = s->cfg;
+	a.block_count = count_imm(pbc);
+	a.table = p.table;
+	a.keys = p.keys;
+	a.count = p.count;
+	a.capacity = capacity;
+	a.error = error;
+	a.lo = lo;
+	a.span = span;
+	register_blocks_kernel<<<grid_for((long long) pbc * span * span * span, 128, 16), 128, 0, s->stream>>>(a);
+	++s->launches;
+	CK(cudaMemcpyAsync(out, p.count, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+	return (int) cudaStreamSynchronize(s->stream);
+}
 
-// initial_setup  gmpm_simulator.cuh:637-781 (counts are read back here: one-time cost).  With `rs` (restore) it differs in three
-// places: the bins get the saved channels, grid[0] gets the saved blocks (no MGSP halo reduction: they hold the full sums), and the
-// step state gets the saved clock.
-static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
+// initial_setup  gmpm_simulator.cuh:637-781 (counts are read back here: one-time cost), from the parts `src` has and the models'
+// positions: the bins get the start state or the saved rows, grid[0] the rasterised particles or the saved blocks (no MGSP halo
+// reduction: they hold the full sums), the step state the fresh clock or the saved one.
+static int setup_impl(cb200_sim* s, const StartSrc& src) {
 	if(!s || s->setup_done || s->models.empty()) return (int) cudaErrorInvalidValue;
 	cudaStream_t st = s->stream;
 	const Cfg& cfg = s->cfg;
 	const int R = s->rollid, Rn = R ^ 1;
 	const int cap = s->desc.max_blocks;
+	const bool mgsp = s->desc.mgsp_world > 1;
 	int* err = &s->d_state->error;
 	int pbc = 0, nbc = 0, ebc = 0;
+	cb200_partition& P = s->part[Rn];  // the partition set-up builds
 
+	// it builds into P and roll R's buckets: both start empty (stream-ordered only: MGSP ranks set up concurrently)
+	CK(fill_arrays(s, partition_arrays(s, P, (size_t) cap)));
 	for(Model& m : s->models) {
-		activate_blocks_kernel<true><<<grid_for(m.n, 256, 16), 256, 0, st>>>(cfg, m.n, m.d_pos, s->part[Rn].index_table, s->part[Rn].active_keys, s->part[Rn].count, cap, err);
+		DevArrays a;
+		buffer_arrays(a, s, m, m.pb[R], (size_t) cap, m.bin_capacity);
+		CK(fill_arrays(s, a));
+	}
+	for(Model& m : s->models) {
+		activate_blocks_kernel<true><<<grid_for(m.n, 256, 16), 256, 0, st>>>(cfg, m.n, m.d_pos, P.index_table, P.active_keys, P.count, cap, err);
 		++s->launches;
 	}
-	CK(cudaMemcpyAsync(&pbc, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToHost, st));
+	CK(cudaMemcpyAsync(&pbc, P.count, sizeof(int), cudaMemcpyDeviceToHost, st));
 	CK(cudaStreamSynchronize(st));
 	if(pbc > cap) return (int) cudaErrorMemoryAllocation;
 	for(Model& m : s->models) {
-		build_particle_cell_buckets_kernel<true><<<grid_for(m.n, 256, 16), 256, 0, st>>>(cfg, m.n, m.d_pos, view(m.pb[R]), s->part[Rn].index_table, err);
+		build_particle_cell_buckets_kernel<true><<<grid_for(m.n, 256, 16), 256, 0, st>>>(cfg, m.n, m.d_pos, view(m.pb[R]), P.index_table, err);
 		cell_bucket_to_block_kernel<<<grid_for(pbc, 1, 16), kBucketThreads, 0, st>>>(cfg, pbc, m.pb[R].cell_particle_counts, m.pb[R].cellbuckets, m.pb[R].particle_bucket_sizes, m.pb[R].blockbuckets, m.celloffs[Rn]);
 		compute_bin_capacity_kernel<<<grid_for(pbc + 1, 256, 16), 256, 0, st>>>(pbc + 1, m.pb[R].particle_bucket_sizes, m.bin_sizes);
 		ScanArgs a {};
@@ -1121,51 +1208,33 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 		a.in = m.bin_sizes;
 		a.out = m.pb[R].bin_offsets;
 		scan_kernel<<<1, 1024, 0, st>>>(a);
-		if(rs) state_to_bins_kernel<<<grid_for(pbc, 1, 16), 128, 0, st>>>(cfg, m.material, pbc, rs->state[&m - s->models.data()], view(m.pb[R]));
-		else array_to_buffer_kernel<<<grid_for(pbc, 1, 16), 128, 0, st>>>(cfg, m.material, pbc, m.d_pos, view(m.pb[R]));
+		array_to_buffer_kernel<<<grid_for(pbc, 1, 16), 128, 0, st>>>(cfg, m.material, pbc, m.d_pos, src.rows[&m - s->models.data()], view(m.pb[R]));
 		s->launches += 5;
 	}
-	{
-		RegisterArgs a {};
-		a.cfg = cfg;
-		a.block_count = count_imm(pbc);
-		a.table = s->part[Rn].index_table;
-		a.keys = s->part[Rn].active_keys;
-		a.count = s->part[Rn].count;
-		a.capacity = cap;
-		a.error = err;
-		a.lo = 0;
-		a.span = 2;
-		register_blocks_kernel<<<grid_for((long long) pbc * 8, 128, 16), 128, 0, st>>>(a);
-		CK(cudaMemcpyAsync(&nbc, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToHost, st));
-		CK(cudaStreamSynchronize(st));
-		if(s->desc.mgsp_world > 1) {  // halo_tagging of the initial partition (mgsp_benchmark.cuh:633), with the kernels of the sub-step
-			if(!s->peers_ready) return (int) cudaErrorNotReady;
-			const MgspView v = mgsp_view(s);
-			DeviceScratch* scr = s->scr;
-			CK(cudaMemcpyAsync(&scr->new_nbc, &nbc, sizeof(int), cudaMemcpyHostToDevice, st));  // key count of the exchange
-			CK(cudaMemsetAsync(&scr->local_max, 0, sizeof(float), st));
-			CK(cudaMemsetAsync(&scr->global_max, 0, sizeof(float), st));
-			mgsp_tag_reset_kernel<<<grid_blocks(1), 256, 0, st>>>(v, s->part[Rn].overlap_marks, &scr->new_nbc);
-			// the next grid is still all zero from cb200_sim_create: the clear changes nothing, and the flag still goes out behind it
-			mgsp_clear_publish_kernel<<<grid_blocks(2), 256, 0, st>>>(v, s->part[Rn].active_keys, &scr->new_nbc, &scr->local_max, s->grid[1]);
-			mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(cfg, v, s->part[Rn].index_table, s->part[Rn].overlap_marks, &scr->new_nbc, &scr->local_max, &scr->global_max, 0, FinalizeArgs {});
-			s->launches += 3;
-		}
-		a.lo = -1;
-		a.span = 3;
-		register_blocks_kernel<<<grid_for((long long) pbc * 27, 128, 16), 128, 0, st>>>(a);
-		CK(cudaMemcpyAsync(&ebc, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToHost, st));
-		CK(cudaStreamSynchronize(st));
-		s->launches += 2;
+	CK(register_ring(s, view(P), cap, err, pbc, 0, 2, &nbc));
+	if(mgsp) {  // halo_tagging of the initial partition (mgsp_benchmark.cuh:633), with the kernels of the sub-step
+		if(!s->peers_ready) return (int) cudaErrorNotReady;
+		const MgspView v = mgsp_view(s);
+		DeviceScratch* scr = s->scr;
+		CK(cudaMemcpyAsync(&scr->new_nbc, &nbc, sizeof(int), cudaMemcpyHostToDevice, st));  // key count of the exchange
+		CK(cudaMemsetAsync(&scr->local_max, 0, sizeof(float), st));
+		CK(cudaMemsetAsync(&scr->global_max, 0, sizeof(float), st));
+		mgsp_tag_reset_kernel<<<grid_blocks(1), 256, 0, st>>>(v, P.overlap_marks, &scr->new_nbc);
+		// the next grid is still all zero from cb200_sim_create: the clear changes nothing, and the flag still goes out behind it
+		mgsp_clear_publish_kernel<<<grid_blocks(2), 256, 0, st>>>(v, P.active_keys, &scr->new_nbc, &scr->local_max, s->grid[1]);
+		mgsp_tag_kernel<<<grid_blocks(1), 256, 0, st>>>(cfg, v, P.index_table, P.overlap_marks, &scr->new_nbc, &scr->local_max, &scr->global_max, 0, FinalizeArgs {});
+		s->launches += 3;
 	}
+	CK(register_ring(s, view(P), cap, err, pbc, -1, 3, &ebc));
 	if(nbc > cap || ebc > cap) return (int) cudaErrorMemoryAllocation;
+	// a blob that passed inspect but does not rebuild the saved partition (hand-edited): nothing to step
+	if(src.expect && (pbc != src.expect->pbc || nbc != src.expect->nbc || ebc != src.expect->ebc)) return (int) cudaErrorIllegalState;
 	// background copies (gmpm_simulator.cuh:745-756); the device count is copied too so that the stale-key
 	// un-insert of the first rebuild knows how many entries the table holds
 	CK(cudaMemcpyAsync(s->part[R].index_table, s->part[Rn].index_table, s->table_entries * sizeof(int), cudaMemcpyDeviceToDevice, st));
 	CK(cudaMemcpyAsync(s->part[R].active_keys, s->part[Rn].active_keys, (size_t) ebc * 3 * sizeof(int), cudaMemcpyDeviceToDevice, st));
 	CK(cudaMemcpyAsync(s->part[R].count, s->part[Rn].count, sizeof(int), cudaMemcpyDeviceToDevice, st));
-	if(s->desc.mgsp_world > 1)  // "need to copy halo tag info as well" (mgsp_benchmark.cuh:639-640)
+	if(mgsp)  // "need to copy halo tag info as well" (mgsp_benchmark.cuh:639-640)
 		CK(cudaMemcpyAsync(s->part[R].overlap_marks, s->part[Rn].overlap_marks, (size_t) nbc * sizeof(int), cudaMemcpyDeviceToDevice, st));
 	for(Model& m : s->models) {
 		CK(cudaMemcpyAsync(m.pb[Rn].bin_offsets, m.pb[R].bin_offsets, (size_t) (pbc + 1) * sizeof(int), cudaMemcpyDeviceToDevice, st));
@@ -1173,15 +1242,18 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 	}
 	clear_grid_kernel<<<grid_for((long long) nbc * 64, 256, 16), 256, 0, st>>>(nbc, s->grid[0]);
 	++s->launches;
-	int* missing = &s->scr->missing;
-	if(rs) {  // the saved blocks by key; a key the rebuilt partition has no neighbour block for is counted, not written
-		const int saved = rs->grid_count;
+	if(src.grid) {  // the saved blocks by key; a key the rebuilt partition has no neighbour block for is counted, not written
+		int* missing = &s->scr->missing;
 		CK(cudaMemsetAsync(missing, 0, sizeof(int), st));
-		scatter_grid_kernel<<<grid_for(saved, 8, 16), 256, 0, st>>>(cfg, saved, rs->keys, rs->grid, s->part[R].index_table, nbc, s->grid[0], missing);
+		scatter_grid_kernel<<<grid_for(src.grid_count, 8, 16), 256, 0, st>>>(cfg, src.grid_count, src.keys, src.grid, s->part[R].index_table, nbc, s->grid[0], missing);
 		++s->launches;
+		int miss = 0;
+		CK(cudaMemcpyAsync(&miss, missing, sizeof(int), cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+		if(miss) return (int) cudaErrorIllegalState;
 	}
 	for(Model& m : s->models) {
-		if(!rs) {
+		if(!src.grid) {
 			rasterize_blocks_kernel<<<grid_for(pbc, 1, 16), 256, 0, st>>>(cfg, m.material, pbc, s->part[R].active_keys, s->part[R].index_table, view(m.pb[R]), s->grid[0], m.pb[R].mass, m.v0[0], m.v0[1], m.v0[2], err);
 			++s->launches;
 		}
@@ -1189,20 +1261,13 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 		++s->launches;
 	}
 	CK(cudaGetLastError());
-	if(rs) {  // a blob that passed inspect but does not rebuild the saved partition (hand-edited): nothing to step
-		int miss = 0;
-		CK(cudaMemcpyAsync(&miss, missing, sizeof(int), cudaMemcpyDeviceToHost, st));
-		CK(cudaStreamSynchronize(st));
-		const cb200_checkpoint_info& I = *rs->info;
-		if(miss || pbc != I.particle_block_count || nbc != I.neighbor_block_count || ebc != I.exterior_block_count) return (int) cudaErrorIllegalState;
-	}
-	if(s->desc.mgsp_world > 1 && !rs) {  // the rasterised halo blocks are partial sums: reduce them (mgsp_benchmark.cuh:653-654, 723-776)
+	if(mgsp && !src.grid) {  // the rasterised halo blocks are partial sums: reduce them (mgsp_benchmark.cuh:653-654, 723-776)
 		mgsp_pack_send_kernel<<<grid_blocks(2), 256, 0, st>>>(cfg, mgsp_view(s), s->grid[0], s->part[R].index_table);
 		mgsp_wait_reduce_kernel<<<grid_blocks(2), 256, 0, st>>>(cfg, mgsp_view(s), s->grid[0], s->part[R].index_table, err);
 		s->launches += 2;
 		CK(cudaGetLastError());
 	}
-	// device-resident step state; initial dt as in main_loop's preamble (gmpm_simulator.cuh:305-315)
+	// device-resident step state
 	CK(pull_state(s));
 	StepState& h = *s->h_state;
 	h.pbc = pbc;
@@ -1211,42 +1276,29 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 	h.prev_nbc = nbc;
 	h.prev_ebc = ebc;
 	h.dt_default = s->desc.dt_default;
-	h.frame_time = s->desc.fps > 0 ? 1.f / (float) s->desc.fps : 0.f;
-	h.step_time = 0.f;
-	h.sim_time = 0.0;
-	if(rs) {
-		const cb200_checkpoint_info& I = *rs->info;
-		h.frame_time = I.frame_time;
-		h.step_time = I.step_time;
-		h.sim_time = I.sim_time;
-		h.dt = I.dt;
-		h.next_dt = I.next_dt;
-		h.steps = I.steps;
-		h.error |= I.error;
-		h.max_vel_sq = 0.f;
-		s->frames_done = I.frames;
-		CK(push_state(s));
+	Clock c {};
+	if(src.clock) {
+		c = *src.clock;
+	} else {  // main_loop's preamble (gmpm_simulator.cuh:305-315)
+		c.frame_time = s->desc.fps > 0 ? 1.f / (float) s->desc.fps : 0.f;
+		float mv = 0.f;
+		for(const Model& m : s->models) mv = fmaxf(mv, sqrtf(m.v0[0] * m.v0[0] + m.v0[1] * m.v0[1] + m.v0[2] * m.v0[2]));
+		if(mgsp) {  // every rank must start from the same dt: max over the ranks' initial speeds
+			h.max_vel_sq = mv * mv;
+			CK(push_state(s));
+			mgsp_allreduce_maxvel_kernel<<<1, 32, 0, st>>>(mgsp_view(s), &s->d_state->max_vel_sq);
+			++s->launches;
+			CK(pull_state(s));
+			mv = sqrtf(h.max_vel_sq);
+		}
+		c.dt = cfl_dt(cfg, h.dt_default, mv);
+		if(c.frame_time > 0.f) c.dt = fminf(c.dt, c.frame_time);
+		c.next_dt = c.dt;
 	}
-	float mv = 0.f;
-	for(const Model& m : s->models) mv = fmaxf(mv, sqrtf(m.v0[0] * m.v0[0] + m.v0[1] * m.v0[1] + m.v0[2] * m.v0[2]));
-	if(s->desc.mgsp_world > 1 && !rs) {  // every rank must start from the same dt: max over the ranks' initial speeds
-		h.max_vel_sq = mv * mv;
-		CK(push_state(s));
-		mgsp_allreduce_maxvel_kernel<<<1, 32, 0, st>>>(mgsp_view(s), &s->d_state->max_vel_sq);
-		++s->launches;
-		CK(pull_state(s));
-		mv = sqrtf(s->h_state->max_vel_sq);
-	}
-	if(!rs) {
-		float dt = h.dt_default;
-		if(mv > 0.f) dt = fminf(dt, cfg.dx * cfg.cfl / mv);
-		if(h.frame_time > 0.f) dt = fminf(dt, h.frame_time);
-		h.dt = dt;
-		h.next_dt = dt;
-		h.max_vel_sq = 0.f;
-		CK(push_state(s));
-	}
-	if(s->desc.mgsp_world > 1) {
+	set_clock(h, s->frames_done, c);
+	h.max_vel_sq = 0.f;
+	CK(push_state(s));
+	if(mgsp) {
 		// global max |v|^2 of the start grid (later sub-steps get it from the end-of-step exchange of the previous one)
 		if(s->has_collider) grid_max_kernel<true><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->collider);
 		else grid_max_kernel<false><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, ColliderView {});
@@ -1262,25 +1314,10 @@ static int setup_impl(cb200_sim* s, const RestoreSrc* rs) {
 	return 0;
 }
 int cb200_sim_initial_setup(cb200_sim* s) {
-	if(!s || !s->restore_pending) return setup_impl(s, nullptr);
-	RestoreSrc rs {};
-	rs.info = &s->restore_info;
-	for(int m = 0; m < kMaxModels; ++m) rs.state[m] = s->restore_state[m];
-	rs.grid = reinterpret_cast<const float*>(s->restore_grid);
-	rs.keys = reinterpret_cast<const int*>(s->restore_grid + s->restore_info.grid_bytes);
-	rs.grid_count = s->restore_info.neighbor_block_count;
-	int e = setup_impl(s, &rs);
-	if(!e) e = (int) cudaStreamSynchronize(s->stream);
-	if(!e) {  // the staged state is in the bins and the grid now
-		for(float*& p : s->restore_state) {
-			g_pool.release(p);
-			p = nullptr;
-		}
-		g_pool.release(s->restore_grid);
-		s->restore_grid = nullptr;
-		s->restore_pending = false;
-	}
-	return e;
+	if(!s) return (int) cudaErrorInvalidValue;
+	CK(setup_impl(s, s->restore.start()));
+	s->restore.release();  // (setup_impl has synchronised: a staged state is in the bins and the grid now)
+	return 0;
 }
 
 static int set_frame_roll(cb200_sim* s, int on) {
@@ -1592,14 +1629,15 @@ int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	I.fps = s->desc.fps;
 	I.mgsp_rank = s->desc.mgsp_world > 1 ? s->desc.mgsp_rank : 0;
 	I.mgsp_world = s->desc.mgsp_world;
-	I.error = h.error;
-	I.dt = h.dt;
-	I.next_dt = h.next_dt;
-	I.step_time = h.step_time;
-	I.frame_time = h.frame_time;
-	I.sim_time = h.sim_time;
-	I.steps = h.steps;
-	I.frames = s->frames_done;
+	const Clock c = clock_of(h, s->frames_done);
+	I.error = c.error;
+	I.dt = c.dt;
+	I.next_dt = c.next_dt;
+	I.step_time = c.step_time;
+	I.frame_time = c.frame_time;
+	I.sim_time = c.sim_time;
+	I.steps = c.steps;
+	I.frames = c.frames;
 	I.particle_block_count = h.pbc;
 	I.neighbor_block_count = h.nbc;
 	I.exterior_block_count = h.ebc;
@@ -1637,7 +1675,7 @@ int cb200_sim_checkpoint_end(cb200_sim* s, const void** blob, size_t* bytes) {
 
 int cb200_sim_restore_models(cb200_sim* s, const void* blob, size_t bytes) {
 	cb200_checkpoint_info I;
-	if(!s || s->setup_done || s->restore_pending || !s->models.empty() || ck_parse(blob, bytes, &I) != 0) return (int) cudaErrorInvalidValue;
+	if(!s || s->setup_done || s->restore.pending || !s->models.empty() || ck_parse(blob, bytes, &I) != 0) return (int) cudaErrorInvalidValue;
 	output_idle(s);
 	const cb200_config& c = s->desc.cfg;
 	if(c.domain_bits != I.cfg.domain_bits || c.max_ppc != I.cfg.max_ppc || c.boundary != I.cfg.boundary || memcmp(&c.gravity, &I.cfg.gravity, sizeof(float)) != 0 ||
@@ -1647,25 +1685,25 @@ int cb200_sim_restore_models(cb200_sim* s, const void* blob, size_t bytes) {
 	if(s->desc.max_blocks < I.exterior_block_count) return (int) cudaErrorMemoryAllocation;
 	const unsigned char* src = static_cast<const unsigned char*>(blob);
 	cudaStream_t st = s->stream;
-	s->restore_info = I;
-	s->restore_pending = true;
+	RestoreStaging& rs = s->restore;
+	rs.pending = true;
+	rs.clock = Clock {I.dt, I.next_dt, I.step_time, I.frame_time, I.sim_time, I.steps, I.frames, I.error};
+	rs.counts = BlockCounts {I.particle_block_count, I.neighbor_block_count, I.exterior_block_count};
 	for(int m = 0; m < I.n_models; ++m) {
 		const cb200_checkpoint_model& md = I.models[m];
-		Model model;
-		model.material = md.material;
-		model.n = (int) md.count;
-		CK(alloc_model(s, model));
-		for(cb200_particle_buffer& pb : model.pb) copy_params(pb, md.params);
-		s->models.push_back(model);
-		CK(pool_alloc(&s->restore_state[m], md.bytes));
-		CK(cudaMemcpyAsync(s->restore_state[m], src + md.offset, md.bytes, cudaMemcpyHostToDevice, st));
-		state_positions_kernel<<<num_sms() * 4, 256, 0, st>>>(md.count, md.channels, s->restore_state[m], s->models.back().d_pos);
-		++s->launches;
+		CK(add_model(s, md.material, (int) md.count, nullptr, nullptr, [&](Model& model) {
+			for(cb200_particle_buffer& pb : model.pb) copy_params(pb, md.params);
+			CK(pool_alloc(&rs.rows[m], md.bytes));
+			CK(cudaMemcpyAsync(rs.rows[m], src + md.offset, md.bytes, cudaMemcpyHostToDevice, st));
+			state_positions_kernel<<<num_sms() * 4, 256, 0, st>>>(md.count, md.channels, rs.rows[m], model.d_pos);
+			++s->launches;
+			return (int) cudaGetLastError();
+		}));
 	}
-	CK(pool_alloc(&s->restore_grid, (size_t) I.grid_bytes + (size_t) I.keys_bytes));
-	CK(cudaMemcpyAsync(s->restore_grid, src + I.grid_offset, I.grid_bytes, cudaMemcpyHostToDevice, st));
-	CK(cudaMemcpyAsync(s->restore_grid + I.grid_bytes, src + I.keys_offset, I.keys_bytes, cudaMemcpyHostToDevice, st));
-	CK(cudaGetLastError());
+	rs.grid_bytes = I.grid_bytes;
+	CK(pool_alloc(&rs.grid, (size_t) I.grid_bytes + (size_t) I.keys_bytes));
+	CK(cudaMemcpyAsync(rs.grid, src + I.grid_offset, I.grid_bytes, cudaMemcpyHostToDevice, st));
+	CK(cudaMemcpyAsync(rs.grid + I.grid_bytes, src + I.keys_offset, I.keys_bytes, cudaMemcpyHostToDevice, st));
 	return (int) cudaStreamSynchronize(st);
 }
 
@@ -1883,16 +1921,8 @@ int cb200_sim_init_model_sdf(cb200_sim* s, int material, const cb200_sdf_header*
 	r.st = s->stream;
 	CK(r.run_count(s->desc.cfg, *header, phi_host, *sampling));
 	if(r.count <= 0 || r.count >= (1LL << 31)) return (int) cudaErrorInvalidValue;
-	Model m;
-	m.material = material;
-	m.n = (int) r.count;
-	for(int d = 0; d < 3; ++d) m.v0[d] = v0 ? v0[d] : 0.f;
-	CK(alloc_model(s, m));
-	CK(r.run_write(m.d_pos));
-	CK(cudaStreamSynchronize(s->stream));
-	if(model_id) *model_id = (int) s->models.size();
-	if(n_out) *n_out = m.n;
-	s->models.push_back(m);
+	CK(add_model(s, material, (int) r.count, v0, model_id, [&](Model& m) { return r.run_write(m.d_pos); }));
+	if(n_out) *n_out = (int) r.count;
 	return 0;
 }
 
@@ -1981,30 +2011,18 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	emit_insert_keys_kernel<<<grid_for(h0.pbc, 256, 16), 256, 0, st>>>(cfg, h0.pbc, s->part[s->rollid].active_keys, eb.table, eb.keys, eb.word, cap_s);
 	activate_blocks_kernel<true><<<grid_for(k, 256, 16), 256, 0, st>>>(cfg, k, eb.kept, eb.table, eb.keys, eb.word, cap_s, nullptr);
 	s->launches += 2;
-	int cnt[3] = {0, 0, 0};  // the union's pbc, nbc, ebc
-	CK(cudaMemcpyAsync(&cnt[0], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
+	BlockCounts u {};  // the union's
+	CK(cudaMemcpyAsync(&u.pbc, eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
 	CK(cudaStreamSynchronize(st));
-	RegisterArgs ra {};
-	ra.cfg = cfg;
-	ra.block_count = count_imm(cnt[0]);
-	ra.table = eb.table;
-	ra.keys = eb.keys;
-	ra.count = eb.word;
-	ra.capacity = cap_s;
-	ra.lo = 0;
-	ra.span = 2;
-	register_blocks_kernel<<<grid_for((long long) cnt[0] * 8, 128, 16), 128, 0, st>>>(ra);
-	CK(cudaMemcpyAsync(&cnt[1], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
-	ra.lo = -1;
-	ra.span = 3;
-	register_blocks_kernel<<<grid_for((long long) cnt[0] * 27, 128, 16), 128, 0, st>>>(ra);
-	CK(cudaMemcpyAsync(&cnt[2], eb.word, sizeof(int), cudaMemcpyDeviceToHost, st));
+	const Part scratch {eb.word, eb.table, eb.keys};
+	CK(register_ring(s, scratch, cap_s, nullptr, u.pbc, 0, 2, &u.nbc));
+	CK(register_ring(s, scratch, cap_s, nullptr, u.pbc, -1, 3, &u.ebc));
 	// (3) no cell above max_ppc, existing and new particles together
-	CK(pool_alloc(&eb.cells, (size_t) cnt[0] * kBlockVol * sizeof(int)));
-	CK(cudaMemsetAsync(eb.cells, 0, (size_t) cnt[0] * kBlockVol * sizeof(int), st));
+	CK(pool_alloc(&eb.cells, (size_t) u.pbc * kBlockVol * sizeof(int)));
+	CK(cudaMemsetAsync(eb.cells, 0, (size_t) u.pbc * kBlockVol * sizeof(int), st));
 	emit_count_kernel<<<grid_for(k, 256, 16), 256, 0, st>>>(cfg, k, eb.kept, eb.table, eb.cells);
 	emit_overflow_kernel<<<grid_for(k, 256, 16), 256, 0, st>>>(occ, k, eb.kept, eb.table, eb.cells, eb.word + 1);
-	s->launches += 4;
+	s->launches += 2;
 	CK(cudaGetLastError());
 	CK(cudaMemcpyAsync(&bad, eb.word + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
 	CK(cudaStreamSynchronize(st));
@@ -2012,9 +2030,9 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	if((long long) s->models[model].n + k > 0x7fffffffLL) return (int) cudaErrorInvalidValue;  // n bounds the model's live count
 	// (4) capacity: the union's exterior blocks must fit (auto_grow: grow to 4/3 of them, after everything else that can fail)
 	int new_mb = s->desc.max_blocks;
-	if(cnt[2] > new_mb) {
+	if(u.ebc > new_mb) {
 		if(!s->desc.auto_grow) return (int) cudaErrorMemoryAllocation;
-		new_mb = (int) (((long long) cnt[2] * 4 + 2) / 3);
+		new_mb = (int) (((long long) u.ebc * 4 + 2) / 3);
 	}
 	// (5) gather the current state (checkpoint layout) and allocate what the commit swaps in: nothing live is written yet
 	CK(pool_alloc(&eb.blob, ck_capacity(s)));
@@ -2039,54 +2057,31 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	CK(cudaStreamSynchronize(st));
 	// the last step that can reject: cb200_sim_reserve (an out-of-memory failure there leaves a valid simulator, part-grown)
 	if(new_mb > s->desc.max_blocks) CK(cb200_sim_reserve(s, new_mb));
-	// (6) commit: initial_setup's restore path over the union, then the new particles' mass and momentum added to grid[0]
+	// (6) commit: initial_setup over the union's saved rows and grid[0], then the new particles' mass and momentum added to grid[0]
 	drop_graphs(s);
 	if(eb.bins[0] && new_bins > md.bin_capacity) {  // (reserve may have grown the bins past the new count's rule already)
 		for(int i = 0; i < 2; ++i) std::swap(md.pb[i].bins, eb.bins[i]);
 		md.bin_capacity = new_bins;
 	}
 	std::swap(md.d_pos, eb.pos);
-	RestoreSrc rs {};
+	StartSrc src;
 	for(int m = 0; m < nm; ++m) {
 		Model& mm = s->models[m];
 		mm.n = (int) (m == model ? n_union : counts[m]);
-		rs.state[m] = m == model ? eb.rows : reinterpret_cast<const float*>(eb.blob + L.model_off[m]);
-		state_positions_kernel<<<num_sms() * 4, 256, 0, st>>>(mm.n, ck_channels(mm.material), rs.state[m], mm.d_pos);
+		src.rows[m] = m == model ? eb.rows : reinterpret_cast<const float*>(eb.blob + L.model_off[m]);
+		state_positions_kernel<<<num_sms() * 4, 256, 0, st>>>(mm.n, ck_channels(mm.material), src.rows[m], mm.d_pos);
 		++s->launches;
 	}
-	rs.keys = reinterpret_cast<const int*>(eb.blob + L.keys_off);
-	rs.grid = reinterpret_cast<const float*>(eb.blob + L.grid_off);
-	rs.grid_count = h0.nbc;
-	{  // setup_impl starts from an empty partition (roll Rn) and zero cell counts / bucket sizes in the buffers it buckets into (roll R):
-		// both as allocation leaves them
-		const int R = s->rollid, Rn = R ^ 1;
-		const size_t mb = (size_t) s->desc.max_blocks;
-		CK(fill_arrays(s, partition_arrays(s, s->part[Rn], mb)));
-		for(Model& mm : s->models) {
-			DevArrays a;
-			buffer_arrays(a, s, mm, mm.pb[R], mb, mm.bin_capacity);
-			CK(fill_arrays(s, a));
-		}
-	}
+	src.keys = reinterpret_cast<const int*>(eb.blob + L.keys_off);
+	src.grid = reinterpret_cast<const float*>(eb.blob + L.grid_off);
+	src.grid_count = h0.nbc;
+	src.expect = &u;
 	// the clock stays; dt and next_dt follow initial_setup's rule for v0
-	cb200_checkpoint_info I;
-	memset(&I, 0, sizeof(I));
-	I.particle_block_count = cnt[0];
-	I.neighbor_block_count = cnt[1];
-	I.exterior_block_count = cnt[2];
-	I.error = h0.error;
-	I.step_time = h0.step_time;
-	I.frame_time = h0.frame_time;
-	I.sim_time = h0.sim_time;
-	I.steps = h0.steps;
-	I.frames = s->frames_done;
-	float dt = h0.dt;
-	const float mv = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
-	if(mv > 0.f) dt = fminf(dt, cfg.dx * cfg.cfl / mv);
-	I.dt = I.next_dt = dt;
-	rs.info = &I;
+	Clock clock = clock_of(h0, s->frames_done);
+	clock.dt = clock.next_dt = cfl_dt(cfg, h0.dt, sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]));
+	src.clock = &clock;
 	s->setup_done = false;
-	CK(setup_impl(s, &rs));
+	CK(setup_impl(s, src));
 	// every stencil node of a new particle inside the domain lies in a neighbour block of its particle block; nodes past the top face
 	// are dropped, as rasterize_blocks_kernel drops them
 	rasterize_kernel<<<grid_for(k, 256, 16), 256, 0, st>>>(cfg, k, eb.kept, s->grid[0], s->part[s->rollid].index_table, md.pb[0].mass, v[0], v[1], v[2], nullptr);

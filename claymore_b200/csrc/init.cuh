@@ -44,26 +44,22 @@ __global__ void build_particle_cell_buckets_kernel(Cfg cfg, int n, const float* 
 	}
 }
 
-// array_to_buffer (mgmpm_kernels.cuh:221-323)
-__global__ void array_to_buffer_kernel(Cfg cfg, int material, int block_count, const float* pos, PBuf pb) {
-	const int binf = material == CB200_J_FLUID ? 128 : 512;
+// array_to_buffer (mgmpm_kernels.cuh:221-323): every bucketed particle's row into its bin slot.  The row of particle p is its start
+// state at pos[p] or, with `rows` (a restore, an emission), the saved row rows[p] of ck_channels(material) channels.
+__global__ void array_to_buffer_kernel(Cfg cfg, int material, int block_count, const float* pos, const float* rows, PBuf pb) {
+	const int binf = bin_floats(material), C = ck_channels(material);
 	for(int b = blockIdx.x; b < block_count; b += gridDim.x) {
 		const int n = pb.particle_bucket_sizes[b];
 		const int* bucket = pb.blockbuckets + ((size_t) b << cfg.ppb_shift);
 		for(int i = threadIdx.x; i < n; i += blockDim.x) {
 			const int pid = bucket[i];
-			float* bin = pb.bins + ((size_t) pb.bin_offsets[b] + (i >> 5)) * binf + (i & 31);
-			bin[0] = pos[3 * pid];
-			bin[32] = pos[3 * pid + 1];
-			bin[64] = pos[3 * pid + 2];
-			if(material == CB200_J_FLUID) {
-				bin[96] = 1.f;
-			} else {
-#pragma unroll
-				for(int d = 0; d < 9; ++d) bin[(3 + d) * 32] = (d % 4 == 0) ? 1.f : 0.f;
-				if(material == CB200_SAND) bin[12 * 32] = 0.f;     // ParticleBuffer<SAND>::LOG_JP_0  particle_buffer.cuh:207
-				if(material == CB200_NACC) bin[12 * 32] = -0.01f;  // ParticleBuffer<NACC>::LOG_JP_0  particle_buffer.cuh:241
+			float* bin = bin_slot(pb.bins, pb.bin_offsets[b], i, binf);
+			if(!rows) {
+				start_state(material, pos + 3 * pid, bin, kBinCap);
+				continue;
 			}
+			const float* row = rows + (size_t) pid * C;
+			for(int c = 0; c < C; ++c) bin[c * kBinCap] = row[c];
 		}
 	}
 }
@@ -108,7 +104,7 @@ __global__ void rasterize_kernel(Cfg cfg, int n, const float* pos, float* grid, 
 __global__ void __launch_bounds__(256) rasterize_blocks_kernel(Cfg cfg, int material, int block_count, const int* keys, const int* table, PBuf pb, float* grid, float mass, float v0x, float v0y, float v0z, int* error) {
 	__shared__ float arena[8 * 64];
 	__shared__ int s_bno[8];
-	const int binf = material == CB200_J_FLUID ? 128 : 512;
+	const int binf = bin_floats(material);
 	for(int b = blockIdx.x; b < block_count; b += gridDim.x) {
 		const int n = pb.particle_bucket_sizes[b];
 		if(n == 0) continue;
@@ -116,14 +112,14 @@ __global__ void __launch_bounds__(256) rasterize_blocks_kernel(Cfg cfg, int mate
 		for(int i = threadIdx.x; i < 512; i += blockDim.x) arena[i] = 0.f;
 		if(threadIdx.x < 8) s_bno[threadIdx.x] = table_query(cfg, table, kx + ((threadIdx.x >> 2) & 1), ky + ((threadIdx.x >> 1) & 1), kz + (threadIdx.x & 1));
 		__syncthreads();
-		const float* bins = pb.bins + (size_t) pb.bin_offsets[b] * binf;
+		const int first = pb.bin_offsets[b];
 		// the bucket is cell-major: neighbouring lanes would hold particles of one cell and fight over the same 27 nodes (a shared float
 		// atomicAdd is a compare-and-swap loop).  A lane takes every (n/32)-th particle instead, so a warp's lanes sit in different cells.
 		const int per_lane = (n + 31) >> 5;
 		for(int t = threadIdx.x; t < per_lane * 32; t += blockDim.x) {
 			const int i = (t & 31) * per_lane + (t >> 5);
 			if(i >= n) continue;
-			const float* bin = bins + (size_t) (i >> 5) * binf + (i & 31);
+			const float* bin = bin_slot(pb.bins, first, i, binf);
 			int ab[3];
 			float w[3][3];
 #pragma unroll
@@ -178,7 +174,7 @@ __global__ void init_adv_bucket_kernel(Cfg cfg, int block_count, const int* size
 // retrieve_particle_buffer (mgmpm_kernels.cuh:1087-1122); nch > 3 also exports the remaining channels
 // (F / J / logJp) -- the reference exports positions only, so a run can be checkpointed here.
 __global__ void retrieve_kernel(Cfg cfg, int material, Count block_count, const int* keys, const int* prev_table, PBuf pb, PBuf next_pb, float* out, int nch, int* parcount) {
-	const int binf = material == CB200_J_FLUID ? 128 : 512;
+	const int binf = bin_floats(material);
 	const int n = block_count.get();
 	__shared__ int s_base;
 	for(int b = blockIdx.x; b < n; b += gridDim.x) {
@@ -193,7 +189,7 @@ __global__ void retrieve_kernel(Cfg cfg, int material, Count block_count, const 
 			const int dir = advect >> cfg.ppb_shift, sp = advect & (cfg.ppb - 1);
 			const int sno = table_query(cfg, prev_table, kx + dir / 9 - 1, ky + (dir / 3) % 3 - 1, kz + dir % 3 - 1);
 			if(sno < 0) continue;
-			const float* bin = pb.bins + ((size_t) pb.bin_offsets[sno] + (sp >> 5)) * binf + (sp & 31);
+			const float* bin = bin_slot(pb.bins, pb.bin_offsets[sno], sp, binf);
 			for(int c = 0; c < nch; ++c) out[(size_t) (base + i) * nch + c] = bin[c * 32];
 		}
 	}
