@@ -347,6 +347,13 @@ __global__ void test_stress_kernel(int material, int mode, Mat m, int n, const f
 	}
 	if(log_jp_out) log_jp_out[i] = lj;
 }
+// reference-layout cell buckets (cell-major rows of max_ppc slots) into the step driver's slot-grouped layout
+__global__ void regroup_cell_buckets_kernel(Cfg cfg, long long n, const int* __restrict__ rows, int* __restrict__ grouped) {
+	for(long long i = blockIdx.x * (long long) blockDim.x + threadIdx.x; i < n; i += (long long) gridDim.x * blockDim.x) {
+		const int r = (int) (i & (cfg.ppb - 1));
+		grouped[grouped_cell_slot(cfg, (size_t) (i >> cfg.ppb_shift), r >> cfg.ppc_shift, r & (cfg.max_ppc - 1))] = rows[i];
+	}
+}
 }  // namespace cb200
 
 extern "C" {
@@ -364,8 +371,17 @@ int cb200_test_stress(int material, int mode, cb200_particle_buffer params, int 
 int cb200_test_warp_flatten(const cb200_config* c, int block_count, const int* cell_particle_counts, const int* cellbuckets, int* particle_bucket_sizes, int* buckets, unsigned short* cell_offsets, void* stream) {
 	CB_CFG(c);
 	if(block_count <= 0) return 0;
-	warp_flatten_kernel<<<(block_count + 7) / 8, 256, 0, (cudaStream_t) stream>>>(cfg, block_count, cell_particle_counts, cellbuckets, particle_bucket_sizes, buckets, cell_offsets);
-	return (int) cudaGetLastError();
+	// the caller's buckets are in the reference's layout: regroup them the way the step driver stores its own, then run the driver's flatten
+	const cudaStream_t st = (cudaStream_t) stream;
+	const long long n = (long long) block_count << cfg.ppb_shift;
+	int* grouped = nullptr;
+	cudaError_t e = cudaMallocAsync((void**) &grouped, (size_t) n * sizeof(int), st);
+	if(e != cudaSuccess) return (int) e;
+	regroup_cell_buckets_kernel<<<grid_for(n, 256, 8), 256, 0, st>>>(cfg, n, cellbuckets, grouped);
+	warp_flatten_kernel<<<(block_count + 7) / 8, 256, 0, st>>>(cfg, block_count, cell_particle_counts, grouped, particle_bucket_sizes, buckets, cell_offsets);
+	e = cudaGetLastError();
+	const cudaError_t f = cudaFreeAsync(grouped, st);
+	return (int) (e != cudaSuccess ? e : f);
 }
 // ParticleBuffer<M> defaults (particle_buffer.cuh:141-264) as the step driver sets them (engine.cu)
 void cb200_default_material(const cb200_config* cfg, int material, cb200_particle_buffer* out);

@@ -151,6 +151,13 @@ __device__ __forceinline__ void start_state(int material, const float* x, float*
 __device__ __forceinline__ bool in_domain(const Cfg& c, int x, int y, int z) { return ((unsigned) x < (unsigned) c.gsize) & ((unsigned) y < (unsigned) c.gsize) & ((unsigned) z < (unsigned) c.gsize); }
 __device__ __forceinline__ int table_offset(const Cfg& c, int x, int y, int z) { return (((x << c.gbits) + y) << c.gbits) + z; }
 __device__ __forceinline__ int table_query(const Cfg& c, const int* __restrict__ table, int x, int y, int z) { return in_domain(c, x, y, z) ? __ldg(table + table_offset(c, x, y, z)) : -1; }
+// Slot `slot` of cell `cell` of block `block` in the step driver's cell buckets.  The reference's rows ((block * 64 + cell) * max_ppc
+// + slot) are kept by the kernel-level ABI; the driver groups slots by eight inside each block's ppb slice, [max_ppc / 8][64 cells][8],
+// so that slots 0-7 of all 64 cells of a block (every tag of a block whose cells hold at most eight) are 2 KiB of contiguous memory,
+// and one warp load of the flatten (eight slots of four cells) is one 128-byte line.  max_ppc is a power of two >= 8 (cfg_valid).
+__device__ __forceinline__ size_t grouped_cell_slot(const Cfg& c, size_t block, int cell, int slot) {
+	return (block << c.ppb_shift) + ((slot >> 3) << 9) + (cell << 3) + (slot & 7);
+}
 // get_block_id (utility_funcs.hpp:21-23): round-half-away-from-zero of p * dx_inv
 __device__ __forceinline__ int cell_index(const Cfg& c, float p) { return __float2int_rn(roundf(p * c.dx_inv)); }
 

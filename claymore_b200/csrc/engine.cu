@@ -857,7 +857,7 @@ void preload_kernels() {
 	preload(summary_kernel);
 	preload(rebuild_kernel);
 	preload(register_blocks_kernel);
-	preload(cell_bucket_to_block_kernel);
+	preload(warp_flatten_kernel);
 	preload(compute_bin_capacity_kernel);
 	preload(activate_blocks_kernel<true>);
 	preload(build_particle_cell_buckets_kernel<true>);
@@ -1201,7 +1201,8 @@ static int setup_impl(cb200_sim* s, const StartSrc& src) {
 	if(pbc > cap) return (int) cudaErrorMemoryAllocation;
 	for(Model& m : s->models) {
 		build_particle_cell_buckets_kernel<true><<<grid_for(m.n, 256, 16), 256, 0, st>>>(cfg, m.n, m.d_pos, view(m.pb[R]), P.index_table, err);
-		cell_bucket_to_block_kernel<<<grid_for(pbc, 1, 16), kBucketThreads, 0, st>>>(cfg, pbc, m.pb[R].cell_particle_counts, m.pb[R].cellbuckets, m.pb[R].particle_bucket_sizes, m.pb[R].blockbuckets, m.celloffs[Rn]);
+		// the sub-step's flatten, in place: the driver's cell buckets have one (slot-grouped) layout whoever wrote them
+		warp_flatten_kernel<<<grid_for(pbc, 8, 8), 256, 0, st>>>(cfg, pbc, m.pb[R].cell_particle_counts, m.pb[R].cellbuckets, m.pb[R].particle_bucket_sizes, m.pb[R].blockbuckets, m.celloffs[Rn]);
 		compute_bin_capacity_kernel<<<grid_for(pbc + 1, 256, 16), 256, 0, st>>>(pbc + 1, m.pb[R].particle_bucket_sizes, m.bin_sizes);
 		ScanArgs a {};
 		a.count = count_imm(pbc + 1);

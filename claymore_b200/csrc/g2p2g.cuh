@@ -546,8 +546,10 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 						atomicSub(M.next.cell_particle_counts + rb_cell, 1);
 						if(a.error) atomicOr(a.error, kErrCellOverflow);
 					} else {
-						// cellbuckets index = block * ppb + cell * max_ppc + slot == (block*64 + cell) * max_ppc + slot
-						M.next.cellbuckets[(rb_cell << cfg.ppc_shift) + rb_slot] = rb_tag;
+						// SORTED (the step driver): its own slot-grouped layout, which its flatten reads (grouped_cell_slot).  Otherwise the
+						// reference's rows of the kernel-level ABI: block * ppb + cell * max_ppc + slot == (block*64 + cell) * max_ppc + slot
+						if constexpr(SORTED) M.next.cellbuckets[grouped_cell_slot(cfg, rb_cell >> 6, (int) rb_cell & 63, rb_slot)] = rb_tag;
+						else M.next.cellbuckets[(rb_cell << cfg.ppc_shift) + rb_slot] = rb_tag;
 					}
 				}
 

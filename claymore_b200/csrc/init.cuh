@@ -22,7 +22,8 @@ __global__ void activate_blocks_kernel(Cfg cfg, int n, const float* pos, int* ta
 	}
 }
 
-// build_particle_cell_buckets (mgmpm_kernels.cuh:36-68)
+// build_particle_cell_buckets (mgmpm_kernels.cuh:36-68).  FLOOR = true is the step driver's: it writes the driver's slot-grouped cell
+// buckets (grouped_cell_slot), which its warp flatten reads; the kernel-level drop-in writes the reference's cell-major rows.
 template<bool FLOOR>
 __global__ void build_particle_cell_buckets_kernel(Cfg cfg, int n, const float* pos, PBuf pb, const int* table, int* error) {
 	for(int p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
@@ -40,7 +41,8 @@ __global__ void build_particle_cell_buckets_kernel(Cfg cfg, int n, const float* 
 			if(error) atomicOr(error, kErrCellOverflow);
 			continue;
 		}
-		pb.cellbuckets[((size_t) bno << cfg.ppb_shift) + (cellno << cfg.ppc_shift) + slot] = p;
+		if(FLOOR) pb.cellbuckets[grouped_cell_slot(cfg, bno, cellno, slot)] = p;
+		else pb.cellbuckets[((size_t) bno << cfg.ppb_shift) + (cellno << cfg.ppc_shift) + slot] = p;
 	}
 }
 

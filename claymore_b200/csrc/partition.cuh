@@ -113,10 +113,11 @@ __global__ void scan_inverse_kernel(int num, const int* map, int* map_inv) {
 // writes (each thread finds its cell by a 6-step search of the 65-entry prefix in shared memory), instead of
 // 128 rounds of warp-aggregated atomics each ending in a block barrier.  Bucket order is CELL-MAJOR: lanes of
 // a warp in g2p2g then share stencil nodes and read near-contiguous source slots.
-// dst_block lets the caller write straight into the compacted numbering (fuses update_buckets, :979-1000).
+// It reads the reference's cell-major rows: it serves the kernel-level entry cb200_cell_bucket_to_block.  The step driver's cell
+// buckets are slot-grouped (grouped_cell_slot) and flattened by warp_flatten_block below.
 // ------------------------------------------------------------------------------------------------
 constexpr int kBucketThreads = 128;
-__device__ __forceinline__ int flatten_block(const Cfg& cfg, const int* __restrict__ cell_counts_blk, const int* __restrict__ cellbuckets_blk, int* __restrict__ dst, int* s_prefix, unsigned short* __restrict__ offs = nullptr) {
+__device__ __forceinline__ int flatten_block(const Cfg& cfg, const int* __restrict__ cell_counts_blk, const int* __restrict__ cellbuckets_blk, int* __restrict__ dst, int* s_prefix) {
 	const int tid = threadIdx.x, lane = tid & 31;
 	if(tid < 32) {
 		const int2 c = reinterpret_cast<const int2*>(cell_counts_blk)[lane];
@@ -133,7 +134,6 @@ __device__ __forceinline__ int flatten_block(const Cfg& cfg, const int* __restri
 	}
 	__syncthreads();
 	const int total = s_prefix[64];
-	if(offs && tid < 64) offs[tid] = (unsigned short) s_prefix[tid];  // where the cells start inside the cell-major bucket (read by g2p2g's phase 2)
 	for(int i = tid; i < total; i += kBucketThreads) {
 		int c = 0;
 #pragma unroll
@@ -145,10 +145,10 @@ __device__ __forceinline__ int flatten_block(const Cfg& cfg, const int* __restri
 	return total;
 }
 
-__global__ void __launch_bounds__(kBucketThreads) cell_bucket_to_block_kernel(Cfg cfg, int block_count, const int* cell_particle_counts, const int* cellbuckets, int* particle_bucket_sizes, int* buckets, unsigned short* cell_offsets = nullptr) {
+__global__ void __launch_bounds__(kBucketThreads) cell_bucket_to_block_kernel(Cfg cfg, int block_count, const int* cell_particle_counts, const int* cellbuckets, int* particle_bucket_sizes, int* buckets) {
 	__shared__ int s_prefix[65];
 	for(int b = blockIdx.x; b < block_count; b += gridDim.x) {
-		const int total = flatten_block(cfg, cell_particle_counts + (size_t) b * kBlockVol, cellbuckets + ((size_t) b << cfg.ppb_shift), buckets + ((size_t) b << cfg.ppb_shift), s_prefix, cell_offsets ? cell_offsets + (size_t) b * kBlockVol : nullptr);
+		const int total = flatten_block(cfg, cell_particle_counts + (size_t) b * kBlockVol, cellbuckets + ((size_t) b << cfg.ppb_shift), buckets + ((size_t) b << cfg.ppb_shift), s_prefix);
 		if(threadIdx.x == 0) particle_bucket_sizes[b] += total;
 	}
 }
@@ -321,14 +321,15 @@ __global__ void __launch_bounds__(kSummaryThreads) summary_kernel(const SummaryA
 	}
 }
 
-// one WARP per old block, no search: the block's tags are walked in the order they lie in `cellbuckets` (cell-major rows of
-// max_ppc slots), eight slots of four cells per step, and the bucket is those tags with the empty slots left out.  A lane
-// therefore knows its destination from its cell's count and exclusive prefix alone (one shuffle each from the lane that scanned
-// the cell): every load of a step is one 32-byte sector per cell, independent of every other load, kBatch steps are in flight
-// per warp before the first is consumed, and the valid tags of a step land in one contiguous run of the bucket.
-// Cells holding more than eight tags take further passes over the slots [8 g, 8 g + 8); the order inside a cell is its slot order.
-constexpr int kFlattenBatch = 8;
-__device__ __forceinline__ int warp_flatten_block(const Cfg& cfg, const int2 c, const int* __restrict__ cellbuckets_blk, int* __restrict__ dst, unsigned short* __restrict__ offs) {
+// one WARP per old block, no search: the block's tags are walked in the order they lie in the driver's slot-grouped cell buckets
+// (grouped_cell_slot: [max_ppc / 8 slot groups][64 cells][8 slots]), eight slots of four cells per step, and the bucket is those
+// tags with the empty slots left out.  A lane therefore knows its destination from its cell's count and exclusive prefix alone (one
+// shuffle each from the lane that scanned the cell): the load of a step is one 128-byte line (lane = 8 sub + slot inside the group,
+// cell 4 k + sub), independent of every other load, kFlattenBatch steps are in flight per warp before the first is consumed, and
+// the valid tags of a step land in one contiguous run of the bucket.  Cells holding more than eight tags take further passes over
+// the slot groups [8 g, 8 g + 8); the order inside a cell is its slot order, so the bucket is the reference flatten's.
+constexpr int kFlattenBatch = 4;   // steps in flight per warp: 4, 8 and 16 measured 0.150, 0.153 and 0.209 ms on the 40 M-particle scene (DESIGN section 4)
+__device__ __forceinline__ int warp_flatten_block(const int2 c, const int* __restrict__ cellbuckets_blk, int* __restrict__ dst, unsigned short* __restrict__ offs) {
 	const int lane = threadIdx.x & 31;
 	const int pair = c.x + c.y;
 	int inc = pair;
@@ -357,7 +358,7 @@ __device__ __forceinline__ int warp_flatten_block(const Cfg& cfg, const int2 c, 
 				const int mo = __shfl_sync(0xffffffffu, meta_odd, cell >> 1);
 				const int meta = (cell & 1) ? mo : me;
 				at[u] = slot < (meta & 0xff) ? (meta >> 8) + slot : -1;
-				if(at[u] >= 0) tag[u] = __ldg(cellbuckets_blk + (cell << cfg.ppc_shift) + slot);
+				if(at[u] >= 0) tag[u] = __ldg(cellbuckets_blk + g8 * 64 + 32 * (k0 + u) + lane);  // == grouped_cell_slot(cfg, 0, cell, slot)
 			}
 #pragma unroll
 			for(int u = 0; u < kFlattenBatch; ++u)
@@ -367,12 +368,13 @@ __device__ __forceinline__ int warp_flatten_block(const Cfg& cfg, const int2 c, 
 	return total;
 }
 
-// the flatten above on its own, one warp per block in place (no renumbering): what the tests hold against cell_bucket_to_block_kernel
+// the flatten above on its own, one warp per block in place (no renumbering): the driver's set-up flattens the cell buckets that
+// build_particle_cell_buckets_kernel<true> wrote with it, so the driver has one layout and one flatten whoever wrote the buckets
 __global__ void __launch_bounds__(256) warp_flatten_kernel(Cfg cfg, int block_count, const int* cell_particle_counts, const int* cellbuckets, int* particle_bucket_sizes, int* buckets, unsigned short* cell_offsets) {
 	const int lane = threadIdx.x & 31;
 	for(int b = blockIdx.x * 8 + (threadIdx.x >> 5); b < block_count; b += gridDim.x * 8) {
 		const int2 c = reinterpret_cast<const int2*>(cell_particle_counts + (size_t) b * kBlockVol)[lane];
-		const int total = warp_flatten_block(cfg, c, cellbuckets + ((size_t) b << cfg.ppb_shift), buckets + ((size_t) b << cfg.ppb_shift), cell_offsets + (size_t) b * kBlockVol);
+		const int total = warp_flatten_block(c, cellbuckets + ((size_t) b << cfg.ppb_shift), buckets + ((size_t) b << cfg.ppb_shift), cell_offsets + (size_t) b * kBlockVol);
 		if(lane == 0) particle_bucket_sizes[b] = total;
 	}
 }
@@ -466,7 +468,7 @@ __global__ void __launch_bounds__(kRebuildThreads, 5) rebuild_kernel(const Rebui
 				if(++nmod == nm) nmod = 0, ++nj;
 				advance(nj, nmod);
 				if(nj < PER_WARP) next_row = count_row(nj, nmod);
-				total = warp_flatten_block(cfg, row, a.cellbuckets[m] + ((size_t) b << cfg.ppb_shift), a.dst_buckets[m] + ((size_t) nb << cfg.ppb_shift),
+				total = warp_flatten_block(row, a.cellbuckets[m] + ((size_t) b << cfg.ppb_shift), a.dst_buckets[m] + ((size_t) nb << cfg.ppb_shift),
 				                           a.dst_offs[m] ? a.dst_offs[m] + (size_t) nb * kBlockVol : nullptr);
 			}
 			if(lane == 0) {

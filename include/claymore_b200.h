@@ -18,6 +18,8 @@
  *                    count int[1]                                            hash_table.cuh:75-135
  *   buckets        : cellbuckets/blockbuckets int[blocks*64*max_ppc]; tag = dir*(64*max_ppc) | pidib
  *                                                                            particle_buffer.cuh:134
+ *                    (cellbuckets: cell-major rows, slot s of cell c of block b at (b*64 + c)*max_ppc + s; the step
+ *                    driver's internal cell buckets group the slots by eight instead and are not visible through the ABI)
  */
 #ifndef CLAYMORE_B200_H
 #define CLAYMORE_B200_H
@@ -445,7 +447,8 @@ CB200_API int cb200_sim_add_particles_sdf(cb200_sim* sim, int model, const cb200
 CB200_API int cb200_test_svd3(int n, const float* F, float* U, float* S, float* V, void* stream);
 CB200_API int cb200_test_stress(int material, int mode, cb200_particle_buffer params, int n, const float* F_in, const float* log_jp_in, float* F_out, float* PF_out, float* log_jp_out, void* stream);
 /* The step driver's bucket flatten (the rebuild's warp-per-block copy) on caller-supplied DEVICE containers of `block_count` blocks, in place
- * of cb200_cell_bucket_to_block: sizes are SET (not added to), and cell_offsets[64 * block_count] receives every cell's start in its bucket. */
+ * of cb200_cell_bucket_to_block: sizes are SET (not added to), and cell_offsets[64 * block_count] receives every cell's start in its bucket.
+ * `cellbuckets` is in the reference's layout; the hook regroups it into the driver's own in a stream-ordered scratch allocation first. */
 CB200_API int cb200_test_warp_flatten(const cb200_config* cfg, int block_count, const int* cell_particle_counts, const int* cellbuckets, int* particle_bucket_sizes, int* buckets, unsigned short* cell_offsets, void* stream);
 /* ParticleBuffer<M> default parameters (particle_buffer.cuh:141-264) for `material` on the grid of `cfg` (pointers zero) */
 CB200_API void cb200_default_material(const cb200_config* cfg, int material, cb200_particle_buffer* out);

@@ -27,7 +27,7 @@ SECTOR = 32
 
 def byte_model(pbc, nbc, ebc, particles, models, max_ppc):
     """{kernel: bytes one sub-step's launch has to move}.  pbc / nbc / ebc: particle, + neighbour, + exterior blocks."""
-    tags_in = particles * 4   # the eight or so tags of a cell fill one 32-byte sector of its max_ppc row
+    tags_in = particles * 4   # the eight or so tags of a cell are its first slot group: 32 contiguous bytes of the block's 2 KiB group 0
     return {
         # read + write every grid block, zero the next grid's, zero every model's cell counts over the exterior blocks
         "grid_update_kernel": nbc * 3 * GRID_BLOCK + ebc * models * COUNT_ROW,
