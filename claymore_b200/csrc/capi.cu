@@ -385,4 +385,17 @@ int cb200_test_warp_flatten(const cb200_config* c, int block_count, const int* c
 }
 // ParticleBuffer<M> defaults (particle_buffer.cuh:141-264) as the step driver sets them (engine.cu)
 void cb200_default_material(const cb200_config* cfg, int material, cb200_particle_buffer* out);
+#ifdef CB200_G2P2G_PHASE_CLOCKS
+// g2p2g's per-phase cycle sums (G2P2GClock order, kClkCount values) since the last reset, summed over every CTA of every launch
+// on the current device; reset != 0 zeroes them after the read.  Exported only by the instrumented build (tools/g2p2g_phase_clocks.py).
+CB200_API int cb200_g2p2g_phase_clocks(unsigned long long* out, int reset) {
+	cudaError_t e = cudaDeviceSynchronize();
+	if(e == cudaSuccess && out) e = cudaMemcpyFromSymbol(out, g2p2g_phase_clocks, sizeof(g2p2g_phase_clocks));
+	if(e == cudaSuccess && reset) {
+		const unsigned long long zero[kClkCount] = {};
+		e = cudaMemcpyToSymbol(g2p2g_phase_clocks, zero, sizeof(zero));
+	}
+	return (int) e;
+}
+#endif
 }

@@ -87,6 +87,18 @@ __device__ __forceinline__ int acc_off_x(int X) { return ((X >> 2) << 2) * 256 +
 __device__ __forceinline__ int acc_off_y(int Y) { return ((Y >> 2) << 1) * 256 + ((Y & 3) << 2); }
 __device__ __forceinline__ int acc_off_z(int Z) { return (Z >> 2) * 256 + (Z & 3); }
 
+// What a particle block's processing starts from.  Resolved one block ahead (the CTA knows its next ticket during the whole
+// current block), in shared memory only, by cp.async copies issued where the current block waits anyway: so a block starts
+// with its TMA copy and its first positions in flight right away instead of after five dependent round trips.
+struct G2P2GHeader {
+	int blk;                // the particle block this header describes (-1: none)
+	int key[3];
+	int size[kMaxModels];   // bucket size of every model
+	int nbr[27];            // neighbour block numbers (next partition)
+	int prevno[27];         // the same neighbours' block numbers in the previous partition
+	int srcbin[27];         // their first bins in the source buffer of the block's first non-empty model (then of the model processed)
+};
+
 struct G2P2GSmem {
 	float4 vel4[512];                // node-major velocity arena (v_y, v_z, v_x, gather tag in flight), index (X*8+Y)*8+Z
 	float acc[8 * 256];              // accumulation arena (grid-block layout)
@@ -96,14 +108,69 @@ struct G2P2GSmem {
 	unsigned short movers[kChunk];   // staged slots of particles that changed cell
 	unsigned short offs[66];         // SORTED: cell starts of the current model's bucket, [64] = bucket size
 	int cnt[64];
-	int nbr[27];
-	int prevno[27];
-	int srcbin[27];
+	G2P2GHeader hdr[2];              // the current block's header and the next one's, being resolved
 	int nmovers;
-	int cur_blk, next_blk;
+	int cur_blk, next_blk, hsel;     // hsel: hdr[hsel] is the current block's
 	unsigned valid;                  // bit b: grid block b of the 2x2x2 neighbourhood exists
 	unsigned long long bar;
+#ifdef CB200_G2P2G_PHASE_CLOCKS
+	long long clk_t0, clk_mark;      // thread 0's clock at kernel entry and at the last phase boundary
+	unsigned long long clk[8];       // this CTA's sums, added to g2p2g_phase_clocks when it exits
+#endif
 };
+
+// Per-phase cycle counters (off by default; `make EXTRA=-DCB200_G2P2G_PHASE_CLOCKS`, read by tools/g2p2g_phase_clocks.py).
+// Thread 0 of every CTA reads clock64() at the phase boundaries below and adds the intervals up; the sums of all CTAs are
+// added into this array when they exit.  Without the switch the macros expand to nothing and the kernel is unchanged.
+enum G2P2GClock {
+	kClkPrologue = 0,  // block top (from the previous block's B6) to S2: a header not resolved ahead, neighbourhood, first positions; empty blocks
+	kClkPhase1,        // S2 (or a chunk's own prologue) to B1
+	kClkPhase2,        // B1 to the second arena-round barrier
+	kClkPhase3,        // node-parallel movers
+	kClkFlush,         // end of the last chunk's phase 3 to B6
+	kClkChunkPrologue, // every chunk after a block's first (later chunks, later models): barriers, source bins, tags, first positions
+	kClkLateFirst,     // count: blocks whose first non-empty model is not model 0
+	kClkTotal,         // whole CTA, kernel entry to exit
+	kClkCount
+};
+#ifdef CB200_G2P2G_PHASE_CLOCKS
+static_assert(kClkCount <= 8, "G2P2GSmem::clk");
+__device__ unsigned long long g2p2g_phase_clocks[kClkCount];
+#define CB200_CLK_START()                                                                      \
+	do {                                                                                       \
+		if(threadIdx.x == 0) {                                                                 \
+			for(int k_ = 0; k_ < kClkCount; ++k_) sm.clk[k_] = 0;                              \
+			sm.clk_t0 = sm.clk_mark = clock64();                                               \
+		}                                                                                      \
+	} while(0)
+#define CB200_CLK_MARK(k)                                                                      \
+	do {                                                                                       \
+		if(threadIdx.x == 0) {                                                                 \
+			const long long now_ = clock64();                                                  \
+			sm.clk[(k)] += (unsigned long long) (now_ - sm.clk_mark);                          \
+			sm.clk_mark = now_;                                                                \
+		}                                                                                      \
+	} while(0)
+#define CB200_CLK_COUNT(k)                                                                     \
+	do {                                                                                       \
+		if(threadIdx.x == 0) sm.clk[(k)] += 1;                                                 \
+	} while(0)
+#define CB200_CLK_END()                                                                        \
+	do {                                                                                       \
+		if(threadIdx.x == 0) {                                                                 \
+			sm.clk[kClkTotal] = (unsigned long long) (clock64() - sm.clk_t0);                  \
+			for(int k_ = 0; k_ < kClkCount; ++k_) atomicAdd(&g2p2g_phase_clocks[k_], sm.clk[k_]); \
+		}                                                                                      \
+	} while(0)
+#else
+#define CB200_CLK_START() do {} while(0)
+#define CB200_CLK_MARK(k) do {} while(0)
+#define CB200_CLK_COUNT(k) do {} while(0)
+#define CB200_CLK_END() do {} while(0)
+#endif
+
+// four CTAs per SM: 228 KB of shared memory per SM, 1 KB of it reserved per CTA
+static_assert(CB200_G2P2G_MIN_CTAS * (sizeof(G2P2GSmem) + 1024) <= 228 * 1024, "G2P2GSmem no longer fits the CTAs per SM of the launch bounds");
 
 // Staged records are XOR-swizzled: cell-major buckets put the p-th particles of consecutive cells 8 slots = 128 B apart,
 // i.e. in the same four banks; unswizzled, phase 2 spent 3-5 wavefronts per 16-byte read (profiles/r01_final_*).
@@ -145,6 +212,10 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 	// others (whose kernels are larger or whose phase 1 is shorter) the extra code cost 2-5 % on sand and fluid scenes that have no
 	// movers (H100, DESIGN section 2.1), so their movers all take phase 3 as before.
 	constexpr bool ARRIVALS = SORTED && MAT == CB200_FIXED_COROTATED;
+	// Block headers resolved one block ahead (G2P2GHeader) in the fixed-corotated and fluid builds.  The sand build was 4-5 % slower
+	// with them on the sand column (H100, DESIGN section 4), so it and the NACC build (the same SVD-heavy phase 1, not measured)
+	// resolve each block's header at its top, one load after another, as before.
+	constexpr bool AHEAD = MAT == CB200_FIXED_COROTATED || MAT == CB200_J_FLUID;
 
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	G2P2GSmem& sm = *reinterpret_cast<G2P2GSmem*>(smem_raw);
@@ -166,6 +237,7 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 		sm.nmovers = 0;
 	}
 	if(threadIdx.x < 64) sm.cnt[threadIdx.x] = 0;
+	CB200_CLK_START();
 	__syncthreads();
 	unsigned phase = 0;
 	const float dx = cfg.dx, dx_inv = cfg.dx_inv, d_inv = cfg.d_inv;
@@ -174,7 +246,7 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 	// block queue: CTAs pull particle blocks from a device counter, so a launch that shares the SMs with another launch or
 	// starts late still balances.  The queue runs two blocks ahead: thread 0 keeps the newest ticket in a register, so the
 	// atomic's round trip hides behind a whole block, and the queue shift rides on the flush barrier of the block before.
-	// Barriers per (single-chunk) block: S1, S2, B1, B2, two for the arena rounds, B6.
+	// Barriers per (single-chunk) block: S2, B1, B2 (any-order form only), two for the arena rounds, B6; without AHEAD also S1.
 	int q_pending = 0;
 	if(threadIdx.x == 0) {
 		if(a.work_counter) {
@@ -184,42 +256,119 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 			sm.cur_blk = (int) blockIdx.x;
 			sm.next_blk = (int) (blockIdx.x + gridDim.x);
 		}
+		sm.hdr[0].blk = sm.hdr[1].blk = -1;
+		sm.hsel = 0;
 	}
 	__syncthreads();
+
+	// ---- the block header (G2P2GHeader), in stages.  Every thread that issues one of these copies waits for it with a
+	// cp_async_wait<0> before any counted wait of phase 1 (they ride in the positions' group, or are followed by the wait<0>
+	// before B6), and each is published by a barrier or read only by the thread that copied it.
+	// sizes and key of block b (warp 1)
+	auto hdr_sizes_key = [&](G2P2GHeader& h, int b) {
+		const int t = opaque_tid() - 32;
+		if(t >= 0 && t < a.n_models) cp_async4(&h.size[t], a.m[t].next.particle_bucket_sizes + b);
+		else if(t >= kMaxModels && t < kMaxModels + 3) cp_async4(&h.key[t - kMaxModels], a.keys + 3 * b + (t - kMaxModels));
+	};
+	// neighbour block numbers in both partitions, from the landed key (thread 32 + d: neighbour d)
+	auto hdr_tables = [&](G2P2GHeader& h) {
+		const int d = opaque_tid() - 32;
+		if(d >= 0 && d < 27) {
+			const int x = h.key[0] + d / 9 - 1, y = h.key[1] + (d / 3) % 3 - 1, z = h.key[2] + d % 3 - 1;
+			if(in_domain(cfg, x, y, z)) {
+				const int o = table_offset(cfg, x, y, z);
+				cp_async4(&h.nbr[d], a.table + o);
+				cp_async4(&h.prevno[d], a.prev_table + o);
+			} else {
+				h.nbr[d] = h.prevno[d] = -1;
+			}
+		}
+	};
+	// first model from `from` on with particles in the block (n_models: none)
+	auto hdr_first = [&](const G2P2GHeader& h, int from) {
+		int f = from;
+		while(f < a.n_models && h.size[f] == 0) ++f;
+		return f;
+	};
+	// source bins of model f, by the thread that copied prevno[d] (it waits for its own copies: no barrier)
+	auto hdr_srcbin = [&](G2P2GHeader& h, int f) {
+		const int d = opaque_tid() - 32;
+		if(d >= 0 && d < 27) {
+			cp_async_wait<0>();
+			const int pno = h.prevno[d];
+			if(pno >= 0) cp_async4(&h.srcbin[d], a.m[f].cur.bin_offsets + pno);
+			else h.srcbin[d] = -1;
+		}
+	};
+	// gather tags of the first chunk of model f, into the unused w components of the velocity arena (512 words for 512 staged
+	// particles); thread t fetches the tags it will consume itself
+	auto hdr_tags = [&](const G2P2GHeader& h, int b, int f) {
+		const int t = opaque_tid();
+		const int size0 = min(h.size[f], kChunk);
+		const int* bucket0 = a.m[f].next.blockbuckets + ((size_t) b << cfg.ppb_shift);
+#pragma unroll
+		for(int it = 0; it < ITERS; ++it)
+			if(it * T + t < size0) cp_async4(&sm.vel4[it * T + t].w, bucket0 + it * T + t);
+	};
+
 	for(;;) {
 		const int tid = opaque_tid();  // (not loop-invariant to the compiler: see opaque_tid)
 		const int qi = sm.cur_blk, qn = sm.next_blk;  // published by the last barrier every thread passed
 		if(qi >= nblocks) break;
 		if(tid == 0) q_pending = a.work_counter ? atomicAdd(a.work_counter, 1) : qn + (int) gridDim.x;
 		const int blk = qi;
-		int total_size = 0;
-		for(int mi = 0; mi < a.n_models; ++mi) total_size += a.m[mi].next.particle_bucket_sizes[blk];
-		if(total_size == 0) {
+		G2P2GHeader& H = sm.hdr[AHEAD ? sm.hsel : 0];
+		int kx = 0, ky = 0, kz = 0;  // without AHEAD: the key, in registers
+		int first;  // first model with particles in the block (n_models: none)
+		if constexpr(AHEAD) {
+			if(H.blk != qi) {
+				// not resolved ahead (the CTA's first block, or the one after an empty block): the stages one after another
+				hdr_sizes_key(H, qi);
+				cp_async_commit();
+				cp_async_wait<0>();
+				__syncthreads();  // R1: sizes, key
+				hdr_tables(H);
+				const int f = hdr_first(H, 0);
+				if(f < a.n_models) hdr_tags(H, qi, f);
+				cp_async_commit();
+				if(f < a.n_models) hdr_srcbin(H, f);
+				cp_async_commit();
+				cp_async_wait<0>();
+				__syncthreads();  // R2: tables, source bins, tags
+			}
+			first = hdr_first(H, 0);
+		} else {
+			first = 0;
+			while(first < a.n_models && a.m[first].next.particle_bucket_sizes[blk] == 0) ++first;
+		}
+		if(first == a.n_models) {
 			__syncthreads();
 			if(tid == 0) {
 				sm.cur_blk = qn;
 				sm.next_blk = q_pending;
+				if(AHEAD) sm.hsel ^= 1;
 			}
 			__syncthreads();
+			CB200_CLK_MARK(kClkPrologue);
 			continue;
 		}
-		const int kx = a.keys[3 * blk], ky = a.keys[3 * blk + 1], kz = a.keys[3 * blk + 2];
-		// Gather tags of the first chunk: copied asynchronously into the unused w components of the velocity arena (512 words
-		// for 512 staged particles) while the neighbourhood is staged.  Thread t fetches the tags it will consume itself.
-		{
-			const int size0 = min(a.m[0].next.particle_bucket_sizes[blk], kChunk);
-			const int* bucket0 = a.m[0].next.blockbuckets + ((size_t) blk << cfg.ppb_shift);
+		if constexpr(!AHEAD) {
+			kx = a.keys[3 * blk], ky = a.keys[3 * blk + 1], kz = a.keys[3 * blk + 2];
+			// gather tags of the first chunk, copied while the neighbourhood is staged (thread t fetches the tags it consumes itself)
+			const int size0 = min(a.m[first].next.particle_bucket_sizes[blk], kChunk);
+			const int* bucket0 = a.m[first].next.blockbuckets + ((size_t) blk << cfg.ppb_shift);
 #pragma unroll
 			for(int it = 0; it < ITERS; ++it)
 				if(it * T + tid < size0) cp_async4(&sm.vel4[it * T + tid].w, bucket0 + it * T + tid);
 			cp_async_commit();
 		}
 
-		// ---- stage the neighbourhood -------------------------------------------------------------
+		// ---- stage the neighbourhood, request the first positions --------------------------------------------
 		// (the landing zone aliases the records of the previous block: its last readers are behind that block's B6)
 		if(tid < 32) {
 			const int lb = tid & 7;
-			const int bno = table_query(cfg, a.table, kx + ((lb >> 2) & 1), ky + ((lb >> 1) & 1), kz + (lb & 1));
+			const int bno = AHEAD ? H.nbr[(((lb >> 2) & 1) + 1) * 9 + (((lb >> 1) & 1) + 1) * 3 + (lb & 1) + 1]
+			                      : table_query(cfg, a.table, kx + ((lb >> 2) & 1), ky + ((lb >> 1) & 1), kz + (lb & 1));
 			const unsigned valid = __ballot_sync(0xffffffffu, tid < 8 && bno >= 0);
 			if(tid == 0) {
 				sm.valid = valid;  // released by the arrive, acquired by every thread's wait
@@ -227,13 +376,13 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 			}
 			__syncwarp();
 			if(tid < 8 && bno >= 0) tma_load_1d(velsoa + lb * 192, a.grid + (size_t) bno * kGridBlockFloats + 64, 768, bar);
-		} else if(tid < 32 + 27) {
+		} else if(!AHEAD && tid < 32 + 27) {
 			const int d = tid - 32;
 			const int ox = d / 9 - 1, oy = (d / 3) % 3 - 1, oz = d % 3 - 1;
-			sm.nbr[d] = table_query(cfg, a.table, kx + ox, ky + oy, kz + oz);
+			H.nbr[d] = table_query(cfg, a.table, kx + ox, ky + oy, kz + oz);
 			const int pno = table_query(cfg, a.prev_table, kx + ox, ky + oy, kz + oz);
-			sm.prevno[d] = pno;
-			sm.srcbin[d] = pno >= 0 ? a.m[0].cur.bin_offsets[pno] : -1;  // model 0; further models resolve theirs below
+			H.prevno[d] = pno;
+			H.srcbin[d] = pno >= 0 ? a.m[first].cur.bin_offsets[pno] : -1;  // further models resolve theirs below
 		}
 		bool acc_dirty = true;  // the arena still feeds the previous block's bulk reductions: it is drained and zeroed just
 		                        // before this block's first accumulation, i.e. behind its whole phase 1
@@ -241,7 +390,7 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 		auto src_of = [&](const float* bins, int slot) {
 			const int tag = __float_as_int(sm.vel4[slot].w);
 			const int sp = tag & ppb_mask;
-			return bins + ((size_t) sm.srcbin[tag >> cfg.ppb_shift] + (sp >> 5)) * BINF + (sp & 31);
+			return bins + ((size_t) H.srcbin[tag >> cfg.ppb_shift] + (sp >> 5)) * BINF + (sp & 31);
 		};
 		auto fetch_pos = [&](const float* bins, int slot) {
 			const float* sb = src_of(bins, slot);
@@ -250,16 +399,17 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 			cp_async4(dst + 1, sb + 32);
 			cp_async4(dst + 2, sb + 64);
 		};
-		bool primed = false;  // tags and first positions of (model 0, chunk 0) already requested
-		{
-			const int size0 = min(a.m[0].next.particle_bucket_sizes[blk], kChunk);
+		if constexpr(AHEAD) {
+			// the next block's sizes and key ride in the first positions' group (waited for in phase 1 or before B1)
+			if(qn < nblocks) hdr_sizes_key(sm.hdr[sm.hsel ^ 1], qn);
+			if(tid < min(H.size[first], kChunk)) fetch_pos(a.m[first].cur.bins, tid);
+			cp_async_commit();
+		} else {
+			const int size0 = min(a.m[first].next.particle_bucket_sizes[blk], kChunk);
 			__syncthreads();  // S1: srcbin
-			if(size0 > 0) {
-				cp_async_wait<0>();  // this thread's tags
-				if(tid < size0) fetch_pos(a.m[0].cur.bins, tid);
-				cp_async_commit();
-				primed = true;
-			}
+			cp_async_wait<0>();  // this thread's tags
+			if(tid < size0) fetch_pos(a.m[first].cur.bins, tid);
+			cp_async_commit();
 		}
 		mbar_wait(bar, phase);
 		phase ^= 1;
@@ -270,18 +420,20 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				const int X = n >> 6, Y = (n >> 3) & 7, Z = n & 7;
 				const int bi = ((X >> 2) << 2) | ((Y >> 2) << 1) | (Z >> 2);
 				const int o = bi * 192 + (((X & 3) << 4) | ((Y & 3) << 2) | (Z & 3));
-				const bool ok = (valid >> bi) & 1u;  // w holds a gather tag in flight: write x, y, z only
+				const bool ok = (valid >> bi) & 1u;  // w holds a gather tag: write x, y, z only
 				// node layout (v_y, v_z, v_x, -): G2P's packed arithmetic pairs the components (1, 2)
 				*reinterpret_cast<float2*>(&sm.vel4[n].x) = ok ? make_float2(velsoa[o + 64], velsoa[o + 128]) : make_float2(0.f, 0.f);
 				sm.vel4[n].z = ok ? velsoa[o] : 0.f;
 			}
 		}
-		__syncthreads();  // S2: vel4, nbr, prevno, srcbin
+		__syncthreads();  // S2: vel4
+		CB200_CLK_MARK(kClkPrologue);
+		if(first != 0) CB200_CLK_COUNT(kClkLateFirst);
 
 		bool first_chunk = true;
-		for(int mi = 0; mi < a.n_models; ++mi) {
+		for(int mi = first; mi < a.n_models; ++mi) {
 		const G2P2GModel& M = a.m[mi];
-		const int bucket_size = M.next.particle_bucket_sizes[blk];
+		const int bucket_size = AHEAD ? H.size[mi] : M.next.particle_bucket_sizes[blk];
 		if(bucket_size == 0) continue;
 		const float mass = M.mat.mass;
 		const int dst_bin0 = M.next.bin_offsets[blk];
@@ -292,35 +444,32 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 			if constexpr(SORTED) {  // previous readers of sm.offs are behind a barrier (B6 / the arena rounds); B1 publishes the new values
 				if(c0 == 0 && tid <= 64) sm.offs[tid] = tid < 64 ? M.next_offs[(size_t) blk * kBlockVol + tid] : (unsigned short) bucket_size;
 			}
-			{
-				// every chunk after the first of a block waits for the previous one's phase 3; a further model resolves its bins
-				const bool need_srcbin = mi > 0 && c0 == 0;
-				if(!first_chunk || need_srcbin) {
-					if(!first_chunk) __syncthreads();
-					if(!first_chunk && tid == 0) sm.nmovers = 0;
-					if(need_srcbin && tid < 27) {
-						const int pno = sm.prevno[tid];
-						sm.srcbin[tid] = pno >= 0 ? M.cur.bin_offsets[pno] : -1;
-					}
-					__syncthreads();
-				}
-				first_chunk = false;
-			}
 			// Software pipeline of the gathers (no registers held, no reliance on the few KB of L1 left beside 208 KB of shared
 			// memory): tags sit in vel4[].w; the position of particle `slot` is copied into rec[0][slot] and its F / J / logJp into
 			// rec[1..3][slot] -- the particle's own record slot, which is written only at the end of its iteration.  Positions
-			// run one iteration ahead, F is in flight during G2P.
-			if(!(primed && mi == 0 && c0 == 0)) {
-				if(!(mi == 0 && c0 == 0)) {  // (model 0, chunk 0): tags were requested at the top of the block
-#pragma unroll
-					for(int it = 0; it < ITERS; ++it)
-						if(it * T + tid < nchunk) cp_async4(&sm.vel4[it * T + tid].w, bucket + c0 + it * T + tid);
-					cp_async_commit();
+			// run one iteration ahead, F is in flight during G2P.  The first chunk of the first non-empty model came with the
+			// header: its tags and source bins were resolved ahead and its positions requested at the top of the block.
+			if(!first_chunk) {
+				// every chunk after the first of a block waits for the previous one's phase 3; a further model resolves its bins
+				__syncthreads();
+				if(tid == 0) sm.nmovers = 0;
+				if(c0 == 0 && tid < 27) {
+					const int pno = H.prevno[tid];
+					H.srcbin[tid] = pno >= 0 ? M.cur.bin_offsets[pno] : -1;
 				}
+				__syncthreads();
+#pragma unroll
+				for(int it = 0; it < ITERS; ++it)
+					if(it * T + tid < nchunk) cp_async4(&sm.vel4[it * T + tid].w, bucket + c0 + it * T + tid);
+				cp_async_commit();
 				cp_async_wait<0>();
 				if(tid < nchunk) fetch_pos(M.cur.bins, tid);
 				cp_async_commit();
+				CB200_CLK_MARK(kClkChunkPrologue);
 			}
+			first_chunk = false;
+			// the block's last chunk resolves the next block's header (stages after B1, in the arena rounds, before B6)
+			auto resolves_next = [&]() { return AHEAD && qn < nblocks && c0 + kChunk >= bucket_size && hdr_first(H, mi + 1) == a.n_models; };
 			int cr0 = -1, cr1 = -1, cr2 = -1;  // (home cell << 16) | rank of the up-to-three particles of this thread
 			static_assert(ITERS <= 3, "cellrank registers");
 
@@ -445,12 +594,12 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 						nb[d] = cell_index(cfg, pos[d]) - 1;
 						cell[d] = nb[d] - 1;
 					}
-					rel[0] = (cell[0] >> 2) - kx;
-					rel[1] = (cell[1] >> 2) - ky;
-					rel[2] = (cell[2] >> 2) - kz;
+					rel[0] = (cell[0] >> 2) - (AHEAD ? H.key[0] : kx);
+					rel[1] = (cell[1] >> 2) - (AHEAD ? H.key[1] : ky);
+					rel[2] = (cell[2] >> 2) - (AHEAD ? H.key[2] : kz);
 #pragma unroll
 					for(int d = 0; d < 3; ++d) far |= (rel[d] < -1) | (rel[d] > 1);
-					const int bno = far ? -1 : sm.nbr[(rel[0] + 1) * 9 + (rel[1] + 1) * 3 + rel[2] + 1];
+					const int bno = far ? -1 : H.nbr[(rel[0] + 1) * 9 + (rel[1] + 1) * 3 + rel[2] + 1];
 					if(bno >= 0) {
 						const int dirtag = (1 - rel[0]) * 9 + (1 - rel[1]) * 3 + (1 - rel[2]);
 						const int cellno = ((cell[0] & 3) << 4) | ((cell[1] & 3) << 2) | (cell[2] & 3);
@@ -614,6 +763,17 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				acc_dirty = false;
 			}
 			__syncthreads();  // B1: records, cell counts and the mover list of this chunk are complete; the arena is zero
+			CB200_CLK_MARK(kClkPhase1);
+			if(resolves_next()) {
+				// the next block's tables from its landed key, and the tags of its first chunk: phases 2 and 3 do not read vel4, and a
+				// later chunk or model of this block would still read its own tags there
+				G2P2GHeader& Nx = sm.hdr[sm.hsel ^ 1];
+				hdr_tables(Nx);
+				const int nf = hdr_first(Nx, 0);
+				if(nf < a.n_models) hdr_tags(Nx, qn, nf);
+				cp_async_commit();
+				if(tid == 0) Nx.blk = qn;  // read at the top of the next block, behind B6 and every thread's wait<0> before it
+			}
 			// ================= phase 2: cell-parallel accumulation =====================================
 			// thread = (home cell hc, x-slice sl of its 3x3x3 stencil); a half-warp holds the 16 cells of one x-plane.
 			// The thread's cell, weight polynomial and nine arena offsets are derived from a fresh read of the thread index (see
@@ -780,7 +940,14 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 				}
 				__syncthreads();
 				if(wrp == 5) add_quad();
+				else if(wrp == 1 && resolves_next()) {  // the next block's source bins, from its landed previous-partition numbers
+					G2P2GHeader& Nx = sm.hdr[sm.hsel ^ 1];
+					const int nf = hdr_first(Nx, 0);
+					if(nf < a.n_models) hdr_srcbin(Nx, nf);
+					cp_async_commit();
+				}
 				__syncthreads();
+				CB200_CLK_MARK(kClkPhase2);
 				// arrival counts for the next chunk / block (ordered before its phase 1 by the barrier that starts it)
 				if(ARRIVALS && tid < 64) sm.cnt[tid] = 0;
 			}
@@ -808,19 +975,23 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 					atomicAdd(&sm.acc[o + 128], W * (r1.x + fi * r1.z + fj * r2.x + fk * r2.z));
 					atomicAdd(&sm.acc[o + 192], W * (r1.y + fi * r1.w + fj * r2.y + fk * r2.w));
 				}
+				CB200_CLK_MARK(kClkPhase3);
 			}
 		}
 		}  // models
 
 		// ---- arena -> next grid: eight 1-KiB bulk add-reductions ----------------------------------
 		const int ft = tid - (T - 32);  // the flush is issued by the first eight lanes of the LAST warp (they also drain it, see above)
-		const int flush_bno = (ft >= 0 && ft < 8) ? sm.nbr[(((ft >> 2) & 1) + 1) * 9 + (((ft >> 1) & 1) + 1) * 3 + (ft & 1) + 1] : -1;
+		const int flush_bno = (ft >= 0 && ft < 8) ? H.nbr[(((ft >> 2) & 1) + 1) * 9 + (((ft >> 1) & 1) + 1) * 3 + (ft & 1) + 1] : -1;
 		fence_proxy_async();
-		if(tid == 0) {  // queue shift: every thread read cur/next at the top of this block, barriers ago
+		if constexpr(AHEAD) cp_async_wait<0>();  // the next block's header copies this thread issued
+		if(tid == 0) {  // queue shift: every thread read cur/next/hsel at the top of this block, barriers ago
 			sm.cur_blk = qn;
 			sm.next_blk = q_pending;
+			if(AHEAD) sm.hsel ^= 1;
 		}
 		__syncthreads();  // B6: arena, records and neighbour tables of this block are no longer written or read by the SM
+		CB200_CLK_MARK(kClkFlush);
 		if(tid == 0) sm.nmovers = 0;
 		if(ft >= 0 && ft < 8) {
 			const int bno = flush_bno;
@@ -841,6 +1012,7 @@ __global__ void __launch_bounds__(kG2P2GThreads, CB200_G2P2G_MIN_CTAS) g2p2g_ker
 		}
 	}
 	if((int) threadIdx.x >= kG2P2GThreads - 32 && (int) threadIdx.x < kG2P2GThreads - 24) tma_wait_all<0>();
+	CB200_CLK_END();
 }
 
 }  // namespace cb200
