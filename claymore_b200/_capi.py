@@ -75,6 +75,17 @@ class Collider(C.Structure):
                 ("dsdt", C.c_float), ("scale", C.c_float), ("friction", C.c_float), ("type", C.c_int)]
 
 
+SHAPE_PLANE, SHAPE_BOX, SHAPE_SPHERE, SHAPE_CYLINDER = 0, 1, 2, 3   # CB200_SHAPE_*
+MAX_COLLISION_OBJECTS = 16                                           # CB200_MAX_COLLISION_OBJECTS
+
+
+class CollisionObject(C.Structure):
+    """cb200_collision_object: an analytic shape (a, b: its two vectors, see claymore_b200.objects) with the collider's motion fields."""
+    _fields_ = [("shape", C.c_int), ("type", C.c_int), ("friction", C.c_float), ("a", C.c_float * 3), ("b", C.c_float * 3),
+                ("rot_mat", C.c_float * 9), ("trans", C.c_float * 3), ("trans_vel", C.c_float * 3), ("omega", C.c_float * 3),
+                ("dsdt", C.c_float), ("scale", C.c_float)]
+
+
 OUTPUT_V, OUTPUT_J = 1, 2        # CB200_OUTPUT_V / CB200_OUTPUT_J: per-particle attributes of a frame's .bgeo files
 ERROR_OUTPUT_IO = 2000           # CB200_ERROR_OUTPUT_IO
 
@@ -135,6 +146,7 @@ _SIGNATURES = {
     "cb200_g2p2g": [_CFG, _F, _F, _I, ParticleBuffer, ParticleBuffer, Partition, Partition, _P, _P, _P],
     "cb200_update_grid_velocity_query_max": [_CFG, _I, _P, Partition, _F, _P, _P],
     "cb200_update_grid_velocity_query_max_collider": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), _F, _P, _P],
+    "cb200_update_grid_velocity_query_max_objects": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), C.POINTER(CollisionObject), _I, _F, _P, _P],
     "cb200_clear_grid": [_I, _P, _P],
     "cb200_cell_bucket_to_block": [_CFG, _I, _P, _P, _P, _P, _P],
     "cb200_mark_active_grid_blocks": [_I, _P, _P, _P],
@@ -180,6 +192,7 @@ _SIGNATURES = {
     "cb200_sim_grid": [_P, _P, _I, C.POINTER(_I)],
     "cb200_sim_set_collider": [_P, C.POINTER(Collider), _P],
     "cb200_sim_clear_collider": [_P],
+    "cb200_sim_set_collision_objects": [_P, C.POINTER(CollisionObject), _I],
     "cb200_sim_time": [_P, C.POINTER(C.c_double)],
     "cb200_sim_mgsp_inbox": [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_size_t)],
     "cb200_sim_mgsp_ipc_handle": [_P, _P],

@@ -158,6 +158,35 @@ int cb200_update_grid_velocity_query_max_collider(const cb200_config* c, int blo
 	return (int) cudaGetLastError();
 }
 
+int cb200_update_grid_velocity_query_max_objects(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream) {
+	CB_CFG(c);
+	ObjectList l;
+	if(!objects_prepare(objs, n, l)) return (int) cudaErrorInvalidValue;
+	if(n == 0) return collider ? cb200_update_grid_velocity_query_max_collider(c, block_count, grid, partition, dt, collider, time, max_vel, stream)
+	                           : cb200_update_grid_velocity_query_max(c, block_count, grid, partition, dt, max_vel, stream);
+	if(collider && (!collider_valid(collider) || !collider->sdf)) return (int) cudaErrorInvalidValue;
+	if(block_count <= 0) return 0;
+	GridUpdateArgs a {};
+	a.cfg = cfg;
+	a.state = nullptr;
+	a.nbc = block_count;
+	a.ebc = 0;
+	a.dt = dt;
+	a.grid = grid;
+	a.keys = partition.active_keys;
+	a.max_vel = max_vel;
+	a.clear_grid = nullptr;
+	a.n_clear = 0;
+	a.time = time;
+	if(collider) {
+		a.col = *collider;
+		grid_update_objects_kernel<true><<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a, l);
+	} else {
+		grid_update_objects_kernel<false><<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a, l);
+	}
+	return (int) cudaGetLastError();
+}
+
 int cb200_clear_grid(int block_count, float* grid, void* stream) {
 	if(block_count <= 0) return 0;
 	clear_grid_kernel<<<grid_for((long long) block_count * 64, 256), 256, 0, (cudaStream_t) stream>>>(block_count, grid);

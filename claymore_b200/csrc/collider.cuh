@@ -51,7 +51,9 @@ __device__ __forceinline__ void collider_mat_mul(const float* a, const float* b,
 		for(int i = 0; i < 3; ++i) c[3 * j + i] = a[i] * b[3 * j] + a[3 + i] * b[3 * j + 1] + a[6 + i] * b[3 * j + 2];
 }
 
-__device__ __forceinline__ void collider_make_frame(const ColliderView& c, float t, ColliderFrame& f) {
+// P: any struct with the cb200_collider motion fields (cb200_collider, cb200_collision_object)
+template<class P>
+__device__ __forceinline__ void collider_make_frame(const P& c, float t, ColliderFrame& f) {
 	float cur[9], r[9], prev[9];
 #pragma unroll
 	for(int i = 0; i < 9; ++i) cur[i] = c.rot_mat[i];
@@ -176,6 +178,189 @@ __device__ __forceinline__ void collider_resolve(const ColliderView& c, const Co
 	vz = v[2] + vo[2];
 }
 
+// collider_resolve over any query (P: a struct with the collider's motion, type and friction fields): query(x, n) tests the
+// material-space point x and writes the material-space normal n (0 where it has none).  The analytic objects use it; the
+// level-set path keeps collider_resolve above as it is, whose instructions this form, inlined there, would reorder.
+template<class P, class Q>
+__device__ __forceinline__ void collider_resolve_query(const P& c, const ColliderFrame& f, float dx, int nx, int ny, int nz, float& vx, float& vy, float& vz, Q&& query) {
+	const float xm[3] = {(float) nx * dx - f.b[0], (float) ny * dx - f.b[1], (float) nz * dx - f.b[2]};
+	const float x0[3] = {xm[0] * f.s_inv, xm[1] * f.s_inv, xm[2] * f.s_inv};
+	const float* R = f.rot;
+	float x[3];
+#pragma unroll
+	for(int d = 0; d < 3; ++d) x[d] = (R[3 * d] * x0[0] + R[3 * d + 1] * x0[1] + R[3 * d + 2] * x0[2]) * c.scale + c.trans[d];  // mat_t_mul_vec_3d
+	float on[3];
+	if(!query(x, on)) return;
+	const float* w = c.omega;
+	float vo[3] = {w[1] * xm[2] - w[2] * xm[1], w[2] * xm[0] - w[0] * xm[2], w[0] * xm[1] - w[1] * xm[0]};
+	const float ds = c.dsdt / c.scale;
+#pragma unroll
+	for(int d = 0; d < 3; ++d) vo[d] += xm[d] * ds;
+	{
+		const float r[3] = {x[0] - c.trans[0], x[1] - c.trans[1], x[2] - c.trans[2]};
+		const float mv[3] = {w[1] * r[2] + w[2] * r[1] + c.trans_vel[0], w[2] * r[0] + w[0] * r[2] + c.trans_vel[1], w[0] * r[1] + w[1] * r[0] + c.trans_vel[2]};
+#pragma unroll
+		for(int d = 0; d < 3; ++d) vo[d] += (R[d] * mv[0] + R[3 + d] * mv[1] + R[6 + d] * mv[2]) * c.scale + c.trans_vel[d];  // matrix_vector_multiplication_3d
+	}
+	float v[3] = {vx - vo[0], vy - vo[1], vz - vo[2]};
+	if(c.type == CB200_STICKY) {
+		v[0] = v[1] = v[2] = 0.f;
+	} else {
+		if(c.type == CB200_SEPARATE && on[0] == 0.f && on[1] == 0.f && on[2] == 0.f) {
+			vx = vy = vz = 0.f;  // :222-225 returns before the object velocity is added back
+			return;
+		}
+		float n[3];
+#pragma unroll
+		for(int d = 0; d < 3; ++d) n[d] = R[d] * on[0] + R[3 + d] * on[1] + R[6 + d] * on[2];
+		const float vn = n[0] * v[0] + n[1] * v[1] + n[2] * v[2];
+		const bool slip = c.type == CB200_SLIP;
+		if(slip || vn < 0.f) {
+#pragma unroll
+			for(int d = 0; d < 3; ++d) v[d] -= n[d] * vn;
+			if((slip ? c.friction > 0.f : c.friction != 0.f) && vn < 0.f) {
+				const float len = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+				if(-vn * c.friction < len) {
+					const float fr = vn * c.friction;
+#pragma unroll
+					for(int d = 0; d < 3; ++d) v[d] += v[d] / len * fr;
+				} else {
+					v[0] = v[1] = v[2] = 0.f;
+				}
+			}
+		}
+	}
+	vx = v[0] + vo[0];
+	vy = v[1] + vo[1];
+	vz = v[2] + vo[2];
+}
+// ---- analytic collision objects (DESIGN.md section 2.9) ----------------------------------------------------------------------
+// Passed by value as a kernel parameter beside the argument struct, so the kernels without objects keep their parameter block.
+struct ObjectList {
+	int n;
+	cb200_collision_object o[CB200_MAX_COLLISION_OBJECTS];
+};
+
+inline bool finite_all(const float* v, int n) {
+	for(int i = 0; i < n; ++i)
+		if(!std::isfinite(v[i])) return false;
+	return true;
+}
+// checks every entry of objs[0, n) and copies them into out, the plane normals made unit length in double; false (out
+// unchanged) on an unknown shape or type, scale 0, a non-finite value, a zero plane normal, lo > hi, a radius or half height
+// <= 0, or n outside [0, CB200_MAX_COLLISION_OBJECTS]
+inline bool objects_prepare(const cb200_collision_object* objs, int n, ObjectList& out) {
+	if(n < 0 || n > CB200_MAX_COLLISION_OBJECTS || (n > 0 && !objs)) return false;
+	ObjectList l {};
+	l.n = n;
+	for(int i = 0; i < n; ++i) {
+		cb200_collision_object o = objs[i];
+		if(o.shape < CB200_SHAPE_PLANE || o.shape > CB200_SHAPE_CYLINDER || o.type < CB200_STICKY || o.type > CB200_SEPARATE || o.scale == 0.f) return false;
+		if(!finite_all(&o.friction, 1) || !finite_all(o.a, 3) || !finite_all(o.b, 3) || !finite_all(o.rot_mat, 9) || !finite_all(o.trans, 3) ||
+		   !finite_all(o.trans_vel, 3) || !finite_all(o.omega, 3) || !finite_all(&o.dsdt, 1) || !finite_all(&o.scale, 1))
+			return false;
+		if(o.shape == CB200_SHAPE_PLANE) {
+			const double len = std::sqrt((double) o.b[0] * o.b[0] + (double) o.b[1] * o.b[1] + (double) o.b[2] * o.b[2]);
+			if(!(len > 0.0)) return false;
+			for(int d = 0; d < 3; ++d) o.b[d] = (float) (o.b[d] / len);
+		} else if(o.shape == CB200_SHAPE_BOX) {
+			if(o.a[0] > o.b[0] || o.a[1] > o.b[1] || o.a[2] > o.b[2]) return false;
+		} else if(!(o.b[0] > 0.f) || (o.shape == CB200_SHAPE_CYLINDER && !(o.b[1] > 0.f))) {
+			return false;
+		}
+		l.o[i] = o;
+	}
+	out = l;
+	return true;
+}
+
+// hit test (phi <= 0) and material-space normal of one shape at the material-space point x; the distance is not needed
+__device__ __forceinline__ bool object_query(const cb200_collision_object& o, const float* x, float* n) {
+	const float *a = o.a, *b = o.b;
+	n[0] = n[1] = n[2] = 0.f;
+	if(o.shape == CB200_SHAPE_PLANE) {  // a: point, b: unit normal
+		if((x[0] - a[0]) * b[0] + (x[1] - a[1]) * b[1] + (x[2] - a[2]) * b[2] > 0.f) return false;
+		n[0] = b[0];
+		n[1] = b[1];
+		n[2] = b[2];
+		return true;
+	}
+	if(o.shape == CB200_SHAPE_BOX) {  // a: lo, b: hi
+		if(!(a[0] <= x[0] && x[0] <= b[0] && a[1] <= x[1] && x[1] <= b[1] && a[2] <= x[2] && x[2] <= b[2])) return false;
+		int axis = 0;
+		float best = -INFINITY, sgn = 1.f;
+#pragma unroll
+		for(int d = 0; d < 3; ++d) {
+			const float ql = a[d] - x[d], qh = x[d] - b[d];
+			const float q = fmaxf(ql, qh);
+			if(q > best) {  // the lowest axis wins a tie
+				best = q;
+				axis = d;
+				sgn = ql > qh ? -1.f : 1.f;  // the low face when strictly nearer: +1 at the exact centre
+			}
+		}
+		n[0] = axis == 0 ? sgn : 0.f;  // no dynamic index: n stays in registers
+		n[1] = axis == 1 ? sgn : 0.f;
+		n[2] = axis == 2 ? sgn : 0.f;
+		return true;
+	}
+	const float d0 = x[0] - a[0], d1 = x[1] - a[1], d2 = x[2] - a[2];
+	const float r = b[0];
+	if(o.shape == CB200_SHAPE_SPHERE) {  // a: centre, b[0]: radius
+		const float dd = d0 * d0 + d1 * d1 + d2 * d2;
+		if(dd > r * r) return false;
+		if(dd > 0.f) {
+			const float len = sqrtf(dd);
+			n[0] = d0 / len;
+			n[1] = d1 / len;
+			n[2] = d2 / len;
+		}
+		return true;
+	}
+	// CYLINDER: a: centre, b[0]: radius, b[1]: half height, axis along material-space y, capped
+	const float rho2 = d0 * d0 + d2 * d2, h = b[1];
+	if(rho2 > r * r || fabsf(d1) > h) return false;
+	const float rho = sqrtf(rho2);
+	if(h - fabsf(d1) < r - rho) {
+		n[1] = d1 < 0.f ? -1.f : 1.f;
+	} else if(rho > 0.f) {
+		n[0] = d0 / rho;
+		n[2] = d2 / rho;
+	}
+	return true;
+}
+
+// the per-CTA state of the objects kernels: the level-set collider's frame (COLLIDE), and each object's parameters and frame
+struct ObjectFrames {
+	ColliderFrame col;
+	ColliderFrame f[CB200_MAX_COLLISION_OBJECTS];
+	cb200_collision_object o[CB200_MAX_COLLISION_OBJECTS];
+};
+// thread 0 builds the collider's frame, thread 32 + i object i's (another warp, so that the two run side by side); one barrier
+template<bool COLLIDE>
+__device__ __forceinline__ const ObjectFrames& object_frames_cta(const ColliderView& c, const ObjectList& l, float t) {
+	__shared__ ObjectFrames s;
+	if constexpr(COLLIDE) {
+		if(threadIdx.x == 0) collider_make_frame(c, t, s.col);
+	}
+	const int i = (int) threadIdx.x - 32;
+	if(i >= 0 && i < l.n) {
+		s.o[i] = l.o[i];
+		collider_make_frame(s.o[i], t, s.f[i]);
+	}
+	__syncthreads();
+	return s;
+}
+// the level-set collider (COLLIDE), then the n objects in list order, each resolving the velocity the previous one left
+template<bool COLLIDE>
+__device__ __forceinline__ void objects_resolve(const ColliderView& c, const ObjectFrames& s, int n, const Cfg& cfg, int nx, int ny, int nz, float& vx, float& vy, float& vz) {
+	if constexpr(COLLIDE) collider_resolve(c, s.col, cfg, nx, ny, nz, vx, vy, vz);
+	for(int i = 0; i < n; ++i) {
+		const cb200_collision_object& o = s.o[i];
+		collider_resolve_query(o, s.f[i], cfg.dx, nx, ny, nz, vx, vy, vz, [&](const float* x, float* nn) { return object_query(o, x, nn); });
+	}
+}
+
 // grid-update velocity of one cell (wall mask, gravity on y, collider) and its |v|^2, NaN -> +inf; no mass -> 0
 __device__ __forceinline__ float cell_vel_sq_collide(float m, float p0, float p1, float p2, bool wx, bool wy, bool wz, float gdt, const ColliderView& c, const ColliderFrame& f, const Cfg& cfg, int nx, int ny, int nz) {
 	if(!node_has_mass(m)) return 0.f;
@@ -190,6 +375,23 @@ __device__ __forceinline__ float cell_pair_vel_sq_collide(const Cfg& cfg, const 
 	const float2 m = s2[lane], p0 = s2[32 + lane], p1 = s2[64 + lane], p2 = s2[96 + lane];
 	const int nx = 4 * kx + (lane >> 3), ny = 4 * ky + ((lane >> 1) & 3), nz = 4 * kz + 2 * (lane & 1);
 	return fmaxf(cell_vel_sq_collide(m.x, p0.x, p1.x, p2.x, wx, wy, wz, gdt, c, f, cfg, nx, ny, nz), cell_vel_sq_collide(m.y, p0.y, p1.y, p2.y, wx, wy, wz, gdt, c, f, cfg, nx, ny, nz + 1));
+}
+// the same two functions with the collider (COLLIDE) and then the n objects of s
+template<bool COLLIDE>
+__device__ __forceinline__ float cell_vel_sq_objects(float m, float p0, float p1, float p2, bool wx, bool wy, bool wz, float gdt, const ColliderView& c, const ObjectFrames& s, int n, const Cfg& cfg, int nx, int ny, int nz) {
+	if(!node_has_mass(m)) return 0.f;
+	const float mi = 1.f / m;
+	float a = wx ? 0.f : p0 * mi, b = (wy ? 0.f : p1 * mi) + gdt, d = wz ? 0.f : p2 * mi;
+	objects_resolve<COLLIDE>(c, s, n, cfg, nx, ny, nz, a, b, d);
+	const float sq = a * a + b * b + d * d;
+	return isnan(sq) ? INFINITY : sq;
+}
+template<bool COLLIDE>
+__device__ __forceinline__ float cell_pair_vel_sq_objects(const Cfg& cfg, const ColliderView& c, const ObjectFrames& s, int n, const float2* s2, int lane, int kx, int ky, int kz, bool wx, bool wy, bool wz, float gdt) {
+	const float2 m = s2[lane], p0 = s2[32 + lane], p1 = s2[64 + lane], p2 = s2[96 + lane];
+	const int nx = 4 * kx + (lane >> 3), ny = 4 * ky + ((lane >> 1) & 3), nz = 4 * kz + 2 * (lane & 1);
+	return fmaxf(cell_vel_sq_objects<COLLIDE>(m.x, p0.x, p1.x, p2.x, wx, wy, wz, gdt, c, s, n, cfg, nx, ny, nz),
+	             cell_vel_sq_objects<COLLIDE>(m.y, p0.y, p1.y, p2.y, wx, wy, wz, gdt, c, s, n, cfg, nx, ny, nz + 1));
 }
 
 }  // namespace cb200

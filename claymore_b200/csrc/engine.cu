@@ -375,6 +375,8 @@ struct cb200_sim {
 	bool has_collider = false;
 	ColliderView collider {};
 	float* sdf = nullptr;
+	// analytic collision objects (cb200_sim_set_collision_objects), resolved after the collider in list order; n = 0: none
+	ObjectList objects {};
 	long long frames_done = 0;  // frames finished by cb200_sim_advance_frame (restored from a checkpoint)
 	// the rows each particle block starts at in every read-out, per model: the scans of the bucket sizes, [kMaxModels][max_blocks + 1]
 	int* ck_base = nullptr;
@@ -595,8 +597,11 @@ int enqueue_grid_update(cb200_sim* s, int R) {
 	}
 	gu.n_clear = (int) s->models.size();
 	for(size_t m = 0; m < s->models.size(); ++m) gu.clear_counts[m] = s->models[m].pb[Rn].cell_particle_counts;
-	if(s->has_collider) {  // placed at StepState::sim_time, the start of this sub-step
-		gu.col = s->collider;
+	if(s->has_collider) gu.col = s->collider;  // placed at StepState::sim_time, the start of this sub-step, as are the objects
+	if(s->objects.n > 0) {
+		if(s->has_collider) grid_update_objects_kernel<true><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu, s->objects);
+		else grid_update_objects_kernel<false><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu, s->objects);
+	} else if(s->has_collider) {
 		grid_update_kernel<true><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu);
 	} else {
 		grid_update_kernel<false><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu);
@@ -722,8 +727,11 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 		a.old_grid = s->grid[1];
 		a.new_grid = s->grid[0];
 		a.next_max_vel = mgsp ? &scr->local_max : nullptr;
-		if(mgsp && s->has_collider) {  // the predicted max must be the one the next grid update finds
-			a.col = s->collider;
+		if(mgsp && s->has_collider) a.col = s->collider;  // the predicted max must be the one the next grid update finds
+		if(mgsp && s->objects.n > 0) {
+			if(s->has_collider) carry_grid_objects_kernel<true><<<grid_blocks(4), 256, 0, st>>>(a, s->objects);
+			else carry_grid_objects_kernel<false><<<grid_blocks(4), 256, 0, st>>>(a, s->objects);
+		} else if(mgsp && s->has_collider) {
 			carry_grid_kernel<true><<<grid_blocks(4), 256, 0, st>>>(a);
 		} else {
 			carry_grid_kernel<false><<<grid_blocks(4), 256, 0, st>>>(a);
@@ -853,6 +861,10 @@ void preload_kernels() {
 	preload(clear_grid_kernel);
 	preload(carry_grid_kernel<false>);
 	preload(carry_grid_kernel<true>);
+	preload(grid_update_objects_kernel<false>);
+	preload(grid_update_objects_kernel<true>);
+	preload(carry_grid_objects_kernel<false>);
+	preload(carry_grid_objects_kernel<true>);
 	preload(scan_kernel);
 	preload(summary_kernel);
 	preload(rebuild_kernel);
@@ -876,6 +888,8 @@ void preload_kernels() {
 	preload(mgsp_clear_publish_kernel);
 	preload(grid_max_kernel<false>);
 	preload(grid_max_kernel<true>);
+	preload(grid_max_objects_kernel<false>);
+	preload(grid_max_objects_kernel<true>);
 	preload(snapshot_kernel);
 	preload(state_positions_kernel);
 	preload(scatter_grid_kernel);
@@ -1301,7 +1315,10 @@ static int setup_impl(cb200_sim* s, const StartSrc& src) {
 	CK(push_state(s));
 	if(mgsp) {
 		// global max |v|^2 of the start grid (later sub-steps get it from the end-of-step exchange of the previous one)
-		if(s->has_collider) grid_max_kernel<true><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->collider);
+		const ColliderView col = s->has_collider ? s->collider : ColliderView {};
+		if(s->objects.n > 0 && s->has_collider) grid_max_objects_kernel<true><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, col, s->objects);
+		else if(s->objects.n > 0) grid_max_objects_kernel<false><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, col, s->objects);
+		else if(s->has_collider) grid_max_kernel<true><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->collider);
 		else grid_max_kernel<false><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, ColliderView {});
 		mgsp_allreduce_maxvel_kernel<<<1, 32, 0, st>>>(mgsp_view(s), &s->d_state->max_vel_sq);
 		s->launches += 2;
@@ -1444,7 +1461,7 @@ int cb200_sim_grid(cb200_sim* s, float* grid_host, int capacity_blocks, int* n_o
 }
 long long cb200_sim_launch_count(cb200_sim* s) { return s ? s->launches : 0; }
 
-// The sub-step graphs hold the grid-update and carry launches of the collider state they were captured with: drop them and,
+// The sub-step graphs hold the grid-update and carry launches of the collider and object state they were captured with: drop them and,
 // once set up, instantiate both roll parities again right away (never later, while an MGSP peer may be waiting on this rank).
 static int recapture(cb200_sim* s) {
 	drop_graphs(s);
@@ -1484,6 +1501,13 @@ int cb200_sim_clear_collider(cb200_sim* s) {
 	s->collider = ColliderView {};
 	g_pool.release(s->sdf);
 	s->sdf = nullptr;
+	return recapture(s);
+}
+int cb200_sim_set_collision_objects(cb200_sim* s, const cb200_collision_object* objs, int n) {
+	ObjectList l;
+	if(!s || !objects_prepare(objs, n, l)) return (int) cudaErrorInvalidValue;
+	CK(cudaStreamSynchronize(s->stream));
+	s->objects = l;
 	return recapture(s);
 }
 int cb200_sim_time(cb200_sim* s, double* time) {

@@ -29,11 +29,14 @@ struct GridUpdateArgs {
 // NaN -> +inf (B #3).
 // COLLIDE: the MGSP form with a SignedDistanceGrid (mgmpm_kernels.cuh:323-399): after gravity, cells with mass resolve against
 // the collider (collider.cuh); the max is |v|^2 where that kernel reports 2|v|^2 (Appendix B #11).
-template<bool COLLIDE>
-__global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpdateArgs a) {
+// OBJECTS: then the analytic objects of `objs` in list order (collider.cuh, DESIGN.md section 2.9), placed at the collider's time.
+template<bool COLLIDE, bool OBJECTS>
+__device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const ObjectList* objs) {
 	__shared__ unsigned s_max[kGridThreads / 32];
 	const ColliderFrame* fr = nullptr;
-	if constexpr(COLLIDE) fr = &collider_frame_cta(a.col, a.state ? (float) a.state->sim_time : a.time);
+	const ObjectFrames* of = nullptr;
+	if constexpr(OBJECTS) of = &object_frames_cta<COLLIDE>(a.col, *objs, a.state ? (float) a.state->sim_time : a.time);
+	else if constexpr(COLLIDE) fr = &collider_frame_cta(a.col, a.state ? (float) a.state->sim_time : a.time);
 	const Cfg& cfg = a.cfg;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int nbc = a.state ? a.state->nbc : a.nbc;
@@ -57,7 +60,8 @@ __global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpd
 				v0.x = wx ? 0.f : v0.x * mi;
 				v1.x = (wy ? 0.f : v1.x * mi) + gdt;
 				v2.x = wz ? 0.f : v2.x * mi;
-				if constexpr(COLLIDE) collider_resolve(a.col, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
+				if constexpr(OBJECTS) objects_resolve<COLLIDE>(a.col, *of, objs->n, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
+				else if constexpr(COLLIDE) collider_resolve(a.col, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
 				sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
 			}
 			if(hy) {
@@ -65,7 +69,8 @@ __global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpd
 				v0.y = wx ? 0.f : v0.y * mi;
 				v1.y = (wy ? 0.f : v1.y * mi) + gdt;
 				v2.y = wz ? 0.f : v2.y * mi;
-				if constexpr(COLLIDE) collider_resolve(a.col, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
+				if constexpr(OBJECTS) objects_resolve<COLLIDE>(a.col, *of, objs->n, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
+				else if constexpr(COLLIDE) collider_resolve(a.col, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
 				sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
 			}
 			if(hx || hy) {
@@ -96,6 +101,12 @@ __global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpd
 		if(m) atomicMax(reinterpret_cast<unsigned*>(a.max_vel), m);
 	}
 }
+template<bool COLLIDE>
+__global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpdateArgs a) { grid_update_body<COLLIDE, false>(a, nullptr); }
+// the same with analytic objects (objs.n >= 1): the list is a parameter of its own, so the kernels above keep their parameter block
+template<bool COLLIDE>
+__global__ void __launch_bounds__(kGridThreads, 2) grid_update_objects_kernel(const GridUpdateArgs a, const __grid_constant__ ObjectList objs) { grid_update_body<COLLIDE, true>(a, &objs); }
+static_assert(sizeof(GridUpdateArgs) + sizeof(ObjectList) <= 4096, "the objects grid update's parameters must fit the 4 KiB kernel-parameter limit");
 
 // clear_grid (mgmpm_kernels.cuh:106-115)
 __global__ void clear_grid_kernel(int block_count, float* grid) {
@@ -126,8 +137,8 @@ struct CarryArgs {
 	int* overlap_marks;
 	ColliderView col;  // COLLIDE: the predictor applies the collider at the time the next grid update sees
 };
-template<bool COLLIDE>
-__global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
+template<bool COLLIDE, bool OBJECTS>
+__device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const ObjectList* objs) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int n = *a.new_count;
 	const int old_nbc = a.state->nbc;
@@ -136,7 +147,9 @@ __global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
 	float gdt = 0.f;
 	if(a.next_max_vel) gdt = a.cfg.gravity * device_compute_dt(a.cfg, a.state->max_vel_sq, a.state->step_time, a.state->frame_time, a.state->dt_default);
 	const ColliderFrame* fr = nullptr;
-	if constexpr(COLLIDE) fr = &collider_frame_cta(a.col, (float) (a.state->sim_time + (double) a.state->dt));  // the clock rolls by this sub-step's dt
+	const ObjectFrames* of = nullptr;
+	if constexpr(OBJECTS) of = &object_frames_cta<COLLIDE>(a.col, *objs, (float) (a.state->sim_time + (double) a.state->dt));
+	else if constexpr(COLLIDE) fr = &collider_frame_cta(a.col, (float) (a.state->sim_time + (double) a.state->dt));  // the clock rolls by this sub-step's dt
 	unsigned vmax = 0u;
 	for(int j = blockIdx.x * 8 + warp; j < n; j += gridDim.x * 8) {
 		const int kx = a.new_keys[3 * j], ky = a.new_keys[3 * j + 1], kz = a.new_keys[3 * j + 2];
@@ -153,7 +166,8 @@ __global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
 			if(a.next_max_vel) {
 				const float2* s2 = reinterpret_cast<const float2*>(s);
 				const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
-				if constexpr(COLLIDE) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_collide(a.cfg, a.col, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+				if constexpr(OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_objects<COLLIDE>(a.cfg, a.col, *of, objs->n, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+				else if constexpr(COLLIDE) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_collide(a.cfg, a.col, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
 				else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 			}
 		} else {
@@ -166,6 +180,12 @@ __global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) {
 		if(lane == 0 && vmax) atomicMax(reinterpret_cast<unsigned*>(a.next_max_vel), vmax);
 	}
 }
+template<bool COLLIDE>
+__global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) { carry_grid_body<COLLIDE, false>(a, nullptr); }
+// OBJECTS: the predictor applies the objects too (MGSP; objs.n >= 1)
+template<bool COLLIDE>
+__global__ void __launch_bounds__(256, 2) carry_grid_objects_kernel(const CarryArgs a, const __grid_constant__ ObjectList objs) { carry_grid_body<COLLIDE, true>(a, &objs); }
+static_assert(sizeof(CarryArgs) + sizeof(ObjectList) <= 4096, "the objects carry's parameters must fit the 4 KiB kernel-parameter limit");
 
 // max |v|^2 the grid update will find, without touching the grid (MGSP start-up)
 template<bool COLLIDE>
@@ -182,6 +202,23 @@ __global__ void __launch_bounds__(256) grid_max_kernel(Cfg cfg, const StepState*
 		const float2* s2 = reinterpret_cast<const float2*>(grid + (size_t) b * kGridBlockFloats);
 		if constexpr(COLLIDE) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_collide(cfg, col, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
 		else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
+	}
+	vmax = __reduce_max_sync(0xffffffffu, vmax);
+	if(lane == 0 && vmax) atomicMax(reinterpret_cast<unsigned*>(max_vel), vmax);
+}
+// the same with the analytic objects after the collider (objs.n >= 1)
+template<bool COLLIDE>
+__global__ void __launch_bounds__(256, 2) grid_max_objects_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const ColliderView col, const __grid_constant__ ObjectList objs) {
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	const int g = cfg.gsize, bc = cfg.boundary;
+	const float gdt = cfg.gravity * state->dt;
+	const ObjectFrames& of = object_frames_cta<COLLIDE>(col, objs, (float) state->sim_time);
+	unsigned vmax = 0u;
+	for(int b = blockIdx.x * 8 + warp; b < state->nbc; b += gridDim.x * 8) {
+		const int kx = keys[3 * b], ky = keys[3 * b + 1], kz = keys[3 * b + 2];
+		const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
+		const float2* s2 = reinterpret_cast<const float2*>(grid + (size_t) b * kGridBlockFloats);
+		vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_objects<COLLIDE>(cfg, col, of, objs.n, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
 	}
 	vmax = __reduce_max_sync(0xffffffffu, vmax);
 	if(lane == 0 && vmax) atomicMax(reinterpret_cast<unsigned*>(max_vel), vmax);

@@ -13,6 +13,14 @@ A "box" collider spans [offset, offset + span], a "sphere" has diameter min(span
 through offset and is solid behind `normal`.  The collider is the reference's SignedDistanceGrid (init_boundary,
 Projects/MGSP/mgsp_benchmark.cuh:257-266); "velocity" is its trans_vel.
 
+     "boundaries": [{"shape": "plane"|"box"|"sphere"|"cylinder", + the "collider" keys offset, span, normal, type, friction,
+                     velocity, omega, scale, dsdt}, ...]
+
+Analytic collision objects (claymore_b200.objects, DESIGN.md section 2.9), resolved after the collider in list order, at most
+CB200_MAX_COLLISION_OBJECTS.  Box, sphere and plane are placed as the collider's are; a "cylinder" fills [offset, offset + span]
+with its axis along y and radius min(span_x, span_z) / 2.  Unknown keys or shapes, too many entries or a bad value raise
+ValueError before any device work; "collider" and "boundaries" may both be present.
+
 The reference only loads `.sdf` level sets (gmpm.cu:152-159).  Here "file": "<name>.sdf" is sampled on the device by
 GmpmSimulator.init_model_sdf with the optional keys "sampler" ("random", the default, or "lattice"), "ppc" (particles per
 simulation cell, default 8: the reference's MODEL_PPC, settings.h:51) and "seed" (default 0); the level set is fitted into
@@ -92,6 +100,46 @@ def _collider(sim, c, cfg, base_dir):
         sdf, grad = levelset.load(cfg, kind if os.path.isabs(kind) else os.path.join(base_dir, kind))
     sim.set_collider(sdf, grad, type=c.get("type", "sticky"), friction=c.get("friction", 0.3), trans_vel=c.get("velocity", [0, 0, 0]),
                      omega=c.get("omega", [0, 0, 0]), scale=c.get("scale", 1.0), dsdt=c.get("dsdt", 0.0))
+
+
+BOUNDARY_KEYS = ("shape", "offset", "span", "normal", "type", "friction", "velocity", "omega", "scale", "dsdt")
+
+
+def boundaries(doc):
+    """The scene's "boundaries" as validated collision objects (ValueError on a bad entry), before any device work."""
+    from . import objects
+    bs = doc.get("boundaries", [])
+    if not isinstance(bs, list):
+        raise ValueError("\"boundaries\" must be a list of objects")
+    if len(bs) > objects.MAX_COLLISION_OBJECTS:
+        raise ValueError(f"at most {objects.MAX_COLLISION_OBJECTS} \"boundaries\", not {len(bs)}")
+    out = []
+    for i, b in enumerate(bs):
+        if not isinstance(b, dict):
+            raise ValueError(f"boundary {i} must be an object with keys {', '.join(BOUNDARY_KEYS)}")
+        unknown = sorted(set(b) - set(BOUNDARY_KEYS))
+        if unknown:
+            raise ValueError(f"boundary {i}: unknown keys {unknown} (known: {', '.join(BOUNDARY_KEYS)})")
+        shape = b.get("shape")
+        if shape not in objects.SHAPES:
+            raise ValueError(f"boundary {i}: unknown shape {shape!r} (known: {', '.join(objects.SHAPES)})")
+        try:
+            offset = np.asarray(b.get("offset", [0, 0, 0]), dtype=np.float64).reshape(3)
+            span = np.asarray(b.get("span", [1, 1, 1]), dtype=np.float64).reshape(3)
+            motion = dict(type=b.get("type", "sticky"), friction=float(b.get("friction", 0.3)), trans_vel=b.get("velocity", [0, 0, 0]),
+                          omega=b.get("omega", [0, 0, 0]), scale=float(b.get("scale", 1.0)), dsdt=float(b.get("dsdt", 0.0)))
+            if shape == "box":
+                o = objects.box(offset, offset + span, **motion)
+            elif shape == "sphere":
+                o = objects.sphere(offset + span / 2, float(span.min()) / 2, **motion)
+            elif shape == "plane":
+                o = objects.plane(offset, b.get("normal", [0, 1, 0]), **motion)
+            else:
+                o = objects.cylinder(offset + span / 2, float(min(span[0], span[2])) / 2, float(span[1]) / 2, **motion)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"boundary {i} ({shape}): {e}") from None
+        out.append(o)
+    return out
 
 
 EMIT_KEYS = ("start", "every", "until", "fill")
@@ -185,7 +233,7 @@ def _check_resume(doc, cfg, resume):
 def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_kwargs):
     """parse_scene (gmpm.cu:60-165): returns an initialised GmpmSimulator with every model registered.
     resume: path of a checkpoint of this scene.  It is checked against the document before any simulator exists; the scene's
-    collider is set and the checkpoint restored in place of the models (max_blocks defaults to the saved capacity).  MGSP runs
+    collider and boundaries are set and the checkpoint restored in place of the models (max_blocks defaults to the saved capacity).  MGSP runs
     resume rank by rank instead: GmpmSimulator.from_checkpoint, wire the peers, restore."""
     if isinstance(path_or_dict, dict):
         doc, base = path_or_dict, os.getcwd()
@@ -198,6 +246,7 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
     if emit_schedule(doc) and sim_kwargs.get("mgsp_world", 1) > 1:
         raise ValueError("\"emit\" is not supported in MGSP mode")
     models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
+    objs = boundaries(doc)
     if resume is not None:
         inf = _check_resume(doc, cfg, resume)
         emitters = _emitters(doc, cfg, base, _level_sets(models, base))
@@ -205,6 +254,8 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
                             frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max(max_blocks, inf["max_blocks"]), **sim_kwargs)
         if "collider" in doc:
             _collider(sim, doc["collider"], cfg, base)
+        if objs:
+            sim.set_collision_objects(objs)
         sim.restore(resume)
         sim.emitters = emitters
         return sim
@@ -234,5 +285,7 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
             sim.update_sand_parameters(model["rho"], model["volume"], model["youngs_modulus"], model["poisson_ratio"], model=mid)
     if "collider" in doc:
         _collider(sim, doc["collider"], cfg, base)
+    if objs:
+        sim.set_collision_objects(objs)
     sim.emitters = emitters
     return sim

@@ -218,6 +218,17 @@ class GmpmSimulator:
     def clear_collider(self):
         check(self.L.cb200_sim_clear_collider(self.h), "clear_collider")
 
+    # ---- analytic collision objects (claymore_b200.objects, DESIGN.md section 2.9) ---------------------------------------------
+    def set_collision_objects(self, objs):
+        """Replaces the analytic collision objects by `objs` (claymore_b200.objects.plane / box / sphere / cylinder; [] clears them).
+        From the next sub-step on the grid update resolves the level-set collider, then these in list order (synchronises)."""
+        from . import objects
+        objs = list(objs)
+        check(self.L.cb200_sim_set_collision_objects(self.h, objects.array(objs), len(objs)), "set_collision_objects")
+
+    def clear_collision_objects(self):
+        check(self.L.cb200_sim_set_collision_objects(self.h, None, 0), "clear_collision_objects")
+
     def sim_time(self):
         """Simulated time since initial_setup (sum of the dt of every finished sub-step)."""
         t = C.c_double(0.0)

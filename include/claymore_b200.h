@@ -111,6 +111,36 @@ typedef struct cb200_collider {
  * half of what that kernel reports (it adds every square twice). */
 CB200_API int cb200_update_grid_velocity_query_max_collider(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, float time, float* max_vel, void* stream);
 
+/* Analytic collision objects (DESIGN.md section 2.9): closed-form shapes with the collider's boundary types and motion model,
+ * up to CB200_MAX_COLLISION_OBJECTS per simulator, no device memory.  A shape is defined in the collider's material space, the
+ * point x = R(t)^T (node dx - trans - trans_vel t) / (1 + dsdt t) * scale + trans that the level-set collider queries (R(t) =
+ * rot_mat Rx(omega_x t) Ry(omega_y t) Rz(omega_z t)); for a static object (rot_mat = I, scale 1, no velocities) that is world
+ * space.  The shape vectors a and b:
+ *   CB200_SHAPE_PLANE     a = a point p, b = the normal n (made unit length in double): solid where (x - p) . n <= 0, normal n
+ *   CB200_SHAPE_BOX       a = lo, b = hi, axis-aligned: solid where lo <= x <= hi; normal of the nearest face (largest
+ *                         max(lo_d - x_d, x_d - hi_d), ties to the lowest axis; -1 towards lo only where strictly nearer)
+ *   CB200_SHAPE_SPHERE    a = centre c, b[0] = radius r: solid where |x - c|^2 <= r^2; normal (x - c) / |x - c|, 0 at c
+ *   CB200_SHAPE_CYLINDER  a = centre c, b[0] = radius r, b[1] = half height h, axis along material-space y (orient it with
+ *                         rot_mat), capped: solid where (x-c)_x^2 + (x-c)_z^2 <= r^2 and |(x-c)_y| <= h; normal +-y when
+ *                         h - |(x-c)_y| < r - rho, else radial (0 on the axis)
+ * type and friction act as the level-set collider's (a zero normal: SEPARATE sets v to 0, SLIP leaves it).  Unused b
+ * components are ignored. */
+enum { CB200_SHAPE_PLANE = 0, CB200_SHAPE_BOX = 1, CB200_SHAPE_SPHERE = 2, CB200_SHAPE_CYLINDER = 3 };
+#define CB200_MAX_COLLISION_OBJECTS 16
+typedef struct cb200_collision_object {
+	int shape, type;
+	float friction;
+	float a[3], b[3];
+	float rot_mat[9];
+	float trans[3], trans_vel[3], omega[3];
+	float dsdt, scale;
+} cb200_collision_object;
+
+/* The grid update with the level-set collider `collider` (NULL: none) and then the n objects objs[0, n) in list order, all placed
+ * at `time`.  n = 0 runs exactly cb200_update_grid_velocity_query_max (collider NULL) or ..._collider.  cudaErrorInvalidValue
+ * for an invalid object (see cb200_sim_set_collision_objects) or collider. */
+CB200_API int cb200_update_grid_velocity_query_max_objects(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream);
+
 /* clear_grid  mgmpm_kernels.cuh:106-115 via GridBuffer::reset  grid_buffer.cuh:32-35 */
 CB200_API int cb200_clear_grid(int block_count, float* grid, void* stream);
 
@@ -227,6 +257,13 @@ CB200_API int cb200_sim_grid(cb200_sim* sim, float* grid_host, int capacity_bloc
  * synchronise and re-capture the sub-step graphs; call them between sub-steps. */
 CB200_API int cb200_sim_set_collider(cb200_sim* sim, const cb200_collider* params, const float* sdf_host);
 CB200_API int cb200_sim_clear_collider(cb200_sim* sim);
+/* Replaces the simulator's analytic collision objects by objs[0, n) (n = 0 clears them).  Every entry is checked first: an
+ * unknown shape or type, scale 0, a non-finite value, a zero plane normal, lo > hi, a radius or half height <= 0 or n outside
+ * [0, CB200_MAX_COLLISION_OBJECTS] return cudaErrorInvalidValue with the simulator unchanged.  Each sub-step's grid update
+ * resolves the level-set collider first, then the objects in list order (overlapping objects depend on that order), all placed
+ * at the simulated time at the start of the sub-step.  Synchronises and re-captures the sub-step graphs; call it between
+ * sub-steps.  Objects are scene input: a checkpoint does not store them, set them before cb200_sim_restore. */
+CB200_API int cb200_sim_set_collision_objects(cb200_sim* sim, const cb200_collision_object* objs, int n);
 /* simulated time since initial_setup: the sum of the dt of every finished sub-step (synchronises) */
 CB200_API int cb200_sim_time(cb200_sim* sim, double* time);
 /* number of kernels this library launched on behalf of `sim` since creation */
@@ -252,7 +289,7 @@ CB200_API long long cb200_sim_launch_count(cb200_sim* sim);
  *     int32 keys[nbc][3]: the grid blocks of grid[0] (particle blocks first)
  *     float grid[nbc][256]: mass and momentum the next sub-step's grid update starts from, layout of a grid block
  * Particle rows are in partition order, then bucket order inside a block: two checkpoints of an unchanged simulator are
- * byte-identical.  The collider field is not stored: set it before cb200_sim_restore. */
+ * byte-identical.  The collider field and the collision objects are not stored: set them before cb200_sim_restore. */
 #define CB200_CHECKPOINT_VERSION 1
 #define CB200_CHECKPOINT_HEADER_BYTES 1024
 typedef struct cb200_checkpoint_model {

@@ -5,6 +5,13 @@ with no collider, alternating the two in one process, and prints JSON lines: the
 run the sub-step time (CUDA events, graph replay) and the per-phase milliseconds of profile_phases (grid_update first).
 
     python tools/collider_bench.py [--steps 50] [--warmup 10] [--rounds 3]
+
+--objects compares, in alternating rounds, no collider, the level-set floor, the same floor as one analytic box, and 4 and 16
+analytic objects (the floor box, then spheres and cylinders off to the sides of the spheres, and planes below the floor).  Each
+run also reports the grid update's kernel time per sub-step from torch.profiler (a run of its own) and the device memory the
+collider or the objects add (free memory before and after they are set).
+
+    python tools/collider_bench.py --objects [--steps 50] [--warmup 10] [--rounds 3]
 """
 import argparse
 import json
@@ -15,12 +22,18 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
-def run(scene, field, args, stream):
+def run(scene, field, args, stream, objs=None):
     import torch
     from claymore_b200 import scenes
     sim = scenes.build_engine(scene, dt=args.dt, max_blocks=scenes.max_blocks_for(scene), stream=stream.cuda_stream, auto_grow=False)
+    torch.cuda.synchronize()
+    free0 = torch.cuda.mem_get_info()[0]
     if field is not None:
         sim.set_collider(field[0], field[1], type="sticky")
+    if objs:
+        sim.set_collision_objects(objs)
+    torch.cuda.synchronize()
+    added = free0 - torch.cuda.mem_get_info()[0]
     sim.step(args.warmup)
     sim.sync()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -34,10 +47,35 @@ def run(scene, field, args, stream):
     phases = {k: round(v / args.steps, 4) for k, v in sim.profile_phases().items()}
     sim.profile_read()
     sim.profile(False)
+    kernel_ms = None
+    if args.objects:
+        from torch.profiler import ProfilerActivity, profile
+        sim.sync()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            sim.step(args.steps)
+            sim.sync()
+        us = sum(e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total for e in prof.key_averages() if "grid_update" in e.key)
+        kernel_ms = round(us / 1000.0 / args.steps, 4)
     st = sim.stats()
     sim.close()
     assert st.error == 0, f"engine error bits {st.error}"
-    return {"substep_ms": round(substep_ms, 4), "phases_ms": phases}
+    return {"substep_ms": round(substep_ms, 4), "phases_ms": phases, "grid_update_kernel_ms": kernel_ms, "added_device_bytes": added}
+
+
+def object_sets(top):
+    """the analytic variants of --objects: the floor box alone, 4 and 16 objects (the floor first)"""
+    from claymore_b200 import objects
+    floor = objects.box((0.1, 0.1, 0.1), (0.9, top, 0.9), type="sticky")
+    extra = []
+    for i in range(15):
+        k = i % 3
+        if k == 0:
+            extra.append(objects.sphere((0.12 + 0.05 * i, 0.75, 0.12), 0.03, type="slip", friction=0.3))
+        elif k == 1:
+            extra.append(objects.cylinder((0.88, 0.6, 0.12 + 0.05 * i), 0.03, 0.1, type="separate", friction=0.3, omega=(0.0, 1.0, 0.0)))
+        else:
+            extra.append(objects.plane((0.5, 0.1 - 0.005 * i, 0.5), (0.0, 1.0, 0.0), type="slip"))
+    return {"analytic_floor": [floor], "objects4": [floor] + extra[:3], "objects16": [floor] + extra}
 
 
 def main():
@@ -46,6 +84,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--dt", type=float, default=1e-4)
+    ap.add_argument("--objects", action="store_true", help="also the analytic floor box, 4 and 16 analytic objects")
     args = ap.parse_args()
 
     import torch
@@ -61,10 +100,12 @@ def main():
     top = 0.5 - 0.1645 - 0.5 / (1 << scene["domain_bits"])
     field = levelset.box(Config(domain_bits=scene["domain_bits"]), (0.1, 0.1, 0.1), (0.9, top, 0.9))
     stream = torch.cuda.Stream()
+    sets = object_sets(top) if args.objects else {}
+    names = ["floor", "none"] + sorted(sets)
     for r in range(args.rounds):
-        order = ("floor", "none") if r % 2 == 0 else ("none", "floor")
+        order = names if r % 2 == 0 else names[::-1]
         for name in order:
-            res = run(scene, field if name == "floor" else None, args, stream)
+            res = run(scene, field if name == "floor" else None, args, stream, sets.get(name))
             print(json.dumps({"round": r, "collider": name, "steps": args.steps, **res}), flush=True)
 
 
