@@ -112,6 +112,7 @@ class CheckpointInfo(C.Structure):
 
 SDF_RANDOM, SDF_LATTICE = 0, 1   # CB200_SDF_RANDOM / CB200_SDF_LATTICE
 EMIT_EMPTY_CELLS = 1             # CB200_EMIT_EMPTY_CELLS: add only particles whose cell held none before the call
+REMOVE_OUTSIDE = 1               # CB200_REMOVE_OUTSIDE: remove the particles outside the union of the regions instead of inside it
 
 
 class SdfHeader(C.Structure):
@@ -214,6 +215,8 @@ _SIGNATURES = {
     "cb200_sim_init_model_sdf": [_P, _I, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.POINTER(_I), C.POINTER(_I)],
     "cb200_sim_add_particles": [_P, _I, _P, _I, _P, C.c_uint, C.POINTER(_I)],
     "cb200_sim_add_particles_sdf": [_P, _I, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.c_uint, C.POINTER(_I)],
+    "cb200_sim_remove_particles": [_P, C.c_uint, C.POINTER(CollisionObject), _I, C.c_uint, C.POINTER(C.c_longlong)],
+    "cb200_sim_remove_rows": [_P, _I, _P, C.c_longlong, C.POINTER(C.c_longlong)],
     "cb200_test_svd3": [_I, _P, _P, _P, _P, _P],
     "cb200_test_stress": [_I, _I, ParticleBuffer, _I, _P, _P, _P, _P, _P, _P],
     "cb200_test_warp_flatten": [_CFG, _I, _P, _P, _P, _P, _P, _P],

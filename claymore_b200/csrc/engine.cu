@@ -34,6 +34,7 @@
 #include "mgsp.cuh"
 #include "output.cuh"
 #include "partition.cuh"
+#include "remove.cuh"
 #include "sdf.cuh"
 
 namespace cb200 {
@@ -272,6 +273,9 @@ struct StartSrc {
 	int grid_count = 0;                  // a checkpoint's nbc; an emission's old nbc, a subset of the rebuilt partition's
 	const Clock* clock = nullptr;        // absent: the fresh clock of desc and the models' v0
 	const BlockCounts* expect = nullptr; // the block counts the rebuild must reproduce; absent: no check
+	const float* vel = nullptr;          // [vel_count][256] saved grid blocks with their keys [vel_count][3] whose node velocities p / m
+	const int* vel_keys = nullptr;       // the rasterised mass takes (a removal); absent: the models' v0.  Not with `grid`.
+	int vel_count = 0;
 };
 
 // cb200_sim_restore_models: the checkpoint's state, clock and block counts, staged on the device until initial_setup consumes them
@@ -1187,7 +1191,9 @@ static int register_ring(cb200_sim* s, Part p, int capacity, int* error, int pbc
 
 // initial_setup  gmpm_simulator.cuh:637-781 (counts are read back here: one-time cost), from the parts `src` has and the models'
 // positions: the bins get the start state or the saved rows, grid[0] the rasterised particles or the saved blocks (no MGSP halo
-// reduction: they hold the full sums), the step state the fresh clock or the saved one.
+// reduction: they hold the full sums) or, with src.vel, the rasterised mass at the saved velocities, the step state the fresh clock or
+// the saved one.
+constexpr float kZeroVel[3] = {0.f, 0.f, 0.f};
 static int setup_impl(cb200_sim* s, const StartSrc& src) {
 	if(!s || s->setup_done || s->models.empty()) return (int) cudaErrorInvalidValue;
 	cudaStream_t st = s->stream;
@@ -1269,10 +1275,15 @@ static int setup_impl(cb200_sim* s, const StartSrc& src) {
 	}
 	for(Model& m : s->models) {
 		if(!src.grid) {
-			rasterize_blocks_kernel<<<grid_for(pbc, 1, 16), 256, 0, st>>>(cfg, m.material, pbc, s->part[R].active_keys, s->part[R].index_table, view(m.pb[R]), s->grid[0], m.pb[R].mass, m.v0[0], m.v0[1], m.v0[2], err);
+			const float* v0 = src.vel ? kZeroVel : m.v0;
+			rasterize_blocks_kernel<<<grid_for(pbc, 1, 16), 256, 0, st>>>(cfg, m.material, pbc, s->part[R].active_keys, s->part[R].index_table, view(m.pb[R]), s->grid[0], m.pb[R].mass, v0[0], v0[1], v0[2], err);
 			++s->launches;
 		}
 		init_adv_bucket_kernel<<<grid_for(pbc, 1, 16), 128, 0, st>>>(cfg, pbc, m.pb[Rn].particle_bucket_sizes, m.pb[Rn].blockbuckets);
+		++s->launches;
+	}
+	if(src.vel) {
+		keep_velocity_kernel<<<grid_for(src.vel_count, 8, 16), 256, 0, st>>>(cfg, src.vel_count, src.vel_keys, src.vel, s->part[R].index_table, nbc, s->grid[0]);
 		++s->launches;
 	}
 	CK(cudaGetLastError());
@@ -1631,6 +1642,8 @@ int cb200_sim_particle_state(cb200_sim* s, int model, float* state_host, int* n_
 
 int cb200_sim_checkpoint_begin(cb200_sim* s, size_t* bytes) {
 	if(!s || !s->setup_done) return (int) cudaErrorInvalidValue;
+	for(const Model& m : s->models)
+		if(m.n == 0) return (int) cudaErrorNotSupported;  // format version 1 holds no empty model
 	CK(s->ck.wait());  // the pinned blob and the staging blob are re-used
 	s->ck_bytes = 0;
 	CK(s->ck.open_stream());
@@ -1975,6 +1988,34 @@ struct EmitBuffers {
 	}
 };
 
+// The live state of every model, gathered (checkpoint layout) into a blob from the pool that the caller releases: each model's count
+// and the layout of the sections, for the grid of nbc blocks.  Reads the live state only.
+int gather_live(cb200_sim* s, long long nbc, unsigned char** blob, long long* counts, CkLayout* L) {
+	CK(pool_alloc(blob, ck_capacity(s)));
+	SnapshotArgs sa {};
+	sa.grid = s->grid[0];
+	sa.out = *blob;
+	CK(read_out(s, snapshot_kernel, sa, counts));
+	*L = models_layout(s, counts, nbc);
+	return 0;
+}
+
+// The commit of an emission or a removal: model m becomes the n[m] state rows rows[m] (device), its positions follow from them (into
+// its d_pos, which holds n[m] positions), and initial_setup runs over src with those rows, re-capturing the sub-step graphs.  The old
+// graphs are dropped first: from here on a failure leaves a simulator that cannot step.
+int commit_rows(cb200_sim* s, const long long* n, const float* const* rows, StartSrc& src) {
+	drop_graphs(s);
+	for(int m = 0; m < (int) s->models.size(); ++m) {
+		Model& mm = s->models[m];
+		mm.n = (int) n[m];
+		src.rows[m] = rows[m];
+		state_positions_kernel<<<num_sms() * 4, 256, 0, s->stream>>>(mm.n, ck_channels(mm.material), src.rows[m], mm.d_pos);
+		++s->launches;
+	}
+	s->setup_done = false;
+	return setup_impl(s, src);
+}
+
 int emit_precheck(cb200_sim* s, int model, unsigned flags, const float* v0) {
 	if(!s) return (int) cudaErrorInvalidValue;
 	if(s->desc.mgsp_world > 1) return (int) cudaErrorNotSupported;  // a rank's rebuild would have to be agreed with its peers
@@ -2060,13 +2101,9 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 		new_mb = (int) (((long long) u.ebc * 4 + 2) / 3);
 	}
 	// (5) gather the current state (checkpoint layout) and allocate what the commit swaps in: nothing live is written yet
-	CK(pool_alloc(&eb.blob, ck_capacity(s)));
-	SnapshotArgs sa {};
-	sa.grid = s->grid[0];
-	sa.out = eb.blob;
 	long long counts[kMaxModels];
-	CK(read_out(s, snapshot_kernel, sa, counts));
-	const CkLayout L = models_layout(s, counts, h0.nbc);
+	CkLayout L;
+	CK(gather_live(s, h0.nbc, &eb.blob, counts, &L));
 	Model& md = s->models[model];
 	const int C = ck_channels(md.material);
 	const long long n_union = counts[model] + k;
@@ -2083,20 +2120,18 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	// the last step that can reject: cb200_sim_reserve (an out-of-memory failure there leaves a valid simulator, part-grown)
 	if(new_mb > s->desc.max_blocks) CK(cb200_sim_reserve(s, new_mb));
 	// (6) commit: initial_setup over the union's saved rows and grid[0], then the new particles' mass and momentum added to grid[0]
-	drop_graphs(s);
 	if(eb.bins[0] && new_bins > md.bin_capacity) {  // (reserve may have grown the bins past the new count's rule already)
 		for(int i = 0; i < 2; ++i) std::swap(md.pb[i].bins, eb.bins[i]);
 		md.bin_capacity = new_bins;
 	}
 	std::swap(md.d_pos, eb.pos);
-	StartSrc src;
+	long long n_rows[kMaxModels];
+	const float* rows[kMaxModels];
 	for(int m = 0; m < nm; ++m) {
-		Model& mm = s->models[m];
-		mm.n = (int) (m == model ? n_union : counts[m]);
-		src.rows[m] = m == model ? eb.rows : reinterpret_cast<const float*>(eb.blob + L.model_off[m]);
-		state_positions_kernel<<<num_sms() * 4, 256, 0, st>>>(mm.n, ck_channels(mm.material), src.rows[m], mm.d_pos);
-		++s->launches;
+		n_rows[m] = m == model ? n_union : counts[m];
+		rows[m] = m == model ? eb.rows : reinterpret_cast<const float*>(eb.blob + L.model_off[m]);
 	}
+	StartSrc src;
 	src.keys = reinterpret_cast<const int*>(eb.blob + L.keys_off);
 	src.grid = reinterpret_cast<const float*>(eb.blob + L.grid_off);
 	src.grid_count = h0.nbc;
@@ -2105,8 +2140,7 @@ int emit_impl(cb200_sim* s, int model, EmitBuffers& eb, int n, const float* v0, 
 	Clock clock = clock_of(h0, s->frames_done);
 	clock.dt = clock.next_dt = cfl_dt(cfg, h0.dt, sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]));
 	src.clock = &clock;
-	s->setup_done = false;
-	CK(setup_impl(s, src));
+	CK(commit_rows(s, n_rows, rows, src));
 	// every stencil node of a new particle inside the domain lies in a neighbour block of its particle block; nodes past the top face
 	// are dropped, as rasterize_blocks_kernel drops them
 	rasterize_kernel<<<grid_for(k, 256, 16), 256, 0, st>>>(cfg, k, eb.kept, s->grid[0], s->part[s->rollid].index_table, md.pb[0].mass, v[0], v[1], v[2], nullptr);
@@ -2146,6 +2180,117 @@ int cb200_sim_add_particles_sdf(cb200_sim* s, int model, const cb200_sdf_header*
 	CK(pool_alloc(&eb.cand, (size_t) r.count * 3 * sizeof(float)));
 	CK(r.run_write(eb.cand));
 	return emit_impl(s, model, eb, (int) r.count, v0, flags, n_added);
+}
+
+// ---- removing particles at a sub-step boundary (kernels: remove.cuh) ------------------------------------------------------------------
+}  // extern "C"
+namespace {
+// every buffer one call allocates, and the selection runs (their tile offsets)
+struct RemoveBuffers {
+	unsigned char* blob = nullptr;  // the gathered state, checkpoint layout
+	unsigned char* mask = nullptr;  // cb200_sim_remove_rows: the host mask
+	float* rows[kMaxModels] = {};   // per model with removals, the survivors' rows
+	SdfRun runs[kMaxModels];
+	~RemoveBuffers() {
+		g_pool.release(blob);
+		g_pool.release(mask);
+		for(float* p : rows) g_pool.release(p);
+	}
+};
+
+int remove_precheck(cb200_sim* s, long long* removed) {
+	if(removed)
+		for(int m = 0; m < kMaxModels; ++m) removed[m] = 0;
+	if(!s) return (int) cudaErrorInvalidValue;
+	if(s->desc.mgsp_world > 1) return (int) cudaErrorNotSupported;  // a rank's rebuild would have to be agreed with its peers
+	return s->setup_done ? 0 : (int) cudaErrorInvalidValue;
+}
+
+// The shared path of both entries: the models of `mask` lose the rows `sel` (a RemoveRegions or RemoveMask with everything but the
+// rows set) does not keep.  The gather, the selection and the compaction read the live state and write scratch only, so a rejection,
+// or a call that removes nothing, leaves the simulator as it was.  mask_host / mask_n: RemoveMask's host bytes (one model).
+template<class Sel>
+int remove_impl(cb200_sim* s, unsigned mask, Sel sel, const unsigned char* mask_host, long long mask_n, long long* removed) {
+	cudaStream_t st = s->stream;
+	const int nm = (int) s->models.size();
+	CK(cudaStreamSynchronize(st));
+	CK(pull_state(s));
+	const StepState h0 = *s->h_state;
+	RemoveBuffers rb;
+	long long counts[kMaxModels];
+	CkLayout L;
+	CK(gather_live(s, h0.nbc, &rb.blob, counts, &L));
+	if constexpr(std::is_same<Sel, RemoveMask>::value) {
+		if(mask_n != counts[__builtin_ctz(mask)]) return (int) cudaErrorInvalidValue;
+		if(mask_n) {
+			CK(pool_alloc(&rb.mask, (size_t) mask_n));
+			CK(cudaMemcpyAsync(rb.mask, mask_host, (size_t) mask_n, cudaMemcpyHostToDevice, st));
+		}
+		sel.mask = rb.mask;
+	}
+	// (1) per selected model, the survivors' count
+	long long n_rows[kMaxModels], live = 0, gone = 0;
+	for(int m = 0; m < nm; ++m) {
+		n_rows[m] = counts[m];
+		if(mask >> m & 1) {
+			rb.runs[m].st = st;
+			CK(pool_alloc(&rb.runs[m].done, sizeof(unsigned)));
+			sel.in = reinterpret_cast<const float*>(rb.blob + L.model_off[m]);
+			sel.C = ck_channels(s->models[m].material);
+			CK(rb.runs[m].count_pass(sel, counts[m], &n_rows[m]));
+			gone += counts[m] - n_rows[m];
+		}
+		live += n_rows[m];
+	}
+	if(gone == 0) return 0;
+	if(live == 0) return (int) cudaErrorInvalidValue;  // a sub-step over no particle block is not a state the driver runs
+	// (2) the survivors' rows, in row order
+	const float* rows[kMaxModels];
+	for(int m = 0; m < nm; ++m) {
+		rows[m] = reinterpret_cast<const float*>(rb.blob + L.model_off[m]);
+		if(!(mask >> m & 1) || n_rows[m] == counts[m]) continue;
+		sel.in = rows[m];
+		sel.C = ck_channels(s->models[m].material);
+		CK(pool_alloc(&rb.rows[m], (size_t) std::max(1LL, n_rows[m]) * sel.C * sizeof(float)));
+		sel.out = rb.rows[m];
+		CK(rb.runs[m].write_pass(sel));
+		s->launches += 2;
+		rows[m] = rb.rows[m];
+	}
+	// (3) commit: initial_setup over the survivors, grid[0] the survivors' mass at the velocities of the saved grid; the clock is kept
+	StartSrc src;
+	src.vel = reinterpret_cast<const float*>(rb.blob + L.grid_off);
+	src.vel_keys = reinterpret_cast<const int*>(rb.blob + L.keys_off);
+	src.vel_count = h0.nbc;
+	const Clock clock = clock_of(h0, s->frames_done);
+	src.clock = &clock;
+	CK(commit_rows(s, n_rows, rows, src));
+	if(removed)
+		for(int m = 0; m < nm; ++m) removed[m] = counts[m] - n_rows[m];
+	return 0;
+}
+}  // namespace
+extern "C" {
+
+int cb200_sim_remove_particles(cb200_sim* s, unsigned model_mask, const cb200_collision_object* regions, int n, unsigned flags, long long* removed) {
+	CK(remove_precheck(s, removed));
+	RemoveRegions sel {};
+	const int nm = (int) s->models.size();
+	if(!model_mask || (model_mask >> nm) || (flags & ~CB200_REMOVE_OUTSIDE) || !objects_prepare(regions, n, sel.l)) return (int) cudaErrorInvalidValue;
+	if(n == 0) return 0;
+	CK(cudaStreamSynchronize(s->stream));
+	CK(pull_state(s));
+	sel.t = (float) s->h_state->sim_time;
+	sel.outside = (flags & CB200_REMOVE_OUTSIDE) ? 1 : 0;
+	return remove_impl(s, model_mask, sel, nullptr, 0, removed);
+}
+
+int cb200_sim_remove_rows(cb200_sim* s, int model, const unsigned char* remove_host, long long n, long long* removed) {
+	CK(remove_precheck(s, removed));
+	if(model < 0 || model >= (int) s->models.size() || n < 0 || (n > 0 && !remove_host)) return (int) cudaErrorInvalidValue;
+	RemoveMask sel {};
+	static const unsigned char kNone = 0;
+	return remove_impl(s, 1u << model, sel, n ? remove_host : &kNone, n, removed);
 }
 
 // ---- MGSP peer wiring ------------------------------------------------------------------------------------------

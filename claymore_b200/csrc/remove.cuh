@@ -1,0 +1,93 @@
+// remove.cuh -- taking particles out of a set-up simulator at a sub-step boundary (cb200_sim_remove_particles / _rows,
+// include/claymore_b200.h, DESIGN.md section 2.10).
+//   * select and compact: sdf.cuh's count / write pair over one model's gathered rows (checkpoint layout), with an item kind per way
+//     of choosing the rows; an item is kept (survives) unless it is selected, and a kept row is copied whole, in row order;
+//   * the velocity-kept rule of the commit: grid[0]'s mass is rasterised from the survivors, and every node then takes the velocity
+//     p / m it had before the call.
+#pragma once
+#include "checkpoint.cuh"
+#include "collider.cuh"
+#include "sdf.cuh"
+
+namespace cb200 {
+
+// the survivors' rows, C channels each, from the gathered rows `in`
+struct RemoveRows {
+	const float* in;
+	float* out;
+	int C;
+	using Row = long long;  // the source row
+	__device__ __forceinline__ void emit(long long r, const Row& i) const {
+		for(int c = 0; c < C; ++c) out[r * C + c] = __ldg(in + i * C + c);
+	}
+};
+
+// by region: a row is removed when its position, mapped into object k's material space with k's frame at time t as the collider maps
+// a node (collider_resolve_query), lies in any of the n objects (object_query); with `outside`, when it lies in none
+struct RemoveRegions : RemoveRows {
+	ObjectList l;
+	float t;
+	int outside;
+	static __device__ __forceinline__ ObjectFrames& frames() {
+		__shared__ ObjectFrames s;
+		return s;
+	}
+	// thread i builds object i's frame once per CTA (object_frames_cta's work, without the level-set collider)
+	__device__ __forceinline__ void prepare() const {
+		ObjectFrames& s = frames();
+		const int i = (int) threadIdx.x;
+		if(i < l.n) {
+			s.o[i] = l.o[i];
+			collider_make_frame(s.o[i], t, s.f[i]);
+		}
+		__syncthreads();
+	}
+	__device__ __forceinline__ bool eval(long long i, Row& row) const {
+		const ObjectFrames& s = frames();
+		const float p[3] = {__ldg(in + i * C), __ldg(in + i * C + 1), __ldg(in + i * C + 2)};
+		bool hit = false;
+		for(int k = 0; k < l.n; ++k) {
+			const cb200_collision_object& o = s.o[k];
+			const ColliderFrame& f = s.f[k];
+			const float xm[3] = {p[0] - f.b[0], p[1] - f.b[1], p[2] - f.b[2]};
+			const float x0[3] = {xm[0] * f.s_inv, xm[1] * f.s_inv, xm[2] * f.s_inv};
+			const float* R = f.rot;
+			float x[3], n[3];
+#pragma unroll
+			for(int d = 0; d < 3; ++d) x[d] = (R[3 * d] * x0[0] + R[3 * d + 1] * x0[1] + R[3 * d + 2] * x0[2]) * o.scale + o.trans[d];
+			hit |= object_query(o, x, n);
+		}
+		row = i;
+		return hit == (outside != 0);
+	}
+};
+
+// by mask: a row is removed when its byte is non-zero
+struct RemoveMask : RemoveRows {
+	const unsigned char* mask;
+	__device__ __forceinline__ bool eval(long long i, Row& row) const {
+		row = i;
+		return __ldg(mask + i) == 0;
+	}
+};
+
+// The velocity-kept rule, in scatter_grid_kernel's form: a warp per saved block (its key, its 1 KiB), a table query, absent keys
+// skipped.  A node of the rebuilt grid[0] holds the survivors' mass m'; it takes the momentum m' (p / m) from the saved node (m, p),
+// 0 where m = 0.  Each lane takes two nodes of every channel (float2, cell_pair_vel_sq's split).
+__global__ void __launch_bounds__(256) keep_velocity_kernel(Cfg cfg, int count, const int* keys, const float* blocks, const int* table, int nbc, float* grid) {
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	for(int h = blockIdx.x * 8 + warp; h < count; h += gridDim.x * 8) {
+		const int bno = table_query(cfg, table, keys[3 * h], keys[3 * h + 1], keys[3 * h + 2]);
+		if(bno < 0 || bno >= nbc) continue;
+		const float2* s = reinterpret_cast<const float2*>(blocks + (size_t) h * kGridBlockFloats);
+		float2* d = reinterpret_cast<float2*>(grid + (size_t) bno * kGridBlockFloats);
+		const float2 m = s[lane], mn = d[lane];
+#pragma unroll
+		for(int c = 1; c < 4; ++c) {
+			const float2 p = s[32 * c + lane];
+			d[32 * c + lane] = make_float2(m.x != 0.f ? mn.x * (p.x / m.x) : 0.f, m.y != 0.f ? mn.y * (p.y / m.y) : 0.f);
+		}
+	}
+}
+
+}  // namespace cb200

@@ -8,6 +8,7 @@
 //       lattice   items = k^3 points per simulation cell of the range that covers the node box, kept inside the box where phi < 0.
 //     count: per tile a kept count, the last CTA turns the counts into exclusive tile offsets (summary_kernel's pattern);
 //     write: a second launch re-evaluates each item and writes it at its tile offset + warp-ballot rank, so rows are in item order.
+//     (remove.cuh instantiates the pair twice more, over a model's rows, to keep the survivors of a removal in row order.)
 // phi is read through the read-only path; the dragons' 14.6 MB stay in L2 between the passes.
 // Every floating-point step of phi and of the positions is an explicitly rounded double operation, so the rows are bitwise those of
 // the float64 restatement (tests/sdf_ref.py).
@@ -17,6 +18,8 @@
 #include <cmath>
 #include <cstdlib>
 #include <string>
+#include <type_traits>
+#include <utility>
 
 #include "common.cuh"
 
@@ -243,6 +246,13 @@ struct SdfLattice {
 	}
 };
 
+// A kind may build per-CTA state (shared memory) before its first eval: prepare(), run by every thread once, barrier included.  The
+// kinds without one compile to the kernels they had before it existed.
+template<class G, class = void>
+struct has_prepare : std::false_type {};
+template<class G>
+struct has_prepare<G, std::void_t<decltype(std::declval<const G&>().prepare())>> : std::true_type {};
+
 // items [tile T, tile (T + 1)) with T = kSdfThreads * rounds; in round r thread t takes item tile_base + r kSdfThreads + t
 struct SdfScan {
 	long long n_items;
@@ -255,6 +265,7 @@ template<class G>
 __global__ void __launch_bounds__(kSdfThreads) sdf_count_kernel(const G g, const SdfScan a) {
 	__shared__ int s_warp[kSdfThreads / 32];
 	__shared__ bool s_last;
+	if constexpr(has_prepare<G>::value) g.prepare();
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const long long base = (long long) blockIdx.x * kSdfThreads * a.rounds;
 	int cnt = 0;
@@ -315,6 +326,7 @@ __global__ void __launch_bounds__(kSdfThreads) sdf_count_kernel(const G g, const
 template<class G>
 __global__ void __launch_bounds__(kSdfThreads) sdf_write_kernel(const G g, const SdfScan a) {
 	__shared__ int s_warp[2][kSdfThreads / 32];
+	if constexpr(has_prepare<G>::value) g.prepare();
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const long long base = (long long) blockIdx.x * kSdfThreads * a.rounds;
 	long long run = a.tile_off[blockIdx.x];

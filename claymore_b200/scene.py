@@ -35,6 +35,16 @@ sampled again and added with the model's "velocity" (GmpmSimulator.add_particles
 holds no particle, so a repeating source refills only the cells its material has left.  Frame 1 starts from the model's initial
 particles; a resumed run emits exactly the frames an uninterrupted run emits after the checkpoint's frame.  Bad "emit" keys or
 values, or "emit" in MGSP mode, raise ValueError before any device work.
+
+     "sinks": [{"shape", "offset", "span", "normal", "velocity", "omega", "scale", "dsdt", "models": [...], "outside": false,
+                "start": 1, "every": 1, "until": <frames>}, ...]
+
+Outlets (GmpmSimulator.remove_particles, DESIGN.md section 2.10).  A sink's region is placed as a "boundaries" entry of its shape is
+placed, at the simulated time; "models" (scene model indices) defaults to all of them, and "outside": true removes what lies outside
+the region instead of inside it.  At the start of frames start, start + every, ... <= until ("until" defaults to the scene's frame
+count), before the sources emit, the sinks due at that frame with the same "models" and "outside" are removed in one call (at most
+CB200_MAX_COLLISION_OBJECTS sinks in one such group).  A resumed run applies exactly the frames after the checkpoint's frame.  Bad
+keys or values, too many sinks in one group, or "sinks" in MGSP mode raise ValueError before any device work.
 """
 import json
 import os
@@ -105,6 +115,33 @@ def _collider(sim, c, cfg, base_dir):
 BOUNDARY_KEYS = ("shape", "offset", "span", "normal", "type", "friction", "velocity", "omega", "scale", "dsdt")
 
 
+def _object(b, what, keys):
+    """The collision object of one "boundaries" or "sinks" entry `b` (ValueError naming `what` on a bad entry or a key not in `keys`)."""
+    from . import objects
+    if not isinstance(b, dict):
+        raise ValueError(f"{what} must be an object with keys {', '.join(keys)}")
+    unknown = sorted(set(b) - set(keys))
+    if unknown:
+        raise ValueError(f"{what}: unknown keys {unknown} (known: {', '.join(keys)})")
+    shape = b.get("shape")
+    if shape not in objects.SHAPES:
+        raise ValueError(f"{what}: unknown shape {shape!r} (known: {', '.join(objects.SHAPES)})")
+    try:
+        offset = np.asarray(b.get("offset", [0, 0, 0]), dtype=np.float64).reshape(3)
+        span = np.asarray(b.get("span", [1, 1, 1]), dtype=np.float64).reshape(3)
+        motion = dict(type=b.get("type", "sticky"), friction=float(b.get("friction", 0.3)), trans_vel=b.get("velocity", [0, 0, 0]),
+                      omega=b.get("omega", [0, 0, 0]), scale=float(b.get("scale", 1.0)), dsdt=float(b.get("dsdt", 0.0)))
+        if shape == "box":
+            return objects.box(offset, offset + span, **motion)
+        if shape == "sphere":
+            return objects.sphere(offset + span / 2, float(span.min()) / 2, **motion)
+        if shape == "plane":
+            return objects.plane(offset, b.get("normal", [0, 1, 0]), **motion)
+        return objects.cylinder(offset + span / 2, float(min(span[0], span[2])) / 2, float(span[1]) / 2, **motion)
+    except (TypeError, ValueError) as e:
+        raise ValueError(f"{what} ({shape}): {e}") from None
+
+
 def boundaries(doc):
     """The scene's "boundaries" as validated collision objects (ValueError on a bad entry), before any device work."""
     from . import objects
@@ -113,33 +150,84 @@ def boundaries(doc):
         raise ValueError("\"boundaries\" must be a list of objects")
     if len(bs) > objects.MAX_COLLISION_OBJECTS:
         raise ValueError(f"at most {objects.MAX_COLLISION_OBJECTS} \"boundaries\", not {len(bs)}")
+    return [_object(b, f"boundary {i}", BOUNDARY_KEYS) for i, b in enumerate(bs)]
+
+
+SINK_KEYS = ("shape", "offset", "span", "normal", "velocity", "omega", "scale", "dsdt", "models", "outside", "start", "every", "until")
+
+
+def sinks(doc):
+    """The scene's validated "sinks": [{"object", "models" (sorted tuple of scene model indices), "outside", "frames" (list)}], in
+    document order (ValueError on a bad entry, or on more than CB200_MAX_COLLISION_OBJECTS sinks due in one group), before any
+    device work."""
+    from . import objects
+    frames = doc.get("simulation", {}).get("frames", GmpmSimulator.DEFAULT_FRAMES)
+    n_models = len([m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES])
+    ss = doc.get("sinks", [])
+    if not isinstance(ss, list):
+        raise ValueError("\"sinks\" must be a list of objects")
     out = []
-    for i, b in enumerate(bs):
-        if not isinstance(b, dict):
-            raise ValueError(f"boundary {i} must be an object with keys {', '.join(BOUNDARY_KEYS)}")
-        unknown = sorted(set(b) - set(BOUNDARY_KEYS))
-        if unknown:
-            raise ValueError(f"boundary {i}: unknown keys {unknown} (known: {', '.join(BOUNDARY_KEYS)})")
-        shape = b.get("shape")
-        if shape not in objects.SHAPES:
-            raise ValueError(f"boundary {i}: unknown shape {shape!r} (known: {', '.join(objects.SHAPES)})")
-        try:
-            offset = np.asarray(b.get("offset", [0, 0, 0]), dtype=np.float64).reshape(3)
-            span = np.asarray(b.get("span", [1, 1, 1]), dtype=np.float64).reshape(3)
-            motion = dict(type=b.get("type", "sticky"), friction=float(b.get("friction", 0.3)), trans_vel=b.get("velocity", [0, 0, 0]),
-                          omega=b.get("omega", [0, 0, 0]), scale=float(b.get("scale", 1.0)), dsdt=float(b.get("dsdt", 0.0)))
-            if shape == "box":
-                o = objects.box(offset, offset + span, **motion)
-            elif shape == "sphere":
-                o = objects.sphere(offset + span / 2, float(span.min()) / 2, **motion)
-            elif shape == "plane":
-                o = objects.plane(offset, b.get("normal", [0, 1, 0]), **motion)
-            else:
-                o = objects.cylinder(offset + span / 2, float(min(span[0], span[2])) / 2, float(span[1]) / 2, **motion)
-        except (TypeError, ValueError) as e:
-            raise ValueError(f"boundary {i} ({shape}): {e}") from None
-        out.append(o)
+    for i, e in enumerate(ss):
+        what = f"sink {i}"
+        o = _object(e, what, SINK_KEYS)
+        models = e.get("models", list(range(n_models)))
+        if not isinstance(models, list) or not models:
+            raise ValueError(f"{what}: \"models\" must be a non-empty list of model indices, not {models!r}")
+        for m in models:
+            if isinstance(m, bool) or not isinstance(m, int) or not 0 <= m < n_models:
+                raise ValueError(f"{what}: unknown model {m!r} (the scene has {n_models})")
+        outside = e.get("outside", False)
+        if not isinstance(outside, bool):
+            raise ValueError(f"{what}: \"outside\" must be true or false, not {outside!r}")
+        spec = {k: e.get(k, d) for k, d in (("start", 1), ("every", 1), ("until", None))}
+        if spec["until"] is None:   # the last frame; a scene shorter than `start` then never removes
+            spec["until"] = max(frames, spec["start"]) if isinstance(spec["start"], int) else frames
+        for k, v in spec.items():
+            if isinstance(v, bool) or not isinstance(v, int):
+                raise ValueError(f"{what}: \"{k}\" must be an integer, not {v!r}")
+        if spec["start"] < 1:
+            raise ValueError(f"{what}: \"start\" must be at least 1, not {spec['start']}")
+        if spec["every"] < 1:
+            raise ValueError(f"{what}: \"every\" must be at least 1, not {spec['every']}")
+        if spec["until"] < spec["start"]:
+            raise ValueError(f"{what}: \"until\" ({spec['until']}) must not precede \"start\" ({spec['start']})")
+        out.append({"object": o, "models": tuple(sorted(set(models))), "outside": outside,
+                    "frames": list(range(spec["start"], min(spec["until"], frames) + 1, spec["every"]))})
+    for f, groups in _sink_groups(out).items():
+        for (models, outside), idx in groups.items():
+            if len(idx) > objects.MAX_COLLISION_OBJECTS:
+                raise ValueError(f"frame {f}: {len(idx)} sinks of models {list(models)} (outside={outside}) are due together; at most "
+                                 f"{objects.MAX_COLLISION_OBJECTS}")
     return out
+
+
+def _sink_groups(specs, after=0):
+    """{frame: {(models, outside): [sink indices]}} over the frames > after, groups and indices in document order."""
+    out = {}
+    for i, sp in enumerate(specs):
+        for f in sp["frames"]:
+            if f > after:
+                out.setdefault(f, {}).setdefault((sp["models"], sp["outside"]), []).append(i)
+    return dict(sorted(out.items()))
+
+
+def sink_schedule(doc, after=0):
+    """{frame: [(models, outside, [sink indices]), ...]}: the removal calls of every frame > `after` (a resumed run's checkpoint
+    frame), one per group of sinks due together with the same models and outside, in document order.  Validates "sinks"."""
+    return {f: [(m, o, idx) for (m, o), idx in g.items()] for f, g in _sink_groups(sinks(doc), after).items()}
+
+
+def _sink_hook(doc, after=0):
+    """main_loop's per-frame hook that applies the scene's sinks (None without any), built before any device work."""
+    specs = sinks(doc)
+    todo = sink_schedule(doc, after)
+    if not todo:
+        return None
+
+    def remove(s, f):
+        for models, outside, idx in todo.get(f, ()):
+            s.remove_particles([specs[i]["object"] for i in idx], models=models, outside=outside)
+    return remove
 
 
 EMIT_KEYS = ("start", "every", "until", "fill")
@@ -245,11 +333,14 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
     s = doc.get("simulation", {})
     if emit_schedule(doc) and sim_kwargs.get("mgsp_world", 1) > 1:
         raise ValueError("\"emit\" is not supported in MGSP mode")
+    if doc.get("sinks") and sim_kwargs.get("mgsp_world", 1) > 1:
+        raise ValueError("\"sinks\" are not supported in MGSP mode")
     models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
     objs = boundaries(doc)
     if resume is not None:
         inf = _check_resume(doc, cfg, resume)
         emitters = _emitters(doc, cfg, base, _level_sets(models, base))
+        sink = _sink_hook(doc, inf["frames"])
         sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                             frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max(max_blocks, inf["max_blocks"]), **sim_kwargs)
         if "collider" in doc:
@@ -257,12 +348,13 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
         if objs:
             sim.set_collision_objects(objs)
         sim.restore(resume)
-        sim.emitters = emitters
+        sim.emitters = ([sink] if sink else []) + emitters
         return sim
     for model in models:
         if model.get("constitutive") not in CONSTITUTIVE:
             raise ValueError(f"unknown constitutive model {model.get('constitutive')!r}")
     level_sets = _level_sets(models, base)
+    sink = _sink_hook(doc)
     emitters = _emitters(doc, cfg, base, level_sets)
     sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                         frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max_blocks, **sim_kwargs)
@@ -287,5 +379,5 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
         _collider(sim, doc["collider"], cfg, base)
     if objs:
         sim.set_collision_objects(objs)
-    sim.emitters = emitters
+    sim.emitters = ([sink] if sink else []) + emitters
     return sim

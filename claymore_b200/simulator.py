@@ -124,6 +124,39 @@ class GmpmSimulator:
         self.counts[model] += n.value
         return n.value
 
+    # ---- sinks: particles removed from a set-up simulator at the current sub-step boundary (synchronises) -----------------
+    def remove_particles(self, regions, models=None, outside=False):
+        """Removes, from the models `models` (indices; default all of them), the particles whose position lies in any of `regions`
+        (claymore_b200.objects constructors, placed at the simulated time; type and friction are ignored), or with outside=True the
+        particles in none of them.  Survivors keep every channel and their velocity; the clock is kept.  Returns the count removed
+        per model; counts drops by it.  An empty region list removes nothing."""
+        from . import objects
+        regions = list(regions)
+        models = range(len(self.materials)) if models is None else list(models)
+        mask = 0
+        for m in models:
+            if isinstance(m, bool) or not isinstance(m, (int, np.integer)) or not 0 <= m < len(self.materials):
+                raise ValueError(f"unknown model {m!r} (the simulator has {len(self.materials)})")
+            mask |= 1 << int(m)
+        removed = (C.c_longlong * 8)()
+        check(self.L.cb200_sim_remove_particles(self.h, mask, objects.array(regions), len(regions), _capi.REMOVE_OUTSIDE if outside else 0,
+                                                removed), "remove_particles")
+        return self._removed(removed)
+
+    def remove_rows(self, model, mask):
+        """Removes the rows of `model` where `mask` is true (non-zero); row i is row i of particle_state / retrieve now, and the mask
+        has one entry per row.  Returns the count removed per model, as remove_particles."""
+        m = np.ascontiguousarray(np.asarray(mask).reshape(-1) != 0, dtype=np.uint8)
+        removed = (C.c_longlong * 8)()
+        check(self.L.cb200_sim_remove_rows(self.h, model, m.ctypes.data_as(C.c_void_p), m.size, removed), "remove_rows")
+        return self._removed(removed)
+
+    def _removed(self, removed):
+        out = [int(removed[m]) for m in range(len(self.materials))]
+        for m, n in enumerate(out):
+            self.counts[m] -= n
+        return out
+
     def update_fr_parameters(self, rho, vol, ym, pr, model=-1):
         check(self.L.cb200_sim_update_fr_parameters(self.h, self._m(model), rho, vol, ym, pr), "update_fr_parameters")
 
@@ -341,6 +374,8 @@ class GmpmSimulator:
             check(self.L.cb200_sim_retrieve(self.h, model, out.ctypes.data_as(C.c_void_p), C.byref(n)), "retrieve")
             return out.reshape(-1, 3)[: n.value]
         check(self.L.cb200_sim_retrieve_pinned(self.h, model, C.byref(p), C.byref(n)), "retrieve")
+        if n.value == 0:   # an emptied model: there may be no staging buffer to view
+            return np.zeros((0, 3), np.float32)
         view = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(n.value, 3))
         return view.copy() if copy else view
 

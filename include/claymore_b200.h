@@ -321,7 +321,8 @@ typedef struct cb200_checkpoint_info {
 CB200_API int cb200_checkpoint_inspect(const void* blob, size_t bytes, cb200_checkpoint_info* info);
 /* Snapshot at the current sub-step boundary, enqueued on the simulator's stream; waits for the snapshot kernel (not for the sub-steps
  * queued after it), then queues the copy into a pinned buffer the simulator owns on a stream of its own and returns.  *bytes: size
- * of the blob.  Sub-steps enqueued afterwards overlap with the copy. */
+ * of the blob.  Sub-steps enqueued afterwards overlap with the copy.  Format version 1 holds no empty model: while a model has no
+ * particle (after cb200_sim_remove_particles / _rows took them all) it returns cudaErrorNotSupported and changes nothing. */
 CB200_API int cb200_sim_checkpoint_begin(cb200_sim* sim, size_t* bytes);
 /* waits for the copy of the last begin; *blob_pinned stays valid until the next begin, reserve or destroy */
 CB200_API int cb200_sim_checkpoint_end(cb200_sim* sim, const void** blob_pinned, size_t* bytes);
@@ -475,6 +476,42 @@ CB200_API int cb200_sim_add_particles(cb200_sim* sim, int model, const float* po
 /* The same with positions sampled on the device from a level set, as cb200_sim_init_model_sdf samples them (no host copy). */
 CB200_API int cb200_sim_add_particles_sdf(cb200_sim* sim, int model, const cb200_sdf_header* header, const float* phi_host,
                                           const cb200_sdf_sampling* sampling, const float* v0, unsigned flags, int* n_added);
+
+/* ------------------------------------------------------------------------------------------------
+ * Removing particles from a running simulation (sinks: outlets, drains, discarding what leaves a region of interest).  Both entries
+ * share one path and differ only in how the rows to remove are chosen.  The call synchronises and acts at the current sub-step
+ * boundary.
+ *   Rejections, all before anything changes (a checkpoint taken after one is byte-identical to one taken before it):
+ *     cudaErrorNotSupported    MGSP mode (a rank's rebuild would have to be agreed with its peers, as for emission);
+ *     cudaErrorInvalidValue    a simulator that is not set up, an empty or unknown model mask or an unknown model, unknown flag bits,
+ *                              a region cb200_sim_set_collision_objects rejects, n outside [0, CB200_MAX_COLLISION_OBJECTS], a mask
+ *                              length other than the model's row count, or a removal that would leave the whole simulator without
+ *                              a particle.
+ *   Removing nothing (n = 0, regions that hit nothing, an all-zero mask) is a successful no-op: nothing is rebuilt.
+ *   A device error after the commit has begun leaves a simulator that cannot step, as for emission.
+ *   After the call, at the same boundary:
+ *     - every surviving particle keeps all its channels bitwise (as a multiset of rows); the removed rows are exactly those selected;
+ *     - the partition's particle / neighbour / exterior keys are the ones initial_setup builds for the survivors' positions; the bins
+ *       keep their capacity;
+ *     - grid[0]'s mass is the survivors' rasterisation, and every node keeps the velocity it had: momentum_i = m'_i (p_i / m_i) in
+ *       float32, 0 where m_i = 0.  The next sub-step reads only grid[0]'s velocities, so the survivors feel no impulse and their
+ *       velocity (as cb200_sim_frame_output's v defines it) is unchanged; blocks no survivor reaches are dropped;
+ *     - the whole clock is kept bitwise: dt, next_dt, steps, sim_time, step_time, frame_time, the frames finished, the error bits;
+ *     - every model's particle count becomes its live count, as after an emission; the sub-step graphs are re-captured.
+ *   A model may become empty: it stays registered, steps as nothing, cb200_sim_retrieve / particle_state return 0 rows, its frame
+ *   files hold 0 points, and cb200_sim_add_particles* can refill it.  cb200_sim_checkpoint_begin refuses while a model is empty.
+ *   A checkpoint_begin copy or a frame_output frame in flight still delivers the state from before the call.
+ * ---------------------------------------------------------------------------------------------- */
+#define CB200_REMOVE_OUTSIDE 1u  /* remove the particles outside the union of the regions instead of inside it */
+/* Removes, from every model whose bit is set in model_mask, the particles whose position lies in any of regions[0, n): a region is a
+ * cb200_collision_object (shape and motion as in section 2.9; type and friction are ignored), placed at the simulated time, and the
+ * point tested is the particle's position mapped into the object's material space as the collider maps a node.  removed[m]
+ * (nullable, 8 entries): rows removed from model m. */
+CB200_API int cb200_sim_remove_particles(cb200_sim* sim, unsigned model_mask, const cb200_collision_object* regions, int n,
+                                         unsigned flags, long long* removed);
+/* Removes the rows of `model` whose byte in remove_host[0, n) is non-zero; row i is row i of cb200_sim_retrieve / particle_state
+ * at this boundary, and n must equal that row count. */
+CB200_API int cb200_sim_remove_rows(cb200_sim* sim, int model, const unsigned char* remove_host, long long n, long long* removed);
 
 /* ------------------------------------------------------------------------------------------------
  * Test-only hooks (used by tests/, not part of the drop-in surface): the device 3x3 SVD and constitutive models of g2p2g on
