@@ -19,7 +19,8 @@ Conventions the engine keeps (DESIGN.md section 3, quirks):
 * a cell takes at most max_ppc particles at re-bucketing; the rest leave the next partition (``cell_overflow``);
 * nodes outside the domain do not exist: what a particle would add there is dropped;
 * a signed-distance collider (DESIGN.md section 2.4, C1-C6) acts after the wall mask and gravity on the nodes with mass
-  (collider_resolve); nodes near one of its discontinuities, and what reads them, are left out of the checks and counted.
+  (collider_resolve), then the analytic objects in list order (section 2.9, object_chain); nodes near one of their
+  discontinuities, and what reads them, are left out of the checks and counted.
 
 Every output comes with a magnitude M such that an FP32 implementation of the same operations differs from the float64
 value by at most a small multiple of 2^-24 * M.  The tests fix that multiple (kappa) per quantity.
@@ -181,14 +182,16 @@ def compute_dt(cfg, max_vsq, dt_default, time_left=np.inf):
     return min(dt, time_left)
 
 
-def grid_update(cfg, keys, grid, dt, collider=None, t=0.0):
+def grid_update(cfg, keys, grid, dt, collider=None, t=0.0, objects=None):
     """v = mv / m, wall mask on both faces (key < boundary or key >= G - boundary), then gravity, on the nodes whose mass
     is at least FLT_MIN (a subnormal FP32 mass is no mass: the reference flushes subnormals to zero); other nodes keep
     their momentum channels as they are (0 where nothing was added).  With ``collider`` = (col, sdf, grad) the nodes with
     mass then resolve against it, placed at time ``t`` (collider_resolve), and the max is |v|^2 after the collider (C2).
     Returns (vel[nb,3,64], magnitude[nb,3,64], max |v|^2 over the nodes with mass, NaN -> +inf), and with a collider a
     fourth item: dict(near[nb,64], branch[nb,64], margin[nb,64], vo[nb,3,64], mx_lo, mx_hi, mx_err), the max over every
-    choice of the near nodes' branches lying in [mx_lo, mx_hi], and each other node's |v|^2 within kappa 2^-24 mx_err."""
+    choice of the near nodes' branches lying in [mx_lo, mx_hi], and each other node's |v|^2 within kappa 2^-24 mx_err.
+    ``objects`` (a non-empty list of cb200_collision_object or object_params) resolve after the collider, in list order
+    (object_chain); the info then also holds shape_branch[nb,64] and per list entry its labels (stages)."""
     keys = np.asarray(keys, np.int64)
     grid = np.asarray(grid, np.float64)
     G, bc = 1 << (cfg.domain_bits - 2), cfg.boundary
@@ -203,15 +206,34 @@ def grid_update(cfg, keys, grid, dt, collider=None, t=0.0):
     v[:, 1] += np.where(has, gdt, 0.0)
     mag[:, 1] += np.where(has, abs(gdt), 0.0)
     info = None
-    if collider is not None:
-        col, sdf, grad = collider
+    objects = [object_params(o) for o in objects] if objects else []
+    if collider is not None or objects:
         nb = len(keys)
         info = dict(near=np.zeros((nb, 64), bool), branch=np.full((nb, 64), "", dtype=object), margin=np.full((nb, 64), np.inf),
                     vo=np.zeros((nb, 3, 64)))
         b, c = np.nonzero(has)
         nodes = keys[b] * 4 + _CELLS[c]
-        r = collider_resolve(cfg, col, sdf, grad, t, nodes, v[b, :, c], mag[b, :, c])
+        if objects:
+            r = object_chain(cfg, collider, objects, t, nodes, v[b, :, c], mag[b, :, c])
+            info["shape_branch"] = np.full((nb, 64), "", dtype=object)
+            info["shape_branch"][b, c] = r["shape_branch"]
+            info["stages"] = []
+            for lab in r["labels"]:
+                st = {k: np.full((nb, 64), "" if k.endswith("branch") else False, dtype=object if k.endswith("branch") else bool) for k in lab}
+                for k in lab:
+                    st[k][b, c] = lab[k]
+                info["stages"].append(st)
+        else:
+            col, sdf, grad = collider
+            r = collider_resolve(cfg, col, sdf, grad, t, nodes, v[b, :, c], mag[b, :, c])
         v[b, :, c], mag[b, :, c] = r["v"], r["mag"]
+        # g2p2g reads mag as each velocity's scale (the magnitude M of its own roundings), and a velocity resolved exactly
+        # (E = 0: the object velocity of a translating static frame, an axis-aligned normal) still has its size.  On the
+        # collider path mag stays E, so its g2p2g bound is the tighter one there (too tight, never too loose: with the same
+        # floor moving_floor_frame_end's worst F falls from 1.14 to 0.79 of KAPPA); it is kept so that the collider tests'
+        # recorded ratios stay comparable.  The objects path, whose exact branches are common, takes the floor.
+        if objects:
+            mag[b, :, c] = np.maximum(r["mag"], np.abs(r["v"]))
         for f in ("near", "branch", "margin"):
             info[f][b, c] = r[f]
         info["vo"][b, :, c] = r["vo"]
@@ -237,8 +259,9 @@ def grid_update(cfg, keys, grid, dt, collider=None, t=0.0):
 #   the 8 corners, plus its sensitivity to the rounding of x, sum_d |d phi / d x_d| E_x,d with |d phi / d x_d| the largest
 #   one-sided slope of the cell and of its two neighbours along d (the 1/dx amplification at a box's edges);
 #   normalisation: |dn| <= 2 |dn_raw| / |n_raw|, plus the roundings of the sqrt and the division;
-#   friction: v += v / len * (vn f) as the products and sums it is, with |vn f| / len taken at most 1 (the slide side at the
-#   stick switch, where both sides are 0).
+#   friction: v += v / len * (vn f) as the products and sums it is, with |vn f| / len taken at most 1 for a positive friction
+#   (the slide side at the stick switch, where both sides are 0); a negative friction never sticks and pushes v by more than
+#   len where |vn f| > len.
 # Exact zeros and exact copies (STICKY's v = 0, the identity frame of a static collider) carry E = 0, so a node of a static
 # collider on the lattice is not near the wall band edge it sits on.
 # Discontinuities: the hit test (sd <= 0), the wall band (x < lo, x >= hi), the top guard (node gc + 1 >= 4G) and the exact
@@ -366,30 +389,35 @@ def _slope(f, gc, w, N, dx):
     return out
 
 
-def collider_resolve(cfg, col, sdf, grad, t, nodes, v, vmag):
-    """detect_and_resolve_collision of the velocities v[n, 3] (magnitudes vmag[n, 3]) at the grid nodes nodes[n, 3], the
-    collider col (collider_params) placed at the float32 time t, its level set the dense sdf[(N, N, N)], grad[(3, N, N, N)]
-    read by node index.  Returns dict(v, mag (E of each component), vo (the object velocity), hit, branch (label), margin
-    (distance to the nearest discontinuity in units of 2^-24 E), near, vsq_lo, vsq_hi (|v|^2 over both sides of a near
-    node's branch))."""
+def material_point(cfg, col, t, nodes):
+    """The collider's (or an object's) frame at the float32 time t and the material-space point of each node nodes[n, 3]:
+    dict(f (collider_frame), col (collider_params), Rb (the rotation per node, (value, E)), xm (node dx - b), x (the
+    material-space point R (node dx - b) s_inv scale + trans)), every vector as (value[n, 3], E[n, 3])."""
     f = collider_frame(col, t)
     col = f["col"]
     nodes = np.asarray(nodes, np.int64).reshape(-1, 3)
     n = len(nodes)
-    G = 1 << (cfg.domain_bits - 2)
-    N, bc = 4 * G, cfg.boundary
     dx = 1.0 / (1 << cfg.domain_bits)
-    vin = (np.asarray(v, np.float64).reshape(n, 3), np.asarray(vmag, np.float64).reshape(n, 3))
     R = f["rot"]
     Rb = (np.broadcast_to(R[0], (n, 9)), np.broadcast_to(R[1], (n, 9)))
-    # material-space point: x = R (node dx - b) s_inv scale + trans
     xm = _sub(_exact(nodes * dx), (np.broadcast_to(f["b"][0], (n, 3)), np.broadcast_to(f["b"][1], (n, 3))))
     x0 = _mul(xm, f["s_inv"])
     y = [_dot3(Rb, x0, lambda k, d=d: 3 * d + k, lambda k: k) for d in range(3)]
     y = (np.stack([a[0] for a in y], -1), np.stack([a[1] for a in y], -1))
     x = _add(_mul(y, _exact(col["scale"])), _exact(col["trans"]))
-    tol = EPS32 * NEAR
-    # query: wall band, top guard, trilinear distance and gradient
+    return dict(f=f, col=col, Rb=Rb, xm=xm, x=x)
+
+
+def levelset_query(cfg, sdf, grad, x):
+    """collider_query of the dense level set sdf[(N, N, N)], grad[(3, N, N, N)] (read by node index) at the material-space
+    points x = (value[n, 3], E[n, 3]).  Returns the query dict collider_resolve takes: hit, on / eon (the material-space
+    normal and its E), zero (no normal), m_zero (its margin), margin (of the wall band, the top guard and the hit test),
+    branch (the label of a node that is not hit)."""
+    n = len(x[0])
+    G = 1 << (cfg.domain_bits - 2)
+    N, bc = 4 * G, cfg.boundary
+    dx = 1.0 / (1 << cfg.domain_bits)
+    # wall band, top guard, trilinear distance and gradient
     lo, hi = float(bc) * dx * 4.0, float(G - bc) * 4.0 * dx
     band = np.any((x[0] < lo) | (x[0] >= hi), axis=1)
     with np.errstate(divide="ignore", invalid="ignore"):
@@ -419,6 +447,29 @@ def collider_resolve(cfg, col, sdf, grad, t, nodes, v, vmag):
         m_zero = np.where(zero, np.where(enr_len > 0, 0.0, np.inf), ln / (EPS32 * enr_len))
         on = np.where(zero[:, None], 0.0, nr / np.where(zero, 1.0, ln)[:, None])
         eon = np.where(zero[:, None], 0.0, (2 * enr_len / np.where(zero, 1.0, ln))[:, None] + 3 * np.abs(on))
+    branch = np.where(band, "band", np.where(top, "top", "miss")).astype(object)
+    margin = np.where(band | top, np.minimum(m_band, m_top), np.minimum(np.minimum(m_band, m_top), m_hit))
+    return dict(hit=hit, on=on, eon=eon, zero=zero, m_zero=m_zero, margin=margin, branch=branch)
+
+
+def collider_resolve(cfg, col, sdf, grad, t, nodes, v, vmag):
+    """detect_and_resolve_collision of the velocities v[n, 3] (magnitudes vmag[n, 3]) at the grid nodes nodes[n, 3], the
+    collider col (collider_params) placed at the float32 time t, its level set the dense sdf[(N, N, N)], grad[(3, N, N, N)]
+    read by node index.  Returns dict(v, mag (E of each component), vo (the object velocity), hit, branch (label), margin
+    (distance to the nearest discontinuity in units of 2^-24 E), near, vsq_lo, vsq_hi (|v|^2 over both sides of a near
+    node's branch)) and what object_chain needs to follow a near node's branches."""
+    p = material_point(cfg, col, t, nodes)
+    return resolve_query(p, levelset_query(cfg, sdf, grad, p["x"]), v, vmag)
+
+
+def resolve_query(p, q, v, vmag):
+    """The object velocity and the response of the collider or object p["col"] (material_point p) to the query q at the nodes
+    with velocities v[n, 3] (magnitudes vmag[n, 3]), shared by the level set and the analytic shapes (collider_resolve)."""
+    col, Rb, xm, x = p["col"], p["Rb"], p["xm"], p["x"]
+    n = len(xm[0])
+    vin = (np.asarray(v, np.float64).reshape(n, 3), np.asarray(vmag, np.float64).reshape(n, 3))
+    tol = EPS32 * NEAR
+    hit, on, eon, zero, m_zero = q["hit"], q["on"], q["eon"], q["zero"], q["m_zero"]
     # object velocity: omega x xm + xm dsdt / scale + R^T (omega (all-plus) r + trans_vel) scale + trans_vel, r = x - trans
     wv = _exact(np.broadcast_to(col["omega"], (n, 3)))
     cross = [_sub(_mul((wv[0][:, a], wv[1][:, a]), (xm[0][:, b], xm[1][:, b])), _mul((wv[0][:, b], wv[1][:, b]), (xm[0][:, a], xm[1][:, a])))
@@ -438,8 +489,9 @@ def collider_resolve(cfg, col, sdf, grad, t, nodes, v, vmag):
     vr = _sub(vin, vo)
     typ, fr = col["type"], col["friction"]
     out_v, out_e = vin[0].copy(), vin[1].copy()
-    branch = np.where(band, "band", np.where(top, "top", "miss")).astype(object)
-    margin = np.where(band | top, np.minimum(m_band, m_top), np.minimum(np.minimum(m_band, m_top), m_hit))
+    branch = q["branch"].copy()
+    margin = q["margin"]
+    m_hit = np.nan_to_num(margin, nan=np.inf)                               # the hit test's: a near node may miss or hit
     zero_alt = np.zeros(n, bool)
     res_v, res_e = vo[0].copy(), vo[1].copy()                               # STICKY: v = 0 + vo
     if typ == STICKY:
@@ -455,11 +507,11 @@ def collider_resolve(cfg, col, sdf, grad, t, nodes, v, vmag):
         eplen = np.where(plen > 0, (np.abs(proj[0]) * proj[1]).sum(1) / np.where(plen > 0, plen, 1.0), np.sqrt((proj[1] ** 2).sum(1))) + _rnd(plen)
         vnf = _mul(vn, _exact(fr))
         with np.errstate(divide="ignore", invalid="ignore"):
-            q = np.minimum(np.abs(vnf[0]) / plen, 1.0)
-            q = np.where(plen > 0, q, 1.0)
+            qf = np.abs(vnf[0]) / plen                                  # a negative friction has no stick side: |vn f| / len may exceed 1
+            qf = np.where(plen > 0, np.minimum(qf, 1.0) if fr > 0 else qf, 1.0)
             unit = proj[0] / np.where(plen > 0, plen, 1.0)[:, None]
         slide_v = proj[0] + unit * vnf[0][:, None]
-        slide_e = proj[1] * (1 + q)[:, None] + np.abs(unit) * (vnf[1] + q * eplen)[:, None] + _rnd(slide_v)
+        slide_e = proj[1] * (1 + qf)[:, None] + np.abs(unit) * (vnf[1] + qf * eplen)[:, None] + _rnd(slide_v)
         stick = -vnf[0] >= plen
         with np.errstate(divide="ignore", invalid="ignore"):
             near_stick = np.abs(plen + vnf[0]) <= tol * (eplen + vnf[1])
@@ -497,12 +549,233 @@ def collider_resolve(cfg, col, sdf, grad, t, nodes, v, vmag):
     alt_miss = (vin[0] ** 2).sum(1)
     lo_sq = np.where(near, np.minimum(alt_hit, alt_miss), vsq)
     hi_sq = np.where(near, np.maximum(alt_hit, alt_miss), vsq)
+    span = np.zeros(n)
+    ovo = np.sqrt((vo[0] ** 2).sum(1))
     if typ != STICKY:
         span = (1 + abs(fr)) * np.sqrt((vr[0] ** 2).sum(1))
-        ovo = np.sqrt((vo[0] ** 2).sum(1))
         lo_sq = np.where(zero_alt, np.minimum(lo_sq, np.maximum(ovo - span, 0.0) ** 2), lo_sq)
         hi_sq = np.where(zero_alt, np.maximum(hi_sq, (ovo + span) ** 2), hi_sq)
-    return dict(v=out_v, mag=out_e, vo=vo[0], hit=hit, branch=branch, margin=margin, near=near, vsq_lo=lo_sq, vsq_hi=hi_sq)
+    return dict(v=out_v, mag=out_e, vo=vo[0], hit=hit, branch=branch, margin=margin, near=near, vsq_lo=lo_sq, vsq_hi=hi_sq,
+                res_v=res_v, near_hit=m_hit <= NEAR, normal_alt=zero_alt, ovo=ovo, span=span, shape_branch=q.get("shape_branch"),
+                type=typ, friction=fr)
+
+
+# ---- analytic collision objects (DESIGN.md section 2.9, object_query in collider.cuh) ------------------------------------
+# The object's frame, material-space point, object velocity and response are the collider's (material_point, resolve_query);
+# only the query differs.  Each query's quantities carry E by the rules above, plus sqrt(a) near 0: at most sqrt(Ea / 2^-24)
+# in units of 2^-24 (|sqrt(a + e) - sqrt(a)| <= sqrt(|e|)).  Discontinuities and their margins (distance / (2^-24 E)):
+#   plane  phi = (x - a) . b <= 0, b the stored unit normal (exact);
+#   box    the six comparisons a_d <= x_d <= b_d (a miss flips only if every failing one does: its margin is their largest),
+#          the axis of the largest q_d = max(a_d - x_d, x_d - b_d) (a strict > : the lowest axis wins a tie), and the face's
+#          sign ql > qh (+1 at the exact centre);
+#   sphere dd = |x - a|^2 <= r * r (with the rounding of r * r), the zero-normal test dd > 0, n = d / sqrt(dd);
+#   cylinder rho2 = d0^2 + d2^2 <= r * r and |d1| <= h, the cap / side switch h - |d1| < r - rho, the cap's sign d1 < 0, the
+#          side's zero-normal test rho > 0, n = (d0, 0, d2) / rho.
+# An exact quantity exactly on a switch (E = 0: 0 / 0) is decided alike, as above.  A hit node near a normal switch (box axis
+# or sign, cylinder cap or side, a zero normal) may take any unit normal in FP32: object_chain bounds it by the span bound.
+PLANE, BOX, SPHERE, CYLINDER = 0, 1, 2, 3
+MAX_CANDIDATES = 8     # object_chain: a node's branch candidates beyond this many collapse into one speed interval
+
+
+def object_params(o):
+    """An object's float32 fields as float64 values (a cb200_collision_object or a dict with its fields), the plane normal as
+    cb200_sim_set_collision_objects stores it: made unit length in double once more and rounded to float32."""
+    get = (lambda k: o[k]) if isinstance(o, dict) else (lambda k: getattr(o, k))
+    p = collider_params(o)
+    f32 = lambda x: np.asarray(np.asarray(x, np.float32), np.float64)   # noqa: E731
+    p.update(shape=int(get("shape")), a=f32(list(get("a"))), b=f32(list(get("b"))))
+    if p["shape"] == PLANE:
+        p["b"] = f32(p["b"] / np.sqrt((p["b"] * p["b"]).sum()))
+    return p
+
+
+def _col(x, k):
+    return x[0][:, k], x[1][:, k]
+
+
+def _margin(dist, err):
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.abs(dist) / (EPS32 * err)
+
+
+def _sqrt(a):
+    v = np.sqrt(a[0])
+    with np.errstate(divide="ignore", invalid="ignore"):
+        flat = np.sqrt(a[1] / EPS32)
+        e = np.where(v > 0, np.minimum(a[1] / (2 * np.where(v > 0, v, 1.0)), flat), flat)
+    return v, e + _rnd(v)
+
+
+def _both(conds, margins):
+    """hit = every condition, and its margin: the smallest over all when it holds, else the largest over the failing ones."""
+    conds, margins = np.stack(conds, 1), np.nan_to_num(np.stack(margins, 1), nan=np.inf)
+    hit = conds.all(1)
+    return hit, np.where(hit, margins.min(1), np.where(conds, 0.0, margins).max(1))
+
+
+def object_query(o, x):
+    """object_query of the object o (object_params) at the material-space points x = (value[n, 3], E[n, 3]): the query dict of
+    resolve_query (the normal margins folded into m_zero, so that a node near any normal switch is near and bounded by
+    the span bound), plus shape_branch (the shape's branch label of each hit node)."""
+    n = len(x[0])
+    a, b, shape = o["a"], o["b"], o["shape"]
+    on, eon = np.zeros((n, 3)), np.zeros((n, 3))
+    zero = np.zeros(n, bool)
+    m_norm = np.full(n, np.inf)
+    d = [_sub(_col(x, k), _exact(a[k])) for k in range(3)]
+    if shape == PLANE:
+        phi = _add(_add(_mul(d[0], _exact(b[0])), _mul(d[1], _exact(b[1]))), _mul(d[2], _exact(b[2])))
+        hit, margin = phi[0] <= 0, _margin(phi[0], phi[1])
+        on[:] = b
+        sb = np.full(n, "plane", dtype=object)
+    elif shape == BOX:
+        conds, ms = [], []
+        for k in range(3):
+            conds += [a[k] <= x[0][:, k], x[0][:, k] <= b[k]]
+            ms += [_margin(x[0][:, k] - a[k], x[1][:, k]), _margin(x[0][:, k] - b[k], x[1][:, k])]
+        hit, margin = _both(conds, ms)
+        ql = [_sub(_exact(a[k]), _col(x, k)) for k in range(3)]
+        qh = [_sub(_col(x, k), _exact(b[k])) for k in range(3)]
+        qv = np.stack([np.maximum(ql[k][0], qh[k][0]) for k in range(3)], 1)
+        qe = np.stack([np.maximum(ql[k][1], qh[k][1]) for k in range(3)], 1)
+        axis = np.argmax(qv, 1)                                             # the first of equal maxima: the lowest axis
+        i = np.arange(n)
+        for k in range(3):
+            m_ax = np.nan_to_num(_margin(qv[i, axis] - qv[:, k], qe[i, axis] + qe[:, k]), nan=np.inf)
+            m_norm = np.minimum(m_norm, np.where(axis == k, np.inf, m_ax))
+        qlv = np.stack([c[0] for c in ql], 1)[i, axis]
+        qhv = np.stack([c[0] for c in qh], 1)[i, axis]
+        sgn = np.where(qlv > qhv, -1.0, 1.0)
+        m_sgn = _margin(qlv - qhv, np.stack([c[1] for c in ql], 1)[i, axis] + np.stack([c[1] for c in qh], 1)[i, axis])
+        m_norm = np.minimum(m_norm, np.nan_to_num(m_sgn, nan=np.inf))
+        on[i, axis] = sgn
+        sb = np.array([f"box_{'xyz'[k]}{'-' if s < 0 else '+'}" for k, s in zip(axis, sgn)], dtype=object)
+    elif shape == SPHERE:
+        dd = _add(_add(_mul(d[0], d[0]), _mul(d[1], d[1])), _mul(d[2], d[2]))
+        rr = _mul(_exact(b[0]), _exact(b[0]))
+        hit, margin = dd[0] <= rr[0], _margin(dd[0] - rr[0], dd[1] + rr[1])
+        zero = dd[0] == 0
+        m_norm = np.nan_to_num(_margin(dd[0], dd[1]), nan=np.inf)
+        ln = _sqrt(dd)
+        safe = (np.where(zero, 1.0, ln[0]), ln[1])
+        for k in range(3):
+            c = _div(d[k], safe)
+            on[:, k], eon[:, k] = np.where(zero, 0.0, c[0]), np.where(zero, 0.0, c[1])
+        sb = np.where(zero, "sphere_zero", "sphere").astype(object)
+    else:
+        h = b[1]
+        rho2 = _add(_mul(d[0], d[0]), _mul(d[2], d[2]))
+        rr = _mul(_exact(b[0]), _exact(b[0]))
+        ad1 = (np.abs(d[1][0]), d[1][1])
+        hit, margin = _both([rho2[0] <= rr[0], ad1[0] <= h], [_margin(rho2[0] - rr[0], rho2[1] + rr[1]), _margin(ad1[0] - h, ad1[1])])
+        rho = _sqrt(rho2)
+        A, B = _sub(_exact(h), ad1), _sub(_exact(b[0]), rho)
+        cap = A[0] < B[0]
+        m_cap = np.nan_to_num(_margin(A[0] - B[0], A[1] + B[1]), nan=np.inf)
+        m_csgn = np.nan_to_num(_margin(d[1][0], d[1][1]), nan=np.inf)
+        zero = ~cap & (rho[0] == 0)
+        m_zero_side = np.nan_to_num(_margin(rho2[0], rho2[1]), nan=np.inf)
+        m_norm = np.minimum(m_cap, np.where(cap, m_csgn, m_zero_side))
+        on[:, 1] = np.where(cap, np.where(d[1][0] < 0, -1.0, 1.0), 0.0)
+        safe = (np.where(rho[0] > 0, rho[0], 1.0), rho[1])
+        for k in (0, 2):
+            c = _div(d[k], safe)
+            side = ~cap & ~zero
+            on[:, k], eon[:, k] = np.where(side, c[0], 0.0), np.where(side, c[1], 0.0)
+        tie = (A[0] == B[0]) & (A[1] == 0) & (B[1] == 0)                    # an exact cap / side tie: the side wins
+        sb = np.where(cap, np.where(d[1][0] < 0, "cyl_cap-", "cyl_cap+"), np.where(zero, "cyl_zero", np.where(tie, "cyl_side_tie", "cyl_side"))).astype(object)
+    return dict(hit=hit, on=on, eon=eon, zero=zero, m_zero=m_norm, margin=margin, branch=np.full(n, "miss", dtype=object),
+                shape_branch=np.where(hit, sb, "miss").astype(object))
+
+
+def object_resolve(cfg, o, t, nodes, v, vmag):
+    """collider_resolve with the analytic object o (object_params) in place of the level set."""
+    p = material_point(cfg, o, t, nodes)
+    return resolve_query(p, object_query(o, p["x"]), v, vmag)
+
+
+def object_chain(cfg, collider, objects, t, nodes, v, vmag):
+    """The level-set collider = (col, sdf, grad) (or None), then each object (object_params) in list order, each resolving
+    the velocity and E the previous one left, all placed at the float32 time t.  Returns collider_resolve's dict with near
+    the union over the list, margin the smallest, branch the last hit's label (shape_branch likewise: labels[i] per stage in
+    ``labels``), and vsq_lo / vsq_hi over every branch choice of the near nodes: their candidate velocities are carried
+    through the list, each near decision adding the other branch; a near normal switch (any unit normal) and a node with more
+    than MAX_CANDIDATES candidates carry a speed interval instead."""
+    nodes = np.asarray(nodes, np.int64).reshape(-1, 3)
+    stages = []
+    if collider is not None:
+        col, sdf, grad = collider
+        stages.append(lambda nd, vv, vm: collider_resolve(cfg, col, sdf, grad, t, nd, vv, vm))
+    for o in objects:
+        stages.append(lambda nd, vv, vm, o=o: object_resolve(cfg, o, t, nd, vv, vm))
+    n = len(nodes)
+    v0 = np.asarray(v, np.float64).reshape(n, 3)
+    cur, mag = v0, np.asarray(vmag, np.float64).reshape(n, 3)
+    near, margin = np.zeros(n, bool), np.full(n, np.inf)
+    branch, shape_branch = np.full(n, "miss", dtype=object), np.full(n, "miss", dtype=object)
+    labels, vo = [], np.zeros((n, 3))
+    for st in stages:
+        r = st(nodes, cur, mag)
+        cur, mag = r["v"], r["mag"]
+        near |= r["near"]
+        margin = np.minimum(margin, r["margin"])
+        branch = np.where(r["hit"], r["branch"], branch)
+        sb = r["shape_branch"] if r["shape_branch"] is not None else np.where(r["hit"], "levelset", "miss").astype(object)
+        shape_branch = np.where(r["hit"], sb, shape_branch)
+        vo = np.where(r["hit"][:, None], r["vo"], vo)
+        labels.append(dict(hit=r["hit"], near=r["near"], branch=r["branch"], shape_branch=sb))
+    vsq = (cur ** 2).sum(1)
+    lo, hi = vsq.copy(), vsq.copy()
+    S = np.flatnonzero(near)
+    if len(S):
+        # candidate rows: (owner in S, velocity) or (owner, speed interval [slo, shi]) with a NaN velocity
+        own = np.arange(len(S))
+        rv = v0[S].copy()
+        iv = np.full((len(S), 2), np.nan)
+        for st in stages:
+            isint = ~np.isnan(iv[:, 0])
+            r = st(nodes[S][own], np.where(isint[:, None], 0.0, rv), np.zeros((len(own), 3)))
+            sticky, fr = r["type"] == STICKY, abs(r["friction"])
+            no, nv, ni = [], [], []
+            for j in range(len(own)):
+                hit, nh, ovo, span = bool(r["hit"][j]), bool(r["near_hit"][j]), r["ovo"][j], r["span"][j]
+                if hit or nh:                                           # the hit branch
+                    if sticky:
+                        no.append(own[j]), nv.append(r["vo"][j]), ni.append((np.nan, np.nan))
+                    elif isint[j]:                                      # |v - vo| <= (1 + |friction|) |v_in - vo|
+                        no.append(own[j]), nv.append(np.zeros(3)), ni.append((0.0, ovo + (1 + fr) * (iv[j][1] + ovo)))
+                    elif r["normal_alt"][j]:                            # any unit normal (SEPARATE's zero normal: 0)
+                        no.append(own[j]), nv.append(np.zeros(3)), ni.append((0.0 if r["type"] == SEPARATE else max(ovo - span, 0.0), ovo + span))
+                    else:
+                        no.append(own[j]), nv.append(r["res_v"][j]), ni.append((np.nan, np.nan))
+                if nh or not hit:                                       # the miss branch: the row as it is
+                    no.append(own[j]), nv.append(rv[j]), ni.append(iv[j])
+            own, rv, iv = np.asarray(no, np.int64), np.asarray(nv, np.float64).reshape(-1, 3), np.asarray(ni, np.float64).reshape(-1, 2)
+            own, rv, iv = _cap_candidates(own, rv, iv)
+        sp_lo = np.where(np.isnan(iv[:, 0]), np.sqrt((rv ** 2).sum(1)), iv[:, 0])
+        sp_hi = np.where(np.isnan(iv[:, 0]), np.sqrt((rv ** 2).sum(1)), iv[:, 1])
+        clo, chi = np.full(len(S), np.inf), np.zeros(len(S))
+        np.minimum.at(clo, own, sp_lo ** 2)
+        np.maximum.at(chi, own, sp_hi ** 2)
+        lo[S], hi[S] = clo, chi
+    return dict(v=cur, mag=mag, vo=vo, near=near, margin=margin, branch=branch, shape_branch=shape_branch, labels=labels,
+                vsq_lo=lo, vsq_hi=hi)
+
+
+def _cap_candidates(own, rv, iv):
+    """A node with more than MAX_CANDIDATES rows keeps one: the speed interval over them."""
+    cnt = np.bincount(own, minlength=own.max(initial=-1) + 1)
+    big = cnt[own] > MAX_CANDIDATES
+    if not big.any():
+        return own, rv, iv
+    sp = np.sqrt((rv ** 2).sum(1))
+    slo, shi = np.where(np.isnan(iv[:, 0]), sp, iv[:, 0]), np.where(np.isnan(iv[:, 0]), sp, iv[:, 1])
+    keep = ~big
+    out_o, out_v, out_i = [own[keep]], [rv[keep]], [iv[keep]]
+    for o in np.unique(own[big]):
+        m = own == o
+        out_o.append(np.array([o])), out_v.append(np.zeros((1, 3))), out_i.append(np.array([[slo[m].min(), shi[m].max()]]))
+    return np.concatenate(out_o), np.concatenate(out_v), np.concatenate(out_i)
 
 
 # ---- constitutive models (exact float64) -------------------------------------------------------------------------------
@@ -714,13 +987,13 @@ def g2p2g(cfg, models, vkeys, vel, vmag, dt, new_dt, near=None):
     return dict(models=out, keys=keys, grid=g[:, :4], mag=g[:, 4:8], stress=g[:, 8:12], taint=g[:, 12])
 
 
-def substep(cfg, models, keys, grid, dt, dt_default, time_left=np.inf, collider=None, t=0.0):
-    """The whole sub-step: grid update at dt (with ``collider`` = (col, sdf, grad) placed at the float32 time t), new_dt
-    from its max, g2p2g with (dt, new_dt).  ``dt_range`` = (new_dt of mx_hi, new_dt of mx_lo): the new dt over every branch
-    choice of the collider's near nodes; ``collider_info`` is grid_update's."""
-    u = grid_update(cfg, keys, grid, dt, collider, t)
+def substep(cfg, models, keys, grid, dt, dt_default, time_left=np.inf, collider=None, t=0.0, objects=None):
+    """The whole sub-step: grid update at dt (with ``collider`` = (col, sdf, grad), then ``objects``, placed at the float32
+    time t), new_dt from its max, g2p2g with (dt, new_dt).  ``dt_range`` = (new_dt of mx_hi, new_dt of mx_lo): the new dt over
+    every branch choice of the near nodes; ``collider_info`` is grid_update's."""
+    u = grid_update(cfg, keys, grid, dt, collider, t, objects)
     vel, vmag, mx = u[:3]
-    info = u[3] if collider is not None else dict(near=None, mx_lo=mx, mx_hi=mx, mx_err=0.0)
+    info = u[3] if len(u) > 3 else dict(near=None, mx_lo=mx, mx_hi=mx, mx_err=0.0)
     new_dt = compute_dt(cfg, mx, dt_default, time_left)
     r = g2p2g(cfg, models, keys, vel, vmag, dt, new_dt, info["near"])
     r.update(max_vsq=mx, new_dt=new_dt, vel=vel, vel_mag=vmag, collider_info=info,

@@ -3,7 +3,8 @@
 A case is dict(domain_bits, models=[dict(material, pos, v0, rho, vol, args)], dt, steps, cfl, max_ppc, gravity, boundary): ``args``
 are the material setter's arguments after (rho, vol); ``steps`` the sub-steps k at which one sub-step is checked.  A case with
 a ``collider`` = dict(field=(kind, *args), type, friction, rot_mat, trans, trans_vel, omega, dsdt, scale) has a signed-distance
-collider (collider_field, collider_struct; the other keys default to SignedDistanceGrid's).
+collider (collider_field, collider_struct; the other keys default to SignedDistanceGrid's).  A case with ``objects`` has
+analytic collision objects after it (OBJECT_CASES, object_structs).
 """
 import numpy as np
 
@@ -274,7 +275,15 @@ def config(case):
 def build_oracle(ob, case, max_blocks=6000):
     cfg = ob.make_config(domain_bits=case["domain_bits"], max_ppc=case["max_ppc"], cfl=case["cfl"], gravity=case.get("gravity", -9.8),
                          boundary=case.get("boundary", 2))
-    if case.get("collider"):
+    if case.get("objects"):
+        import collider_oracle_binding as cob
+        import objects_oracle_binding as oob
+        sim = oob.ObjectsOracleSim(cfg, case["dt"], max_blocks)
+        if case.get("collider"):
+            sdf, grad = collider_field(case)
+            sim.set_collider(collider_struct(cob.Collider(), case["collider"]), sdf, grad)
+        sim.set_collision_objects(object_structs(case))
+    elif case.get("collider"):
         import collider_oracle_binding as cob
         sim = cob.ColliderOracleSim(cfg, case["dt"], max_blocks)
         sdf, grad = collider_field(case)
@@ -300,6 +309,8 @@ def build_engine(case, use_graph=True, max_blocks=6000):
         p = collider_spec(case["collider"])
         sim.set_collider(sdf, grad, type=p["type"], friction=p["friction"], trans=p["trans"], trans_vel=p["trans_vel"], omega=p["omega"],
                          rot=np.asarray(p["rot_mat"]).reshape(3, 3), scale=p["scale"], dsdt=p["dsdt"])
+    if case.get("objects"):
+        sim.set_collision_objects(object_structs(case))
     sim.initial_setup()
     return sim
 
@@ -418,4 +429,112 @@ COLLIDER_CASES = {
     # the wall thickness without a collider
     "walls_boundary1": _walls(FIXED_COROTATED, boundary=1),
     "fc_cube_boundary0": _cube(FIXED_COROTATED, steps=[0, 3], boundary=0),
+}
+
+
+# ---- analytic collision objects (DESIGN.md section 2.9) -------------------------------------------------------------------
+# A case with ``objects`` = [(shape, args, keywords)] has analytic collision objects (claymore_b200.objects.<shape>(*args,
+# **keywords)), resolved after its collider, if any, in list order (object_structs, ref_objects).
+def make_object(shape, args, **kw):
+    """claymore_b200.objects.<shape>(*args, **kw); shape "raw_plane" is a plane whose stored normal is the caller's as given,
+    not of unit length: only cb200_sim_set_collision_objects' own normalisation makes it one."""
+    from claymore_b200 import objects
+    if shape != "raw_plane":
+        return getattr(objects, shape)(*args, **kw)
+    o = objects.plane(*args, **kw)
+    o.b[:] = [float(v) for v in args[1]]
+    return o
+
+
+def object_structs(case):
+    """The case's objects as cb200_collision_object structs (make_object)."""
+    return [make_object(shape, args, **kw) for shape, args, kw in case.get("objects", ())]
+
+
+def ref_objects(case):
+    """The ``objects`` argument of ref64.grid_update / substep for a case (None without objects)."""
+    return object_structs(case) or None
+
+
+FLOOR_LO, FLOOR_HI = FLOOR[1], FLOOR[2]
+# every motion at once, as _paddle's collider: a non-identity rot_mat, trans, trans_vel, all three omega components, scale, dsdt
+PADDLE_MOTION = dict(rot=_rot(0.4, -0.3, 0.25), trans=(0.40, 0.40, 0.40), trans_vel=(3.0, 0.5, -1.0), omega=(0.5, -0.7, 1.1), scale=1.1, dsdt=0.3)
+
+
+def _on_object_floor(material, typ, friction=0.3, steps=(12, 30), **kw):
+    """_on_floor with FLOOR as an analytic box."""
+    dx = 1.0 / 64
+    return _case(6, [model(material, box(dx, (26, 21, 26), (34, 27, 34)), (0.3, -6.0, 0.2), dx)], list(steps), dt=2e-4,
+                 objects=[("box", (FLOOR_LO, FLOOR_HI), dict(type=typ, friction=friction))], **kw)
+
+
+def _falling(lo, hi, objs, steps=(10, 24), v0=(0.3, -6.0, 0.2), material=FIXED_COROTATED, dt=2e-4, **kw):
+    """A block [lo, hi) (cells) falling onto the objects objs."""
+    dx = 1.0 / 64
+    return _case(6, [model(material, box(dx, lo, hi), v0, dx)], list(steps), dt=dt, objects=objs, **kw)
+
+
+def _sixteen():
+    """The longest list: five container planes around a fluid block and eleven small boxes and spheres inside the container,
+    the last of them a sphere in the block's path."""
+    objs = [("plane", ((0.5, 0.25, 0.5), (0.0, 1.0, 0.05)), dict(type=SLIP, friction=0.2)),
+            ("plane", ((0.22, 0.5, 0.5), (1.0, 0.0, 0.0)), dict(type=SEPARATE, friction=0.0)),
+            ("plane", ((0.62, 0.5, 0.5), (-1.0, 0.1, 0.0)), dict(type=SLIP, friction=0.0)),
+            ("plane", ((0.5, 0.5, 0.22), (0.0, 0.0, 1.0)), dict(type=STICKY)),
+            ("plane", ((0.5, 0.5, 0.62), (0.0, -0.05, -1.0)), dict(type=SEPARATE, friction=0.3))]
+    for i in range(10):
+        c = (0.27 + 0.033 * i, 0.3 + 0.011 * (i % 3), 0.27 + 0.031 * ((3 * i) % 10))
+        if i % 2:
+            objs.append(("sphere", (c, 0.017), dict(type=(SLIP, SEPARATE, STICKY)[i % 3], friction=0.3)))
+        else:
+            objs.append(("box", (tuple(x - 0.015 for x in c), tuple(x + 0.015 for x in c)), dict(type=(SLIP, SEPARATE, STICKY)[i % 3], friction=0.2)))
+    objs.append(("sphere", ((0.47, 0.33, 0.46), 0.03), dict(type=SLIP, friction=0.3, trans_vel=(0.2, 0.0, 0.0))))
+    return _falling((24, 20, 24), (36, 28, 36), objs, material=J_FLUID, v0=(0.2, -4.0, -0.1))
+
+
+OBJECT_CASES = {
+    "obj_floor_fc_sticky": _on_object_floor(FIXED_COROTATED, STICKY),
+    "obj_floor_fc_slip": _on_object_floor(FIXED_COROTATED, SLIP),
+    "obj_floor_fc_separate": _on_object_floor(FIXED_COROTATED, SEPARATE),
+    "obj_floor_fluid_slip": _on_object_floor(J_FLUID, SLIP),
+    "obj_floor_sand_sticky": dict(_on_object_floor(SAND, STICKY), max_near_branch=1.0),   # F = I at sub-step 0: the cone tip
+    "obj_floor_nacc_separate": _on_object_floor(NACC, SEPARATE),
+    # a tilted plane: a normal off every axis, passed without normalising it, and no lattice node within rounding of the plane
+    "obj_tilted_plane_slip": _falling((24, 22, 24), (36, 28, 36), [("raw_plane", ((0.5, 0.3037, 0.5), (0.31, 1.0, -0.23)), dict(type=SLIP, friction=0.3))]),
+    # frictionless SEPARATE on a sphere: normals in every direction
+    "obj_sphere_separate": _falling((26, 22, 26), (38, 28, 38), [("sphere", ((0.5, 0.25, 0.5), 0.09), dict(type=SEPARATE, friction=0.0))],
+                                    steps=(0, 10), v0=(0.0, -2.0, 0.0), dt=1e-4),
+    # a capped cylinder tilted by rot_mat, under a block wider than it: the material meets the cap and the side
+    "obj_cylinder_tilted": _falling((18, 23, 18), (46, 27, 46), [("cylinder", ((0.5, 0.26, 0.5), 0.1, 0.07), dict(type=SLIP, friction=0.3, rot=_rot(0.5, 0.3, 0.0), trans=(0.5, 0.26, 0.5)))],
+                                    steps=(10, 20)),
+    # static and lattice-aligned: faces at nodes 24 / 40 (x, z) and 16 / 24 (y), the centre at node (32, 20, 32); the nodes
+    # equidistant from two faces and the centre are exact ties (E = 0), which the lowest axis and the + sign win.  A small
+    # block rests at the centre, another falls onto the top face
+    "obj_lattice_box": _case(6, [model(FIXED_COROTATED, box(1.0 / 64, (30, 18, 30), (34, 22, 34)), (0.0, 0.0, 0.0), 1.0 / 64),
+                                 model(FIXED_COROTATED, box(1.0 / 64, (22, 25, 22), (42, 29, 42)), (0.0, -3.0, 0.0), 1.0 / 64)], [6, 12], dt=2e-4,
+                             objects=[("box", ((0.375, 0.25, 0.375), (0.625, 0.375, 0.625)), dict(type=SLIP, friction=0.0))]),
+    # static, centred on node (32, 16, 32), r = 8 dx, h = 12 dx: where d2 = 0 the nodes with |d1| = rho + 4 dx are exact cap / side
+    # ties (E = 0), which the side wins (h - |d1| < r - rho is false); a block falls onto the cap and round its rim
+    "obj_lattice_cylinder": _case(6, [model(FIXED_COROTATED, box(1.0 / 64, (22, 28, 22), (42, 32, 42)), (0.0, -3.0, 0.0), 1.0 / 64)], [0, 8], dt=2e-4,
+                                  objects=[("cylinder", ((0.5, 0.25, 0.5), 0.125, 0.1875), dict(type=SLIP, friction=0.0))]),
+    # the paddle with every motion at once through resting fluid: it sets the CFL-bound dt
+    "obj_paddle_combined": _case(6, [model(J_FLUID, box(1.0 / 64, (18, 18, 18), (34, 34, 34)), (0.0, 0.0, 0.0), 1.0 / 64)], [0, 14], dt=1e-3, cfl=0.05,
+                                 objects=[("box", ((0.36, 0.30, 0.37), (0.43, 0.50, 0.44)), dict(type=SLIP, friction=0.3, **PADDLE_MOTION))]),
+    # overlapping objects: the list order decides where they overlap
+    "obj_overlap": _falling((22, 24, 22), (42, 30, 42), [("sphere", ((0.5, 0.3, 0.5), 0.07), dict(type=STICKY, trans_vel=(0.1, 0.0, 0.0))),
+                                                         ("box", ((0.4, 0.2, 0.4), (0.6, 0.33, 0.58)), dict(type=SLIP, friction=0.3)),
+                                                         ("cylinder", ((0.45, 0.3, 0.52), 0.06, 0.08), dict(type=SEPARATE, friction=0.0, omega=(0.0, 0.7, 0.0)))]),
+    # the level-set collider and two objects (the COLLIDE forms of the objects kernels)
+    "obj_collider_plus_two": _falling((26, 22, 26), (38, 28, 38), [("box", (FLOOR_LO, (0.85, 0.2, 0.85)), dict(type=STICKY, trans_vel=(0.1, 0.0, 0.0))),
+                                                                  ("sphere", ((0.56, 0.3, 0.45), 0.05), dict(type=SEPARATE, friction=0.3))],
+                                      collider=dict(field=("sphere", (0.45, 0.25, 0.5), 0.09), type=SLIP, friction=0.3, trans_vel=(0.2, 0.0, 0.0))),
+    "obj_sixteen": _sixteen(),
+    # objects have no wall-band guard: a slip box through the floor band (cells y < 8) under a column standing in it, and at
+    # boundary 0 a sticky box over the top faces, where node 63 = 4G - 1 has mass
+    "obj_wall_band": dict(_floor(FIXED_COROTATED, [0, 10]), objects=[("box", ((0.1, -0.1, 0.1), (0.9, 0.2, 0.9)), dict(type=SLIP, friction=0.3, trans_vel=(0.2, 0.0, 0.0)))]),
+    "obj_top_boundary0": _case(6, [model(FIXED_COROTATED, box(1.0 / 64, (26, 57, 26), (34, 63, 34)), (0.2, 1.0, -0.1), 1.0 / 64)], [0, 2], boundary=0,
+                               gravity=0.0, objects=[("box", ((0.0, 0.95, 0.0), (1.0, 1.1, 1.0)), dict(type=STICKY))]),
+    # a moving floor at the frame end: fps = 390 makes sub-step 25 end the frame with new_dt = 0.64 dt
+    "obj_moving_floor_frame_end": dict(_floor(FIXED_COROTATED, [24, 25, 26]), fps=390,
+                                       objects=[("box", ((0.15, 0.05, 0.15), (0.85, 0.2, 0.85)), dict(type=SLIP, friction=0.3, trans_vel=(0.2, 0.05, 0.0)))]),
 }

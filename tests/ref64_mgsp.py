@@ -96,19 +96,20 @@ def _union_models(per_rank, n_models):
     return out
 
 
-def substep(cfg, ranks, dt, dt_default, time_left=np.inf, n_models=None, collider=None, t=0.0):
+def substep(cfg, ranks, dt, dt_default, time_left=np.inf, n_models=None, collider=None, t=0.0, objects=None):
     """The reference sub-step of all ranks: every rank's grid update and g2p2g on its own view (fresh copies filled), the
     next grid summed key-wise over the ranks (magnitudes and stress columns likewise), new_dt from the max over the ranks'
-    maxima.  ``collider`` = (col, sdf, grad) acts in every rank's grid update at the float32 time t (ref64.grid_update); the
+    maxima.  ``collider`` = (col, sdf, grad) and then ``objects`` act in every rank's grid update at the float32 time t
+    (ref64.grid_update); the
     engine's ranks agree on a max their next-max predictor computed at the end of the previous sub-step, at the time this
     grid update sees.  Returns a dict ref64.compare-like (keys, grid, mag, stress, models per scene model, new_dt) plus owners
     (contributing ranks per cell), pre_keys (every rank's key hashes before the sub-step), fresh_in (copies filled), and per
     rank its models' results (per_rank: [(scene model, result)]) and its P2G (partials: (keys, grid))."""
     views, fresh_in = _fill_fresh(ranks)
-    ups = [ref64.grid_update(cfg, r["keys"], v, dt, collider, t) for r, v in zip(ranks, views)]
+    ups = [ref64.grid_update(cfg, r["keys"], v, dt, collider, t, objects) for r, v in zip(ranks, views)]
     mx = max((u[2] for u in ups), default=0.0)
     new_dt = ref64.compute_dt(cfg, mx, dt_default, time_left)
-    infos = [u[3] if collider is not None else dict(near=None, mx_lo=u[2], mx_hi=u[2], mx_err=0.0) for u in ups]
+    infos = [u[3] if len(u) > 3 else dict(near=None, mx_lo=u[2], mx_hi=u[2], mx_err=0.0) for u in ups]
     mx_lo, mx_hi = max((i["mx_lo"] for i in infos), default=0.0), max((i["mx_hi"] for i in infos), default=0.0)
     mx_err = max((i["mx_err"] for i in infos), default=0.0)
     if n_models is None:

@@ -70,7 +70,7 @@ def _engine_state(sim, nm):
 
 def engine_collider_check(case, use_graph, label):
     sim = S.build_engine(case, use_graph=use_graph)
-    ccol = S.ref_collider(case)
+    ccol, objs = S.ref_collider(case), S.ref_objects(case)
     nm = len(case["models"])
     done, expect = 0, 0
     counts = new_counts()
@@ -81,7 +81,7 @@ def engine_collider_check(case, use_graph, label):
         keys, grid, before = _engine_state(sim, nm)
         t = sim.sim_time()
         r = ref64.substep(sim.cfg, ref_models(case, before), keys, grid, st.dt, case["dt"], S.engine_time_left(sim, case), ccol,
-                          np.float32(t) if ccol is not None else 0.0)
+                          np.float32(t) if ccol is not None or objs else 0.0, objects=objs)
         sim.step(1)
         done = k + 1
         assert sim.sim_time() == t + float(np.float32(st.dt)), f"{label}: sim_time {sim.sim_time()!r} after a sub-step of {st.dt!r} from {t!r}"
@@ -106,11 +106,9 @@ def test_engine_collider_substep_matches_ref64(cuda_lib, name, use_graph):
 
 # ---- MGSP -------------------------------------------------------------------------------------------------------------------
 def build_ranks_with_collider(case, parts, use_graph, max_blocks=6000):
-    """The ranks of test_gpu_mgsp_ref64.build_ranks with the case's collider set before initial_setup, so that the set-up's
-    next-max predictor (grid_max_kernel<true>) applies it."""
+    """The ranks of test_gpu_mgsp_ref64.build_ranks with the case's collider and objects set before initial_setup, so that the
+    set-up's next-max predictor (grid_max_kernel<true>, grid_max_objects_kernel) applies them."""
     from claymore_b200.simulator import GmpmSimulator
-    sdf, grad = S.collider_field(case)
-    p = S.collider_spec(case["collider"])
     sims = []
     for r, ps in enumerate(parts):
         sim = GmpmSimulator(dt=case["dt"], fps=case.get("fps", 0), config=S.config(case), max_blocks=max_blocks, use_graph=use_graph,
@@ -118,8 +116,13 @@ def build_ranks_with_collider(case, parts, use_graph, max_blocks=6000):
         for q in ps:
             mid = sim.init_model(q["material"], q["pos"], q["v0"])
             getattr(sim, S.SETTER[q["material"]])(q["rho"], q["vol"], *q["args"], model=mid)
-        sim.set_collider(sdf, grad, type=p["type"], friction=p["friction"], trans=p["trans"], trans_vel=p["trans_vel"], omega=p["omega"],
-                         rot=np.asarray(p["rot_mat"]).reshape(3, 3), scale=p["scale"], dsdt=p["dsdt"])
+        if case.get("collider"):
+            sdf, grad = S.collider_field(case)
+            p = S.collider_spec(case["collider"])
+            sim.set_collider(sdf, grad, type=p["type"], friction=p["friction"], trans=p["trans"], trans_vel=p["trans_vel"], omega=p["omega"],
+                             rot=np.asarray(p["rot_mat"]).reshape(3, 3), scale=p["scale"], dsdt=p["dsdt"])
+        if case.get("objects"):
+            sim.set_collision_objects(S.object_structs(case))
         sims.append(sim)
     ptrs = [s.mgsp_inbox() for s in sims]
     for s in sims:
@@ -138,7 +141,7 @@ def mgsp_collider_check(case, parts, use_graph, label):
     sub-step 0's dt is the set-up predictor's (grid_max_kernel<true> at t = 0), every later one the carry kernel's."""
     sims = build_ranks_with_collider(case, parts, use_graph)
     cfg = sims[0].cfg
-    ccol = S.ref_collider(case)
+    ccol, objs = S.ref_collider(case), S.ref_objects(case)
     nm = len(case["models"])
     for s in sims:
         assert s.stats().error == 0
@@ -157,7 +160,7 @@ def mgsp_collider_check(case, parts, use_graph, label):
         M.check_dts(dts, dts[0], 0)
         t = sims[0].sim_time()
         assert all(s.sim_time() == t for s in sims)
-        r = M.substep(cfg, ranks, dts[0], case["dt"], S.engine_time_left(sims[0], case), n_models=nm, collider=ccol, t=np.float32(t))
+        r = M.substep(cfg, ranks, dts[0], case["dt"], S.engine_time_left(sims[0], case), n_models=nm, collider=ccol, t=np.float32(t), objects=objs)
         on_threads(sims, lambda s: (s.step(1), s.sync()))
         done = k + 1
         for s in sims:

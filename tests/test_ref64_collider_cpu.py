@@ -110,10 +110,10 @@ def oracle_update(cob, ob, cfg, keys, grid, dt, col, t):
     return g, float(mv[0])
 
 
-def check_collider_update(cfg, keys, pre, post, mx_impl, dt, ccol, t, label):
-    """One implementation's collider grid update against ref64 -> (worst ratio, near nodes, resolved nodes, branches away)."""
-    col, sdf, grad = ccol
-    vel, vmag, mx, info = ref64.grid_update(cfg, keys, pre.astype(np.float64), dt, ccol, t)
+def check_collider_update(cfg, keys, pre, post, mx_impl, dt, ccol, t, label, objects=None):
+    """One implementation's collider grid update (``ccol`` = (col, sdf, grad) or None, then ``objects``) against ref64 ->
+    (worst ratio, near nodes, resolved nodes, branches away; with objects also each shape's branches, per list entry)."""
+    vel, vmag, mx, info = ref64.grid_update(cfg, keys, pre.astype(np.float64), dt, ccol, t, objects)
     post = np.asarray(post, np.float64)
     assert np.array_equal(post[:, 0], pre[:, 0]), f"{label}: the grid update changed the mass channel"
     has = pre[:, 0] >= ref64.FLT_MIN32
@@ -137,7 +137,11 @@ def check_collider_update(cfg, keys, pre, post, mx_impl, dt, ccol, t, label):
     hi = info["mx_hi"] * (1 + COLLIDER_MAX_REL * ref64.EPS32) + slack
     assert lo <= mx_impl <= hi, f"{label}: max |v|^2 {mx_impl!r} outside [{info['mx_lo']!r}, {info['mx_hi']!r}] (ref64 {mx!r}, slack {slack:.3g})"
     away = has & ~near
-    return float(ratio.max(initial=0.0)), int((near & has).sum()), int(has.sum()), set(info["branch"][away].tolist())
+    branches = set(info["branch"][away].tolist())
+    for st in info.get("stages", ()):
+        on = has & st["hit"] & ~st["near"]
+        branches |= set(st["branch"][on].tolist()) | set(st["shape_branch"][on].tolist())
+    return float(ratio.max(initial=0.0)), int((near & has).sum()), int(has.sum()), branches
 
 
 def kernel_matrix(run, ob, field, boundary, motion, label):
@@ -238,16 +242,17 @@ def new_counts():
 def oracle_collider_check(ob, case, label):
     osim = S.build_oracle(ob, case)
     clock = S.OracleClock(osim)
-    ccol = S.ref_collider(case)
+    ccol, objs = S.ref_collider(case), S.ref_objects(case)
     nm = len(case["models"])
     done = 0
     counts = new_counts()
     for k in case["steps"]:
         clock.step(k - done)
-        t = np.float32(osim.sim_time) if ccol is not None else 0.0
+        t = np.float32(osim.sim_time) if ccol is not None or objs else 0.0
         _, nbc, _ = osim.block_counts()
         before = [osim.particle_state(i) for i in range(nm)]
-        r = ref64.substep(osim.cfg, ref_models(case, before), osim.active_keys()[:nbc], osim.grid(), osim.dt, case["dt"], clock.time_left(), ccol, t)
+        r = ref64.substep(osim.cfg, ref_models(case, before), osim.active_keys()[:nbc], osim.grid(), osim.dt, case["dt"], clock.time_left(), ccol, t,
+                          objects=objs)
         clock.step(1)
         done = k + 1
         _, nbc, _ = osim.block_counts()
