@@ -119,8 +119,16 @@ int cb200_g2p2g(const cb200_config* c, float dt, float new_dt, int pbc, cb200_pa
 	return (int) launch_g2p2g(cur.material, a, pbc, (cudaStream_t) stream);
 }
 
-int cb200_update_grid_velocity_query_max(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, float* max_vel, void* stream) {
+// The three kernel-level grid updates: the level set when collider is non-null (valid, with a field), then objs[0, n), placed at time
+static int update_grid_boundaries(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream) {
 	CB_CFG(c);
+	Boundaries bd {};
+	if(!objects_prepare(objs, n, bd.objects)) return (int) cudaErrorInvalidValue;
+	if(collider) {
+		if(!collider_valid(collider) || !collider->sdf) return (int) cudaErrorInvalidValue;
+		bd.has_collider = true;
+		bd.col = *collider;
+	}
 	if(block_count <= 0) return 0;
 	GridUpdateArgs a {};
 	a.cfg = cfg;
@@ -133,58 +141,22 @@ int cb200_update_grid_velocity_query_max(const cb200_config* c, int block_count,
 	a.max_vel = max_vel;
 	a.clear_grid = nullptr;
 	a.n_clear = 0;
-	grid_update_kernel<false><<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a);
+	a.time = time;
+	launch_grid_update(a, bd, grid_for(block_count, kGridThreads / 32), (cudaStream_t) stream);
 	return (int) cudaGetLastError();
+}
+
+int cb200_update_grid_velocity_query_max(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, float* max_vel, void* stream) {
+	return update_grid_boundaries(c, block_count, grid, partition, dt, nullptr, nullptr, 0, 0.f, max_vel, stream);
 }
 
 int cb200_update_grid_velocity_query_max_collider(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, float time, float* max_vel, void* stream) {
-	CB_CFG(c);
-	if(!collider_valid(collider) || !collider->sdf) return (int) cudaErrorInvalidValue;
-	if(block_count <= 0) return 0;
-	GridUpdateArgs a {};
-	a.cfg = cfg;
-	a.state = nullptr;
-	a.nbc = block_count;
-	a.ebc = 0;
-	a.dt = dt;
-	a.grid = grid;
-	a.keys = partition.active_keys;
-	a.max_vel = max_vel;
-	a.clear_grid = nullptr;
-	a.n_clear = 0;
-	a.col = *collider;
-	a.time = time;
-	grid_update_kernel<true><<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a);
-	return (int) cudaGetLastError();
+	if(!collider) return (int) cudaErrorInvalidValue;
+	return update_grid_boundaries(c, block_count, grid, partition, dt, collider, nullptr, 0, time, max_vel, stream);
 }
 
 int cb200_update_grid_velocity_query_max_objects(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream) {
-	CB_CFG(c);
-	ObjectList l;
-	if(!objects_prepare(objs, n, l)) return (int) cudaErrorInvalidValue;
-	if(n == 0) return collider ? cb200_update_grid_velocity_query_max_collider(c, block_count, grid, partition, dt, collider, time, max_vel, stream)
-	                           : cb200_update_grid_velocity_query_max(c, block_count, grid, partition, dt, max_vel, stream);
-	if(collider && (!collider_valid(collider) || !collider->sdf)) return (int) cudaErrorInvalidValue;
-	if(block_count <= 0) return 0;
-	GridUpdateArgs a {};
-	a.cfg = cfg;
-	a.state = nullptr;
-	a.nbc = block_count;
-	a.ebc = 0;
-	a.dt = dt;
-	a.grid = grid;
-	a.keys = partition.active_keys;
-	a.max_vel = max_vel;
-	a.clear_grid = nullptr;
-	a.n_clear = 0;
-	a.time = time;
-	if(collider) {
-		a.col = *collider;
-		grid_update_objects_kernel<true><<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a, l);
-	} else {
-		grid_update_objects_kernel<false><<<grid_for(block_count, kGridThreads / 32), kGridThreads, 0, (cudaStream_t) stream>>>(a, l);
-	}
-	return (int) cudaGetLastError();
+	return update_grid_boundaries(c, block_count, grid, partition, dt, collider, objs, n, time, max_vel, stream);
 }
 
 int cb200_clear_grid(int block_count, float* grid, void* stream) {

@@ -2,8 +2,8 @@
 //
 // The level set is dense over the whole domain in the reference's layout (signed_distance_field_, boundary_condition.cuh:15-16):
 // one 1 KiB block per grid block, blocks row-major (x*G*G + y*G + z), inside a block 4 channels SoA (distance, gradient x, y, z)
-// of 64 cells (cell = x*16 + y*4 + z).  Every caller (the grid update and the two next-max predictors of grid.cuh) shares
-// collider_resolve, so the max the MGSP ranks agree on is the max the next grid update finds.
+// of 64 cells (cell = x*16 + y*4 + z).  Every caller (the grid update and the two next-max predictors of grid.cuh) applies the
+// same boundary chain (boundaries_resolve), so the max the MGSP ranks agree on is the max the next grid update finds.
 #pragma once
 #include "common.cuh"
 
@@ -71,14 +71,6 @@ __device__ __forceinline__ void collider_make_frame(const P& c, float t, Collide
 	f.s_inv = 1.f / (1.f + c.dsdt * t);
 }
 
-// one thread builds the frame, the CTA reads it from shared memory
-__device__ __forceinline__ const ColliderFrame& collider_frame_cta(const ColliderView& c, float t) {
-	__shared__ ColliderFrame s_frame;
-	if(threadIdx.x == 0) collider_make_frame(c, t, s_frame);
-	__syncthreads();
-	return s_frame;
-}
-
 // get_signed_distance_and_normal + query_sdf (:98-143) at the material-space point x.  The wall band reports no hit (kept); the
 // normal is normalised only when it is non-zero (the reference divides 0 by 0); the +1 node must lie in the domain (the reference
 // always has a wall band there).  Reads go through the read-only path at addresses computed from the node's block key.
@@ -122,73 +114,29 @@ __device__ __forceinline__ bool collider_query(const ColliderView& c, const Cfg&
 	return sd <= 0.f;
 }
 
-// detect_and_resolve_collision (:159-249) of the velocity v at grid node (nx, ny, nz).  The object velocity takes a true
-// omega x r where the reference's vec3_cross_vec3 (:92-95) adds all products; get_material_velocity keeps MnBase's
-// vec_cross_mul_vec_3d as it is (MatrixUtils.h:54-58).
-__device__ __forceinline__ void collider_resolve(const ColliderView& c, const ColliderFrame& f, const Cfg& cfg, int nx, int ny, int nz, float& vx, float& vy, float& vz) {
-	const float xm[3] = {(float) nx * cfg.dx - f.b[0], (float) ny * cfg.dx - f.b[1], (float) nz * cfg.dx - f.b[2]};
+// the point p's image in the material space of an object placed by f (P: its parameters): x = R^T ((p - b) s_inv) scale + trans;
+// xm = p - b, the offset the object velocity is taken at
+template<class P>
+__device__ __forceinline__ void collider_material_point(const P& c, const ColliderFrame& f, const float* p, float* xm, float* x) {
+#pragma unroll
+	for(int d = 0; d < 3; ++d) xm[d] = p[d] - f.b[d];
 	const float x0[3] = {xm[0] * f.s_inv, xm[1] * f.s_inv, xm[2] * f.s_inv};
 	const float* R = f.rot;
-	float x[3];
 #pragma unroll
 	for(int d = 0; d < 3; ++d) x[d] = (R[3 * d] * x0[0] + R[3 * d + 1] * x0[1] + R[3 * d + 2] * x0[2]) * c.scale + c.trans[d];  // mat_t_mul_vec_3d
-	float on[3];
-	if(!collider_query(c, cfg, x, on)) return;
-	const float* w = c.omega;
-	float vo[3] = {w[1] * xm[2] - w[2] * xm[1], w[2] * xm[0] - w[0] * xm[2], w[0] * xm[1] - w[1] * xm[0]};
-	const float ds = c.dsdt / c.scale;
-#pragma unroll
-	for(int d = 0; d < 3; ++d) vo[d] += xm[d] * ds;
-	{
-		const float r[3] = {x[0] - c.trans[0], x[1] - c.trans[1], x[2] - c.trans[2]};
-		const float mv[3] = {w[1] * r[2] + w[2] * r[1] + c.trans_vel[0], w[2] * r[0] + w[0] * r[2] + c.trans_vel[1], w[0] * r[1] + w[1] * r[0] + c.trans_vel[2]};
-#pragma unroll
-		for(int d = 0; d < 3; ++d) vo[d] += (R[d] * mv[0] + R[3 + d] * mv[1] + R[6 + d] * mv[2]) * c.scale + c.trans_vel[d];  // matrix_vector_multiplication_3d
-	}
-	float v[3] = {vx - vo[0], vy - vo[1], vz - vo[2]};
-	if(c.type == CB200_STICKY) {
-		v[0] = v[1] = v[2] = 0.f;
-	} else {
-		if(c.type == CB200_SEPARATE && on[0] == 0.f && on[1] == 0.f && on[2] == 0.f) {
-			vx = vy = vz = 0.f;  // :222-225 returns before the object velocity is added back
-			return;
-		}
-		float n[3];
-#pragma unroll
-		for(int d = 0; d < 3; ++d) n[d] = R[d] * on[0] + R[3 + d] * on[1] + R[6 + d] * on[2];
-		const float vn = n[0] * v[0] + n[1] * v[1] + n[2] * v[2];
-		const bool slip = c.type == CB200_SLIP;
-		if(slip || vn < 0.f) {
-#pragma unroll
-			for(int d = 0; d < 3; ++d) v[d] -= n[d] * vn;
-			if((slip ? c.friction > 0.f : c.friction != 0.f) && vn < 0.f) {
-				const float len = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
-				if(-vn * c.friction < len) {
-					const float fr = vn * c.friction;
-#pragma unroll
-					for(int d = 0; d < 3; ++d) v[d] += v[d] / len * fr;
-				} else {
-					v[0] = v[1] = v[2] = 0.f;
-				}
-			}
-		}
-	}
-	vx = v[0] + vo[0];
-	vy = v[1] + vo[1];
-	vz = v[2] + vo[2];
 }
 
-// collider_resolve over any query (P: a struct with the collider's motion, type and friction fields): query(x, n) tests the
-// material-space point x and writes the material-space normal n (0 where it has none).  The analytic objects use it; the
-// level-set path keeps collider_resolve above as it is, whose instructions this form, inlined there, would reorder.
+// detect_and_resolve_collision (:159-249) of the velocity v at grid node (nx, ny, nz) against the object with parameters c (P: a
+// struct with the collider's motion, type and friction fields) placed by f.  query(x, n) tests the material-space point x and
+// writes the material-space normal n (0 where it has none): collider_query for the level set, object_query for an analytic shape.
+// The object velocity takes a true omega x r where the reference's vec3_cross_vec3 (:92-95) adds all products;
+// get_material_velocity keeps MnBase's vec_cross_mul_vec_3d as it is (MatrixUtils.h:54-58).
 template<class P, class Q>
-__device__ __forceinline__ void collider_resolve_query(const P& c, const ColliderFrame& f, float dx, int nx, int ny, int nz, float& vx, float& vy, float& vz, Q&& query) {
-	const float xm[3] = {(float) nx * dx - f.b[0], (float) ny * dx - f.b[1], (float) nz * dx - f.b[2]};
-	const float x0[3] = {xm[0] * f.s_inv, xm[1] * f.s_inv, xm[2] * f.s_inv};
+__device__ __forceinline__ void collider_resolve(const P& c, const ColliderFrame& f, float dx, int nx, int ny, int nz, float& vx, float& vy, float& vz, Q&& query) {
+	const float p[3] = {(float) nx * dx, (float) ny * dx, (float) nz * dx};
+	float xm[3], x[3];
+	collider_material_point(c, f, p, xm, x);
 	const float* R = f.rot;
-	float x[3];
-#pragma unroll
-	for(int d = 0; d < 3; ++d) x[d] = (R[3 * d] * x0[0] + R[3 * d + 1] * x0[1] + R[3 * d + 2] * x0[2]) * c.scale + c.trans[d];  // mat_t_mul_vec_3d
 	float on[3];
 	if(!query(x, on)) return;
 	const float* w = c.omega;
@@ -234,8 +182,8 @@ __device__ __forceinline__ void collider_resolve_query(const P& c, const Collide
 	vy = v[1] + vo[1];
 	vz = v[2] + vo[2];
 }
+
 // ---- analytic collision objects (DESIGN.md section 2.9) ----------------------------------------------------------------------
-// Passed by value as a kernel parameter beside the argument struct, so the kernels without objects keep their parameter block.
 struct ObjectList {
 	int n;
 	cb200_collision_object o[CB200_MAX_COLLISION_OBJECTS];
@@ -330,68 +278,73 @@ __device__ __forceinline__ bool object_query(const cb200_collision_object& o, co
 	return true;
 }
 
-// the per-CTA state of the objects kernels: the level-set collider's frame (COLLIDE), and each object's parameters and frame
-struct ObjectFrames {
+// ---- the boundary chain -------------------------------------------------------------------------------------------------------
+// The solid boundaries of a simulator, applied in this order: the level-set collider (has_collider), then the analytic objects in
+// list order, each resolving the velocity the previous one left.  Passed by value as a kernel parameter of its own beside the argument
+// struct, so the plain kernels keep their parameter block; which of the two parts a kernel compiles in is its COLLIDE / OBJECTS flags.
+struct Boundaries {
+	bool has_collider;
+	ColliderView col;
+	ObjectList objects;  // n = 0: none
+};
+
+// the per-CTA state of the chain: the level-set collider's frame (COLLIDE), and each object's parameters and frame (OBJECTS)
+struct BoundaryFrames {
 	ColliderFrame col;
 	ColliderFrame f[CB200_MAX_COLLISION_OBJECTS];
 	cb200_collision_object o[CB200_MAX_COLLISION_OBJECTS];
 };
-// thread 0 builds the collider's frame, thread 32 + i object i's (another warp, so that the two run side by side); one barrier
-template<bool COLLIDE>
-__device__ __forceinline__ const ObjectFrames& object_frames_cta(const ColliderView& c, const ObjectList& l, float t) {
-	__shared__ ObjectFrames s;
+__device__ __forceinline__ BoundaryFrames& boundary_frames() {
+	__shared__ BoundaryFrames s;
+	return s;
+}
+// thread 0 builds the collider's frame at time t and thread i object i's, from thread 32 on with the collider (another warp, so that
+// the two run side by side); one barrier
+template<bool COLLIDE, bool OBJECTS>
+__device__ __forceinline__ const BoundaryFrames& boundary_frames_cta(const Boundaries& b, float t) {
+	BoundaryFrames& s = boundary_frames();
 	if constexpr(COLLIDE) {
-		if(threadIdx.x == 0) collider_make_frame(c, t, s.col);
+		if(threadIdx.x == 0) collider_make_frame(b.col, t, s.col);
 	}
-	const int i = (int) threadIdx.x - 32;
-	if(i >= 0 && i < l.n) {
-		s.o[i] = l.o[i];
-		collider_make_frame(s.o[i], t, s.f[i]);
+	if constexpr(OBJECTS) {
+		const int i = (int) threadIdx.x - (COLLIDE ? 32 : 0);
+		if(i >= 0 && i < b.objects.n) {
+			s.o[i] = b.objects.o[i];
+			collider_make_frame(s.o[i], t, s.f[i]);
+		}
 	}
 	__syncthreads();
 	return s;
 }
-// the level-set collider (COLLIDE), then the n objects in list order, each resolving the velocity the previous one left
-template<bool COLLIDE>
-__device__ __forceinline__ void objects_resolve(const ColliderView& c, const ObjectFrames& s, int n, const Cfg& cfg, int nx, int ny, int nz, float& vx, float& vy, float& vz) {
-	if constexpr(COLLIDE) collider_resolve(c, s.col, cfg, nx, ny, nz, vx, vy, vz);
-	for(int i = 0; i < n; ++i) {
-		const cb200_collision_object& o = s.o[i];
-		collider_resolve_query(o, s.f[i], cfg.dx, nx, ny, nz, vx, vy, vz, [&](const float* x, float* nn) { return object_query(o, x, nn); });
+// the chain at grid node (nx, ny, nz), its frames s built by boundary_frames_cta
+template<bool COLLIDE, bool OBJECTS>
+__device__ __forceinline__ void boundaries_resolve(const Boundaries& b, const BoundaryFrames& s, const Cfg& cfg, int nx, int ny, int nz, float& vx, float& vy, float& vz) {
+	if constexpr(COLLIDE) collider_resolve(b.col, s.col, cfg.dx, nx, ny, nz, vx, vy, vz, [&](const float* x, float* n) { return collider_query(b.col, cfg, x, n); });
+	if constexpr(OBJECTS) {
+		for(int i = 0; i < b.objects.n; ++i) {
+			const cb200_collision_object& o = s.o[i];
+			collider_resolve(o, s.f[i], cfg.dx, nx, ny, nz, vx, vy, vz, [&](const float* x, float* n) { return object_query(o, x, n); });
+		}
 	}
 }
 
-// grid-update velocity of one cell (wall mask, gravity on y, collider) and its |v|^2, NaN -> +inf; no mass -> 0
-__device__ __forceinline__ float cell_vel_sq_collide(float m, float p0, float p1, float p2, bool wx, bool wy, bool wz, float gdt, const ColliderView& c, const ColliderFrame& f, const Cfg& cfg, int nx, int ny, int nz) {
+// grid-update velocity of one cell (wall mask, gravity on y, the chain) and its |v|^2, NaN -> +inf; no mass -> 0
+template<bool COLLIDE, bool OBJECTS>
+__device__ __forceinline__ float cell_vel_sq_boundaries(float m, float p0, float p1, float p2, bool wx, bool wy, bool wz, float gdt, const Boundaries& bd, const BoundaryFrames& s, const Cfg& cfg, int nx, int ny, int nz) {
 	if(!node_has_mass(m)) return 0.f;
 	const float mi = 1.f / m;
 	float a = wx ? 0.f : p0 * mi, b = (wy ? 0.f : p1 * mi) + gdt, d = wz ? 0.f : p2 * mi;
-	collider_resolve(c, f, cfg, nx, ny, nz, a, b, d);
+	boundaries_resolve<COLLIDE, OBJECTS>(bd, s, cfg, nx, ny, nz, a, b, d);
 	const float sq = a * a + b * b + d * d;
 	return isnan(sq) ? INFINITY : sq;
 }
-// cell_pair_vel_sq (common.cuh) with the collider: the two cells lane holds of block (kx, ky, kz), whose grid block is s2 (float2 view)
-__device__ __forceinline__ float cell_pair_vel_sq_collide(const Cfg& cfg, const ColliderView& c, const ColliderFrame& f, const float2* s2, int lane, int kx, int ky, int kz, bool wx, bool wy, bool wz, float gdt) {
+// cell_pair_vel_sq (common.cuh) with the chain: the two cells lane holds of block (kx, ky, kz), whose grid block is s2 (float2 view)
+template<bool COLLIDE, bool OBJECTS>
+__device__ __forceinline__ float cell_pair_vel_sq_boundaries(const Cfg& cfg, const Boundaries& bd, const BoundaryFrames& s, const float2* s2, int lane, int kx, int ky, int kz, bool wx, bool wy, bool wz, float gdt) {
 	const float2 m = s2[lane], p0 = s2[32 + lane], p1 = s2[64 + lane], p2 = s2[96 + lane];
 	const int nx = 4 * kx + (lane >> 3), ny = 4 * ky + ((lane >> 1) & 3), nz = 4 * kz + 2 * (lane & 1);
-	return fmaxf(cell_vel_sq_collide(m.x, p0.x, p1.x, p2.x, wx, wy, wz, gdt, c, f, cfg, nx, ny, nz), cell_vel_sq_collide(m.y, p0.y, p1.y, p2.y, wx, wy, wz, gdt, c, f, cfg, nx, ny, nz + 1));
-}
-// the same two functions with the collider (COLLIDE) and then the n objects of s
-template<bool COLLIDE>
-__device__ __forceinline__ float cell_vel_sq_objects(float m, float p0, float p1, float p2, bool wx, bool wy, bool wz, float gdt, const ColliderView& c, const ObjectFrames& s, int n, const Cfg& cfg, int nx, int ny, int nz) {
-	if(!node_has_mass(m)) return 0.f;
-	const float mi = 1.f / m;
-	float a = wx ? 0.f : p0 * mi, b = (wy ? 0.f : p1 * mi) + gdt, d = wz ? 0.f : p2 * mi;
-	objects_resolve<COLLIDE>(c, s, n, cfg, nx, ny, nz, a, b, d);
-	const float sq = a * a + b * b + d * d;
-	return isnan(sq) ? INFINITY : sq;
-}
-template<bool COLLIDE>
-__device__ __forceinline__ float cell_pair_vel_sq_objects(const Cfg& cfg, const ColliderView& c, const ObjectFrames& s, int n, const float2* s2, int lane, int kx, int ky, int kz, bool wx, bool wy, bool wz, float gdt) {
-	const float2 m = s2[lane], p0 = s2[32 + lane], p1 = s2[64 + lane], p2 = s2[96 + lane];
-	const int nx = 4 * kx + (lane >> 3), ny = 4 * ky + ((lane >> 1) & 3), nz = 4 * kz + 2 * (lane & 1);
-	return fmaxf(cell_vel_sq_objects<COLLIDE>(m.x, p0.x, p1.x, p2.x, wx, wy, wz, gdt, c, s, n, cfg, nx, ny, nz),
-	             cell_vel_sq_objects<COLLIDE>(m.y, p0.y, p1.y, p2.y, wx, wy, wz, gdt, c, s, n, cfg, nx, ny, nz + 1));
+	return fmaxf(cell_vel_sq_boundaries<COLLIDE, OBJECTS>(m.x, p0.x, p1.x, p2.x, wx, wy, wz, gdt, bd, s, cfg, nx, ny, nz),
+	             cell_vel_sq_boundaries<COLLIDE, OBJECTS>(m.y, p0.y, p1.y, p2.y, wx, wy, wz, gdt, bd, s, cfg, nx, ny, nz + 1));
 }
 
 }  // namespace cb200

@@ -375,12 +375,10 @@ struct cb200_sim {
 	bool poll_pending = false;
 	int steps_since_poll = 15;  // the first sub-step polls
 	int grow_events = 0;
-	// signed-distance collider (cb200_sim_set_collider): parameters, and the device field this simulator owns
-	bool has_collider = false;
-	ColliderView collider {};
+	// the signed-distance collider (cb200_sim_set_collider), whose device field this simulator owns (sdf), and the analytic collision
+	// objects (cb200_sim_set_collision_objects) resolved after it in list order
+	Boundaries boundaries {};
 	float* sdf = nullptr;
-	// analytic collision objects (cb200_sim_set_collision_objects), resolved after the collider in list order; n = 0: none
-	ObjectList objects {};
 	long long frames_done = 0;  // frames finished by cb200_sim_advance_frame (restored from a checkpoint)
 	// the rows each particle block starts at in every read-out, per model: the scans of the bucket sizes, [kMaxModels][max_blocks + 1]
 	int* ck_base = nullptr;
@@ -601,15 +599,7 @@ int enqueue_grid_update(cb200_sim* s, int R) {
 	}
 	gu.n_clear = (int) s->models.size();
 	for(size_t m = 0; m < s->models.size(); ++m) gu.clear_counts[m] = s->models[m].pb[Rn].cell_particle_counts;
-	if(s->has_collider) gu.col = s->collider;  // placed at StepState::sim_time, the start of this sub-step, as are the objects
-	if(s->objects.n > 0) {
-		if(s->has_collider) grid_update_objects_kernel<true><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu, s->objects);
-		else grid_update_objects_kernel<false><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu, s->objects);
-	} else if(s->has_collider) {
-		grid_update_kernel<true><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu);
-	} else {
-		grid_update_kernel<false><<<grid_blocks(4), kGridThreads, 0, s->stream>>>(gu);
-	}
+	launch_grid_update(gu, s->boundaries, grid_blocks(4), s->stream);  // placed at StepState::sim_time, the start of this sub-step
 	++s->launches;
 	return (int) cudaGetLastError();
 }
@@ -731,15 +721,8 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 		a.old_grid = s->grid[1];
 		a.new_grid = s->grid[0];
 		a.next_max_vel = mgsp ? &scr->local_max : nullptr;
-		if(mgsp && s->has_collider) a.col = s->collider;  // the predicted max must be the one the next grid update finds
-		if(mgsp && s->objects.n > 0) {
-			if(s->has_collider) carry_grid_objects_kernel<true><<<grid_blocks(4), 256, 0, st>>>(a, s->objects);
-			else carry_grid_objects_kernel<false><<<grid_blocks(4), 256, 0, st>>>(a, s->objects);
-		} else if(mgsp && s->has_collider) {
-			carry_grid_kernel<true><<<grid_blocks(4), 256, 0, st>>>(a);
-		} else {
-			carry_grid_kernel<false><<<grid_blocks(4), 256, 0, st>>>(a);
-		}
+		// MGSP: the boundaries, so that the predicted max is the one the next grid update finds; a single domain predicts nothing
+		launch_carry_grid(a, mgsp ? s->boundaries : Boundaries {}, grid_blocks(4), st);
 		++s->launches;
 	}
 	if(mgsp) {
@@ -860,15 +843,15 @@ void preload_kernels() {
 	preload(g2p2g_kernel<CB200_FIXED_COROTATED, true>);
 	preload(g2p2g_kernel<CB200_SAND, true>);
 	preload(g2p2g_kernel<CB200_NACC, true>);
-	preload(grid_update_kernel<false>);
-	preload(grid_update_kernel<true>);
+	preload(grid_update_kernel);
 	preload(clear_grid_kernel);
-	preload(carry_grid_kernel<false>);
-	preload(carry_grid_kernel<true>);
-	preload(grid_update_objects_kernel<false>);
-	preload(grid_update_objects_kernel<true>);
-	preload(carry_grid_objects_kernel<false>);
-	preload(carry_grid_objects_kernel<true>);
+	preload(carry_grid_kernel);
+	preload(grid_max_kernel);
+	for_each_boundary_instance([](auto C, auto O) {
+		preload(grid_update_boundary_kernel<C, O>);
+		preload(carry_grid_boundary_kernel<C, O>);
+		preload(grid_max_boundary_kernel<C, O>);
+	});
 	preload(scan_kernel);
 	preload(summary_kernel);
 	preload(rebuild_kernel);
@@ -890,10 +873,6 @@ void preload_kernels() {
 	preload(mgsp_done_publish_kernel);
 	preload(mgsp_done_wait_kernel);
 	preload(mgsp_clear_publish_kernel);
-	preload(grid_max_kernel<false>);
-	preload(grid_max_kernel<true>);
-	preload(grid_max_objects_kernel<false>);
-	preload(grid_max_objects_kernel<true>);
 	preload(snapshot_kernel);
 	preload(state_positions_kernel);
 	preload(scatter_grid_kernel);
@@ -1326,11 +1305,7 @@ static int setup_impl(cb200_sim* s, const StartSrc& src) {
 	CK(push_state(s));
 	if(mgsp) {
 		// global max |v|^2 of the start grid (later sub-steps get it from the end-of-step exchange of the previous one)
-		const ColliderView col = s->has_collider ? s->collider : ColliderView {};
-		if(s->objects.n > 0 && s->has_collider) grid_max_objects_kernel<true><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, col, s->objects);
-		else if(s->objects.n > 0) grid_max_objects_kernel<false><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, col, s->objects);
-		else if(s->has_collider) grid_max_kernel<true><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->collider);
-		else grid_max_kernel<false><<<grid_blocks(2), 256, 0, st>>>(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, ColliderView {});
+		launch_grid_max(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->boundaries, grid_blocks(2), st);
 		mgsp_allreduce_maxvel_kernel<<<1, 32, 0, st>>>(mgsp_view(s), &s->d_state->max_vel_sq);
 		s->launches += 2;
 	}
@@ -1500,16 +1475,16 @@ int cb200_sim_set_collider(cb200_sim* s, const cb200_collider* params, const flo
 		CK(cudaMemcpyAsync(s->sdf, f.data(), f.size() * sizeof(float), cudaMemcpyHostToDevice, s->stream));
 		CK(cudaStreamSynchronize(s->stream));
 	}
-	s->collider = *params;
-	s->collider.sdf = s->sdf;
-	s->has_collider = true;
+	s->boundaries.col = *params;
+	s->boundaries.col.sdf = s->sdf;
+	s->boundaries.has_collider = true;
 	return recapture(s);
 }
 int cb200_sim_clear_collider(cb200_sim* s) {
 	if(!s) return (int) cudaErrorInvalidValue;
 	CK(cudaStreamSynchronize(s->stream));
-	s->has_collider = false;
-	s->collider = ColliderView {};
+	s->boundaries.has_collider = false;
+	s->boundaries.col = ColliderView {};
 	g_pool.release(s->sdf);
 	s->sdf = nullptr;
 	return recapture(s);
@@ -1518,7 +1493,7 @@ int cb200_sim_set_collision_objects(cb200_sim* s, const cb200_collision_object* 
 	ObjectList l;
 	if(!s || !objects_prepare(objs, n, l)) return (int) cudaErrorInvalidValue;
 	CK(cudaStreamSynchronize(s->stream));
-	s->objects = l;
+	s->boundaries.objects = l;
 	return recapture(s);
 }
 int cb200_sim_time(cb200_sim* s, double* time) {
@@ -2276,7 +2251,7 @@ int cb200_sim_remove_particles(cb200_sim* s, unsigned model_mask, const cb200_co
 	CK(remove_precheck(s, removed));
 	RemoveRegions sel {};
 	const int nm = (int) s->models.size();
-	if(!model_mask || (model_mask >> nm) || (flags & ~CB200_REMOVE_OUTSIDE) || !objects_prepare(regions, n, sel.l)) return (int) cudaErrorInvalidValue;
+	if(!model_mask || (model_mask >> nm) || (flags & ~CB200_REMOVE_OUTSIDE) || !objects_prepare(regions, n, sel.b.objects)) return (int) cudaErrorInvalidValue;
 	if(n == 0) return 0;
 	CK(cudaStreamSynchronize(s->stream));
 	CK(pull_state(s));

@@ -19,24 +19,26 @@ struct GridUpdateArgs {
 	float* clear_grid;       // nullable: next grid, nbc blocks zeroed        (clear_grid, mgmpm_kernels.cuh:106-115)
 	int n_clear;             // number of cell-count arrays to zero over ebc blocks (cudaMemsetAsync at gmpm_simulator.cuh:389)
 	int* clear_counts[kMaxModels];
-	ColliderView col;        // COLLIDE only
-	float time;              // COLLIDE, state == nullptr: time the collider is placed at (the driver reads StepState::sim_time)
+	float time;              // boundary kernels, state == nullptr: time the boundaries are placed at (the driver reads StepState::sim_time)
 };
+
+// CTAs per SM a boundary instance is compiled for: the level-set-only one fits the driver's 4 at 256 threads (64 registers); the ones
+// with objects take 2, without which ptxas picks 64 registers and spills
+template<bool COLLIDE, bool OBJECTS>
+constexpr int kBoundaryMinCtas = OBJECTS ? 2 : 4;
 
 // update_grid_velocity_query_max (mgmpm_kernels.cuh:325-420): one warp per grid block, two cells per lane as
 // one 8-byte access per channel; warp max by redux, one atomicMax per CTA on the float's bit pattern.
 // Quirks kept: wall blocks zero the masked component BEFORE gravity is added to y (Appendix B #1);
 // NaN -> +inf (B #3).
-// COLLIDE: the MGSP form with a SignedDistanceGrid (mgmpm_kernels.cuh:323-399): after gravity, cells with mass resolve against
-// the collider (collider.cuh); the max is |v|^2 where that kernel reports 2|v|^2 (Appendix B #11).
-// OBJECTS: then the analytic objects of `objs` in list order (collider.cuh, DESIGN.md section 2.9), placed at the collider's time.
+// COLLIDE / OBJECTS: the MGSP form with a Boundary (mgmpm_kernels.cuh:323-399): after gravity, cells with mass resolve against the
+// boundary chain of `bd` (collider.cuh: the SignedDistanceGrid, then the analytic objects of DESIGN.md section 2.9); the max is |v|^2
+// where that kernel reports 2|v|^2 (Appendix B #11).
 template<bool COLLIDE, bool OBJECTS>
-__device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const ObjectList* objs) {
+__device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const Boundaries* bd) {
 	__shared__ unsigned s_max[kGridThreads / 32];
-	const ColliderFrame* fr = nullptr;
-	const ObjectFrames* of = nullptr;
-	if constexpr(OBJECTS) of = &object_frames_cta<COLLIDE>(a.col, *objs, a.state ? (float) a.state->sim_time : a.time);
-	else if constexpr(COLLIDE) fr = &collider_frame_cta(a.col, a.state ? (float) a.state->sim_time : a.time);
+	const BoundaryFrames* fr = nullptr;
+	if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, a.state ? (float) a.state->sim_time : a.time);
 	const Cfg& cfg = a.cfg;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int nbc = a.state ? a.state->nbc : a.nbc;
@@ -60,8 +62,7 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 				v0.x = wx ? 0.f : v0.x * mi;
 				v1.x = (wy ? 0.f : v1.x * mi) + gdt;
 				v2.x = wz ? 0.f : v2.x * mi;
-				if constexpr(OBJECTS) objects_resolve<COLLIDE>(a.col, *of, objs->n, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
-				else if constexpr(COLLIDE) collider_resolve(a.col, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
+				if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
 				sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
 			}
 			if(hy) {
@@ -69,8 +70,7 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 				v0.y = wx ? 0.f : v0.y * mi;
 				v1.y = (wy ? 0.f : v1.y * mi) + gdt;
 				v2.y = wz ? 0.f : v2.y * mi;
-				if constexpr(OBJECTS) objects_resolve<COLLIDE>(a.col, *of, objs->n, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
-				else if constexpr(COLLIDE) collider_resolve(a.col, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
+				if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
 				sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
 			}
 			if(hx || hy) {
@@ -101,12 +101,13 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 		if(m) atomicMax(reinterpret_cast<unsigned*>(a.max_vel), m);
 	}
 }
-template<bool COLLIDE>
-__global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpdateArgs a) { grid_update_body<COLLIDE, false>(a, nullptr); }
-// the same with analytic objects (objs.n >= 1): the list is a parameter of its own, so the kernels above keep their parameter block
-template<bool COLLIDE>
-__global__ void __launch_bounds__(kGridThreads, 2) grid_update_objects_kernel(const GridUpdateArgs a, const __grid_constant__ ObjectList objs) { grid_update_body<COLLIDE, true>(a, &objs); }
-static_assert(sizeof(GridUpdateArgs) + sizeof(ObjectList) <= 4096, "the objects grid update's parameters must fit the 4 KiB kernel-parameter limit");
+__global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpdateArgs a) { grid_update_body<false, false>(a, nullptr); }
+// the same with the boundaries of bd (COLLIDE: bd.has_collider; OBJECTS: bd.objects.n >= 1)
+template<bool COLLIDE, bool OBJECTS>
+__global__ void __launch_bounds__(kGridThreads, (kBoundaryMinCtas<COLLIDE, OBJECTS>)) grid_update_boundary_kernel(const GridUpdateArgs a, const __grid_constant__ Boundaries bd) {
+	grid_update_body<COLLIDE, OBJECTS>(a, &bd);
+}
+static_assert(sizeof(GridUpdateArgs) + sizeof(Boundaries) <= 4096, "the boundary grid update's parameters must fit the 4 KiB kernel-parameter limit");
 
 // clear_grid (mgmpm_kernels.cuh:106-115)
 __global__ void clear_grid_kernel(int block_count, float* grid) {
@@ -135,10 +136,10 @@ struct CarryArgs {
 	int mgsp;
 	MgspView view;
 	int* overlap_marks;
-	ColliderView col;  // COLLIDE: the predictor applies the collider at the time the next grid update sees
 };
+// COLLIDE / OBJECTS (MGSP): the predictor applies the boundaries of bd at the time the next grid update sees
 template<bool COLLIDE, bool OBJECTS>
-__device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const ObjectList* objs) {
+__device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Boundaries* bd) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int n = *a.new_count;
 	const int old_nbc = a.state->nbc;
@@ -146,10 +147,8 @@ __device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Object
 	if(a.mgsp && blockIdx.x == 0 && (int) threadIdx.x < a.view.world) a.view.overlap_count[threadIdx.x] = 0;
 	float gdt = 0.f;
 	if(a.next_max_vel) gdt = a.cfg.gravity * device_compute_dt(a.cfg, a.state->max_vel_sq, a.state->step_time, a.state->frame_time, a.state->dt_default);
-	const ColliderFrame* fr = nullptr;
-	const ObjectFrames* of = nullptr;
-	if constexpr(OBJECTS) of = &object_frames_cta<COLLIDE>(a.col, *objs, (float) (a.state->sim_time + (double) a.state->dt));
-	else if constexpr(COLLIDE) fr = &collider_frame_cta(a.col, (float) (a.state->sim_time + (double) a.state->dt));  // the clock rolls by this sub-step's dt
+	const BoundaryFrames* fr = nullptr;
+	if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, (float) (a.state->sim_time + (double) a.state->dt));  // the clock rolls by this sub-step's dt
 	unsigned vmax = 0u;
 	for(int j = blockIdx.x * 8 + warp; j < n; j += gridDim.x * 8) {
 		const int kx = a.new_keys[3 * j], ky = a.new_keys[3 * j + 1], kz = a.new_keys[3 * j + 2];
@@ -166,8 +165,7 @@ __device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Object
 			if(a.next_max_vel) {
 				const float2* s2 = reinterpret_cast<const float2*>(s);
 				const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
-				if constexpr(OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_objects<COLLIDE>(a.cfg, a.col, *of, objs->n, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
-				else if constexpr(COLLIDE) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_collide(a.cfg, a.col, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+				if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS>(a.cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
 				else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 			}
 		} else {
@@ -180,48 +178,77 @@ __device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Object
 		if(lane == 0 && vmax) atomicMax(reinterpret_cast<unsigned*>(a.next_max_vel), vmax);
 	}
 }
-template<bool COLLIDE>
-__global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) { carry_grid_body<COLLIDE, false>(a, nullptr); }
-// OBJECTS: the predictor applies the objects too (MGSP; objs.n >= 1)
-template<bool COLLIDE>
-__global__ void __launch_bounds__(256, 2) carry_grid_objects_kernel(const CarryArgs a, const __grid_constant__ ObjectList objs) { carry_grid_body<COLLIDE, true>(a, &objs); }
-static_assert(sizeof(CarryArgs) + sizeof(ObjectList) <= 4096, "the objects carry's parameters must fit the 4 KiB kernel-parameter limit");
+__global__ void __launch_bounds__(256) carry_grid_kernel(const CarryArgs a) { carry_grid_body<false, false>(a, nullptr); }
+template<bool COLLIDE, bool OBJECTS>
+__global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, OBJECTS>)) carry_grid_boundary_kernel(const CarryArgs a, const __grid_constant__ Boundaries bd) {
+	carry_grid_body<COLLIDE, OBJECTS>(a, &bd);
+}
+static_assert(sizeof(CarryArgs) + sizeof(Boundaries) <= 4096, "the boundary carry's parameters must fit the 4 KiB kernel-parameter limit");
 
 // max |v|^2 the grid update will find, without touching the grid (MGSP start-up)
-template<bool COLLIDE>
-__global__ void __launch_bounds__(256) grid_max_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const ColliderView col) {
+template<bool COLLIDE, bool OBJECTS>
+__device__ __forceinline__ void grid_max_body(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries* bd) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int g = cfg.gsize, bc = cfg.boundary;
 	const float gdt = cfg.gravity * state->dt;
-	const ColliderFrame* fr = nullptr;
-	if constexpr(COLLIDE) fr = &collider_frame_cta(col, (float) state->sim_time);
+	const BoundaryFrames* fr = nullptr;
+	if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, (float) state->sim_time);
 	unsigned vmax = 0u;
 	for(int b = blockIdx.x * 8 + warp; b < state->nbc; b += gridDim.x * 8) {
 		const int kx = keys[3 * b], ky = keys[3 * b + 1], kz = keys[3 * b + 2];
 		const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
 		const float2* s2 = reinterpret_cast<const float2*>(grid + (size_t) b * kGridBlockFloats);
-		if constexpr(COLLIDE) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_collide(cfg, col, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+		if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS>(cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
 		else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 	}
 	vmax = __reduce_max_sync(0xffffffffu, vmax);
 	if(lane == 0 && vmax) atomicMax(reinterpret_cast<unsigned*>(max_vel), vmax);
 }
-// the same with the analytic objects after the collider (objs.n >= 1)
-template<bool COLLIDE>
-__global__ void __launch_bounds__(256, 2) grid_max_objects_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const ColliderView col, const __grid_constant__ ObjectList objs) {
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	const int g = cfg.gsize, bc = cfg.boundary;
-	const float gdt = cfg.gravity * state->dt;
-	const ObjectFrames& of = object_frames_cta<COLLIDE>(col, objs, (float) state->sim_time);
-	unsigned vmax = 0u;
-	for(int b = blockIdx.x * 8 + warp; b < state->nbc; b += gridDim.x * 8) {
-		const int kx = keys[3 * b], ky = keys[3 * b + 1], kz = keys[3 * b + 2];
-		const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
-		const float2* s2 = reinterpret_cast<const float2*>(grid + (size_t) b * kGridBlockFloats);
-		vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_objects<COLLIDE>(cfg, col, of, objs.n, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
-	}
-	vmax = __reduce_max_sync(0xffffffffu, vmax);
-	if(lane == 0 && vmax) atomicMax(reinterpret_cast<unsigned*>(max_vel), vmax);
+__global__ void __launch_bounds__(256) grid_max_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel) {
+	grid_max_body<false, false>(cfg, state, grid, keys, max_vel, nullptr);
+}
+template<bool COLLIDE, bool OBJECTS>
+__global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, OBJECTS>)) grid_max_boundary_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const __grid_constant__ Boundaries bd) {
+	grid_max_body<COLLIDE, OBJECTS>(cfg, state, grid, keys, max_vel, &bd);
+}
+
+// ---- launching the three boundary passes ---------------------------------------------------------------------------------------
+// Calls f(COLLIDE, OBJECTS), two std::bool_constant, with the instance flags that apply bd: the level set when bd.has_collider, the
+// objects when the list is non-empty; neither is the plain kernel.  Each pass keeps all four instances, because the level-set-only
+// one fits 4 CTAs per SM and the level set + objects one does not.
+template<class F>
+void with_boundaries(const Boundaries& bd, F&& f) {
+	using T = std::true_type;
+	using N = std::false_type;
+	if(bd.has_collider && bd.objects.n > 0) f(T(), T());
+	else if(bd.has_collider) f(T(), N());
+	else if(bd.objects.n > 0) f(N(), T());
+	else f(N(), N());
+}
+// f(COLLIDE, OBJECTS) for each boundary instance
+template<class F>
+void for_each_boundary_instance(F&& f) {
+	f(std::true_type(), std::false_type());
+	f(std::false_type(), std::true_type());
+	f(std::true_type(), std::true_type());
+}
+inline void launch_grid_update(const GridUpdateArgs& a, const Boundaries& bd, int ctas, cudaStream_t st) {
+	with_boundaries(bd, [&](auto C, auto O) {
+		if constexpr(C || O) grid_update_boundary_kernel<C, O><<<ctas, kGridThreads, 0, st>>>(a, bd);
+		else grid_update_kernel<<<ctas, kGridThreads, 0, st>>>(a);
+	});
+}
+inline void launch_carry_grid(const CarryArgs& a, const Boundaries& bd, int ctas, cudaStream_t st) {
+	with_boundaries(bd, [&](auto C, auto O) {
+		if constexpr(C || O) carry_grid_boundary_kernel<C, O><<<ctas, 256, 0, st>>>(a, bd);
+		else carry_grid_kernel<<<ctas, 256, 0, st>>>(a);
+	});
+}
+inline void launch_grid_max(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries& bd, int ctas, cudaStream_t st) {
+	with_boundaries(bd, [&](auto C, auto O) {
+		if constexpr(C || O) grid_max_boundary_kernel<C, O><<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel, bd);
+		else grid_max_kernel<<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel);
+	});
 }
 
 // copy_selected_grid_blocks (mgmpm_kernels.cuh:1002-1020), drop-in form: scatter marked blocks

@@ -22,40 +22,21 @@ struct RemoveRows {
 	}
 };
 
-// by region: a row is removed when its position, mapped into object k's material space with k's frame at time t as the collider maps
-// a node (collider_resolve_query), lies in any of the n objects (object_query); with `outside`, when it lies in none
+// by region: a row is removed when its position, mapped into object k's material space with k's frame at time t as the boundary chain
+// maps a node (collider_material_point), lies in any of the n objects of b.objects (object_query); with `outside`, when it lies in none
 struct RemoveRegions : RemoveRows {
-	ObjectList l;
+	Boundaries b;  // objects only
 	float t;
 	int outside;
-	static __device__ __forceinline__ ObjectFrames& frames() {
-		__shared__ ObjectFrames s;
-		return s;
-	}
-	// thread i builds object i's frame once per CTA (object_frames_cta's work, without the level-set collider)
-	__device__ __forceinline__ void prepare() const {
-		ObjectFrames& s = frames();
-		const int i = (int) threadIdx.x;
-		if(i < l.n) {
-			s.o[i] = l.o[i];
-			collider_make_frame(s.o[i], t, s.f[i]);
-		}
-		__syncthreads();
-	}
+	__device__ __forceinline__ void prepare() const { boundary_frames_cta<false, true>(b, t); }
 	__device__ __forceinline__ bool eval(long long i, Row& row) const {
-		const ObjectFrames& s = frames();
+		const BoundaryFrames& s = boundary_frames();
 		const float p[3] = {__ldg(in + i * C), __ldg(in + i * C + 1), __ldg(in + i * C + 2)};
 		bool hit = false;
-		for(int k = 0; k < l.n; ++k) {
-			const cb200_collision_object& o = s.o[k];
-			const ColliderFrame& f = s.f[k];
-			const float xm[3] = {p[0] - f.b[0], p[1] - f.b[1], p[2] - f.b[2]};
-			const float x0[3] = {xm[0] * f.s_inv, xm[1] * f.s_inv, xm[2] * f.s_inv};
-			const float* R = f.rot;
-			float x[3], n[3];
-#pragma unroll
-			for(int d = 0; d < 3; ++d) x[d] = (R[3 * d] * x0[0] + R[3 * d + 1] * x0[1] + R[3 * d + 2] * x0[2]) * o.scale + o.trans[d];
-			hit |= object_query(o, x, n);
+		for(int k = 0; k < b.objects.n; ++k) {
+			float xm[3], x[3], n[3];
+			collider_material_point(s.o[k], s.f[k], p, xm, x);
+			hit |= object_query(s.o[k], x, n);
 		}
 		row = i;
 		return hit == (outside != 0);

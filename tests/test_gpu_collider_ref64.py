@@ -4,7 +4,7 @@ test_ref64_collider_cpu.py fixed on the FP32 collider oracle (no re-tuning here)
 Kernel level: cb200_update_grid_velocity_query_max_collider on the synthetic grids and parameter matrix of the CPU test, per
 node.  Step driver: every case of COLLIDER_CASES in graph and stream mode, one sub-step at a time, the collider placed at the
 simulated time the engine reports before the sub-step.  MGSP: the ranks' dt comes from the max their next-max predictor
-(carry_grid_kernel<true>, grid_max_kernel<true> at set-up) computed for the next grid update; it must be bit-identical on
+(carry_grid_boundary_kernel, grid_max_boundary_kernel at set-up) computed for the next grid update; it must be bit-identical on
 every rank and within DT_ULPS of ref64's grid update at that time.
 """
 import ctypes as C
@@ -107,7 +107,7 @@ def test_engine_collider_substep_matches_ref64(cuda_lib, name, use_graph):
 # ---- MGSP -------------------------------------------------------------------------------------------------------------------
 def build_ranks_with_collider(case, parts, use_graph, max_blocks=6000):
     """The ranks of test_gpu_mgsp_ref64.build_ranks with the case's collider and objects set before initial_setup, so that the
-    set-up's next-max predictor (grid_max_kernel<true>, grid_max_objects_kernel) applies them."""
+    set-up's next-max predictor (grid_max_boundary_kernel) applies them."""
     from claymore_b200.simulator import GmpmSimulator
     sims = []
     for r, ps in enumerate(parts):
@@ -138,7 +138,7 @@ def _grid(sim):
 
 def mgsp_collider_check(case, parts, use_graph, label):
     """Set-up grid and case['steps'] sub-steps of the ranks against ref64_mgsp with the collider at the engine's sim_time;
-    sub-step 0's dt is the set-up predictor's (grid_max_kernel<true> at t = 0), every later one the carry kernel's."""
+    sub-step 0's dt is the set-up predictor's (grid_max_boundary_kernel at t = 0), every later one the carry kernel's."""
     sims = build_ranks_with_collider(case, parts, use_graph)
     cfg = sims[0].cfg
     ccol, objs = S.ref_collider(case), S.ref_objects(case)

@@ -217,7 +217,7 @@ def test_kernel_matches_oracle(oracle, cuda_lib, grid, case, collider, t):
 
 
 def test_sphere_object_matches_levelset_collider_away_from_surface(cuda_lib, grid):
-    """The two copies of the response (collider_resolve and collider_resolve_query) on identical inputs: a sphere object and the
+    """The response (collider_resolve) over its two queries on identical inputs: a sphere object and the
     level-set collider on levelset.sphere's field, same type, friction and motion, give the same velocities at every node a cell or
     more from the surface and off the sphere's centre (the trilinear gradient there is the exact normal up to float32 rounding)."""
     torch = _torch()
@@ -370,8 +370,8 @@ def test_emission_with_objects_matches_oracle(oracle, cuda_lib, use_graph):
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize("use_graph", [True, False], ids=["graph", "stream"])
 def test_mgsp_two_ranks_analytic_sticky_floor_match_single_domain(oracle, cuda_lib, use_graph):
-    """The max |v|^2 the ranks agree on comes from grid_max_objects_kernel at set-up and carry_grid_objects_kernel after each
-    sub-step: with a CFL-bound dt (fast cube, dt_default 1e-3) it drives dt, which must equal the single-domain oracle's (whose max
+    """The max |v|^2 the ranks agree on comes from the objects instances of grid_max_boundary_kernel at set-up and of
+    carry_grid_boundary_kernel after each sub-step: with a CFL-bound dt (fast cube, dt_default 1e-3) it drives dt, which must equal the single-domain oracle's (whose max
     is the one its grid update finds) and be bit-identical on both ranks."""
     from claymore_b200 import mgsp
     scene = _sticky_floor_dt_scene()

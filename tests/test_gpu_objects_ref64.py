@@ -5,7 +5,7 @@ Kernel level: cb200_update_grid_velocity_query_max_objects on the synthetic grid
 friction, motion, t and boundary, the 16-object list, the level-set collider with two objects), per node and in the max.
 Step driver: every case of OBJECT_CASES in graph and stream mode, one sub-step at a time, the objects placed at the simulated
 time the engine reports before the sub-step: error bits, the clock, particles and cells, dt.  MGSP: sub-step 0's dt comes
-from the set-up predictor (grid_max_objects_kernel at sim_time), every later one from carry_grid_objects_kernel, which places
+from the set-up predictor (grid_max_boundary_kernel at sim_time), every later one from carry_grid_boundary_kernel, which places
 the objects at sim_time + dt; both must be bit-identical on every rank and within DT_ULPS of ref64's grid update at that time.
 """
 import ctypes as C
