@@ -697,8 +697,11 @@ void orc_register_exterior_blocks(const orc_config* cfg, int block_count, orc_pa
 static inline int node_has_mass(float m) { return m >= FLT_MIN; }
 
 /* ref: Projects/GMPM/mgmpm_kernels.cuh:325-420.  Quirk kept: wall-zeroed y velocity still receives
- * gravity (SURVEY.md Appendix B #1); NaN -> +inf (B #3). */
-void orc_update_grid_velocity_query_max(const orc_config* cfg, int block_count, float* grid, orc_partition part, float dt, float* max_vel) {
+ * gravity (SURVEY.md Appendix B #1); NaN -> +inf (B #3).  The one body of every grid update: `resolve` (NULL: none) is the
+ * boundaries' hook, run on each node with mass after gravity and before |v|^2 (the collider oracle's, collider_oracle.c). */
+typedef void (*orc_node_resolve)(const void* ctx, const int* node, float* v);
+static void boundaries_update(const orc_config* cfg, int block_count, float* grid, orc_partition part, float dt, orc_node_resolve resolve, const void* ctx,
+                              float* max_vel) {
 	const int g = cfg_gsize(cfg), bc = cfg->boundary;
 	float mx = *max_vel;
 #pragma omp parallel for num_threads(g_threads) schedule(static) reduction(max : mx)
@@ -711,22 +714,31 @@ void orc_update_grid_velocity_query_max(const orc_config* cfg, int block_count, 
 			float vsq = 0.f;
 			if(node_has_mass(mass)) {
 				const float mi = 1.f / mass;
-				float v0 =(ob & 4) ? 0.f : blk[64 + c] * mi;
-				float v1 = (ob & 2) ? 0.f : blk[128 + c] * mi;
-				v1 += cfg->gravity * dt;
-				float v2 = (ob & 1) ? 0.f : blk[192 + c] * mi;
-				blk[64 + c] = v0;
-				blk[128 + c] = v1;
-				blk[192 + c] = v2;
-				vsq += v0 * v0;
-				vsq += v1 * v1;
-				vsq += v2 * v2;
+				float v[3];
+				v[0] = (ob & 4) ? 0.f : blk[64 + c] * mi;
+				v[1] = (ob & 2) ? 0.f : blk[128 + c] * mi;
+				v[1] += cfg->gravity * dt;
+				v[2] = (ob & 1) ? 0.f : blk[192 + c] * mi;
+				if(resolve) {
+					const int node[3] = {4 * k[0] + ((c & 0x30) >> 4), 4 * k[1] + ((c & 0xc) >> 2), 4 * k[2] + (c & 0x3)};
+					resolve(ctx, node, v);
+				}
+				blk[64 + c] = v[0];
+				blk[128 + c] = v[1];
+				blk[192 + c] = v[2];
+				vsq += v[0] * v[0];
+				vsq += v[1] * v[1];
+				vsq += v[2] * v[2];
 			}
 			if(isnan(vsq)) vsq = INFINITY;
 			if(vsq > mx) mx = vsq;
 		}
 	}
 	*max_vel = mx;
+}
+
+void orc_update_grid_velocity_query_max(const orc_config* cfg, int block_count, float* grid, orc_partition part, float dt, float* max_vel) {
+	boundaries_update(cfg, block_count, grid, part, dt, NULL, NULL, max_vel);
 }
 
 static inline void dir_components(int dir, int* d) {
@@ -1258,14 +1270,12 @@ void orc_sim_initial_setup(orc_sim* s) {
 	}
 }
 
-/* ref: gmpm_simulator.cuh:324-580 (one pass of the inner loop) */
-void orc_sim_step(orc_sim* s, float time_left) {
+/* ref: gmpm_simulator.cuh:337-579: one sub-step after its grid update (:337-362), which left the max |v|^2 max_vel_sq.  The
+ * collider oracle's sub-step (orc_csim_step) runs it after its own grid update. */
+static void sim_step_after_grid_update(orc_sim* s, float max_vel_sq, float time_left) {
 	const orc_config* cfg = &s->cfg;
 	const int R = s->rollid, Rn = R ^ 1;
-	/* :337-362 */
-	float mv = 0.f;
-	orc_update_grid_velocity_query_max(cfg, s->nbc, s->grids[0], s->parts[R], s->dt, &mv);
-	s->max_vel = sqrtf(mv);
+	s->max_vel = sqrtf(max_vel_sq);
 	s->next_dt = compute_dt(cfg, s->max_vel, time_left, s->dt_default);
 	/* :383-398 */
 	orc_clear_grid(s->nbc, s->grids[1]);
@@ -1323,6 +1333,13 @@ void orc_sim_step(orc_sim* s, float time_left) {
 	/* :578-579 */
 	s->rollid = Rn;
 	s->dt = s->next_dt;
+}
+
+/* ref: gmpm_simulator.cuh:324-580 (one pass of the inner loop) */
+void orc_sim_step(orc_sim* s, float time_left) {
+	float mv = 0.f; /* :337-362 */
+	orc_update_grid_velocity_query_max(&s->cfg, s->nbc, s->grids[0], s->parts[s->rollid], s->dt, &mv);
+	sim_step_after_grid_update(s, mv, time_left);
 }
 
 int orc_sim_counts(orc_sim* s, int* pbc, int* nbc, int* ebc) {

@@ -1,7 +1,7 @@
 /*
  * collider_oracle.c -- see collider_oracle.h.  TEST INFRASTRUCTURE ONLY.
- * The oracle is compiled into this translation unit so that the sub-step restated below can use its simulator's state
- * (struct orc_sim) and helpers; libclaymore_oracle.so itself is unchanged by it.
+ * The oracle is compiled into this translation unit so that the grid update and sub-step below can use its simulator's state
+ * (struct orc_sim) and its grid-update body; libclaymore_oracle.so itself is unchanged by it.
  */
 #include "claymore_oracle.c"
 #include "collider_oracle.h"
@@ -37,7 +37,8 @@ static void col_mat_mul(const float* a, const float* b, float* c) {
 		for(int i = 0; i < 3; ++i) c[3 * j + i] = a[i] * b[3 * j] + a[3 + i] * b[3 * j + 1] + a[6 + i] * b[3 * j + 2];
 }
 /* get_signed_distance_and_normal :98-137 + query_sdf :138-143 */
-static int col_query(const orc_config* cfg, const orc_collider* col, const float* x, float* normal) {
+static int col_query(const orc_config* cfg, const void* ctx, const float* x, float* normal) {
+	const orc_collider* col = (const orc_collider*) ctx;
 	const int G = cfg_gsize(cfg), bc = cfg->boundary;
 	const float dx = cfg_dx(cfg);
 	const float lo = (float) bc * dx * 4.f, hi = (float) (G - bc) * 4.f * dx; /* :139 */
@@ -72,8 +73,70 @@ static int col_query(const orc_config* cfg, const orc_collider* col, const float
 	}
 	return sd <= 0.f; /* :142 */
 }
-/* detect_and_resolve_collision :159-249 */
-void orc_collider_resolve(const orc_config* cfg, const orc_collider* col, float t, const int* node, float* vel) {
+
+/* hit test (phi <= 0) and material-space normal (0 where there is none) of one shape at the material-space point x, restated
+ * from the header's definitions */
+static int object_query(const orc_config* cfg, const void* ctx, const float* x, float* n) {
+	const orc_collision_object* o = (const orc_collision_object*) ctx;
+	const float *a = o->a, *b = o->b;
+	n[0] = n[1] = n[2] = 0.f;
+	if(o->shape == ORC_SHAPE_PLANE) {
+		if((x[0] - a[0]) * b[0] + (x[1] - a[1]) * b[1] + (x[2] - a[2]) * b[2] > 0.f) return 0;
+		for(int d = 0; d < 3; ++d) n[d] = b[d];
+		return 1;
+	}
+	if(o->shape == ORC_SHAPE_BOX) {
+		for(int d = 0; d < 3; ++d)
+			if(!(a[d] <= x[d] && x[d] <= b[d])) return 0;
+		int axis = 0;
+		float best = 0.f, sgn = 1.f;
+		for(int d = 0; d < 3; ++d) {
+			const float ql = a[d] - x[d], qh = x[d] - b[d];
+			const float q = ql > qh ? ql : qh;
+			if(d == 0 || q > best) {
+				best = q;
+				axis = d;
+				sgn = ql > qh ? -1.f : 1.f;
+			}
+		}
+		n[axis] = sgn;
+		return 1;
+	}
+	const float d0 = x[0] - a[0], d1 = x[1] - a[1], d2 = x[2] - a[2], r = b[0];
+	if(o->shape == ORC_SHAPE_SPHERE) {
+		const float dd = d0 * d0 + d1 * d1 + d2 * d2;
+		if(dd > r * r) return 0;
+		if(dd > 0.f) {
+			const float len = sqrtf(dd);
+			n[0] = d0 / len;
+			n[1] = d1 / len;
+			n[2] = d2 / len;
+		}
+		return 1;
+	}
+	const float rho2 = d0 * d0 + d2 * d2, h = b[1];
+	if(rho2 > r * r || fabsf(d1) > h) return 0;
+	const float rho = sqrtf(rho2);
+	if(h - fabsf(d1) < r - rho) {
+		n[1] = d1 < 0.f ? -1.f : 1.f;
+	} else if(rho > 0.f) {
+		n[0] = d0 / rho;
+		n[2] = d2 / rho;
+	}
+	return 1;
+}
+
+/* the motion fields orc_collider and orc_collision_object share */
+typedef struct boundary_motion {
+	const float *rot_mat, *trans, *trans_vel, *omega;
+	float dsdt, scale, friction;
+	int type;
+} boundary_motion;
+#define BOUNDARY_MOTION(p) {(p)->rot_mat, (p)->trans, (p)->trans_vel, (p)->omega, (p)->dsdt, (p)->scale, (p)->friction, (p)->type}
+typedef int (*boundary_query)(const orc_config* cfg, const void* ctx, const float* x, float* normal);
+
+/* detect_and_resolve_collision :159-249 over the query of a level set (col_query) or of a shape (object_query) */
+static void boundary_resolve(const orc_config* cfg, const boundary_motion* col, boundary_query query, const void* ctx, float t, const int* node, float* vel) {
 	const float dx = cfg_dx(cfg);
 	float xm[3], x0[3], x[3], cur[9], prev[9], r[9];
 	for(int d = 0; d < 3; ++d) xm[d] = (float) node[d] * dx - (col->trans[d] + col->trans_vel[d] * t); /* :160 */
@@ -90,7 +153,7 @@ void orc_collider_resolve(const orc_config* cfg, const orc_collider* col, float 
 	}
 	for(int d = 0; d < 3; ++d) x[d] = x[d] * col->scale + col->trans[d]; /* :181 */
 	float on[3];
-	if(!col_query(cfg, col, x, on)) return; /* :185-186 */
+	if(!query(cfg, ctx, x, on)) return; /* :185-186 */
 	const float* w = col->omega;
 	float vo[3] = {w[1] * xm[2] - w[2] * xm[1], w[2] * xm[0] - w[0] * xm[2], w[0] * xm[1] - w[1] * xm[0]}; /* :188, a true cross product */
 	for(int d = 0; d < 3; ++d) vo[d] += xm[d] * (col->dsdt / col->scale); /* :189 */
@@ -137,51 +200,49 @@ void orc_collider_resolve(const orc_config* cfg, const orc_collider* col, float 
 	for(int d = 0; d < 3; ++d) vel[d] += vo[d]; /* :247 */
 }
 
-/* ref: Projects/MGSP/mgmpm_kernels.cuh:323-399: the GMPM grid update (:357-360 as above), then the collider (:362-363) */
-void orc_update_grid_velocity_query_max_collider(const orc_config* cfg, int block_count, float* grid, orc_partition part, float dt, const orc_collider* col, float time, float* max_vel) {
-	const int g = cfg_gsize(cfg), bc = cfg->boundary;
-	float mx = *max_vel;
-#pragma omp parallel for num_threads(g_threads) schedule(static) reduction(max : mx)
-	for(int b = 0; b < block_count; ++b) {
-		const int* k = part.active_keys + 3 * b;
-		const int ob = ((k[0] < bc || k[0] >= g - bc) << 2) | ((k[1] < bc || k[1] >= g - bc) << 1) | (k[2] < bc || k[2] >= g - bc);
-		float* blk = grid + (long) b * 256;
-		for(int c = 0; c < BLOCK_VOL; ++c) {
-			const float mass = blk[c];
-			float vsq = 0.f;
-			if(node_has_mass(mass)) {
-				const float mi = 1.f / mass;
-				float v[3];
-				v[0] = (ob & 4) ? 0.f : blk[64 + c] * mi;
-				v[1] = (ob & 2) ? 0.f : blk[128 + c] * mi;
-				v[1] += cfg->gravity * dt;
-				v[2] = (ob & 1) ? 0.f : blk[192 + c] * mi;
-				const int node[3] = {4 * k[0] + ((c & 0x30) >> 4), 4 * k[1] + ((c & 0xc) >> 2), 4 * k[2] + (c & 0x3)}; /* :362 */
-				orc_collider_resolve(cfg, col, time, node, v);
-				blk[64 + c] = v[0];
-				blk[128 + c] = v[1];
-				blk[192 + c] = v[2];
-				vsq += v[0] * v[0]; /* :364-372 add each square once: |v|^2 */
-				vsq += v[1] * v[1];
-				vsq += v[2] * v[2];
-			}
-			if(isnan(vsq)) vsq = INFINITY;
-			if(vsq > mx) mx = vsq;
-		}
-	}
-	*max_vel = mx;
+void orc_collider_resolve(const orc_config* cfg, const orc_collider* col, float t, const int* node, float* vel) {
+	const boundary_motion m = BOUNDARY_MOTION(col);
+	boundary_resolve(cfg, &m, col_query, col, t, node, vel);
 }
 
+static void object_resolve(const orc_config* cfg, const orc_collision_object* o, float t, const int* node, float* vel) {
+	const boundary_motion m = BOUNDARY_MOTION(o);
+	boundary_resolve(cfg, &m, object_query, o, t, node, vel);
+}
 
-/* ---- the oracle's simulator with a collider -------------------------------------------------------------------------------- */
+/* ref: Projects/MGSP/mgmpm_kernels.cuh:323-399: the GMPM grid update (:357-360, claymore_oracle.c), then the boundaries
+ * (:362-363): the collider, then the objects in list order */
+typedef struct boundaries {
+	const orc_config* cfg;
+	const orc_collider* col;
+	const orc_collision_object* objs;
+	int n_objs;
+	float time;
+} boundaries;
+static void boundaries_resolve(const void* ctx, const int* node, float* v) {
+	const boundaries* b = (const boundaries*) ctx;
+	if(b->col) orc_collider_resolve(b->cfg, b->col, b->time, node, v);
+	for(int i = 0; i < b->n_objs; ++i) object_resolve(b->cfg, &b->objs[i], b->time, node, v);
+}
+void orc_update_grid_velocity_query_max_boundaries(const orc_config* cfg, int block_count, float* grid, orc_partition part, float dt, const orc_collider* col,
+                                                   const orc_collision_object* objs, int n_objs, float time, float* max_vel) {
+	const boundaries b = {cfg, col, objs, n_objs, time};
+	boundaries_update(cfg, block_count, grid, part, dt, boundaries_resolve, &b, max_vel);
+}
+void orc_update_grid_velocity_query_max_collider(const orc_config* cfg, int block_count, float* grid, orc_partition part, float dt, const orc_collider* col, float time, float* max_vel) {
+	orc_update_grid_velocity_query_max_boundaries(cfg, block_count, grid, part, dt, col, NULL, 0, time, max_vel);
+}
+
+/* ---- the oracle's simulator with boundaries ------------------------------------------------------------------------------ */
 struct orc_csim {
 	orc_sim* s;
 	double sim_time;   /* sum of the dt of every finished sub-step */
 	int has_collider;
 	orc_collider col;
 	float* sdf;        /* owned block-layout field of the collider */
+	orc_collision_object* objs;  /* owned copy of the objects */
+	int n_objs;
 };
-
 orc_csim* orc_csim_create(const orc_config* cfg, float dt_default, int max_blocks) {
 	orc_csim* c = (orc_csim*) calloc(1, sizeof(orc_csim));
 	c->s = orc_sim_create(cfg, dt_default, max_blocks);
@@ -191,6 +252,7 @@ void orc_csim_destroy(orc_csim* c) {
 	if(!c) return;
 	orc_sim_destroy(c->s);
 	free(c->sdf);
+	free(c->objs);
 	free(c);
 }
 orc_sim* orc_csim_sim(orc_csim* c) { return c->s; }
@@ -219,72 +281,24 @@ void orc_csim_clear_collider(orc_csim* c) {
 	c->sdf = NULL;
 }
 
-/* orc_sim_step (claymore_oracle.c; ref: gmpm_simulator.cuh:324-580) with the grid update of the MGSP form when a collider is
- * set, placed at the simulated time at the start of the sub-step, and the clock advanced by the dt the sub-step ran with */
+void orc_csim_set_objects(orc_csim* c, const orc_collision_object* objs, int n) {
+	free(c->objs);
+	c->objs = NULL;
+	c->n_objs = n;
+	if(n > 0) {
+		c->objs = (orc_collision_object*) malloc(sizeof(orc_collision_object) * n);
+		memcpy(c->objs, objs, sizeof(orc_collision_object) * n);
+	}
+}
+
+/* orc_sim_step (claymore_oracle.c; ref: gmpm_simulator.cuh:324-580) with the grid update of the MGSP form, the boundaries placed
+ * at the simulated time at the start of the sub-step, and the clock advanced by the dt the sub-step ran with */
 void orc_csim_step(orc_csim* c, float time_left) {
 	orc_sim* s = c->s;
-	const orc_config* cfg = &s->cfg;
-	const int R = s->rollid, Rn = R ^ 1;
-	/* :337-362 */
-	float mv = 0.f;
-	if(c->has_collider)
-		orc_update_grid_velocity_query_max_collider(cfg, s->nbc, s->grids[0], s->parts[R], s->dt, &c->col, (float) c->sim_time, &mv);
-	else
-		orc_update_grid_velocity_query_max(cfg, s->nbc, s->grids[0], s->parts[R], s->dt, &mv);
-	s->max_vel = sqrtf(mv);
-	s->next_dt = compute_dt(cfg, s->max_vel, time_left, s->dt_default);
-	/* :383-398 */
-	orc_clear_grid(s->nbc, s->grids[1]);
-	for(int m = 0; m < s->nmodels; ++m) {
-		memset(s->bins[Rn][m].cell_particle_counts, 0, sizeof(int) * (size_t) s->ebc * BLOCK_VOL);
-		orc_g2p2g(cfg, s->dt, s->next_dt, s->pbc, s->bins[R][m], s->bins[Rn][m], s->parts[Rn], s->parts[R], s->grids[0], s->grids[1]);
-	}
-	/* :424-431 */
-	for(int m = 0; m < s->nmodels; ++m) {
-		orc_particle_buffer pb = s->bins[Rn][m];
-		memset(pb.particle_bucket_sizes, 0, sizeof(int) * (s->ebc + 1));
-		orc_cell_bucket_to_block(cfg, s->ebc, pb.cell_particle_counts, pb.cellbuckets, pb.particle_bucket_sizes, pb.blockbuckets);
-	}
-	/* :438-470 */
-	memset(s->marks, 0, sizeof(int) * s->nbc);
-	orc_mark_active_grid_blocks(s->nbc, s->grids[1], s->marks);
-	memset(s->sources, 0, sizeof(int) * (s->ebc + 1));
-	for(int m = 0; m < s->nmodels; ++m) orc_mark_active_particle_blocks(s->ebc + 1, s->bins[Rn][m].particle_bucket_sizes, s->sources);
-	orc_exclusive_scan(s->ebc + 1, s->sources, s->destinations);
-	const int new_pbc = s->destinations[s->ebc];
-	*s->parts[Rn].count = new_pbc;
-	orc_exclusive_scan_inverse(s->ebc, s->destinations, s->sources);
-	orc_reset_table(cfg, s->parts[Rn]);
-	check_blocks(s, new_pbc, "particle");
-	/* :480-505 */
-	orc_update_partition(cfg, new_pbc, s->sources, s->parts[R], s->parts[Rn]);
-	for(int m = 0; m < s->nmodels; ++m) {
-		orc_update_buckets(cfg, new_pbc, s->sources, s->bins[Rn][m], s->bins[R][m]);
-		s->bins[R][m].particle_bucket_sizes[new_pbc] = 0; /* as orc_sim_step: the reference reads a stale value there */
-		orc_compute_bin_capacity(new_pbc + 1, s->bins[R][m].particle_bucket_sizes, s->bin_sizes);
-		orc_exclusive_scan(new_pbc + 1, s->bin_sizes, s->bins[R][m].bin_offsets);
-		if(s->bins[R][m].bin_offsets[new_pbc] > s->bin_capacity[m]) {
-			fprintf(stderr, "oracle: bin capacity exceeded\n");
-			abort();
-		}
-	}
-	/* :513-524 */
-	orc_register_neighbor_blocks(cfg, new_pbc, s->parts[Rn]);
-	const int prev_nbc = s->nbc;
-	const int new_nbc = *s->parts[Rn].count;
-	check_blocks(s, new_nbc, "neighbour");
-	/* :536-541 */
-	orc_clear_grid(s->ebc > new_nbc ? s->ebc : new_nbc, s->grids[0]);
-	orc_copy_selected_grid_blocks(cfg, prev_nbc, s->parts[R].active_keys, s->parts[Rn], s->marks, s->grids[1], s->grids[0]);
-	/* :560-570 */
-	orc_register_exterior_blocks(cfg, new_pbc, s->parts[Rn]);
-	const int new_ebc = *s->parts[Rn].count;
-	check_blocks(s, new_ebc, "exterior");
-	s->pbc = new_pbc;
-	s->nbc = new_nbc;
-	s->ebc = new_ebc;
-	/* :578-579 */
-	s->rollid = Rn;
-	c->sim_time += (double) s->dt;
-	s->dt = s->next_dt;
+	const float dt = s->dt;
+	float mv = 0.f; /* :337-362 */
+	orc_update_grid_velocity_query_max_boundaries(&s->cfg, s->nbc, s->grids[0], s->parts[s->rollid], dt, c->has_collider ? &c->col : NULL, c->objs, c->n_objs,
+	                                              (float) c->sim_time, &mv);
+	sim_step_after_grid_update(s, mv, time_left);
+	c->sim_time += (double) dt;
 }

@@ -1,6 +1,7 @@
-"""ctypes binding of the CPU oracle with the signed-distance collider (oracle/libclaymore_collider_oracle.so).
+"""ctypes binding of the CPU oracle with the boundaries: the signed-distance collider and the analytic collision objects
+(oracle/libclaymore_collider_oracle.so).
 
-TEST INFRASTRUCTURE ONLY.  The library holds the whole oracle plus the collider (oracle/collider_oracle.c), so a ColliderOracleSim
+TEST INFRASTRUCTURE ONLY.  The library holds the whole oracle plus the boundaries (oracle/collider_oracle.c), so a ColliderOracleSim
 is an OracleSim whose calls go to that library; the plain oracle (oracle_binding) is left as it is.
 """
 import ctypes as C
@@ -10,6 +11,7 @@ import subprocess
 import numpy as np
 
 import oracle_binding as ob
+from claymore_b200._capi import CollisionObject
 
 _ORACLE_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle")
 _LIB_PATH = os.path.join(_ORACLE_DIR, "libclaymore_collider_oracle.so")
@@ -51,6 +53,8 @@ def lib():
             dst.argtypes, dst.restype = src.argtypes, src.restype
         L.orc_collider_resolve.argtypes = [C.POINTER(ob.Config), C.POINTER(Collider), C.c_float, C.c_void_p, C.c_void_p]
         L.orc_update_grid_velocity_query_max_collider.argtypes = [C.POINTER(ob.Config), C.c_int, C.c_void_p, ob.Partition, C.c_float, C.POINTER(Collider), C.c_float, C.c_void_p]
+        L.orc_update_grid_velocity_query_max_boundaries.argtypes = [C.POINTER(ob.Config), C.c_int, C.c_void_p, ob.Partition, C.c_float, C.POINTER(Collider),
+                                                                    C.POINTER(CollisionObject), C.c_int, C.c_float, C.c_void_p]
         L.orc_csim_create.restype = C.c_void_p
         L.orc_csim_create.argtypes = [C.POINTER(ob.Config), C.c_float, C.c_int]
         L.orc_csim_destroy.argtypes = [C.c_void_p]
@@ -58,6 +62,7 @@ def lib():
         L.orc_csim_sim.argtypes = [C.c_void_p]
         L.orc_csim_set_collider.argtypes = [C.c_void_p, C.POINTER(Collider), C.c_void_p]
         L.orc_csim_clear_collider.argtypes = [C.c_void_p]
+        L.orc_csim_set_objects.argtypes = [C.c_void_p, C.POINTER(CollisionObject), C.c_int]
         L.orc_csim_step.argtypes = [C.c_void_p, C.c_float]
         L.orc_csim_time.restype = C.c_double
         L.orc_csim_time.argtypes = [C.c_void_p]
@@ -65,8 +70,19 @@ def lib():
     return _lib
 
 
+def unit_planes(objs):
+    """copies of the objects (orc_collision_object: layout of cb200_collision_object) with plane normals made unit length in double, as
+    cb200_sim_set_collision_objects stores them"""
+    out = (CollisionObject * max(len(objs), 1))(*objs)
+    for o in out[: len(objs)]:
+        if o.shape == 0:
+            n = np.asarray(list(o.b), np.float64)
+            o.b[:] = [float(v) for v in n / np.sqrt((n * n).sum())]
+    return out
+
+
 class ColliderOracleSim(ob.OracleSim):
-    """OracleSim with one collider; every call goes to the collider oracle's library."""
+    """OracleSim with boundaries (a collider, then analytic collision objects); every call goes to the collider oracle's library."""
 
     def __init__(self, cfg, dt_default=1e-4, max_blocks=20000, threads=1):
         self.cfg = cfg
@@ -97,19 +113,11 @@ class ColliderOracleSim(ob.OracleSim):
     def clear_collider(self):
         self.L.orc_csim_clear_collider(self.c)
 
+    def set_collision_objects(self, objs):
+        """objs: cb200_collision_object structs, resolved after the collider in list order; [] clears them"""
+        self.L.orc_csim_set_objects(self.c, unit_planes(list(objs)), len(objs))
+
     @property
     def sim_time(self):
         return self.L.orc_csim_time(self.c)
 
-
-def build_oracle(scene, dt=1e-4, max_blocks=4000, max_ppc=128, threads=1, cfl=0.5):
-    """tests/scenes.build_oracle with a ColliderOracleSim"""
-    import scenes
-    cfg = ob.make_config(domain_bits=scene["domain_bits"], max_ppc=max_ppc, cfl=cfl)
-    sim = ColliderOracleSim(cfg, dt, max_blocks, threads=threads)
-    dx = 1.0 / (1 << scene["domain_bits"])
-    for m in scene["models"]:
-        mid = sim.init_model(m["material"], m["pos"], m["v0"])
-        scenes.apply_material(sim, mid, m["material"], dx, True)
-    sim.initial_setup()
-    return sim

@@ -389,18 +389,20 @@ def _slope(f, gc, w, N, dx):
     return out
 
 
-def material_point(cfg, col, t, nodes):
-    """The collider's (or an object's) frame at the float32 time t and the material-space point of each node nodes[n, 3]:
-    dict(f (collider_frame), col (collider_params), Rb (the rotation per node, (value, E)), xm (node dx - b), x (the
-    material-space point R (node dx - b) s_inv scale + trans)), every vector as (value[n, 3], E[n, 3])."""
+def material_point(cfg, col, t, nodes=None, points=None):
+    """The collider's (or an object's) frame at the float32 time t and the material-space point of each node nodes[n, 3], or
+    of each world-space float32 point points[n, 3] (cfg is then unused): dict(f (collider_frame), col (collider_params), Rb
+    (the rotation per point, (value, E)), xm (node dx - b), x (the material-space point R (node dx - b) s_inv scale + trans)),
+    every vector as (value[n, 3], E[n, 3])."""
     f = collider_frame(col, t)
     col = f["col"]
-    nodes = np.asarray(nodes, np.int64).reshape(-1, 3)
-    n = len(nodes)
-    dx = 1.0 / (1 << cfg.domain_bits)
+    if points is None:
+        points = np.asarray(nodes, np.int64).reshape(-1, 3) * (1.0 / (1 << cfg.domain_bits))
+    points = np.asarray(points, np.float64).reshape(-1, 3)
+    n = len(points)
     R = f["rot"]
     Rb = (np.broadcast_to(R[0], (n, 9)), np.broadcast_to(R[1], (n, 9)))
-    xm = _sub(_exact(nodes * dx), (np.broadcast_to(f["b"][0], (n, 3)), np.broadcast_to(f["b"][1], (n, 3))))
+    xm = _sub(_exact(points), (np.broadcast_to(f["b"][0], (n, 3)), np.broadcast_to(f["b"][1], (n, 3))))
     x0 = _mul(xm, f["s_inv"])
     y = [_dot3(Rb, x0, lambda k, d=d: 3 * d + k, lambda k: k) for d in range(3)]
     y = (np.stack([a[0] for a in y], -1), np.stack([a[1] for a in y], -1))

@@ -275,19 +275,13 @@ def config(case):
 def build_oracle(ob, case, max_blocks=6000):
     cfg = ob.make_config(domain_bits=case["domain_bits"], max_ppc=case["max_ppc"], cfl=case["cfl"], gravity=case.get("gravity", -9.8),
                          boundary=case.get("boundary", 2))
-    if case.get("objects"):
+    if case.get("collider") or case.get("objects"):
         import collider_oracle_binding as cob
-        import objects_oracle_binding as oob
-        sim = oob.ObjectsOracleSim(cfg, case["dt"], max_blocks)
+        sim = cob.ColliderOracleSim(cfg, case["dt"], max_blocks)
         if case.get("collider"):
             sdf, grad = collider_field(case)
             sim.set_collider(collider_struct(cob.Collider(), case["collider"]), sdf, grad)
         sim.set_collision_objects(object_structs(case))
-    elif case.get("collider"):
-        import collider_oracle_binding as cob
-        sim = cob.ColliderOracleSim(cfg, case["dt"], max_blocks)
-        sdf, grad = collider_field(case)
-        sim.set_collider(collider_struct(cob.Collider(), case["collider"]), sdf, grad)
     else:
         sim = ob.OracleSim(cfg, case["dt"], max_blocks)
     sim.frame = np.float32(1.0 / case["fps"]) if case.get("fps") else None

@@ -20,9 +20,11 @@ def apply_material(sim, model_id, material, dx, is_oracle):
         getattr(sim, name)(*args, model=model_id)
 
 
-def build_oracle(ob, scene, dt=1e-4, max_blocks=4000, max_ppc=128, threads=1, cfl=0.5):
+def build_oracle(ob, scene, dt=1e-4, max_blocks=4000, max_ppc=128, threads=1, cfl=0.5, sim_class=None):
+    """The oracle simulator of a scene, set up: an ob.OracleSim, or a sim_class such as collider_oracle_binding.ColliderOracleSim
+    (boundaries)."""
     cfg = ob.make_config(domain_bits=scene["domain_bits"], max_ppc=max_ppc, cfl=cfl)
-    sim = ob.OracleSim(cfg, dt, max_blocks, threads=threads)
+    sim = (sim_class or ob.OracleSim)(cfg, dt, max_blocks, threads=threads)
     dx = 1.0 / (1 << scene["domain_bits"])
     for m in scene["models"]:
         mid = sim.init_model(m["material"], m["pos"], m["v0"])

@@ -179,7 +179,7 @@ def test_frames_resume_where_they_stopped(cuda_lib):
 @pytest.mark.timeout(600)
 def test_moving_paddle_resumes_where_it_was(oracle, cuda_lib):
     scene = scenes.small_cube(material=scenes.J_FLUID, lo=18, hi=34, v0=(0.0, 0.0, 0.0))
-    osim = cob.build_oracle(scene)
+    osim = scenes.build_oracle(oracle, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene)
     p = dict(_params("slip", 0.0, "static"), trans=(-0.08, 0.0, 0.0), trans_vel=(1.5, 0.0, 0.0))
     sdf, grad = _set_both(osim, esim, scene["domain_bits"], "box", p)

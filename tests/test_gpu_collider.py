@@ -66,7 +66,7 @@ def _block_field(domain_bits, sdf, grad):
 @pytest.fixture(scope="module")
 def start_grid(oracle):
     scene = scenes.small_cube()
-    osim = cob.build_oracle(scene)
+    osim = scenes.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     _, nbc, _ = osim.block_counts()
     g0 = osim.grid_array(0)[: nbc * 256].copy()
     keys = osim.partition_arrays(0)["active_keys"][: nbc * 3].copy()
@@ -134,7 +134,7 @@ def test_kernel_wall_band_cells_equal_no_collider(oracle, cuda_lib):
     mass is stopped (STICKY)."""
     torch = _torch()
     scene = scenes.small_cube(lo=4, hi=14, v0=(0.2, -0.5, 0.1))   # reaches into the wall band (2 blocks = 8 cells)
-    osim = cob.build_oracle(scene)
+    osim = scenes.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     _, nbc, _ = osim.block_counts()
     g0 = osim.grid_array(0)[: nbc * 256].copy()
     keys = osim.partition_arrays(0)["active_keys"][: nbc * 3].copy()
@@ -194,7 +194,7 @@ def _set_both(osim, esim, domain_bits, shape, p):
 @pytest.mark.parametrize("material", [scenes.FIXED_COROTATED, scenes.J_FLUID, scenes.SAND, scenes.NACC])
 def test_cube_on_box_collider_matches_oracle(oracle, cuda_lib, material, typ, use_graph):
     scene = scenes.small_cube(material=material, v0=(0.3, -1.5, 0.2))
-    osim = cob.build_oracle(scene)
+    osim = scenes.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene, use_graph=use_graph)
     _set_both(osim, esim, scene["domain_bits"], "floor", _params(typ, 0.3, "static"))
     for k in range(4):
@@ -210,7 +210,7 @@ def test_cube_on_box_collider_matches_oracle(oracle, cuda_lib, material, typ, us
 @pytest.mark.timeout(600)
 def test_fluid_dam_with_moving_paddle_matches_oracle(oracle, cuda_lib):
     scene = scenes.small_cube(material=scenes.J_FLUID, lo=18, hi=34, v0=(0.0, 0.0, 0.0))
-    osim = cob.build_oracle(scene)
+    osim = scenes.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene)
     p = dict(_params("slip", 0.0, "static"), trans=(-0.08, 0.0, 0.0), trans_vel=(1.5, 0.0, 0.0))
     _set_both(osim, esim, scene["domain_bits"], "box", p)
@@ -225,7 +225,7 @@ def test_fluid_dam_with_moving_paddle_matches_oracle(oracle, cuda_lib):
 @pytest.mark.parametrize("use_graph", [True, False], ids=["graph", "stream"])
 def test_set_and_clear_between_substeps(oracle, cuda_lib, use_graph):
     scene = scenes.small_cube(v0=(0.3, -1.5, 0.2))
-    osim = cob.build_oracle(scene)
+    osim = scenes.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene, use_graph=use_graph)
     osim.step(10)
     esim.step(10)
@@ -281,7 +281,7 @@ def test_mgsp_two_ranks_sticky_floor_match_single_domain(oracle, cuda_lib):
     from claymore_b200 import mgsp
     scene = scenes.small_cube(v0=(1.0, -10.0, 0.5))
     dt_default = 1e-3
-    osim = cob.build_oracle(scene, dt=dt_default)
+    osim = scenes.build_oracle(ob, scene, dt=dt_default, sim_class=cob.ColliderOracleSim)
     p = _params("sticky", 0.3, "static")
     sdf, grad = _fields(scene["domain_bits"], "floor")
     osim.set_collider(_fill(cob.Collider(), p), sdf, grad)

@@ -1,5 +1,5 @@
 """GPU tests of the analytic collision objects (DESIGN.md section 2.9): the sm_90a grid update against the float64 reference
-(objects_ref) per node and against the CPU oracle (tests/oracle_objects), the objects entry with no objects against the existing
+(ref64) per node and against the CPU oracle (oracle/collider_oracle.c), the objects entry with no objects against the existing
 entries bit for bit, and the step driver and the MGSP predictors against the oracle with test_gpu_collider's bounds.
 
 Kernel bounds: per node |v - ref| <= 1e-5 (1 + |v_ref|) (the device's sinf / cosf and FMA contraction), nodes near one of the
@@ -13,9 +13,8 @@ import pytest
 import threading
 
 import collider_oracle_binding as cob
-import objects_oracle_binding as oob
-import objects_ref
 import oracle_binding as ob
+import ref64
 import scenes as ts
 import test_gpu_collider as tgc
 from claymore_b200 import _capi, levelset, objects, scenes
@@ -89,7 +88,8 @@ def _run(cuda_lib, keys, g, dt, objs, t, col=None, entry="objects"):
 def _check(cuda_lib, grid, objs, t, dt=1e-3):
     keys, g = grid
     eg, emx = _run(cuda_lib, keys, g, dt, objs, t)
-    ref, near, _, _ = objects_ref.grid_update(Config(domain_bits=DOMAIN_BITS), keys, g, dt, objs, t)
+    ref, _, _, info = ref64.grid_update(Config(domain_bits=DOMAIN_BITS), keys, g, dt, None, t, objects=objs)
+    near = info["near"]
     has = g[:, 0] >= np.finfo(np.float32).tiny
     ok = has & ~near
     err = np.abs(eg[:, 1:] - ref).max(1)
@@ -149,7 +149,8 @@ def test_no_objects_is_the_existing_entry_bit_for_bit(cuda_lib, grid):
     obj = objects.box((0.3, 0.28, 0.33), (0.68, 0.61, 0.7), type="sticky")
     c, _ = _run(cuda_lib, keys, g, 1e-3, [obj], 0.37, col=col, entry="objects")
     d, _ = _run(cuda_lib, keys, g, 1e-3, [obj], 0.37, entry="objects")
-    ref, near, _, _ = objects_ref.grid_update(cfg, keys, g, 1e-3, [obj], 0.37)
+    ref, _, _, info = ref64.grid_update(cfg, keys, g, 1e-3, None, np.float32(0.37), objects=[obj])
+    near = info["near"]
     hit = (ref == 0).all(1) & (g[:, 0] > 0) & ~near
     assert hit.sum() > 1000
     assert np.array_equal(c[:, 1:][np.broadcast_to(hit[:, None], ref.shape)], d[:, 1:][np.broadcast_to(hit[:, None], ref.shape)])
@@ -204,9 +205,9 @@ def test_kernel_matches_oracle(oracle, cuda_lib, grid, case, collider, t):
     part = ob.Partition()
     part.active_keys = keys.ctypes.data
     omv = np.zeros(1, np.float32)
-    arr = oob.unit_planes(objs)
-    oob.lib().orc_update_grid_velocity_query_max_objects(C.byref(ocfg), len(keys), ob.ptr(og), part, 1e-3, C.byref(ocol) if collider else None, arr, len(objs),
-                                                         np.float32(t), ob.ptr(omv))
+    arr = cob.unit_planes(objs)
+    cob.lib().orc_update_grid_velocity_query_max_boundaries(C.byref(ocfg), len(keys), ob.ptr(og), part, 1e-3, C.byref(ocol) if collider else None, arr, len(objs),
+                                                            np.float32(t), ob.ptr(omv))
     eg, emx = _run(cuda_lib, keys, g, 1e-3, objs, np.float32(t), col=ecol if collider else None)
     og = og.reshape(g.shape)
     scale = np.abs(og[:, 1:]).max()
@@ -262,7 +263,7 @@ def _sticky_floor_dt_scene():
 @pytest.mark.parametrize("material", [scenes.FIXED_COROTATED, scenes.J_FLUID, scenes.SAND, scenes.NACC])
 def test_cube_on_analytic_floor_matches_oracle(oracle, cuda_lib, material, typ, use_graph):
     scene = scenes.small_cube(material=material, v0=(0.3, -1.5, 0.2))
-    osim = oob.build_oracle(scene)
+    osim = ts.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene, use_graph=use_graph)
     _set_both(osim, esim, [objects.box(*FLOOR, type=typ, friction=0.3)])
     for k in range(4):
@@ -276,7 +277,7 @@ def test_cube_on_analytic_floor_matches_oracle(oracle, cuda_lib, material, typ, 
 @pytest.mark.timeout(600)
 def test_fluid_in_five_planes_matches_oracle(oracle, cuda_lib):
     scene = scenes.small_cube(material=scenes.J_FLUID, lo=18, hi=34, v0=(0.8, -1.0, -0.6))
-    osim = oob.build_oracle(scene)
+    osim = ts.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene)
     walls = [objects.plane((0.5, 0.27, 0.5), (0, 1, 0), type="slip", friction=0.0),
              objects.plane((0.27, 0.5, 0.5), (1, 0, 0), type="separate", friction=0.2),
@@ -294,7 +295,7 @@ def test_fluid_in_five_planes_matches_oracle(oracle, cuda_lib):
 @pytest.mark.timeout(600)
 def test_fluid_with_moving_cylinder_paddle_matches_oracle(oracle, cuda_lib):
     scene = scenes.small_cube(material=scenes.J_FLUID, lo=18, hi=34, v0=(0.0, 0.0, 0.0))
-    osim = oob.build_oracle(scene)
+    osim = ts.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene)
     paddle = objects.cylinder((0.26, 0.4, 0.40), 0.04, 0.2, type="slip", friction=0.0, trans_vel=(1.5, 0.0, 0.0), omega=(0.0, 0.5, 0.0), trans=(0.26, 0.4, 0.4))
     _set_both(osim, esim, [paddle])
@@ -309,7 +310,7 @@ def test_fluid_with_moving_cylinder_paddle_matches_oracle(oracle, cuda_lib):
 @pytest.mark.parametrize("use_graph", [True, False], ids=["graph", "stream"])
 def test_levelset_collider_with_two_objects_matches_oracle(oracle, cuda_lib, use_graph):
     scene = scenes.small_cube(v0=(0.3, -1.5, 0.2))
-    osim = oob.build_oracle(scene)
+    osim = ts.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene, use_graph=use_graph)
     p = tgc._params("slip", 0.3, "trans_vel")
     tgc._set_both(osim, esim, scene["domain_bits"], "sphere", p)
@@ -326,7 +327,7 @@ def test_levelset_collider_with_two_objects_matches_oracle(oracle, cuda_lib, use
 @pytest.mark.parametrize("use_graph", [True, False], ids=["graph", "stream"])
 def test_set_and_clear_between_substeps(oracle, cuda_lib, use_graph):
     scene = scenes.small_cube(v0=(0.3, -1.5, 0.2))
-    osim = oob.build_oracle(scene)
+    osim = ts.build_oracle(ob, scene, sim_class=cob.ColliderOracleSim)
     esim = scenes.build_engine(scene, use_graph=use_graph)
     osim.step(10)
     esim.step(10)
@@ -358,7 +359,7 @@ def test_emission_with_objects_matches_oracle(oracle, cuda_lib, use_graph):
     esim.set_collision_objects(floor)
     esim.add_particles(0, extra, (0.0, -1.0, 0.0))
     both = dict(scene, models=[dict(scene["models"][0], pos=np.concatenate([scene["models"][0]["pos"], extra]))])
-    osim = oob.build_oracle(both)
+    osim = ts.build_oracle(ob, both, sim_class=cob.ColliderOracleSim)
     osim.set_collision_objects(floor)
     for k in range(4):
         osim.step(10)
@@ -376,7 +377,7 @@ def test_mgsp_two_ranks_analytic_sticky_floor_match_single_domain(oracle, cuda_l
     from claymore_b200 import mgsp
     scene = _sticky_floor_dt_scene()
     dt_default = 1e-3
-    osim = oob.build_oracle(scene, dt=dt_default)
+    osim = ts.build_oracle(ob, scene, dt=dt_default, sim_class=cob.ColliderOracleSim)
     # the floor rises at 6 m/s under the falling cube: a sticky object's velocity (2 trans_vel, 12 m/s) exceeds the cube's, so the
     # predicted max, and so dt, is wrong wherever a predictor leaves the objects out
     floor = [objects.box((0.15, 0.15, 0.15), (0.85, 0.33, 0.85), type="sticky", friction=0.3, trans_vel=(0.0, 6.0, 0.0)),

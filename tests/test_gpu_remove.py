@@ -11,7 +11,6 @@ import os
 import numpy as np
 import pytest
 
-import objects_ref as OR
 import ref64
 import ref64_cases as S
 from claymore_b200 import bgeo, checkpoint, objects
@@ -36,26 +35,16 @@ def _odd_cube(material, v0=(0.3, -1.0, 0.2)):
     return S._case(6, [S.model(material, S.box(DX, (20, 20, 20), (31, 31, 31)), v0, DX)], [])
 
 
-def _material_space(o, pos, t):
-    """float64 restatement of the kernel's map of positions into object o's material space at time t"""
-    p = OR.params(o)
-    cur = p["rot_mat"].copy()
-    for d in range(3):
-        cur = OR._mat_mul(cur, OR._axis_rot(p["omega"][d] * t, d))
-    xm = np.asarray(pos, np.float64) - (p["trans"] + p["trans_vel"] * t)
-    x0 = xm / (1.0 + p["dsdt"] * t)
-    return (x0 @ cur.reshape(3, 3).T) * p["scale"] + p["trans"], p
-
-
-def _expected_removed(regions, pos, t, outside, tol=1e-5):
-    """(removed[n], near[n]) of the union of the regions by the float64 reference; `near` rows lie within tol of a surface"""
+def _expected_removed(regions, pos, t, outside):
+    """(removed[n], near[n]) of the union of the regions by the float64 reference; `near` rows lie within ref64's rounding
+    margin of a surface"""
     hit = np.zeros(len(pos), bool)
     near = np.zeros(len(pos), bool)
     for o in regions:
-        x, p = _material_space(o, pos, t)
-        h, _, nr = OR.query(p, x, tol)
-        hit |= h
-        near |= nr
+        p = ref64.object_params(o)
+        q = ref64.object_query(p, ref64.material_point(None, p, t, points=pos)["x"])
+        hit |= q["hit"]
+        near |= q["margin"] <= ref64.NEAR
     return (~hit if outside else hit), near
 
 

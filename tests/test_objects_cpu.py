@@ -1,5 +1,5 @@
 """CPU tests of the analytic collision objects (DESIGN.md section 2.9): the C ABI's struct and exports, the Python constructors'
-and the scene parser's validation, and the float64 reference (objects_ref) against the level-set collider's fields."""
+and the scene parser's validation, and the float64 reference (ref64.object_query) against the level-set collider's fields."""
 import ctypes as C
 import os
 import re
@@ -9,7 +9,7 @@ import subprocess
 import numpy as np
 import pytest
 
-import objects_ref
+import ref64
 from claymore_b200 import _capi, levelset, objects, scene
 from claymore_b200._capi import Config
 
@@ -137,6 +137,23 @@ def test_scene_placement_conventions():
 
 
 # ---- the reference against the level-set collider's fields ---------------------------------------------------------------------
+def _surface_gap(p, x):
+    """float64 distances at the material-space points x[n, 3] of the box, sphere or plane p (ref64.object_params): |phi| to the
+    surface, and inside the shape the gap to its nearest normal switch (a box's face tie or centre, a sphere's centre)"""
+    sw = np.full(len(x), np.inf)
+    if p["shape"] == ref64.PLANE:
+        return np.abs((x - p["a"]) @ p["b"]), sw
+    if p["shape"] == ref64.BOX:
+        ql, qh = p["a"] - x, x - p["b"]
+        q = np.maximum(ql, qh)
+        srt, i, axis = np.sort(q, 1), np.arange(len(x)), np.argmax(q, 1)
+        phi, sw = srt[:, 2], np.minimum(srt[:, 2] - srt[:, 1], np.abs(ql[i, axis] - qh[i, axis]))
+    else:
+        sw = np.sqrt(((x - p["a"]) ** 2).sum(1))
+        phi = sw - p["b"][0]
+    return np.abs(phi), np.where(phi <= 0, sw, np.inf)
+
+
 @pytest.mark.parametrize("shape", ["box", "sphere", "plane"])
 @pytest.mark.parametrize("typ", [0, 1, 2])
 def test_reference_matches_levelset_fields(shape, typ):
@@ -151,8 +168,11 @@ def test_reference_matches_levelset_fields(shape, typ):
     else:
         o, (sdf, grad) = objects.plane((0.5, 0.55, 0.5), (0.3, -1.0, 0.2), type=typ), levelset.plane(cfg, (0.5, 0.55, 0.5), (0.3, -1.0, 0.2))
     nodes = np.stack(np.meshgrid(*[np.arange(N)] * 3, indexing="ij"), -1).reshape(-1, 3)
-    p = objects_ref.params(o)
-    hit, n, near = objects_ref.query(p, nodes * dx, 1e-6)
+    p = ref64.object_params(o)
+    x = nodes * dx
+    q = ref64.object_query(p, (x, np.zeros_like(x)))
+    hit, n = q["hit"], q["on"]
+    near = np.minimum(*_surface_gap(p, x)) <= 1e-6
     d = sdf.reshape(-1)
     g = grad.reshape(3, -1).T
     keep = ~near & (np.abs(d) > 1e-5)
@@ -163,7 +183,7 @@ def test_reference_matches_levelset_fields(shape, typ):
     assert np.allclose(n[inside], g[inside], atol=1e-6)
     rng = np.random.default_rng(typ)
     v = rng.normal(0, 1, (len(nodes), 3))
-    out, _ = objects_ref.resolve(p, nodes, dx, 0.0, v)
+    out = ref64.object_resolve(cfg, p, 0.0, nodes, v, np.abs(v))["v"]
     assert np.array_equal(out[keep & ~hit], v[keep & ~hit])
     if typ == 0:
         assert (out[inside] == 0).all()
@@ -176,7 +196,6 @@ def test_velocity_matches_dense_collider_reference(shape, typ, t):
     """Velocities through both paths: an analytic object and the float64 reference of the level-set collider (ref64.collider_resolve)
     on the field levelset makes for the same shape, with the same moving parameters, agree at every node that is not near a
     surface, a face tie or the wall band.  This pins the objects' material space and motion to the collider's."""
-    import ref64
     cfg = Config(domain_bits=5, boundary=2)
     N, dx = 4 * cfg.grid_size, cfg.dx
     motion = dict(trans_vel=(0.05, -0.04, 0.03))
@@ -194,12 +213,14 @@ def test_velocity_matches_dense_collider_reference(shape, typ, t):
     nodes = np.stack(np.meshgrid(*[np.arange(lo, hi)] * 3, indexing="ij"), -1).reshape(-1, 3)
     v = rng.normal(0, 1, (len(nodes), 3))
     r = ref64.collider_resolve(cfg, col, sdf, grad, np.float32(t), nodes, v, np.zeros_like(v))
-    out, near = objects_ref.resolve(objects_ref.params(o), nodes, dx, float(np.float32(t)), v, tol=1e-3 * dx)
+    p = ref64.object_params(o)
+    ro = ref64.object_resolve(cfg, p, np.float32(t), nodes, v, np.zeros_like(v))
+    out, ohit = ro["v"], ro["hit"]
     # the trilinear field is exact only a cell away from the surface and from a box's edges and face ties
     x = nodes * dx - np.float32(t) * np.asarray(motion["trans_vel"], np.float32)
-    ohit, _, far = objects_ref.query(objects_ref.params(o), x, 1.5 * dx)
+    far = np.minimum(*_surface_gap(p, x)) <= 1.5 * dx
     band = ((x < (lo + 1) * dx) | (x >= (hi - 1) * dx)).any(1)      # the collider reports no hit in its wall band (C1)
-    keep = ~near & ~r["near"] & ~far & ~band
+    keep = ~ro["near"] & ~r["near"] & ~far & ~band
     if shape == "sphere" and t > 0:   # off the lattice the trilinear gradient of a sphere is not its normal: compare the hit test only
         assert np.array_equal(ohit[keep], r["hit"][keep])
         return

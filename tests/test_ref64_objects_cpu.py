@@ -1,10 +1,10 @@
 """The analytic collision objects against the float64 reference (ref64.object_chain), per node, per sub-step and in the dt.
 
-Kernel level: orc_update_grid_velocity_query_max_objects on synthetic grids (blocks around each object's surface and centre,
+Kernel level: orc_update_grid_velocity_query_max_boundaries on synthetic grids (blocks around each object's surface and centre,
 masses log-uniform from 1e-12 to 1 with zero and subnormal nodes, velocities N(0, 2) m/s) over 4 shapes x 3 types x friction
 {0, 0.3, -0.2} x {static, combined motion} x t {0, 0.37, 3.1} x boundary {2, 0}, plus the 16-object list and the level-set
 collider with two objects.  Per node: |v - ref64| <= COLLIDER_VEL_KAPPA 2^-24 E, nodes near a discontinuity (ref64's margin)
-left out and counted; the max within COLLIDER_MAX_REL of [mx_lo, mx_hi].  Per sub-step: the objects oracle through
+left out and counted; the max within COLLIDER_MAX_REL of [mx_lo, mx_hi].  Per sub-step: the oracle with the objects through
 OBJECT_CASES with COLLIDER_KAPPA.  The kappa values are test_ref64_collider_cpu's: the oracle's worst ratios over this matrix
 stay under them (printed per entry).  The GPU tests (test_gpu_objects_ref64.py) hold the engine to the same values.
 """
@@ -160,7 +160,6 @@ def kernel_matrix(run, ob, entry, boundary, motion, label):
 
 def oracle_kernel(ob):
     import collider_oracle_binding as cob
-    import objects_oracle_binding as oob
 
     def run(cfg, keys, grid, dt, spec, objs, t):
         col = None
@@ -174,8 +173,8 @@ def oracle_kernel(ob):
         part = ob.Partition()
         part.active_keys = k.ctypes.data
         mv = np.zeros(1, np.float32)
-        oob.lib().orc_update_grid_velocity_query_max_objects(C.byref(cfg), len(keys), ob.ptr(g), part, dt, C.byref(col) if col is not None else None,
-                                                             oob.unit_planes(objs), len(objs), np.float32(t), ob.ptr(mv))
+        cob.lib().orc_update_grid_velocity_query_max_boundaries(C.byref(cfg), len(keys), ob.ptr(g), part, dt, C.byref(col) if col is not None else None,
+                                                                cob.unit_planes(objs), len(objs), np.float32(t), ob.ptr(mv))
         return g, float(mv[0])
     return run
 
@@ -199,7 +198,7 @@ def test_objects_kernel_reaches_every_branch(oracle):
     assert want <= got, f"branches never reached away from a margin: {sorted(want - got)}"
 
 
-# ---- per sub-step: the objects oracle through OBJECT_CASES ------------------------------------------------------------------
+# ---- per sub-step: the oracle with the objects through OBJECT_CASES --------------------------------------------------------
 @pytest.mark.parametrize("name", list(S.OBJECT_CASES))
 def test_ref64_object_cases_match_oracle(oracle, name):
     oracle_collider_check(oracle, S.OBJECT_CASES[name], name)
@@ -245,32 +244,3 @@ def test_object_cases_act():
             assert (top & (info["branch"] == "sticky")).any(), "a node at 4G - 1 must be resolved"
         osim.close()
 
-
-# ---- the two float64 restatements of the shapes agree -------------------------------------------------------------------------
-@pytest.mark.parametrize("motion", list(MOTIONS))
-@pytest.mark.parametrize("shape", list(SHAPES))
-def test_ref64_objects_match_objects_ref(shape, motion):
-    """ref64.object_resolve and objects_ref.resolve (the float64 restatement test_gpu_objects and test_gpu_remove use) agree to
-    1e-12 on a few thousand random nodes per shape, motion, t, type and friction wherever neither reports the node near."""
-    import objects_ref
-    from claymore_b200._capi import Config
-    cfg = Config(domain_bits=DOMAIN_BITS, boundary=2)
-    rng = np.random.default_rng(11)
-    nodes, v = rng.integers(8, 56, (3000, 3)), rng.normal(0, 2, (3000, 3))
-    dx = 1.0 / (1 << DOMAIN_BITS)
-    hits = 0
-    for t in TIMES:
-        for typ in TYPES:
-            for fr in FRICTIONS:
-                o = make(*SHAPES[shape], type=typ, friction=fr, **_motion(motion))
-                p = ref64.object_params(o)
-                r = ref64.object_resolve(cfg, p, t, nodes, v, np.abs(v))
-                q = objects_ref.params(o)
-                q["b"] = p["b"]                                        # the stored (renormalised) plane normal
-                w, near = objects_ref.resolve(q, nodes, dx, float(np.float32(t)), v)
-                keep = ~near & ~r["near"]
-                assert keep.mean() > 0.95
-                err = np.abs(w - r["v"])[keep]
-                assert err.max() <= 1e-12 * (1 + np.abs(w[keep]).max()), (t, typ, fr, float(err.max()))
-                hits += int((r["hit"] & keep).sum())
-    assert hits > 1000
