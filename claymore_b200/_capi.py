@@ -77,6 +77,8 @@ class Collider(C.Structure):
 
 SHAPE_PLANE, SHAPE_BOX, SHAPE_SPHERE, SHAPE_CYLINDER = 0, 1, 2, 3   # CB200_SHAPE_*
 MAX_COLLISION_OBJECTS = 16                                           # CB200_MAX_COLLISION_OBJECTS
+SHAPE_LEVELSET = 4                                                   # CB200_SHAPE_LEVELSET
+MAX_COLLISION_LEVELSETS = 16                                         # CB200_MAX_COLLISION_LEVELSETS
 
 
 class CollisionObject(C.Structure):
@@ -120,6 +122,11 @@ class SdfHeader(C.Structure):
     _fields_ = [("ni", C.c_int), ("nj", C.c_int), ("nk", C.c_int), ("min", C.c_float * 3), ("h", C.c_float)]
 
 
+class LevelSetLattice(C.Structure):
+    """cb200_levelset: a prepared level-set lattice on the device (float4 per node) and its node counts."""
+    _fields_ = [("lattice", C.c_void_p), ("ni", C.c_int), ("nj", C.c_int), ("nk", C.c_int)]
+
+
 class SdfSampling(C.Structure):
     """cb200_sdf_sampling: how a level set becomes particles (mode, placement, density, Philox key)."""
     _fields_ = [("mode", C.c_int), ("ppc", C.c_int), ("offset", C.c_double * 3), ("span", C.c_double * 3), ("seed", C.c_ulonglong)]
@@ -148,6 +155,9 @@ _SIGNATURES = {
     "cb200_update_grid_velocity_query_max": [_CFG, _I, _P, Partition, _F, _P, _P],
     "cb200_update_grid_velocity_query_max_collider": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), _F, _P, _P],
     "cb200_update_grid_velocity_query_max_objects": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), C.POINTER(CollisionObject), _I, _F, _P, _P],
+    "cb200_update_grid_velocity_query_max_levelsets": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), C.POINTER(CollisionObject), _I,
+                                                       C.POINTER(LevelSetLattice), _I, _F, _P, _P],
+    "cb200_levelset_prepare": [C.POINTER(SdfHeader), _P, _P, _P],
     "cb200_clear_grid": [_I, _P, _P],
     "cb200_cell_bucket_to_block": [_CFG, _I, _P, _P, _P, _P, _P],
     "cb200_mark_active_grid_blocks": [_I, _P, _P, _P],
@@ -194,6 +204,8 @@ _SIGNATURES = {
     "cb200_sim_set_collider": [_P, C.POINTER(Collider), _P],
     "cb200_sim_clear_collider": [_P],
     "cb200_sim_set_collision_objects": [_P, C.POINTER(CollisionObject), _I],
+    "cb200_sim_add_collision_levelset": [_P, C.POINTER(SdfHeader), _P, C.POINTER(_I)],
+    "cb200_sim_clear_collision_levelsets": [_P],
     "cb200_sim_time": [_P, C.POINTER(C.c_double)],
     "cb200_sim_mgsp_inbox": [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_size_t)],
     "cb200_sim_mgsp_ipc_handle": [_P, _P],

@@ -4,6 +4,7 @@
 #include "g2p2g.cuh"
 #include "grid.cuh"
 #include "init.cuh"
+#include "levelset.cuh"
 #include "partition.cuh"
 
 using namespace cb200;
@@ -119,11 +120,21 @@ int cb200_g2p2g(const cb200_config* c, float dt, float new_dt, int pbc, cb200_pa
 	return (int) launch_g2p2g(cur.material, a, pbc, (cudaStream_t) stream);
 }
 
-// The three kernel-level grid updates: the level set when collider is non-null (valid, with a field), then objs[0, n), placed at time
-static int update_grid_boundaries(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream) {
+// The four kernel-level grid updates: the level set when collider is non-null (valid, with a field), then objs[0, n), placed at time;
+// level-set objects index lattices[0, n_lattices)
+static int update_grid_boundaries(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream,
+                                  const cb200_levelset* lattices = nullptr, int n_lattices = 0) {
 	CB_CFG(c);
+	if(n_lattices < 0 || n_lattices > CB200_MAX_COLLISION_LEVELSETS || (n_lattices > 0 && !lattices)) return (int) cudaErrorInvalidValue;
+	LevelSets ls {};
+	ls.count = n_lattices;
+	for(int i = 0; i < n_lattices; ++i) {
+		const cb200_levelset& l = lattices[i];
+		if(!l.lattice || l.ni < 2 || l.nj < 2 || l.nk < 2 || (long long) l.ni * l.nj * l.nk >= (1LL << 31)) return (int) cudaErrorInvalidValue;
+		ls.v[i] = l;
+	}
 	Boundaries bd {};
-	if(!objects_prepare(objs, n, bd.objects)) return (int) cudaErrorInvalidValue;
+	if(!objects_prepare(objs, n, bd.objects, n_lattices)) return (int) cudaErrorInvalidValue;
 	if(collider) {
 		if(!collider_valid(collider) || !collider->sdf) return (int) cudaErrorInvalidValue;
 		bd.has_collider = true;
@@ -142,7 +153,7 @@ static int update_grid_boundaries(const cb200_config* c, int block_count, float*
 	a.clear_grid = nullptr;
 	a.n_clear = 0;
 	a.time = time;
-	launch_grid_update(a, bd, grid_for(block_count, kGridThreads / 32), (cudaStream_t) stream);
+	launch_grid_update(a, bd, ls, grid_for(block_count, kGridThreads / 32), (cudaStream_t) stream);
 	return (int) cudaGetLastError();
 }
 
@@ -157,6 +168,15 @@ int cb200_update_grid_velocity_query_max_collider(const cb200_config* c, int blo
 
 int cb200_update_grid_velocity_query_max_objects(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream) {
 	return update_grid_boundaries(c, block_count, grid, partition, dt, collider, objs, n, time, max_vel, stream);
+}
+
+int cb200_update_grid_velocity_query_max_levelsets(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, float time, float* max_vel, void* stream) {
+	return update_grid_boundaries(c, block_count, grid, partition, dt, collider, objs, n, time, max_vel, stream, levelsets, n_levelsets);
+}
+
+int cb200_levelset_prepare(const cb200_sdf_header* header, const float* phi, float* lattice, void* stream) {
+	if(!levelset_dims_valid(header) || !phi || !lattice) return (int) cudaErrorInvalidValue;
+	return (int) launch_levelset_prepare(*header, phi, lattice, (cudaStream_t) stream);
 }
 
 int cb200_clear_grid(int block_count, float* grid, void* stream) {

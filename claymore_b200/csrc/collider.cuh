@@ -196,14 +196,16 @@ inline bool finite_all(const float* v, int n) {
 }
 // checks every entry of objs[0, n) and copies them into out, the plane normals made unit length in double; false (out
 // unchanged) on an unknown shape or type, scale 0, a non-finite value, a zero plane normal, lo > hi, a radius or half height
-// <= 0, or n outside [0, CB200_MAX_COLLISION_OBJECTS]
-inline bool objects_prepare(const cb200_collision_object* objs, int n, ObjectList& out) {
+// <= 0, or n outside [0, CB200_MAX_COLLISION_OBJECTS].  CB200_SHAPE_LEVELSET is known only with levelsets > 0 registered lattices:
+// its spacing b[0] must be > 0 and its index b[1] an exact integer in [0, levelsets)
+inline bool objects_prepare(const cb200_collision_object* objs, int n, ObjectList& out, int levelsets = 0) {
 	if(n < 0 || n > CB200_MAX_COLLISION_OBJECTS || (n > 0 && !objs)) return false;
 	ObjectList l {};
 	l.n = n;
+	const int last_shape = levelsets > 0 ? (int) CB200_SHAPE_LEVELSET : (int) CB200_SHAPE_CYLINDER;
 	for(int i = 0; i < n; ++i) {
 		cb200_collision_object o = objs[i];
-		if(o.shape < CB200_SHAPE_PLANE || o.shape > CB200_SHAPE_CYLINDER || o.type < CB200_STICKY || o.type > CB200_SEPARATE || o.scale == 0.f) return false;
+		if(o.shape < CB200_SHAPE_PLANE || o.shape > last_shape || o.type < CB200_STICKY || o.type > CB200_SEPARATE || o.scale == 0.f) return false;
 		if(!finite_all(&o.friction, 1) || !finite_all(o.a, 3) || !finite_all(o.b, 3) || !finite_all(o.rot_mat, 9) || !finite_all(o.trans, 3) ||
 		   !finite_all(o.trans_vel, 3) || !finite_all(o.omega, 3) || !finite_all(&o.dsdt, 1) || !finite_all(&o.scale, 1))
 			return false;
@@ -213,6 +215,8 @@ inline bool objects_prepare(const cb200_collision_object* objs, int n, ObjectLis
 			for(int d = 0; d < 3; ++d) o.b[d] = (float) (o.b[d] / len);
 		} else if(o.shape == CB200_SHAPE_BOX) {
 			if(o.a[0] > o.b[0] || o.a[1] > o.b[1] || o.a[2] > o.b[2]) return false;
+		} else if(o.shape == CB200_SHAPE_LEVELSET) {
+			if(!(o.b[0] > 0.f) || !(o.b[1] >= 0.f) || o.b[1] >= (float) levelsets || o.b[1] != std::floor(o.b[1])) return false;
 		} else if(!(o.b[0] > 0.f) || (o.shape == CB200_SHAPE_CYLINDER && !(o.b[1] > 0.f))) {
 			return false;
 		}
@@ -278,6 +282,73 @@ __device__ __forceinline__ bool object_query(const cb200_collision_object& o, co
 	return true;
 }
 
+// ---- level-set collision objects (DESIGN.md section 2.11) ---------------------------------------------------------------------
+using LevelSetView = cb200_levelset;  // POD: device lattice (float4 per node: phi, g_i, g_j, g_k; i fastest) + its node counts
+// The registered lattices a kernel may query: a kernel parameter of its own beside Boundaries, so that Boundaries and every instance
+// without level sets keep their parameter block.
+struct LevelSets {
+	int count;
+	LevelSetView v[CB200_MAX_COLLISION_LEVELSETS];
+};
+// the CTA's copy of the views, indexed by an object's b[1]
+__device__ __forceinline__ LevelSetView* levelset_views() {
+	__shared__ LevelSetView s[CB200_MAX_COLLISION_LEVELSETS];
+	return s;
+}
+// thread k copies view k (static indices: the views may sit in a by-value kernel parameter); the caller's next barrier publishes them
+__device__ __forceinline__ void levelset_views_cta(const LevelSets& ls) {
+#pragma unroll
+	for(int k = 0; k < CB200_MAX_COLLISION_LEVELSETS; ++k)
+		if((int) threadIdx.x == k && k < ls.count) levelset_views()[k] = ls.v[k];
+}
+
+// hit test (phi <= 0) and material-space normal of the level-set object o (a: node 0, b[0]: spacing c) on its lattice l at the
+// material-space point x: trilinear in the corner order of collider_query, no hit outside the node box
+__device__ __forceinline__ bool levelset_query(const LevelSetView& l, const cb200_collision_object& o, const float* x, float* n) {
+	const int dims[3] = {l.ni, l.nj, l.nk};
+	int i0[3];
+	float w1[3][2];
+	n[0] = n[1] = n[2] = 0.f;
+#pragma unroll
+	for(int d = 0; d < 3; ++d) {
+		const float q = (x[d] - o.a[d]) / o.b[0];  // a true division, as collider_query divides by dx
+		if(!(q >= 0.f && q <= (float) (dims[d] - 1))) return false;
+		i0[d] = min((int) floorf(q), dims[d] - 2);
+		const float t = q - (float) i0[d];
+		w1[d][0] = 1.f - t;
+		w1[d][1] = t;
+	}
+	const float4* node = reinterpret_cast<const float4*>(l.lattice) + ((size_t) i0[2] * l.nj + i0[1]) * l.ni + i0[0];
+	const size_t sj = (size_t) l.ni, sk = (size_t) l.ni * l.nj;
+	float sd = 0.f;
+#pragma unroll
+	for(int i = 0; i < 2; ++i)
+#pragma unroll
+		for(int j = 0; j < 2; ++j)
+#pragma unroll
+			for(int k = 0; k < 2; ++k) {
+				const float w = w1[0][i] * w1[1][j] * w1[2][k];
+				const float4 p = __ldg(node + i + j * sj + k * sk);
+				sd += w * p.x;
+				n[0] += w * p.y;
+				n[1] += w * p.z;
+				n[2] += w * p.w;
+			}
+	const float nn = n[0] * n[0] + n[1] * n[1] + n[2] * n[2];
+	if(nn > 0.f) {
+		const float len = sqrtf(nn);
+		n[0] /= len;
+		n[1] /= len;
+		n[2] /= len;
+	}
+	return sd <= 0.f;
+}
+// object_query with CB200_SHAPE_LEVELSET answered by the lattice levelset_views_cta copied for index b[1]
+__device__ __forceinline__ bool object_query_levelsets(const cb200_collision_object& o, const float* x, float* n) {
+	if(o.shape == CB200_SHAPE_LEVELSET) return levelset_query(levelset_views()[(int) o.b[1]], o, x, n);
+	return object_query(o, x, n);
+}
+
 // ---- the boundary chain -------------------------------------------------------------------------------------------------------
 // The solid boundaries of a simulator, applied in this order: the level-set collider (has_collider), then the analytic objects in
 // list order, each resolving the velocity the previous one left.  Passed by value as a kernel parameter of its own beside the argument
@@ -316,35 +387,40 @@ __device__ __forceinline__ const BoundaryFrames& boundary_frames_cta(const Bound
 	__syncthreads();
 	return s;
 }
-// the chain at grid node (nx, ny, nz), its frames s built by boundary_frames_cta
-template<bool COLLIDE, bool OBJECTS>
+// the chain at grid node (nx, ny, nz), its frames s built by boundary_frames_cta; LEVELSETS (implies OBJECTS): level-set objects are
+// answered from the views levelset_views_cta copied
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
 __device__ __forceinline__ void boundaries_resolve(const Boundaries& b, const BoundaryFrames& s, const Cfg& cfg, int nx, int ny, int nz, float& vx, float& vy, float& vz) {
+	static_assert(OBJECTS || !LEVELSETS, "level-set objects are objects");
 	if constexpr(COLLIDE) collider_resolve(b.col, s.col, cfg.dx, nx, ny, nz, vx, vy, vz, [&](const float* x, float* n) { return collider_query(b.col, cfg, x, n); });
 	if constexpr(OBJECTS) {
 		for(int i = 0; i < b.objects.n; ++i) {
 			const cb200_collision_object& o = s.o[i];
-			collider_resolve(o, s.f[i], cfg.dx, nx, ny, nz, vx, vy, vz, [&](const float* x, float* n) { return object_query(o, x, n); });
+			collider_resolve(o, s.f[i], cfg.dx, nx, ny, nz, vx, vy, vz, [&](const float* x, float* n) {
+				if constexpr(LEVELSETS) return object_query_levelsets(o, x, n);
+				else return object_query(o, x, n);
+			});
 		}
 	}
 }
 
 // grid-update velocity of one cell (wall mask, gravity on y, the chain) and its |v|^2, NaN -> +inf; no mass -> 0
-template<bool COLLIDE, bool OBJECTS>
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
 __device__ __forceinline__ float cell_vel_sq_boundaries(float m, float p0, float p1, float p2, bool wx, bool wy, bool wz, float gdt, const Boundaries& bd, const BoundaryFrames& s, const Cfg& cfg, int nx, int ny, int nz) {
 	if(!node_has_mass(m)) return 0.f;
 	const float mi = 1.f / m;
 	float a = wx ? 0.f : p0 * mi, b = (wy ? 0.f : p1 * mi) + gdt, d = wz ? 0.f : p2 * mi;
-	boundaries_resolve<COLLIDE, OBJECTS>(bd, s, cfg, nx, ny, nz, a, b, d);
+	boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(bd, s, cfg, nx, ny, nz, a, b, d);
 	const float sq = a * a + b * b + d * d;
 	return isnan(sq) ? INFINITY : sq;
 }
 // cell_pair_vel_sq (common.cuh) with the chain: the two cells lane holds of block (kx, ky, kz), whose grid block is s2 (float2 view)
-template<bool COLLIDE, bool OBJECTS>
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
 __device__ __forceinline__ float cell_pair_vel_sq_boundaries(const Cfg& cfg, const Boundaries& bd, const BoundaryFrames& s, const float2* s2, int lane, int kx, int ky, int kz, bool wx, bool wy, bool wz, float gdt) {
 	const float2 m = s2[lane], p0 = s2[32 + lane], p1 = s2[64 + lane], p2 = s2[96 + lane];
 	const int nx = 4 * kx + (lane >> 3), ny = 4 * ky + ((lane >> 1) & 3), nz = 4 * kz + 2 * (lane & 1);
-	return fmaxf(cell_vel_sq_boundaries<COLLIDE, OBJECTS>(m.x, p0.x, p1.x, p2.x, wx, wy, wz, gdt, bd, s, cfg, nx, ny, nz),
-	             cell_vel_sq_boundaries<COLLIDE, OBJECTS>(m.y, p0.y, p1.y, p2.y, wx, wy, wz, gdt, bd, s, cfg, nx, ny, nz + 1));
+	return fmaxf(cell_vel_sq_boundaries<COLLIDE, OBJECTS, LEVELSETS>(m.x, p0.x, p1.x, p2.x, wx, wy, wz, gdt, bd, s, cfg, nx, ny, nz),
+	             cell_vel_sq_boundaries<COLLIDE, OBJECTS, LEVELSETS>(m.y, p0.y, p1.y, p2.y, wx, wy, wz, gdt, bd, s, cfg, nx, ny, nz + 1));
 }
 
 }  // namespace cb200

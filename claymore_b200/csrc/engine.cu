@@ -31,6 +31,7 @@
 #include "g2p2g.cuh"
 #include "grid.cuh"
 #include "init.cuh"
+#include "levelset.cuh"
 #include "mgsp.cuh"
 #include "output.cuh"
 #include "partition.cuh"
@@ -379,6 +380,8 @@ struct cb200_sim {
 	// objects (cb200_sim_set_collision_objects) resolved after it in list order
 	Boundaries boundaries {};
 	float* sdf = nullptr;
+	// the lattices of the level-set collision objects (cb200_sim_add_collision_levelset), owned by this simulator, in registry order
+	LevelSets levelsets {};
 	long long frames_done = 0;  // frames finished by cb200_sim_advance_frame (restored from a checkpoint)
 	// the rows each particle block starts at in every read-out, per model: the scans of the bucket sizes, [kMaxModels][max_blocks + 1]
 	int* ck_base = nullptr;
@@ -599,7 +602,7 @@ int enqueue_grid_update(cb200_sim* s, int R) {
 	}
 	gu.n_clear = (int) s->models.size();
 	for(size_t m = 0; m < s->models.size(); ++m) gu.clear_counts[m] = s->models[m].pb[Rn].cell_particle_counts;
-	launch_grid_update(gu, s->boundaries, grid_blocks(4), s->stream);  // placed at StepState::sim_time, the start of this sub-step
+	launch_grid_update(gu, s->boundaries, s->levelsets, grid_blocks(4), s->stream);  // placed at StepState::sim_time, the start of this sub-step
 	++s->launches;
 	return (int) cudaGetLastError();
 }
@@ -722,7 +725,7 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 		a.new_grid = s->grid[0];
 		a.next_max_vel = mgsp ? &scr->local_max : nullptr;
 		// MGSP: the boundaries, so that the predicted max is the one the next grid update finds; a single domain predicts nothing
-		launch_carry_grid(a, mgsp ? s->boundaries : Boundaries {}, grid_blocks(4), st);
+		launch_carry_grid(a, mgsp ? s->boundaries : Boundaries {}, s->levelsets, grid_blocks(4), st);
 		++s->launches;
 	}
 	if(mgsp) {
@@ -851,6 +854,13 @@ void preload_kernels() {
 		preload(grid_update_boundary_kernel<C, O>);
 		preload(carry_grid_boundary_kernel<C, O>);
 		preload(grid_max_boundary_kernel<C, O>);
+	});
+	for_each_boundary_instance([](auto C, auto O) {
+		if constexpr(O) {
+			preload(grid_update_levelset_kernel<C>);
+			preload(carry_grid_levelset_kernel<C>);
+			preload(grid_max_levelset_kernel<C>);
+		}
 	});
 	preload(scan_kernel);
 	preload(summary_kernel);
@@ -1092,6 +1102,7 @@ int cb200_sim_destroy(cb200_sim* s) {
 	g_pool.release(s->inbox_local);
 	g_pool.release(s->mgsp_sync);
 	g_pool.release(s->sdf);
+	for(int i = 0; i < s->levelsets.count; ++i) g_pool.release(const_cast<float*>(s->levelsets.v[i].lattice));
 	g_pinned.put(s->h_state);
 	g_pinned.put(s->h_poll);
 	if(s->poll_event) cudaEventDestroy(s->poll_event);
@@ -1305,7 +1316,7 @@ static int setup_impl(cb200_sim* s, const StartSrc& src) {
 	CK(push_state(s));
 	if(mgsp) {
 		// global max |v|^2 of the start grid (later sub-steps get it from the end-of-step exchange of the previous one)
-		launch_grid_max(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->boundaries, grid_blocks(2), st);
+		launch_grid_max(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->boundaries, s->levelsets, grid_blocks(2), st);
 		mgsp_allreduce_maxvel_kernel<<<1, 32, 0, st>>>(mgsp_view(s), &s->d_state->max_vel_sq);
 		s->launches += 2;
 	}
@@ -1491,9 +1502,40 @@ int cb200_sim_clear_collider(cb200_sim* s) {
 }
 int cb200_sim_set_collision_objects(cb200_sim* s, const cb200_collision_object* objs, int n) {
 	ObjectList l;
-	if(!s || !objects_prepare(objs, n, l)) return (int) cudaErrorInvalidValue;
+	if(!s || !objects_prepare(objs, n, l, s->levelsets.count)) return (int) cudaErrorInvalidValue;
 	CK(cudaStreamSynchronize(s->stream));
 	s->boundaries.objects = l;
+	return recapture(s);
+}
+// phi is uploaded into scratch, the lattice built from it on the device; the registry takes the lattice only once it is complete
+int cb200_sim_add_collision_levelset(cb200_sim* s, const cb200_sdf_header* header, const float* phi_host, int* id) {
+	if(!s || !levelset_dims_valid(header) || !std::isfinite(header->h) || !(header->h > 0.f) || !phi_host || s->levelsets.count >= CB200_MAX_COLLISION_LEVELSETS)
+		return (int) cudaErrorInvalidValue;
+	CK(cudaStreamSynchronize(s->stream));
+	const size_t nodes = (size_t) header->ni * header->nj * header->nk;
+	float* phi = nullptr;
+	float* lattice = nullptr;
+	cudaError_t e = pool_alloc(&phi, nodes * sizeof(float));
+	if(e == cudaSuccess) e = pool_alloc(&lattice, nodes * 4 * sizeof(float));
+	if(e == cudaSuccess) e = cudaMemcpyAsync(phi, phi_host, nodes * sizeof(float), cudaMemcpyHostToDevice, s->stream);
+	if(e == cudaSuccess) e = launch_levelset_prepare(*header, phi, lattice, s->stream);
+	if(e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
+	g_pool.release(phi);
+	if(e != cudaSuccess) {
+		g_pool.release(lattice);
+		return (int) e;
+	}
+	s->launches += 1;
+	const int k = s->levelsets.count++;
+	s->levelsets.v[k] = cb200_levelset {lattice, header->ni, header->nj, header->nk};
+	if(id) *id = k;
+	return recapture(s);
+}
+int cb200_sim_clear_collision_levelsets(cb200_sim* s) {
+	if(!s || has_levelset_objects(s->boundaries)) return (int) cudaErrorInvalidValue;
+	CK(cudaStreamSynchronize(s->stream));
+	for(int i = 0; i < s->levelsets.count; ++i) g_pool.release(const_cast<float*>(s->levelsets.v[i].lattice));
+	s->levelsets = LevelSets {};
 	return recapture(s);
 }
 int cb200_sim_time(cb200_sim* s, double* time) {
@@ -2251,12 +2293,18 @@ int cb200_sim_remove_particles(cb200_sim* s, unsigned model_mask, const cb200_co
 	CK(remove_precheck(s, removed));
 	RemoveRegions sel {};
 	const int nm = (int) s->models.size();
-	if(!model_mask || (model_mask >> nm) || (flags & ~CB200_REMOVE_OUTSIDE) || !objects_prepare(regions, n, sel.b.objects)) return (int) cudaErrorInvalidValue;
+	if(!model_mask || (model_mask >> nm) || (flags & ~CB200_REMOVE_OUTSIDE) || !objects_prepare(regions, n, sel.b.objects, s->levelsets.count)) return (int) cudaErrorInvalidValue;
 	if(n == 0) return 0;
 	CK(cudaStreamSynchronize(s->stream));
 	CK(pull_state(s));
 	sel.t = (float) s->h_state->sim_time;
 	sel.outside = (flags & CB200_REMOVE_OUTSIDE) ? 1 : 0;
+	if(has_levelset_objects(sel.b)) {
+		RemoveRegionsLevelsets lsel {};
+		static_cast<RemoveRegions&>(lsel) = sel;
+		lsel.ls = s->levelsets;
+		return remove_impl(s, model_mask, lsel, nullptr, 0, removed);
+	}
 	return remove_impl(s, model_mask, sel, nullptr, 0, removed);
 }
 

@@ -34,7 +34,7 @@ constexpr int kBoundaryMinCtas = OBJECTS ? 2 : 4;
 // COLLIDE / OBJECTS: the MGSP form with a Boundary (mgmpm_kernels.cuh:323-399): after gravity, cells with mass resolve against the
 // boundary chain of `bd` (collider.cuh: the SignedDistanceGrid, then the analytic objects of DESIGN.md section 2.9); the max is |v|^2
 // where that kernel reports 2|v|^2 (Appendix B #11).
-template<bool COLLIDE, bool OBJECTS>
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
 __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const Boundaries* bd) {
 	__shared__ unsigned s_max[kGridThreads / 32];
 	const BoundaryFrames* fr = nullptr;
@@ -62,7 +62,7 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 				v0.x = wx ? 0.f : v0.x * mi;
 				v1.x = (wy ? 0.f : v1.x * mi) + gdt;
 				v2.x = wz ? 0.f : v2.x * mi;
-				if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
+				if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
 				sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
 			}
 			if(hy) {
@@ -70,7 +70,7 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 				v0.y = wx ? 0.f : v0.y * mi;
 				v1.y = (wy ? 0.f : v1.y * mi) + gdt;
 				v2.y = wz ? 0.f : v2.y * mi;
-				if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
+				if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
 				sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
 			}
 			if(hx || hy) {
@@ -108,6 +108,13 @@ __global__ void __launch_bounds__(kGridThreads, (kBoundaryMinCtas<COLLIDE, OBJEC
 	grid_update_body<COLLIDE, OBJECTS>(a, &bd);
 }
 static_assert(sizeof(GridUpdateArgs) + sizeof(Boundaries) <= 4096, "the boundary grid update's parameters must fit the 4 KiB kernel-parameter limit");
+// the same with level-set objects among bd's objects, their lattices in ls (DESIGN.md section 2.11); COLLIDE: bd.has_collider
+template<bool COLLIDE>
+__global__ void __launch_bounds__(kGridThreads, (kBoundaryMinCtas<COLLIDE, true>)) grid_update_levelset_kernel(const GridUpdateArgs a, const __grid_constant__ Boundaries bd, const __grid_constant__ LevelSets ls) {
+	levelset_views_cta(ls);  // published by the frame builder's barrier
+	grid_update_body<COLLIDE, true, true>(a, &bd);
+}
+static_assert(sizeof(GridUpdateArgs) + sizeof(Boundaries) + sizeof(LevelSets) <= 4096, "the level-set grid update's parameters must fit the 4 KiB kernel-parameter limit");
 
 // clear_grid (mgmpm_kernels.cuh:106-115)
 __global__ void clear_grid_kernel(int block_count, float* grid) {
@@ -138,7 +145,7 @@ struct CarryArgs {
 	int* overlap_marks;
 };
 // COLLIDE / OBJECTS (MGSP): the predictor applies the boundaries of bd at the time the next grid update sees
-template<bool COLLIDE, bool OBJECTS>
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
 __device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Boundaries* bd) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int n = *a.new_count;
@@ -165,7 +172,7 @@ __device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Bounda
 			if(a.next_max_vel) {
 				const float2* s2 = reinterpret_cast<const float2*>(s);
 				const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
-				if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS>(a.cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+				if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS, LEVELSETS>(a.cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
 				else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 			}
 		} else {
@@ -184,9 +191,15 @@ __global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, OBJECTS>)) car
 	carry_grid_body<COLLIDE, OBJECTS>(a, &bd);
 }
 static_assert(sizeof(CarryArgs) + sizeof(Boundaries) <= 4096, "the boundary carry's parameters must fit the 4 KiB kernel-parameter limit");
+template<bool COLLIDE>
+__global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, true>)) carry_grid_levelset_kernel(const CarryArgs a, const __grid_constant__ Boundaries bd, const __grid_constant__ LevelSets ls) {
+	levelset_views_cta(ls);
+	carry_grid_body<COLLIDE, true, true>(a, &bd);
+}
+static_assert(sizeof(CarryArgs) + sizeof(Boundaries) + sizeof(LevelSets) <= 4096, "the level-set carry's parameters must fit the 4 KiB kernel-parameter limit");
 
 // max |v|^2 the grid update will find, without touching the grid (MGSP start-up)
-template<bool COLLIDE, bool OBJECTS>
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
 __device__ __forceinline__ void grid_max_body(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries* bd) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int g = cfg.gsize, bc = cfg.boundary;
@@ -198,7 +211,7 @@ __device__ __forceinline__ void grid_max_body(const Cfg& cfg, const StepState* s
 		const int kx = keys[3 * b], ky = keys[3 * b + 1], kz = keys[3 * b + 2];
 		const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
 		const float2* s2 = reinterpret_cast<const float2*>(grid + (size_t) b * kGridBlockFloats);
-		if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS>(cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+		if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS, LEVELSETS>(cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
 		else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 	}
 	vmax = __reduce_max_sync(0xffffffffu, vmax);
@@ -211,42 +224,60 @@ template<bool COLLIDE, bool OBJECTS>
 __global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, OBJECTS>)) grid_max_boundary_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const __grid_constant__ Boundaries bd) {
 	grid_max_body<COLLIDE, OBJECTS>(cfg, state, grid, keys, max_vel, &bd);
 }
+template<bool COLLIDE>
+__global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, true>)) grid_max_levelset_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const __grid_constant__ Boundaries bd, const __grid_constant__ LevelSets ls) {
+	levelset_views_cta(ls);
+	grid_max_body<COLLIDE, true, true>(cfg, state, grid, keys, max_vel, &bd);
+}
 
 // ---- launching the three boundary passes ---------------------------------------------------------------------------------------
-// Calls f(COLLIDE, OBJECTS), two std::bool_constant, with the instance flags that apply bd: the level set when bd.has_collider, the
-// objects when the list is non-empty; neither is the plain kernel.  Each pass keeps all four instances, because the level-set-only
-// one fits 4 CTAs per SM and the level set + objects one does not.
+inline bool has_levelset_objects(const Boundaries& bd) {
+	for(int i = 0; i < bd.objects.n; ++i)
+		if(bd.objects.o[i].shape == CB200_SHAPE_LEVELSET) return true;
+	return false;
+}
+// Calls f(COLLIDE, OBJECTS, LEVELSETS), three std::bool_constant, with the instance flags that apply bd: the level set when
+// bd.has_collider, the objects when the list is non-empty, the level-set instances (OBJECTS too) only when an object is a level set;
+// none is the plain kernel.  Each pass keeps all four instances without level sets, because the level-set-only one fits 4 CTAs per SM
+// and the level set + objects one does not.
 template<class F>
 void with_boundaries(const Boundaries& bd, F&& f) {
 	using T = std::true_type;
 	using N = std::false_type;
-	if(bd.has_collider && bd.objects.n > 0) f(T(), T());
-	else if(bd.has_collider) f(T(), N());
-	else if(bd.objects.n > 0) f(N(), T());
-	else f(N(), N());
+	if(has_levelset_objects(bd)) {
+		if(bd.has_collider) f(T(), T(), T());
+		else f(N(), T(), T());
+	} else if(bd.has_collider && bd.objects.n > 0) f(T(), T(), N());
+	else if(bd.has_collider) f(T(), N(), N());
+	else if(bd.objects.n > 0) f(N(), T(), N());
+	else f(N(), N(), N());
 }
-// f(COLLIDE, OBJECTS) for each boundary instance
+// f(COLLIDE, OBJECTS) for each boundary instance without level sets
 template<class F>
 void for_each_boundary_instance(F&& f) {
 	f(std::true_type(), std::false_type());
 	f(std::false_type(), std::true_type());
 	f(std::true_type(), std::true_type());
 }
-inline void launch_grid_update(const GridUpdateArgs& a, const Boundaries& bd, int ctas, cudaStream_t st) {
-	with_boundaries(bd, [&](auto C, auto O) {
-		if constexpr(C || O) grid_update_boundary_kernel<C, O><<<ctas, kGridThreads, 0, st>>>(a, bd);
+// ls: the lattices bd's level-set objects index (read only when one is)
+inline void launch_grid_update(const GridUpdateArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st) {
+	with_boundaries(bd, [&](auto C, auto O, auto L) {
+		if constexpr(L) grid_update_levelset_kernel<C><<<ctas, kGridThreads, 0, st>>>(a, bd, ls);
+		else if constexpr(C || O) grid_update_boundary_kernel<C, O><<<ctas, kGridThreads, 0, st>>>(a, bd);
 		else grid_update_kernel<<<ctas, kGridThreads, 0, st>>>(a);
 	});
 }
-inline void launch_carry_grid(const CarryArgs& a, const Boundaries& bd, int ctas, cudaStream_t st) {
-	with_boundaries(bd, [&](auto C, auto O) {
-		if constexpr(C || O) carry_grid_boundary_kernel<C, O><<<ctas, 256, 0, st>>>(a, bd);
+inline void launch_carry_grid(const CarryArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st) {
+	with_boundaries(bd, [&](auto C, auto O, auto L) {
+		if constexpr(L) carry_grid_levelset_kernel<C><<<ctas, 256, 0, st>>>(a, bd, ls);
+		else if constexpr(C || O) carry_grid_boundary_kernel<C, O><<<ctas, 256, 0, st>>>(a, bd);
 		else carry_grid_kernel<<<ctas, 256, 0, st>>>(a);
 	});
 }
-inline void launch_grid_max(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries& bd, int ctas, cudaStream_t st) {
-	with_boundaries(bd, [&](auto C, auto O) {
-		if constexpr(C || O) grid_max_boundary_kernel<C, O><<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel, bd);
+inline void launch_grid_max(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st) {
+	with_boundaries(bd, [&](auto C, auto O, auto L) {
+		if constexpr(L) grid_max_levelset_kernel<C><<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel, bd, ls);
+		else if constexpr(C || O) grid_max_boundary_kernel<C, O><<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel, bd);
 		else grid_max_kernel<<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel);
 	});
 }

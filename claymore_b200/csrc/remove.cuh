@@ -29,19 +29,33 @@ struct RemoveRegions : RemoveRows {
 	float t;
 	int outside;
 	__device__ __forceinline__ void prepare() const { boundary_frames_cta<false, true>(b, t); }
-	__device__ __forceinline__ bool eval(long long i, Row& row) const {
+	// LEVELSETS: level-set objects answered from the views levelset_views_cta copied
+	template<bool LEVELSETS = false>
+	__device__ __forceinline__ bool select(long long i, Row& row) const {
 		const BoundaryFrames& s = boundary_frames();
 		const float p[3] = {__ldg(in + i * C), __ldg(in + i * C + 1), __ldg(in + i * C + 2)};
 		bool hit = false;
 		for(int k = 0; k < b.objects.n; ++k) {
 			float xm[3], x[3], n[3];
 			collider_material_point(s.o[k], s.f[k], p, xm, x);
-			hit |= object_query(s.o[k], x, n);
+			if constexpr(LEVELSETS) hit |= object_query_levelsets(s.o[k], x, n);
+			else hit |= object_query(s.o[k], x, n);
 		}
 		row = i;
 		return hit == (outside != 0);
 	}
+	__device__ __forceinline__ bool eval(long long i, Row& row) const { return select(i, row); }
 };
+// the same with level-set objects among the regions, their lattices in ls (DESIGN.md section 2.11)
+struct RemoveRegionsLevelsets : RemoveRegions {
+	LevelSets ls;
+	__device__ __forceinline__ void prepare() const {
+		levelset_views_cta(ls);  // published by the frame builder's barrier
+		RemoveRegions::prepare();
+	}
+	__device__ __forceinline__ bool eval(long long i, Row& row) const { return select<true>(i, row); }
+};
+static_assert(sizeof(RemoveRegionsLevelsets) + sizeof(SdfScan) <= 4096, "the level-set sink selection's parameters must fit the 4 KiB kernel-parameter limit");
 
 // by mask: a row is removed when its byte is non-zero
 struct RemoveMask : RemoveRows {

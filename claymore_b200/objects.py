@@ -5,13 +5,16 @@ for a static object, so a shape is placed in world coordinates at t = 0 and move
 motion parameters would.  The keyword arguments and their defaults are GmpmSimulator.set_collider's:
 type ("sticky" / "slip" / "separate" or CB200_*), friction, trans, trans_vel, omega, rot (3x3, row i, column j = rot_mat(i, j)),
 scale, dsdt.
+
+objects.levelset places an SDFGen level set (claymore_b200.sdf.LevelSet) as an obstacle (DESIGN.md section 2.11): the simulator
+registers its lattice on first use and writes the registry index into the object it passes on.
 """
 import math
 
 import numpy as np
 
-from ._capi import (MAX_COLLISION_OBJECTS, SEPARATE, SHAPE_BOX, SHAPE_CYLINDER, SHAPE_PLANE, SHAPE_SPHERE, SLIP, STICKY,
-                    CollisionObject)
+from ._capi import (MAX_COLLISION_LEVELSETS, MAX_COLLISION_OBJECTS, SEPARATE, SHAPE_BOX, SHAPE_CYLINDER, SHAPE_LEVELSET, SHAPE_PLANE,
+                    SHAPE_SPHERE, SLIP, STICKY, CollisionObject)
 
 BOUNDARY_TYPES = {"sticky": STICKY, "slip": SLIP, "separate": SEPARATE}
 SHAPES = {"plane": SHAPE_PLANE, "box": SHAPE_BOX, "sphere": SHAPE_SPHERE, "cylinder": SHAPE_CYLINDER}
@@ -66,10 +69,24 @@ def cylinder(centre, radius, half_height, **motion):
     return _make(SHAPE_CYLINDER, _vec(centre, what="centre"), [float(radius), float(half_height), 0.0], **motion)
 
 
-def validate(o):
+def levelset(ls, offset, span, **motion):
+    """The level set `ls` (claymore_b200.sdf.LevelSet) as an obstacle fitted into [offset, offset + span] with the sampler's uniform
+    fit (sdf.node_box): node (0, 0, 0) at offset, node spacing its cell size.  Solid where phi <= 0.  The box may extend past the
+    domain.  b[1], the registry index, is written by GmpmSimulator when it registers `ls`."""
+    from . import sdf
+    if not min(sdf._vec3(span)) > 0:
+        raise ValueError(f"span {sdf._vec3(span)} must be positive")
+    c, lo, _ = sdf.node_box(ls, offset, span)
+    o = _make(SHAPE_LEVELSET, lo, [c, 0.0, 0.0], **motion)
+    o.levelset = ls
+    return o
+
+
+def validate(o, levelsets=MAX_COLLISION_LEVELSETS):
     """The checks of cb200_sim_set_collision_objects, as ValueError: unknown shape or type, scale 0, a non-finite value, a zero
-    plane normal, lo > hi, a radius or half height <= 0."""
-    if o.shape not in SHAPES.values():
+    plane normal, lo > hi, a radius or half height <= 0, a level set's spacing <= 0 or an index that is not an integer in
+    [0, levelsets) (the registry's size)."""
+    if o.shape not in SHAPES.values() and o.shape != SHAPE_LEVELSET:
         raise ValueError(f"unknown shape {o.shape}")
     if o.type not in BOUNDARY_TYPES.values():
         raise ValueError(f"unknown boundary type {o.type}")
@@ -86,14 +103,19 @@ def validate(o):
         raise ValueError(f"a radius must be positive, not {o.b[0]}")
     if o.shape == SHAPE_CYLINDER and not o.b[1] > 0:
         raise ValueError(f"a half height must be positive, not {o.b[1]}")
+    if o.shape == SHAPE_LEVELSET:
+        if not o.b[0] > 0:
+            raise ValueError(f"a level set's node spacing must be positive, not {o.b[0]}")
+        if not (o.b[1] == int(o.b[1]) and 0 <= o.b[1] < levelsets):
+            raise ValueError(f"a level set's index must be an integer in [0, {levelsets}), not {o.b[1]}")
     return o
 
 
-def array(objs):
-    """ctypes array of the validated objects (at most MAX_COLLISION_OBJECTS)."""
+def array(objs, levelsets=MAX_COLLISION_LEVELSETS):
+    """ctypes array of the validated objects (at most MAX_COLLISION_OBJECTS; level-set indices below `levelsets`)."""
     objs = list(objs)
     if len(objs) > MAX_COLLISION_OBJECTS:
         raise ValueError(f"at most {MAX_COLLISION_OBJECTS} collision objects, not {len(objs)}")
     for o in objs:
-        validate(o)
+        validate(o, levelsets)
     return (CollisionObject * max(len(objs), 1))(*objs)

@@ -18,7 +18,9 @@ Projects/MGSP/mgsp_benchmark.cuh:257-266); "velocity" is its trans_vel.
 
 Analytic collision objects (claymore_b200.objects, DESIGN.md section 2.9), resolved after the collider in list order, at most
 CB200_MAX_COLLISION_OBJECTS.  Box, sphere and plane are placed as the collider's are; a "cylinder" fills [offset, offset + span]
-with its axis along y and radius min(span_x, span_z) / 2.  Unknown keys or shapes, too many entries or a bad value raise
+with its axis along y and radius min(span_x, span_z) / 2.  {"shape": "levelset", "file": "<name>.sdf"} is an SDFGen level set fitted
+into [offset, offset + span] as a model's is (DESIGN.md section 2.11), but it may extend past the domain; each file is read once and
+its lattice registered once per simulator.  Unknown keys or shapes, too many entries, an unreadable file or a bad value raise
 ValueError before any device work; "collider" and "boundaries" may both be present.
 
 The reference only loads `.sdf` level sets (gmpm.cu:152-159).  Here "file": "<name>.sdf" is sampled on the device by
@@ -113,24 +115,45 @@ def _collider(sim, c, cfg, base_dir):
 
 
 BOUNDARY_KEYS = ("shape", "offset", "span", "normal", "type", "friction", "velocity", "omega", "scale", "dsdt")
+LEVELSET_KEYS = ("file",)   # with "shape": "levelset"
 
 
-def _object(b, what, keys):
-    """The collision object of one "boundaries" or "sinks" entry `b` (ValueError naming `what` on a bad entry or a key not in `keys`)."""
+def _obstacle_level_set(b, what, base_dir, cache):
+    """The sdf.LevelSet of a "levelset" entry, read once per path into `cache` (ValueError naming `what` on a bad file)."""
+    f = b.get("file")
+    if not isinstance(f, str) or not f.endswith(".sdf"):
+        raise ValueError(f"{what} (levelset): \"file\" must name an .sdf level set, not {f!r}")
+    path = f if os.path.isabs(f) else os.path.join(base_dir if base_dir is not None else os.getcwd(), f)
+    if path not in cache:
+        try:
+            cache[path] = sdf.read(path)
+        except (OSError, ValueError) as e:
+            raise ValueError(f"{what} (levelset): {f}: {e}") from None
+    return cache[path]
+
+
+def _object(b, what, keys, base_dir=None, cache=None):
+    """The collision object of one "boundaries" or "sinks" entry `b` (ValueError naming `what` on a bad entry or a key not in `keys`).
+    A "levelset" entry's file is read through `cache` ({path: LevelSet}), so that one file is one level set."""
     from . import objects
     if not isinstance(b, dict):
         raise ValueError(f"{what} must be an object with keys {', '.join(keys)}")
+    shape = b.get("shape")
+    if shape == "levelset":
+        keys = tuple(keys) + LEVELSET_KEYS
     unknown = sorted(set(b) - set(keys))
     if unknown:
         raise ValueError(f"{what}: unknown keys {unknown} (known: {', '.join(keys)})")
-    shape = b.get("shape")
-    if shape not in objects.SHAPES:
-        raise ValueError(f"{what}: unknown shape {shape!r} (known: {', '.join(objects.SHAPES)})")
+    if shape not in objects.SHAPES and shape != "levelset":
+        raise ValueError(f"{what}: unknown shape {shape!r} (known: {', '.join(objects.SHAPES)}, levelset)")
     try:
         offset = np.asarray(b.get("offset", [0, 0, 0]), dtype=np.float64).reshape(3)
         span = np.asarray(b.get("span", [1, 1, 1]), dtype=np.float64).reshape(3)
         motion = dict(type=b.get("type", "sticky"), friction=float(b.get("friction", 0.3)), trans_vel=b.get("velocity", [0, 0, 0]),
                       omega=b.get("omega", [0, 0, 0]), scale=float(b.get("scale", 1.0)), dsdt=float(b.get("dsdt", 0.0)))
+        if shape == "levelset":
+            ls = _obstacle_level_set(b, what, base_dir, {} if cache is None else cache)
+            return objects.levelset(ls, offset, span, **motion)
         if shape == "box":
             return objects.box(offset, offset + span, **motion)
         if shape == "sphere":
@@ -142,24 +165,25 @@ def _object(b, what, keys):
         raise ValueError(f"{what} ({shape}): {e}") from None
 
 
-def boundaries(doc):
-    """The scene's "boundaries" as validated collision objects (ValueError on a bad entry), before any device work."""
+def boundaries(doc, base_dir=None, cache=None):
+    """The scene's "boundaries" as validated collision objects (ValueError on a bad entry), before any device work.  Level-set files
+    are relative to base_dir (default: the working directory) and read through `cache` ({path: LevelSet})."""
     from . import objects
     bs = doc.get("boundaries", [])
     if not isinstance(bs, list):
         raise ValueError("\"boundaries\" must be a list of objects")
     if len(bs) > objects.MAX_COLLISION_OBJECTS:
         raise ValueError(f"at most {objects.MAX_COLLISION_OBJECTS} \"boundaries\", not {len(bs)}")
-    return [_object(b, f"boundary {i}", BOUNDARY_KEYS) for i, b in enumerate(bs)]
+    return [_object(b, f"boundary {i}", BOUNDARY_KEYS, base_dir, cache) for i, b in enumerate(bs)]
 
 
 SINK_KEYS = ("shape", "offset", "span", "normal", "velocity", "omega", "scale", "dsdt", "models", "outside", "start", "every", "until")
 
 
-def sinks(doc):
+def sinks(doc, base_dir=None, cache=None):
     """The scene's validated "sinks": [{"object", "models" (sorted tuple of scene model indices), "outside", "frames" (list)}], in
     document order (ValueError on a bad entry, or on more than CB200_MAX_COLLISION_OBJECTS sinks due in one group), before any
-    device work."""
+    device work.  base_dir and cache: as for boundaries."""
     from . import objects
     frames = doc.get("simulation", {}).get("frames", GmpmSimulator.DEFAULT_FRAMES)
     n_models = len([m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES])
@@ -169,7 +193,7 @@ def sinks(doc):
     out = []
     for i, e in enumerate(ss):
         what = f"sink {i}"
-        o = _object(e, what, SINK_KEYS)
+        o = _object(e, what, SINK_KEYS, base_dir, cache)
         models = e.get("models", list(range(n_models)))
         if not isinstance(models, list) or not models:
             raise ValueError(f"{what}: \"models\" must be a non-empty list of model indices, not {models!r}")
@@ -211,16 +235,16 @@ def _sink_groups(specs, after=0):
     return dict(sorted(out.items()))
 
 
-def sink_schedule(doc, after=0):
+def sink_schedule(doc, after=0, base_dir=None, cache=None):
     """{frame: [(models, outside, [sink indices]), ...]}: the removal calls of every frame > `after` (a resumed run's checkpoint
     frame), one per group of sinks due together with the same models and outside, in document order.  Validates "sinks"."""
-    return {f: [(m, o, idx) for (m, o), idx in g.items()] for f, g in _sink_groups(sinks(doc), after).items()}
+    return {f: [(m, o, idx) for (m, o), idx in g.items()] for f, g in _sink_groups(sinks(doc, base_dir, cache), after).items()}
 
 
-def _sink_hook(doc, after=0):
+def _sink_hook(doc, after=0, base_dir=None, cache=None):
     """main_loop's per-frame hook that applies the scene's sinks (None without any), built before any device work."""
-    specs = sinks(doc)
-    todo = sink_schedule(doc, after)
+    specs = sinks(doc, base_dir, cache)
+    todo = sink_schedule(doc, after, base_dir, cache)
     if not todo:
         return None
 
@@ -336,11 +360,12 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
     if doc.get("sinks") and sim_kwargs.get("mgsp_world", 1) > 1:
         raise ValueError("\"sinks\" are not supported in MGSP mode")
     models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
-    objs = boundaries(doc)
+    obstacles = {}   # {path: LevelSet} of the "levelset" boundaries and sinks: one registration per file
+    objs = boundaries(doc, base, obstacles)
     if resume is not None:
         inf = _check_resume(doc, cfg, resume)
         emitters = _emitters(doc, cfg, base, _level_sets(models, base))
-        sink = _sink_hook(doc, inf["frames"])
+        sink = _sink_hook(doc, inf["frames"], base, obstacles)
         sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                             frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max(max_blocks, inf["max_blocks"]), **sim_kwargs)
         if "collider" in doc:
@@ -354,7 +379,7 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
         if model.get("constitutive") not in CONSTITUTIVE:
             raise ValueError(f"unknown constitutive model {model.get('constitutive')!r}")
     level_sets = _level_sets(models, base)
-    sink = _sink_hook(doc)
+    sink = _sink_hook(doc, 0, base, obstacles)
     emitters = _emitters(doc, cfg, base, level_sets)
     sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                         frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max_blocks, **sim_kwargs)

@@ -11,8 +11,8 @@ import os
 import numpy as np
 
 from . import _capi
-from ._capi import (CHANNELS, ERROR_OUTPUT_IO, OUTPUT_J, OUTPUT_V, SEPARATE, SLIP, STICKY, Collider, Config, SimDesc, SimStats, check,
-                    lib)
+from ._capi import (CHANNELS, ERROR_OUTPUT_IO, OUTPUT_J, OUTPUT_V, SEPARATE, SLIP, STICKY, CollisionObject, Collider, Config, SimDesc,
+                    SimStats, check, lib)
 
 BOUNDARY_TYPES = {"sticky": STICKY, "slip": SLIP, "separate": SEPARATE}
 OUTPUT_ATTRIBUTES = {"v": OUTPUT_V, "J": OUTPUT_J}
@@ -43,6 +43,7 @@ class GmpmSimulator:
         self.restored = False
         self.emitters = []   # fn(sim, frame): called by main_loop at the start of each frame, before its sub-steps
         self._output_paths = []   # files of the frame being written (for the error of wait_output)
+        self._levelsets = []      # the sdf.LevelSet of each registered lattice, in registry order
 
     # ---- lifecycle -------------------------------------------------------------------------------
     def close(self):
@@ -139,7 +140,7 @@ class GmpmSimulator:
                 raise ValueError(f"unknown model {m!r} (the simulator has {len(self.materials)})")
             mask |= 1 << int(m)
         removed = (C.c_longlong * 8)()
-        check(self.L.cb200_sim_remove_particles(self.h, mask, objects.array(regions), len(regions), _capi.REMOVE_OUTSIDE if outside else 0,
+        check(self.L.cb200_sim_remove_particles(self.h, mask, self._objects_array(regions), len(regions), _capi.REMOVE_OUTSIDE if outside else 0,
                                                 removed), "remove_particles")
         return self._removed(removed)
 
@@ -255,12 +256,45 @@ class GmpmSimulator:
     def set_collision_objects(self, objs):
         """Replaces the analytic collision objects by `objs` (claymore_b200.objects.plane / box / sphere / cylinder; [] clears them).
         From the next sub-step on the grid update resolves the level-set collider, then these in list order (synchronises)."""
-        from . import objects
         objs = list(objs)
-        check(self.L.cb200_sim_set_collision_objects(self.h, objects.array(objs), len(objs)), "set_collision_objects")
+        check(self.L.cb200_sim_set_collision_objects(self.h, self._objects_array(objs), len(objs)), "set_collision_objects")
 
     def clear_collision_objects(self):
         check(self.L.cb200_sim_set_collision_objects(self.h, None, 0), "clear_collision_objects")
+
+    # ---- level-set collision objects (claymore_b200.objects.levelset, DESIGN.md section 2.11) -------------------------------
+    def _objects_array(self, objs):
+        """objects.array of `objs`, each objects.levelset entry with its level set's registry index: every level set not yet
+        registered is registered once (its lattice stays on the device until clear_collision_levelsets or close).  Every object is
+        validated before the first registration."""
+        from . import objects
+        objs = list(objs)
+        objects.array(objs)
+        out = []
+        for o in objs:
+            ls = getattr(o, "levelset", None)
+            if ls is not None:
+                o = CollisionObject.from_buffer_copy(o)
+                o.b[1] = float(self.add_collision_levelset(ls))
+            out.append(o)
+        return objects.array(out, len(self._levelsets))
+
+    def add_collision_levelset(self, ls):
+        """Registry index of the level set `ls` (claymore_b200.sdf.LevelSet), registering it on first use (synchronises)."""
+        for i, r in enumerate(self._levelsets):
+            if r is ls:
+                return i
+        phi = np.ascontiguousarray(ls.phi, dtype=np.float32)
+        idx = C.c_int(-1)
+        check(self.L.cb200_sim_add_collision_levelset(self.h, C.byref(ls.header), phi.ctypes.data_as(C.c_void_p), C.byref(idx)),
+              "add_collision_levelset")
+        self._levelsets.append(ls)
+        return idx.value
+
+    def clear_collision_levelsets(self):
+        """Frees every registered level set; refused (CB200Error) while a set collision object is a level set."""
+        check(self.L.cb200_sim_clear_collision_levelsets(self.h), "clear_collision_levelsets")
+        self._levelsets = []
 
     def sim_time(self):
         """Simulated time since initial_setup (sum of the dt of every finished sub-step)."""

@@ -141,6 +141,31 @@ typedef struct cb200_collision_object {
  * for an invalid object (see cb200_sim_set_collision_objects) or collider. */
 CB200_API int cb200_update_grid_velocity_query_max_objects(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream);
 
+/* Level-set collision objects (DESIGN.md section 2.11): CB200_SHAPE_LEVELSET, a level set from an SDFGen `.sdf` file evaluated in the
+ * object's material space, in the same list as the analytic shapes and with their types, friction and motion.  Only the file's lattice
+ * is stored on the device: one float4 per node (phi, g_i, g_j, g_k), SDFGen order (i fastest), g the central difference of phi in
+ * index units, 0.5f * (phi[i+1] - phi[i-1]) in float32, one-sided (phi[1] - phi[0], phi[n-1] - phi[n-2]) on the lattice faces.
+ *   CB200_SHAPE_LEVELSET  a = the material-space position of node (0, 0, 0), b[0] = node spacing c > 0, b[1] = the index of the
+ *                         level set in the simulator's registry (an exact integer in [0, count)); b[2] is ignored.
+ * At the material-space point x: q_d = (x_d - a_d) / c (a true division); outside [0, n_d - 1] on any axis no hit; else
+ * i0 = min(floor(q), n - 2), t = q - i0, and the four channels are interpolated trilinearly (the dense collider's corner order).  Solid
+ * where phi <= 0; normal the interpolated g, normalised only when |g|^2 > 0 (a zero normal acts as for the other shapes).  The wall
+ * band does not apply. */
+enum { CB200_SHAPE_LEVELSET = 4 };
+#define CB200_MAX_COLLISION_LEVELSETS 16
+/* one prepared lattice on the device: lattice = float4[ni nj nk] (as float[4 ni nj nk]) */
+typedef struct cb200_levelset {
+	const float* lattice;
+	int ni, nj, nk;
+} cb200_levelset;
+/* Builds the device lattice (float[4 ni nj nk]) from the DEVICE phi (float[ni nj nk]) of `header`.  cudaErrorInvalidValue for a
+ * dimension below 2, ni nj nk >= 2^31 or a null pointer. */
+struct cb200_sdf_header; /* below, with the .sdf sampler */
+CB200_API int cb200_levelset_prepare(const struct cb200_sdf_header* header, const float* phi, float* lattice, void* stream);
+/* cb200_update_grid_velocity_query_max_objects where objs may hold CB200_SHAPE_LEVELSET entries, whose b[1] indexes
+ * levelsets[0, n_levelsets) (at most CB200_MAX_COLLISION_LEVELSETS prepared lattices). */
+CB200_API int cb200_update_grid_velocity_query_max_levelsets(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, float time, float* max_vel, void* stream);
+
 /* clear_grid  mgmpm_kernels.cuh:106-115 via GridBuffer::reset  grid_buffer.cuh:32-35 */
 CB200_API int cb200_clear_grid(int block_count, float* grid, void* stream);
 
@@ -264,6 +289,14 @@ CB200_API int cb200_sim_clear_collider(cb200_sim* sim);
  * at the simulated time at the start of the sub-step.  Synchronises and re-captures the sub-step graphs; call it between
  * sub-steps.  Objects are scene input: a checkpoint does not store them, set them before cb200_sim_restore. */
 CB200_API int cb200_sim_set_collision_objects(cb200_sim* sim, const cb200_collision_object* objs, int n);
+/* Registers a level set for CB200_SHAPE_LEVELSET objects and sinks: phi_host (ni nj nk floats of `header`) is uploaded, its lattice
+ * prepared on the device (16 B per node, kept until cb200_sim_destroy or cb200_sim_clear_collision_levelsets) and its index written to
+ * *id.  cudaErrorInvalidValue, nothing changed, for a bad header (as cb200_sdf_parse), a null pointer or a full registry
+ * (CB200_MAX_COLLISION_LEVELSETS).  Level sets are scene input, as objects are: register them before cb200_sim_restore.  Both calls
+ * synchronise and re-capture the sub-step graphs. */
+CB200_API int cb200_sim_add_collision_levelset(cb200_sim* sim, const struct cb200_sdf_header* header, const float* phi_host, int* id);
+/* Frees every registered level set; cudaErrorInvalidValue, nothing changed, while a set collision object refers to one. */
+CB200_API int cb200_sim_clear_collision_levelsets(cb200_sim* sim);
 /* simulated time since initial_setup: the sum of the dt of every finished sub-step (synchronises) */
 CB200_API int cb200_sim_time(cb200_sim* sim, double* time);
 /* number of kernels this library launched on behalf of `sim` since creation */
@@ -504,7 +537,8 @@ CB200_API int cb200_sim_add_particles_sdf(cb200_sim* sim, int model, const cb200
  * ---------------------------------------------------------------------------------------------- */
 #define CB200_REMOVE_OUTSIDE 1u  /* remove the particles outside the union of the regions instead of inside it */
 /* Removes, from every model whose bit is set in model_mask, the particles whose position lies in any of regions[0, n): a region is a
- * cb200_collision_object (shape and motion as in section 2.9; type and friction are ignored), placed at the simulated time, and the
+ * cb200_collision_object (shape and motion as in section 2.9, or a registered level set as in section 2.11; type and friction are
+ * ignored), placed at the simulated time, and the
  * point tested is the particle's position mapped into the object's material space as the collider maps a node.  removed[m]
  * (nullable, 8 entries): rows removed from model m. */
 CB200_API int cb200_sim_remove_particles(cb200_sim* sim, unsigned model_mask, const cb200_collision_object* regions, int n,

@@ -12,7 +12,15 @@ run also reports the grid update's kernel time per sub-step from torch.profiler 
 collider or the objects add (free memory before and after they are set).
 
     python tools/collider_bench.py --objects [--steps 50] [--warmup 10] [--rounds 3]
+
+--levelsets compares, in alternating rounds, no collider, the dense level-set floor, the analytic floor box, the same floor as a
+level-set collision object (a box level set on a lattice of node spacing dx, two cells wider than the floor on every side), and a
+dragon-shaped obstacle (two_dragons.sdf's 77 x 118 x 401 nodes, two ellipsoids, at node spacing dx) through the spheres' lower
+halves, with the grid update's kernel time and the device memory each adds, as --objects.
+
+    python tools/collider_bench.py --levelsets [--steps 50] [--warmup 10] [--rounds 3]
 """
+import ctypes as C
 import argparse
 import json
 import os
@@ -48,7 +56,7 @@ def run(scene, field, args, stream, objs=None):
     sim.profile_read()
     sim.profile(False)
     kernel_ms = None
-    if args.objects:
+    if args.objects or args.levelsets:
         from torch.profiler import ProfilerActivity, profile
         sim.sync()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -78,6 +86,39 @@ def object_sets(top):
     return {"analytic_floor": [floor], "objects4": [floor] + extra[:3], "objects16": [floor] + extra}
 
 
+def _level_set(phi, h):
+    """an sdf.LevelSet of phi[k, j, i] with node spacing h"""
+    import numpy as np
+    from claymore_b200 import sdf
+    from claymore_b200._capi import SdfHeader
+    nk, nj, ni = phi.shape
+    return sdf.LevelSet(SdfHeader(ni, nj, nk, (C.c_float * 3)(0, 0, 0), h), np.ascontiguousarray(phi, np.float32).reshape(-1))
+
+
+def levelset_sets(top, dx):
+    """the level-set variants of --levelsets: the floor box as a level-set object, and the dragon-shaped obstacle"""
+    import numpy as np
+    from claymore_b200 import objects
+    lo, hi = np.array([0.1, 0.1, 0.1]), np.array([0.9, top, 0.9])
+    org = lo - 2 * dx
+    n = np.floor((hi + 2 * dx - org) / dx).astype(int) + 1
+    x = (org[0] + dx * np.arange(n[0]))[None, None, :]
+    y = (org[1] + dx * np.arange(n[1]))[None, :, None]
+    z = (org[2] + dx * np.arange(n[2]))[:, None, None]
+    phi = np.maximum(np.maximum(np.maximum(lo[0] - x, x - hi[0]), np.maximum(lo[1] - y, y - hi[1])), np.maximum(lo[2] - z, z - hi[2]))
+    floor = objects.levelset(_level_set(phi, dx), org, (n - 1) * dx, type="sticky")
+    dn = (77, 118, 401)
+    L = [(d - 1) * dx for d in dn]
+    x = (dx * np.arange(dn[0]))[None, None, :]
+    y = (dx * np.arange(dn[1]))[None, :, None]
+    z = (dx * np.arange(dn[2]))[:, None, None]
+    a = np.sqrt(((x - 0.5 * L[0]) / (0.4 * L[0])) ** 2 + ((y - 0.45 * L[1]) / (0.4 * L[1])) ** 2 + ((z - 0.25 * L[2]) / (0.2 * L[2])) ** 2) - 1
+    b = np.sqrt(((x - 0.5 * L[0]) / (0.35 * L[0])) ** 2 + ((y - 0.55 * L[1]) / (0.4 * L[1])) ** 2 + ((z - 0.72 * L[2]) / (0.22 * L[2])) ** 2) - 1
+    dragon = objects.levelset(_level_set(np.minimum(a, b) * min(L) * 0.2, dx), (0.5 - 0.5 * L[0], top - 0.05, 0.5 - 0.5 * L[2]),
+                              [v + 1e-9 for v in L], type="slip", friction=0.3)
+    return {"levelset_floor": [floor], "dragon": [dragon]}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=50)
@@ -85,6 +126,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--dt", type=float, default=1e-4)
     ap.add_argument("--objects", action="store_true", help="also the analytic floor box, 4 and 16 analytic objects")
+    ap.add_argument("--levelsets", action="store_true", help="also the analytic floor box, the floor as a level-set object and a dragon")
     args = ap.parse_args()
 
     import torch
@@ -101,6 +143,8 @@ def main():
     field = levelset.box(Config(domain_bits=scene["domain_bits"]), (0.1, 0.1, 0.1), (0.9, top, 0.9))
     stream = torch.cuda.Stream()
     sets = object_sets(top) if args.objects else {}
+    if args.levelsets:
+        sets = {"analytic_floor": object_sets(top)["analytic_floor"], **levelset_sets(top, 1.0 / (1 << scene["domain_bits"]))}
     names = ["floor", "none"] + sorted(sets)
     for r in range(args.rounds):
         order = names if r % 2 == 0 else names[::-1]
