@@ -7,6 +7,6 @@ It fails loudly when the CUDA library is missing: there is no CPU fallback.
 """
 from ._capi import (CB200Error, Config, ParticleBuffer, Partition, SimDesc, SimStats, J_FLUID, FIXED_COROTATED, SAND, NACC, lib, lib_path, build_library)
 from .simulator import GmpmSimulator
-from . import bgeo, checkpoint, levelset, objects, samplers, scene, scenes, sdf
+from . import bgeo, checkpoint, levelset, mesh, objects, samplers, scene, scenes, sdf
 
-__all__ = ["CB200Error", "Config", "ParticleBuffer", "Partition", "SimDesc", "SimStats", "J_FLUID", "FIXED_COROTATED", "SAND", "NACC", "lib", "lib_path", "build_library", "GmpmSimulator", "bgeo", "checkpoint", "levelset", "objects", "samplers", "scene", "scenes", "sdf"]
+__all__ = ["CB200Error", "Config", "ParticleBuffer", "Partition", "SimDesc", "SimStats", "J_FLUID", "FIXED_COROTATED", "SAND", "NACC", "lib", "lib_path", "build_library", "GmpmSimulator", "bgeo", "checkpoint", "levelset", "mesh", "objects", "samplers", "scene", "scenes", "sdf"]

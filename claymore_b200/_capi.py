@@ -127,6 +127,16 @@ class LevelSetLattice(C.Structure):
     _fields_ = [("lattice", C.c_void_p), ("ni", C.c_int), ("nj", C.c_int), ("nk", C.c_int)]
 
 
+class MeshHeader(C.Structure):
+    """cb200_mesh_header: a parsed mesh's vertex and triangle counts and its vertex bounding box."""
+    _fields_ = [("nv", C.c_int), ("nt", C.c_int), ("min", C.c_float * 3), ("max", C.c_float * 3)]
+
+
+class MeshLevelSetParams(C.Structure):
+    """cb200_mesh_levelset_params: SDFGen's node spacing and padding, and make_level_set3's exact band."""
+    _fields_ = [("h", C.c_float), ("padding", C.c_int), ("exact_band", C.c_int)]
+
+
 class SdfSampling(C.Structure):
     """cb200_sdf_sampling: how a level set becomes particles (mode, placement, density, Philox key)."""
     _fields_ = [("mode", C.c_int), ("ppc", C.c_int), ("offset", C.c_double * 3), ("span", C.c_double * 3), ("seed", C.c_ulonglong)]
@@ -225,6 +235,8 @@ _SIGNATURES = {
     "cb200_sdf_parse": [C.c_char_p, C.c_size_t, C.POINTER(SdfHeader), _P, C.c_size_t],
     "cb200_sample_sdf": [_CFG, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.c_longlong, C.POINTER(C.c_longlong), _P],
     "cb200_sim_init_model_sdf": [_P, _I, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.POINTER(_I), C.POINTER(_I)],
+    "cb200_obj_parse": [C.c_char_p, C.c_size_t, C.POINTER(MeshHeader), _P, _P, C.c_size_t, C.c_size_t],
+    "cb200_mesh_levelset": [_P, _I, _P, _I, C.POINTER(MeshLevelSetParams), C.POINTER(SdfHeader), _P, C.c_size_t, _P],
     "cb200_sim_add_particles": [_P, _I, _P, _I, _P, C.c_uint, C.POINTER(_I)],
     "cb200_sim_add_particles_sdf": [_P, _I, C.POINTER(SdfHeader), _P, C.POINTER(SdfSampling), _P, C.c_uint, C.POINTER(_I)],
     "cb200_sim_remove_particles": [_P, C.c_uint, C.POINTER(CollisionObject), _I, C.c_uint, C.POINTER(C.c_longlong)],

@@ -32,6 +32,7 @@
 #include "grid.cuh"
 #include "init.cuh"
 #include "levelset.cuh"
+#include "mesh.cuh"
 #include "mgsp.cuh"
 #include "output.cuh"
 #include "partition.cuh"
@@ -1979,6 +1980,82 @@ int cb200_sim_init_model_sdf(cb200_sim* s, int material, const cb200_sdf_header*
 	CK(add_model(s, material, (int) r.count, v0, model_id, [&](Model& m) { return r.run_write(m.d_pos); }));
 	if(n_out) *n_out = (int) r.count;
 	return 0;
+}
+
+// ---- level sets from triangle meshes (kernels: mesh.cuh) --------------------------------------------------------------------------
+}  // extern "C"
+namespace {
+// every device buffer of one build, from the pool and back to it
+struct MeshRun {
+	float* x = nullptr;
+	int* tri = nullptr;
+	MeshTri* boxes = nullptr;
+	longlong2* counts = nullptr;  // per triangle (band nodes, crossing columns)
+	longlong2* offs = nullptr;    // [nt + 1] their exclusive prefix
+	longlong2* tile = nullptr;
+	unsigned* done = nullptr;
+	unsigned long long* packed = nullptr;  // per node: phi bits << 32 | closest triangle
+	int* cross = nullptr;                  // per node: crossings in (i - 1, i], then phi
+	~MeshRun() {
+		for(void* p : {(void*) x, (void*) tri, (void*) boxes, (void*) counts, (void*) offs, (void*) tile, (void*) done, (void*) packed, (void*) cross}) g_pool.release(p);
+	}
+};
+
+// one CTA per SM: a plane holds at most a few nodes per thread, and the grid barrier, paid 16 (ni + nj + nk) times, costs more
+// the more CTAs it joins
+int mesh_sweep_grid() { return num_sms(); }
+}  // namespace
+extern "C" {
+
+int cb200_obj_parse(const char* text, size_t bytes, cb200_mesh_header* header, float* vertices, int* triangles, size_t v_capacity, size_t t_capacity) {
+	return obj_parse(text, bytes, header, vertices, triangles, v_capacity, t_capacity);
+}
+
+int cb200_mesh_levelset(const float* vertices, int nv, const int* triangles, int nt, const cb200_mesh_levelset_params* params, cb200_sdf_header* out,
+                        float* phi, size_t capacity, void* stream) {
+	if(!params || !out) return (int) cudaErrorInvalidValue;
+	cb200_sdf_header hdr {};
+	CK(mesh_header(vertices, nv, triangles, nt, *params, hdr));
+	const long long nodes = (long long) hdr.ni * hdr.nj * hdr.nk;
+	if(phi && capacity < (size_t) nodes) return (int) cudaErrorInvalidValue;
+	*out = hdr;
+	if(!phi) return 0;
+	const cudaStream_t st = (cudaStream_t) stream;
+	MeshRun r;
+	const int tiles = (nt + kMeshThreads * kMeshScanPer - 1) / (kMeshThreads * kMeshScanPer);
+	CK(pool_alloc(&r.x, (size_t) nv * 3 * sizeof(float)));
+	CK(pool_alloc(&r.tri, (size_t) nt * 3 * sizeof(int)));
+	CK(pool_alloc(&r.boxes, (size_t) nt * sizeof(MeshTri)));
+	CK(pool_alloc(&r.counts, (size_t) nt * sizeof(longlong2)));
+	CK(pool_alloc(&r.offs, (size_t) (nt + 1) * sizeof(longlong2)));
+	CK(pool_alloc(&r.tile, (size_t) tiles * sizeof(longlong2)));
+	CK(pool_alloc(&r.done, sizeof(unsigned)));
+	CK(pool_alloc(&r.packed, (size_t) nodes * sizeof(unsigned long long)));
+	CK(pool_alloc(&r.cross, (size_t) nodes * sizeof(int)));
+	CK(cudaMemcpyAsync(r.x, vertices, (size_t) nv * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
+	CK(cudaMemcpyAsync(r.tri, triangles, (size_t) nt * 3 * sizeof(int), cudaMemcpyHostToDevice, st));
+	CK(cudaMemsetAsync(r.done, 0, sizeof(unsigned), st));
+	MeshGeom g {r.x, r.tri, nt, hdr.min[0], hdr.min[1], hdr.min[2], hdr.h, hdr.ni, hdr.nj, hdr.nk};
+	// phi.assign((ni+nj+nk)*dx): int times float
+	const float init = (float) (hdr.ni + hdr.nj + hdr.nk) * hdr.h;
+	mesh_init_kernel<<<grid_for(nodes, kMeshThreads), kMeshThreads, 0, st>>>(nodes, mesh_pack(init, -1), r.packed, r.cross);
+	mesh_setup_kernel<<<(nt + kMeshThreads - 1) / kMeshThreads, kMeshThreads, 0, st>>>(g, params->exact_band, r.boxes, r.counts);
+	const MeshScan sc {r.counts, r.offs, r.tile, r.done, nt};
+	mesh_scan_tiles_kernel<<<tiles, kMeshThreads, 0, st>>>(sc);
+	mesh_scan_write_kernel<<<tiles, kMeshThreads, 0, st>>>(sc);
+	CK(cudaGetLastError());
+	longlong2 total {};
+	CK(cudaMemcpyAsync(&total, r.offs + nt, sizeof(longlong2), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	mesh_band_kernel<<<grid_for(total.x, kMeshThreads), kMeshThreads, 0, st>>>(g, r.boxes, r.offs, init, r.packed);
+	if(total.y) mesh_cross_kernel<<<grid_for(total.y, kMeshThreads), kMeshThreads, 0, st>>>(g, r.boxes, r.offs, r.cross);
+	CK(cudaGetLastError());
+	void* args[] = {(void*) &g, (void*) &r.packed};
+	CK(cudaLaunchCooperativeKernel((const void*) mesh_sweep_kernel, mesh_sweep_grid(), kMeshThreads, args, 0, st));
+	mesh_sign_kernel<<<grid_for((long long) hdr.nj * hdr.nk * 32, kMeshThreads), kMeshThreads, 0, st>>>(g, r.packed, r.cross);
+	CK(cudaGetLastError());
+	CK(cudaMemcpyAsync(phi, r.cross, (size_t) nodes * sizeof(float), cudaMemcpyDeviceToHost, st));
+	return (int) cudaStreamSynchronize(st);
 }
 
 // ---- adding particles at a sub-step boundary (kernels: emit.cuh) ----------------------------------------------------------------------

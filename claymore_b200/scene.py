@@ -23,6 +23,12 @@ into [offset, offset + span] as a model's is (DESIGN.md section 2.11), but it ma
 its lattice registered once per simulator.  Unknown keys or shapes, too many entries, an unreadable file or a bad value raise
 ValueError before any device work; "collider" and "boundaries" may both be present.
 
+A "file": "<name>.obj" model, boundary or sink is a Wavefront OBJ triangle mesh turned into a level set on the device
+(claymore_b200.mesh, SDFGen's make_level_set3 bit for bit, DESIGN.md section 2.12) with the optional keys "h" (node spacing in mesh
+units; default: the mesh's longest extent x dx / the longest span, about one simulation cell per level-set cell), "padding" (1) and
+"exact_band" (1); from there it is an `.sdf` level set in every respect.  Each distinct (file, h, padding, exact_band) is built
+once, after every file has been read and every entry validated, and registered once.
+
 The reference only loads `.sdf` level sets (gmpm.cu:152-159).  Here "file": "<name>.sdf" is sampled on the device by
 GmpmSimulator.init_model_sdf with the optional keys "sampler" ("random", the default, or "lattice"), "ppc" (particles per
 simulation cell, default 8: the reference's MODEL_PPC, settings.h:51) and "seed" (default 0); the level set is fitted into
@@ -53,7 +59,7 @@ import os
 
 import numpy as np
 
-from . import levelset, samplers, sdf
+from . import levelset, mesh, samplers, sdf
 from ._capi import Config, FIXED_COROTATED, J_FLUID, NACC, SAND
 from .simulator import GmpmSimulator
 
@@ -77,7 +83,7 @@ def _positions(model, cfg, base_dir):
         return np.fromfile(path, dtype=np.float32).reshape(-1, 3)
     if path.endswith(".npy"):
         return np.load(path).astype(np.float32).reshape(-1, 3)
-    raise ValueError(f"unsupported model file {kind!r} (known: box, sphere, *.sdf, *.bin, *.npy)")
+    raise ValueError(f"unsupported model file {kind!r} (known: box, sphere, *.sdf, *.obj, *.bin, *.npy)")
 
 
 def _model_path(model, base_dir):
@@ -85,12 +91,54 @@ def _model_path(model, base_dir):
     return kind if os.path.isabs(kind) else os.path.join(base_dir, kind)
 
 
-def _level_sets(models, base_dir):
-    """Reads every `.sdf` model's level set and checks its node box: {model index: LevelSet}, before any device work."""
+MESH_KEYS = ("h", "padding", "exact_band")   # with a "file": "*.obj" model, boundary or sink
+
+
+def _mesh_level_set(e, path, what, span, dx, cache):
+    """The level set of the `.obj` entry `e`, one per (path, h, padding, exact_band) in `cache`: read and checked on the host here, its
+    phi left None until _build_level_sets (ValueError naming `what`).  h defaults to the mesh's longest extent x dx / the longest
+    span, so that one level-set cell is about one simulation cell."""
+    try:
+        if ("obj", path) not in cache:
+            cache[("obj", path)] = mesh.read_obj(path)
+        m = cache[("obj", path)]
+        lo, hi = m.bounds if len(m.vertices) else (np.zeros(3), np.zeros(3))
+        h = e.get("h", float(np.max(hi - lo)) * dx / max(sdf._vec3(span)))
+        padding, band = e.get("padding", 1), e.get("exact_band", 1)
+        for k, v in (("h", h), ("padding", padding), ("exact_band", band)):
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or (k != "h" and not isinstance(v, int)):
+                raise ValueError(f"\"{k}\" must be a {'number' if k == 'h' else 'integer'}, not {v!r}")
+        key = (path, float(np.float32(h)), padding, band)
+        if key not in cache:
+            ls = sdf.LevelSet(mesh.header(m, h, padding, band), None)
+            ls.source = (m, h, padding, band)
+            cache[key] = ls
+        return cache[key]
+    except (OSError, ValueError) as e:
+        raise ValueError(f"{what}: {os.path.basename(path)}: {e}") from None
+
+
+def _build_level_sets(cache):
+    """Builds, on the current device, every mesh level set of `cache` that has no phi yet (each distinct one once)."""
+    for ls in cache.values():
+        if isinstance(ls, sdf.LevelSet) and ls.phi is None:
+            built = mesh.levelset(*ls.source)
+            ls.header, ls.phi = built.header, built.phi
+
+
+def _level_sets(models, base_dir, dx=None, cache=None):
+    """Reads every `.sdf` model's level set and every `.obj` model's mesh and checks its node box: {model index: LevelSet}, before any
+    device work.  A mesh's level set is built later by _build_level_sets(cache)."""
     out = {}
+    dx = Config().dx if dx is None else dx
+    cache = {} if cache is None else cache
     for i, model in enumerate(models):
-        if str(model.get("file", "box")).endswith(".sdf"):
-            ls = sdf.read(_model_path(model, base_dir))
+        f = str(model.get("file", "box"))
+        if f.endswith(".obj"):
+            ls = _mesh_level_set(model, _model_path(model, base_dir), f"model {i}", model.get("span", [1, 1, 1]), dx, cache)
+        if f.endswith(".sdf") or f.endswith(".obj"):
+            if f.endswith(".sdf"):
+                ls = sdf.read(_model_path(model, base_dir))
             sdf.check_box(ls, model.get("offset", [0, 0, 0]), model.get("span", [1, 1, 1]), what=f"model {i} ({model['file']})")
             sdf.sampling(model.get("offset", [0, 0, 0]), model.get("span", [1, 1, 1]), model.get("ppc", 8), model.get("sampler", "random"),
                          model.get("seed", 0))
@@ -115,15 +163,20 @@ def _collider(sim, c, cfg, base_dir):
 
 
 BOUNDARY_KEYS = ("shape", "offset", "span", "normal", "type", "friction", "velocity", "omega", "scale", "dsdt")
-LEVELSET_KEYS = ("file",)   # with "shape": "levelset"
+LEVELSET_KEYS = ("file",) + MESH_KEYS   # with "shape": "levelset"
 
 
-def _obstacle_level_set(b, what, base_dir, cache):
-    """The sdf.LevelSet of a "levelset" entry, read once per path into `cache` (ValueError naming `what` on a bad file)."""
+def _obstacle_level_set(b, what, base_dir, cache, span=(1, 1, 1), dx=None):
+    """The sdf.LevelSet of a "levelset" entry, read once per path (an .obj mesh: once per path, h, padding and band) into `cache`
+    (ValueError naming `what` on a bad file)."""
     f = b.get("file")
-    if not isinstance(f, str) or not f.endswith(".sdf"):
-        raise ValueError(f"{what} (levelset): \"file\" must name an .sdf level set, not {f!r}")
+    if not isinstance(f, str) or not (f.endswith(".sdf") or f.endswith(".obj")):
+        raise ValueError(f"{what} (levelset): \"file\" must name an .sdf level set or an .obj mesh, not {f!r}")
     path = f if os.path.isabs(f) else os.path.join(base_dir if base_dir is not None else os.getcwd(), f)
+    if f.endswith(".obj"):
+        return _mesh_level_set(b, path, f"{what} (levelset)", span, Config().dx if dx is None else dx, cache)
+    if any(k in b for k in MESH_KEYS):
+        raise ValueError(f"{what} (levelset): {', '.join(k for k in MESH_KEYS if k in b)} only apply to an .obj mesh")
     if path not in cache:
         try:
             cache[path] = sdf.read(path)
@@ -132,7 +185,7 @@ def _obstacle_level_set(b, what, base_dir, cache):
     return cache[path]
 
 
-def _object(b, what, keys, base_dir=None, cache=None):
+def _object(b, what, keys, base_dir=None, cache=None, dx=None):
     """The collision object of one "boundaries" or "sinks" entry `b` (ValueError naming `what` on a bad entry or a key not in `keys`).
     A "levelset" entry's file is read through `cache` ({path: LevelSet}), so that one file is one level set."""
     from . import objects
@@ -152,7 +205,7 @@ def _object(b, what, keys, base_dir=None, cache=None):
         motion = dict(type=b.get("type", "sticky"), friction=float(b.get("friction", 0.3)), trans_vel=b.get("velocity", [0, 0, 0]),
                       omega=b.get("omega", [0, 0, 0]), scale=float(b.get("scale", 1.0)), dsdt=float(b.get("dsdt", 0.0)))
         if shape == "levelset":
-            ls = _obstacle_level_set(b, what, base_dir, {} if cache is None else cache)
+            ls = _obstacle_level_set(b, what, base_dir, {} if cache is None else cache, span, dx)
             return objects.levelset(ls, offset, span, **motion)
         if shape == "box":
             return objects.box(offset, offset + span, **motion)
@@ -165,22 +218,23 @@ def _object(b, what, keys, base_dir=None, cache=None):
         raise ValueError(f"{what} ({shape}): {e}") from None
 
 
-def boundaries(doc, base_dir=None, cache=None):
+def boundaries(doc, base_dir=None, cache=None, dx=None):
     """The scene's "boundaries" as validated collision objects (ValueError on a bad entry), before any device work.  Level-set files
-    are relative to base_dir (default: the working directory) and read through `cache` ({path: LevelSet})."""
+    are relative to base_dir (default: the working directory) and read through `cache` ({path: LevelSet}); dx (default: Config's)
+    sets an .obj mesh's default h."""
     from . import objects
     bs = doc.get("boundaries", [])
     if not isinstance(bs, list):
         raise ValueError("\"boundaries\" must be a list of objects")
     if len(bs) > objects.MAX_COLLISION_OBJECTS:
         raise ValueError(f"at most {objects.MAX_COLLISION_OBJECTS} \"boundaries\", not {len(bs)}")
-    return [_object(b, f"boundary {i}", BOUNDARY_KEYS, base_dir, cache) for i, b in enumerate(bs)]
+    return [_object(b, f"boundary {i}", BOUNDARY_KEYS, base_dir, cache, dx) for i, b in enumerate(bs)]
 
 
 SINK_KEYS = ("shape", "offset", "span", "normal", "velocity", "omega", "scale", "dsdt", "models", "outside", "start", "every", "until")
 
 
-def sinks(doc, base_dir=None, cache=None):
+def sinks(doc, base_dir=None, cache=None, dx=None):
     """The scene's validated "sinks": [{"object", "models" (sorted tuple of scene model indices), "outside", "frames" (list)}], in
     document order (ValueError on a bad entry, or on more than CB200_MAX_COLLISION_OBJECTS sinks due in one group), before any
     device work.  base_dir and cache: as for boundaries."""
@@ -193,7 +247,7 @@ def sinks(doc, base_dir=None, cache=None):
     out = []
     for i, e in enumerate(ss):
         what = f"sink {i}"
-        o = _object(e, what, SINK_KEYS, base_dir, cache)
+        o = _object(e, what, SINK_KEYS, base_dir, cache, dx)
         models = e.get("models", list(range(n_models)))
         if not isinstance(models, list) or not models:
             raise ValueError(f"{what}: \"models\" must be a non-empty list of model indices, not {models!r}")
@@ -235,16 +289,16 @@ def _sink_groups(specs, after=0):
     return dict(sorted(out.items()))
 
 
-def sink_schedule(doc, after=0, base_dir=None, cache=None):
+def sink_schedule(doc, after=0, base_dir=None, cache=None, dx=None):
     """{frame: [(models, outside, [sink indices]), ...]}: the removal calls of every frame > `after` (a resumed run's checkpoint
     frame), one per group of sinks due together with the same models and outside, in document order.  Validates "sinks"."""
-    return {f: [(m, o, idx) for (m, o), idx in g.items()] for f, g in _sink_groups(sinks(doc, base_dir, cache), after).items()}
+    return {f: [(m, o, idx) for (m, o), idx in g.items()] for f, g in _sink_groups(sinks(doc, base_dir, cache, dx), after).items()}
 
 
-def _sink_hook(doc, after=0, base_dir=None, cache=None):
+def _sink_hook(doc, after=0, base_dir=None, cache=None, dx=None):
     """main_loop's per-frame hook that applies the scene's sinks (None without any), built before any device work."""
-    specs = sinks(doc, base_dir, cache)
-    todo = sink_schedule(doc, after, base_dir, cache)
+    specs = sinks(doc, base_dir, cache, dx)
+    todo = sink_schedule(doc, after, base_dir, cache, dx)
     if not todo:
         return None
 
@@ -360,12 +414,15 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
     if doc.get("sinks") and sim_kwargs.get("mgsp_world", 1) > 1:
         raise ValueError("\"sinks\" are not supported in MGSP mode")
     models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
-    obstacles = {}   # {path: LevelSet} of the "levelset" boundaries and sinks: one registration per file
-    objs = boundaries(doc, base, obstacles)
+    # {path or (path, h, padding, band): LevelSet} of the "levelset" boundaries and sinks and the .obj models: one build and one
+    # registration per distinct level set
+    obstacles = {}
+    objs = boundaries(doc, base, obstacles, cfg.dx)
     if resume is not None:
         inf = _check_resume(doc, cfg, resume)
-        emitters = _emitters(doc, cfg, base, _level_sets(models, base))
-        sink = _sink_hook(doc, inf["frames"], base, obstacles)
+        emitters = _emitters(doc, cfg, base, _level_sets(models, base, cfg.dx, obstacles))
+        sink = _sink_hook(doc, inf["frames"], base, obstacles, cfg.dx)
+        _build_level_sets(obstacles)   # deterministic: the same phi as the run that wrote the checkpoint
         sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                             frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max(max_blocks, inf["max_blocks"]), **sim_kwargs)
         if "collider" in doc:
@@ -378,9 +435,10 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
     for model in models:
         if model.get("constitutive") not in CONSTITUTIVE:
             raise ValueError(f"unknown constitutive model {model.get('constitutive')!r}")
-    level_sets = _level_sets(models, base)
-    sink = _sink_hook(doc, 0, base, obstacles)
+    level_sets = _level_sets(models, base, cfg.dx, obstacles)
+    sink = _sink_hook(doc, 0, base, obstacles, cfg.dx)
     emitters = _emitters(doc, cfg, base, level_sets)
+    _build_level_sets(obstacles)
     sim = GmpmSimulator(gpu=s.get("gpuid", 0), dt=s.get("default_dt", GmpmSimulator.DEFAULT_DT), fps=s.get("fps", GmpmSimulator.DEFAULT_FPS),
                         frames=s.get("frames", GmpmSimulator.DEFAULT_FRAMES), config=cfg, max_blocks=max_blocks, **sim_kwargs)
     for i, model in enumerate(models):

@@ -1,6 +1,7 @@
 """Particle models from SDFGen `.sdf` level sets (the reference's read_sdf, Library/MnSystem/IO/ParticleIO.hpp:65-97).
 
     ls = sdf.read("dragon.sdf")                                  # the library's parser (strtof: LoadSDF's values bit for bit)
+    sdf.write(ls, "copy.sdf")                                    # SDFGen text, 9 significant digits: read() returns ls bit for bit
     pos = sdf.sample(ls, cfg, offset, span, ppc=8)               # host positions, e.g. for samplers.split_slabs
     sim.init_model_sdf(material, ls, offset, span, v0)           # sampled straight into the model's device array
 
@@ -57,6 +58,14 @@ def read(path):
         return parse(f.read())
 
 
+def write(ls, path):
+    """Writes `ls` as SDFGen text with 9 significant digits, so that read(path) returns ls bit for bit."""
+    n = ls.n
+    with open(path, "w") as f:
+        f.write(f"{n[0]} {n[1]} {n[2]}\n{' '.join('%.9g' % float(v) for v in ls.header.min)}\n{'%.9g' % ls.h}\n")
+        np.savetxt(f, np.asarray(ls.phi, dtype=np.float32).reshape(-1, 1), fmt="%.9g")
+
+
 def _vec3(v):
     a = np.broadcast_to(np.asarray(v, dtype=np.float64), (3,))
     return [float(x) for x in a]
@@ -106,4 +115,4 @@ def sample(ls, cfg, offset, span, ppc=8, mode="random", seed=0, stream=None):
     return out
 
 
-__all__ = ["LevelSet", "MODES", "parse", "read", "node_box", "check_box", "sampling", "sample", "CB200Error"]
+__all__ = ["LevelSet", "MODES", "parse", "read", "write", "node_box", "check_box", "sampling", "sample", "CB200Error"]

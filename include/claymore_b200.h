@@ -472,6 +472,37 @@ CB200_API int cb200_sim_init_model_sdf(cb200_sim* sim, int material, const cb200
                                        const cb200_sdf_sampling* sampling, const float* v0, int* model_id, int* n_out);
 
 /* ------------------------------------------------------------------------------------------------
+ * Level sets from triangle meshes (DESIGN.md section 2.12): SDFGen's make_level_set3 (Externals/SDFGen/makelevelset3.cpp:118-183)
+ * on the device, bit for bit, and the lattice of SDFGen's main (main.cpp:63-118).  The result is a (cb200_sdf_header, phi) pair that
+ * every .sdf consumer above takes: exact distances within exact_band cells of a triangle, fast-sweeping distances beyond, and the
+ * sign by the parity of crossings along +i (a mesh that is not watertight gives streaks).
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct cb200_mesh_header {
+	int nv, nt;      /* vertices, triangles (a polygon counts as its fan) */
+	float min[3];    /* the vertex bounding box (every vertex, referenced or not) */
+	float max[3];
+} cb200_mesh_header;
+typedef struct cb200_mesh_levelset_params {
+	float h;         /* node spacing, mesh units */
+	int padding;     /* cells between the vertex box and the lattice's faces (below 1 means 1) */
+	int exact_band;  /* 0..8: cells around each triangle's box whose distances are exact */
+} cb200_mesh_levelset_params;
+/* Host only.  Wavefront OBJ text: `v x y z` lines (further values ignored) and `f` lines of 3 or more references `i`, `i/t`, `i//n`
+ * or `i/t/n` (1-based; negative counts back from the last vertex read); a polygon becomes the fan (v0, v_i, v_{i+1}).  Other lines
+ * are ignored.  vertices (nullable): float[3 nv]; triangles (nullable): int[3 nt], 0-based; each filled when its capacity (in
+ * vertices / triangles) allows.  cudaErrorInvalidValue for a `v` line without three finite numbers, an `f` line with fewer than three
+ * references, a reference that is not an integer, 0, or outside the vertices, or a capacity below the count. */
+CB200_API int cb200_obj_parse(const char* text, size_t bytes, cb200_mesh_header* header, float* vertices, int* triangles, size_t v_capacity,
+                              size_t t_capacity);
+/* The level set of HOST vertices[3 nv] / triangles[3 nt] on the current device.  *out: min = vertex box - padding h (float),
+ * n_d = (unsigned) ((max_d - min_d) / h), h.  phi == NULL fills only *out, on the host.  Otherwise phi (HOST, capacity >= ni nj nk
+ * floats) receives the level set, i fastest; synchronises `stream`.  cudaErrorInvalidValue, before any device work, for an h that is
+ * not finite and positive, exact_band outside 0..8, no triangles, an index outside [0, nv), a non-finite vertex, any n_d < 2,
+ * ni nj nk >= 2^31 or a capacity below it. */
+CB200_API int cb200_mesh_levelset(const float* vertices, int nv, const int* triangles, int nt, const cb200_mesh_levelset_params* params,
+                                  cb200_sdf_header* out, float* phi, size_t capacity, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Adding particles to a running simulation (sources: inlets, pouring, an object dropped later).  Both entries share one path and
  * differ only in where the candidate positions come from.  The call synchronises and acts at the current sub-step boundary.
  *   Rejections, all before anything changes (a checkpoint taken after one is byte-identical to one taken before it):
