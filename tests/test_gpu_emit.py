@@ -18,9 +18,9 @@ from claymore_b200 import bgeo, checkpoint
 from claymore_b200._capi import CB200Error, Config
 from claymore_b200.scene import emit_schedule, parse_scene
 from claymore_b200.simulator import GmpmSimulator
+from ref64_checks import BRANCH_MARGIN, F_ALLOW, KAPPA, RASTER_KAPPA, STRESS_ALLOW, check_counts, check_dt, check_report, ref_models
 from test_gpu_checkpoint import _assert_round_trip, _restored, _sorted_rows
 from test_gpu_parity import _compare_state
-from test_ref64_cpu import BRANCH_MARGIN, F_ALLOW, KAPPA, RASTER_KAPPA, STRESS_ALLOW, check_counts, check_dt, check_report, ref_models
 
 pytestmark = pytest.mark.gpu
 

@@ -21,9 +21,9 @@ import sdf_ref
 from claymore_b200 import _capi, objects, samplers, scene, sdf
 from claymore_b200._capi import CB200Error, CollisionObject, Config, LevelSetLattice, Partition, SdfHeader
 from claymore_b200.simulator import GmpmSimulator
+from ref64_checks import COLLIDER_VEL_KAPPA
 from scenes import match_particles
 from test_levelset_objects_cpu import LATTICES, level_set
-from test_ref64_collider_cpu import COLLIDER_VEL_KAPPA
 
 pytestmark = pytest.mark.gpu
 DOMAIN_BITS = 6

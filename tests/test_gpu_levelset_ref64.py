@@ -1,5 +1,5 @@
 """The step driver and the MGSP dt predictors with level-set collision objects (DESIGN.md section 2.11) against the float64
-reference, sub-step by sub-step, with test_gpu_collider_ref64's bounds (COLLIDER_KAPPA per particle and cell, dt within
+reference, sub-step by sub-step, with the boundary bounds of ref64_checks (COLLIDER_KAPPA per particle and cell, dt within
 DT_ULPS).  ref64's sub-step answers the level-set objects through ref64_levelset.registered.
 
 Step driver: a block falling onto a level-set floor for four materials x three types; a fluid block through the moving,
@@ -13,7 +13,7 @@ import pytest
 
 import ref64_cases as S
 import ref64_levelset as RL
-from test_gpu_collider_ref64 import engine_collider_check, mgsp_collider_check
+from ref64_checks import engine_substep_check, mgsp_substep_check
 from test_levelset_objects_cpu import level_set
 from test_ref64_mgsp_cpu import split_case
 
@@ -45,7 +45,7 @@ def _floor(**kw):
 
 def _check(case, use_graph, label):
     with RL.registered(_lattices(case)):
-        engine_collider_check(case, use_graph, label)
+        engine_substep_check(case, use_graph, label)
 
 
 @pytest.mark.timeout(900)
@@ -86,5 +86,5 @@ def test_mgsp_rising_sticky_levelset_floor_two_slabs(cuda_lib, use_graph):
     case = S._case(6, [S.model(S.FIXED_COROTATED, S.box(DX, (24, 24, 24), (36, 30, 34)), (1.0, -3.0, 0.5), DX)], [0, 1, 2, 3, 4],
                    dt=1e-3, objects=[_floor(type=S.STICKY, friction=0.3, trans_vel=(0.0, 15.0, 0.0))])
     with RL.registered(_lattices(case)):
-        r = mgsp_collider_check(case, split_case(case, 2, "x"), use_graph, f"rising level-set floor 2x {'graph' if use_graph else 'stream'}")
+        _, r = mgsp_substep_check(case, split_case(case, 2, "x"), use_graph, f"rising level-set floor 2x {'graph' if use_graph else 'stream'}")
     assert r["new_dt"] < case["dt"], "the dt must be CFL-bound"

@@ -20,7 +20,7 @@ import ref64_levelset as RL
 from claymore_b200 import _capi, mesh, objects, scene, sdf
 from claymore_b200._capi import Config
 from claymore_b200.simulator import GmpmSimulator
-from test_gpu_collider_ref64 import engine_collider_check
+from ref64_checks import engine_substep_check
 
 pytestmark = pytest.mark.gpu
 GOLDENS = sorted(glob.glob(os.path.join(M.GOLDEN, "ref_sdfgen_*.npz")))
@@ -99,7 +99,7 @@ def test_fluid_onto_torus_from_obj_ref64(cuda_lib):
     case = S._case(6, [S.model(S.J_FLUID, S.box(DX, (26, 24, 26), (34, 30, 34)), (0.0, -3.0, 0.0), DX)], [0, 5, 20, 39], dt=2e-4,
                    objects=[obstacle])
     with RL.registered([RL.lattice(torus.n, torus.phi)]):
-        engine_collider_check(case, True, "fluid onto the .obj torus")
+        engine_substep_check(case, True, "fluid onto the .obj torus")
 
 
 def _scene_files(tmp_path):

@@ -7,110 +7,13 @@ at a time: every rank's state at sub-step k, one sub-step on every rank, then ev
 the ranks' particles per scene model and every rank's dt against the reference.  At most 4 ranks: the exchange kernels of
 every rank spin on their peers' flags, and more ranks on one GPU could leave no SM for the last rank's wide kernels.
 """
-import threading
-
-import numpy as np
 import pytest
 
 import ref64_cases as S
-import ref64_mgsp as M
-from test_ref64_cpu import BRANCH_MARGIN, DT_ULPS, F_ALLOW, KAPPA, RASTER_KAPPA, STRESS_ALLOW, check_report
-from test_ref64_mgsp_cpu import rank_models, split_case
+from ref64_checks import ERR_BLOCK_CAPACITY, build_ranks, mgsp_substep_check
+from test_ref64_mgsp_cpu import split_case
 
 pytestmark = pytest.mark.gpu
-
-ERR_BLOCK_CAPACITY, ERR_LOST, ERR_HALO_MAP = 1, 4, 16
-
-
-def on_threads(sims, fn, timeout=120):
-    errs = []
-
-    def go(s):
-        try:
-            fn(s)
-        except Exception as e:  # pragma: no cover
-            errs.append(e)
-    th = [threading.Thread(target=go, args=(s,)) for s in sims]
-    [t.start() for t in th]
-    [t.join(timeout) for t in th]
-    assert not errs and not any(t.is_alive() for t in th), errs
-
-
-def build_ranks(case, parts, use_graph, halo_cap=0, max_blocks=6000):
-    from claymore_b200.simulator import GmpmSimulator
-    sims = []
-    for r, ps in enumerate(parts):
-        sim = GmpmSimulator(dt=case["dt"], fps=case.get("fps", 0), config=S.config(case), max_blocks=max_blocks, use_graph=use_graph,
-                            mgsp_rank=r, mgsp_world=len(parts), mgsp_halo_cap=halo_cap)
-        for p in ps:
-            mid = sim.init_model(p["material"], p["pos"], p["v0"])
-            getattr(sim, S.SETTER[p["material"]])(p["rho"], p["vol"], *p["args"], model=mid)
-        sims.append(sim)
-    ptrs = [s.mgsp_inbox() for s in sims]
-    for s in sims:
-        s.mgsp_set_peers(ptrs)
-    on_threads(sims, lambda s: s.initial_setup())
-    return sims
-
-
-def _grid(sim):
-    g = sim.grid()
-    return sim.active_keys()[: len(g)].astype(np.int64), g
-
-
-def _errors(sims, expect, label):
-    got = [s.stats().error for s in sims]
-    assert not any(e & ERR_HALO_MAP for e in got), f"{label}: kErrHaloMap on a rank ({got})"
-    assert got == expect, f"{label}: error bits {got}, expected {expect}"
-
-
-def mgsp_substep_check(case, parts, use_graph, label):
-    """Set-up grid and case['steps'] sub-steps of the ranks against ref64; returns what the matrix saw (owners, fresh copies)."""
-    sims = build_ranks(case, parts, use_graph)
-    cfg = sims[0].cfg
-    nm = len(case["models"])
-    seen = dict(max_owners=0, fresh=0, fresh_in=0)
-    world = len(sims)
-    expect = [0] * world
-    _errors(sims, expect, f"{label} set-up")
-    ref = M.rasterize(cfg, [[dict(pos=p["pos"], v0=p["v0"], mass=S.ref_params(p)["mass"]) for p in ps] for ps in parts])
-    after = [dict(zip(("keys", "grid"), _grid(s))) for s in sims]
-    check_report(M.compare(cfg, ref, after, RASTER_KAPPA, 0.0, []), f"{label} set-up")
-    done, near = 0, 0
-    f_allow = [F_ALLOW[m["material"]] for m in case["models"]]
-    for k in case["steps"]:
-        if k > done:
-            on_threads(sims, lambda s: (s.step(k - done), s.sync()))
-        _errors(sims, expect, f"{label} at sub-step {k}")
-        ranks = []
-        for s, ps in zip(sims, parts):
-            keys, grid = _grid(s)
-            ranks.append(dict(keys=keys, grid=grid, models=rank_models(ps, [s.particle_state(i) for i in range(len(ps))])))
-        dts = [s.stats().dt for s in sims]
-        M.check_dts(dts, dts[0], 0)
-        r = M.substep(cfg, ranks, dts[0], case["dt"], S.engine_time_left(sims[0], case), n_models=nm)
-        on_threads(sims, lambda s: (s.step(1), s.sync()))
-        done = k + 1
-        for i, per in enumerate(r["per_rank"]):
-            if any(res["dropped"].any() or res["lost"].any() for _, res in per):
-                expect[i] |= ERR_LOST
-        _errors(sims, expect, f"{label} after sub-step {k}")
-        after = []
-        for s, ps in zip(sims, parts):
-            keys, grid = _grid(s)
-            after.append(dict(keys=keys, grid=grid, states={p["model"]: s.particle_state(i) for i, p in enumerate(ps)}))
-        rep = M.compare(cfg, r, after, KAPPA, STRESS_ALLOW, f_allow, margin=BRANCH_MARGIN)
-        check_report(rep, f"{label} sub-step {k}")
-        M.check_dts([s.stats().dt for s in sims], r["new_dt"], DT_ULPS)
-        near += rep["near_branch"]
-        seen["max_owners"] = max(seen["max_owners"], rep["max_owners"])
-        seen["fresh"] += rep["fresh"]
-        seen["fresh_in"] += r["fresh_in"]
-    for s in sims:
-        s.close()
-    total = sum(len(m["pos"]) for m in case["models"]) * len(case["steps"])
-    assert near <= case.get("max_near_branch", 0.01) * total, f"{label}: {near} of {total} particle updates near a branch point"
-    return seen
 
 
 CROSSING = 0.25 / 64 / (2.5 * 1e-4)   # m/s: carries a lattice particle (0.25 dx short of a cell face) across it in sub-step 3
@@ -179,7 +82,7 @@ def test_mgsp_ranks_match_ref64(cuda_lib, name, use_graph):
     lists = [sorted(p["model"] for p in ps) for ps in parts]
     if want.get("models_differ"):
         assert any(a != b for a in lists for b in lists), lists   # a rank holds a model another rank lacks
-    seen = mgsp_substep_check(case, parts, use_graph, f"{name} {'graph' if use_graph else 'stream'}")
+    seen, _ = mgsp_substep_check(case, parts, use_graph, f"{name} {'graph' if use_graph else 'stream'}")
     print(f"{name}: {seen}, model lists {lists}")
     assert seen["max_owners"] >= want["owners"], seen
     if want.get("fresh"):   # zero copies seen after a sub-step, then filled from their owners in the next sub-step's input

@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 import ref64_cases as S
-from test_gpu_collider_ref64 import engine_collider_check, mgsp_collider_check
+from ref64_checks import engine_substep_check, mgsp_substep_check
 from test_ref64_collider_cpu import FIELDS, block_field
 from test_ref64_mgsp_cpu import split_case
 from test_ref64_objects_cpu import KERNEL_MATRIX, kernel_matrix
@@ -63,7 +63,7 @@ def test_engine_objects_kernel_matches_ref64(oracle, engine_objects_kernel, entr
 @pytest.mark.parametrize("use_graph", [True, False], ids=["graph", "stream"])
 @pytest.mark.parametrize("name", list(S.OBJECT_CASES))
 def test_engine_object_substep_matches_ref64(cuda_lib, name, use_graph):
-    engine_collider_check(S.OBJECT_CASES[name], use_graph, f"{name} {'graph' if use_graph else 'stream'}")
+    engine_substep_check(S.OBJECT_CASES[name], use_graph, f"{name} {'graph' if use_graph else 'stream'}")
 
 
 # ---- MGSP -------------------------------------------------------------------------------------------------------------------
@@ -74,7 +74,7 @@ def test_mgsp_analytic_sticky_floor_two_slabs(cuda_lib, use_graph):
     dx = 1.0 / 64
     case = S._case(6, [S.model(S.FIXED_COROTATED, S.box(dx, (24, 20, 24), (36, 28, 34)), (1.0, -10.0, 0.5), dx)], [0, 1, 2, 3, 4], dt=1e-3,
                    objects=[("box", (S.FLOOR_LO, S.FLOOR_HI), dict(type=S.STICKY, friction=0.3))])
-    mgsp_collider_check(case, split_case(case, 2, "x"), use_graph, f"analytic sticky floor 2x {'graph' if use_graph else 'stream'}")
+    mgsp_substep_check(case, split_case(case, 2, "x"), use_graph, f"analytic sticky floor 2x {'graph' if use_graph else 'stream'}")
 
 
 @pytest.mark.timeout(600)
@@ -83,7 +83,7 @@ def test_mgsp_object_paddle_2x2(cuda_lib, use_graph):
     """The combined-motion paddle object on 2 x 2 ranks: the max comes from nodes the paddle resolves and moves with t, so a
     predictor that placed the objects at any other time than the next grid update's would give another dt."""
     case = S.OBJECT_CASES["obj_paddle_combined"]
-    r = mgsp_collider_check(case, split_case(case, 4, "2x2"), use_graph, f"object paddle 2x2 {'graph' if use_graph else 'stream'}")
+    _, r = mgsp_substep_check(case, split_case(case, 4, "2x2"), use_graph, f"object paddle 2x2 {'graph' if use_graph else 'stream'}")
     assert r["new_dt"] < case["dt"], "the paddle's dt must be CFL-bound"
 
 
@@ -91,4 +91,4 @@ def test_mgsp_object_paddle_2x2(cuda_lib, use_graph):
 def test_mgsp_collider_plus_objects_two_slabs(cuda_lib):
     """The level-set collider with two objects on two x slabs: the <true> forms of both predictors."""
     case = S.OBJECT_CASES["obj_collider_plus_two"]
-    mgsp_collider_check(case, split_case(case, 2, "x"), True, "collider + objects 2x graph")
+    mgsp_substep_check(case, split_case(case, 2, "x"), True, "collider + objects 2x graph")

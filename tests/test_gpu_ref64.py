@@ -1,5 +1,5 @@
 """The engine's sub-step against the float64 reference (tests/ref64.py), per grid cell and per particle, with the kappa
-values test_ref64_cpu.py fixed on the FP32 oracle (no re-tuning here), and the engine's set-up rules at the domain's
+values the FP32 oracle fixed (ref64_checks, test_ref64_cpu.py; no re-tuning here), and the engine's set-up rules at the domain's
 faces and limits.
 
 The step driver is the production path (the sorted g2p2g with arrival lists), in graph and stream mode: the engine's
@@ -13,50 +13,10 @@ import pytest
 
 import ref64
 import ref64_cases as S
-from test_ref64_cpu import (BRANCH_MARGIN, F_ALLOW, KAPPA, KERNEL_LEVEL, KERNEL_LEVEL_CASES, RASTER_KAPPA, STRESS_ALLOW, check_counts, check_dt,
-                            check_report, grid_mass, kernel_level_check, ref_models)
+from ref64_checks import ERR_CELL_OVERFLOW, ERR_LOST, RASTER_KAPPA, check_report, engine_substep_check
+from test_ref64_cpu import KERNEL_LEVEL, KERNEL_LEVEL_CASES, grid_mass, kernel_level_check
 
 pytestmark = pytest.mark.gpu
-
-ERR_LOST, ERR_CELL_OVERFLOW = 4, 8
-
-
-def _engine_state(sim, nm):
-    g = sim.grid()
-    return sim.active_keys()[: len(g)], g, [sim.particle_state(i) for i in range(nm)]
-
-
-def engine_substep_check(case, use_graph, label):
-    sim = S.build_engine(case, use_graph=use_graph)
-    nm = len(case["models"])
-    done = 0
-    near = 0
-    expect = 0   # a particle that moves more than one cell (quirk #4) or leaves its block's neighbourhood is flagged lost,
-    #              a cell that gets more than max_ppc particles in g2p2g sets the overflow bit
-    for k in case["steps"]:
-        sim.step(k - done)
-        st = sim.stats()
-        assert st.error == expect, f"{label}: error bits {st.error} at sub-step {k}, expected {expect}"
-        keys, grid, before = _engine_state(sim, nm)
-        r = ref64.substep(sim.cfg, ref_models(case, before), keys, grid, st.dt, case["dt"], S.engine_time_left(sim, case))
-        sim.step(1)
-        done = k + 1
-        st = sim.stats()
-        if any(m["dropped"].any() or m["lost"].any() for m in r["models"]):
-            expect |= ERR_LOST
-        if any(ref64.cell_overflow(m, case["max_ppc"])[1] for m in r["models"]):
-            expect |= ERR_CELL_OVERFLOW
-        assert st.error == expect, f"{label}: error bits {st.error} after sub-step {k}, expected {expect}"
-        keys, grid, states = _engine_state(sim, nm)
-        check_counts(r, before, states, case["max_ppc"], f"{label} sub-step {k}")
-        rep = ref64.compare(r, keys, grid, states, KAPPA, STRESS_ALLOW, [F_ALLOW[m["material"]] for m in case["models"]], margin=BRANCH_MARGIN,
-                            max_ppc=case["max_ppc"])
-        check_report(rep, f"{label} sub-step {k}")
-        check_dt(st.dt, r["new_dt"], f"{label} sub-step {k}")
-        near += rep["near_branch"]
-    sim.close()
-    total = sum(len(m["pos"]) for m in case["models"]) * len(case["steps"])
-    assert near <= case.get("max_near_branch", 0.01) * total, f"{label}: {near} of {total} particle updates near a branch point"
 
 
 @pytest.mark.parametrize("use_graph", [True, False], ids=["graph", "stream"])

@@ -5,7 +5,7 @@ log-uniform from 1e-12 to 1 with zero and subnormal nodes, velocities N(0, 2) m/
 {static, combined motion} x t {0, 0.37, 3.1} x {sphere, box, tilted plane, zero-gradient slab} x boundary {2, 0}; friction
 -0.2 separates SLIP's `friction > 0` from SEPARATE's `friction != 0`.  Per node: |v - ref64| <= COLLIDER_VEL_KAPPA 2^-24 E,
 nodes near a discontinuity (ref64's margin) left out and counted.  Per sub-step: the collider oracle through COLLIDER_CASES
-with the single-domain kappa of test_ref64_cpu (F excepted, COLLIDER_KAPPA); particles that read a near node and the cells
+with ref64_checks' single-domain kappa (F excepted, COLLIDER_KAPPA); particles that read a near node and the cells
 they write are left out and counted, each under its cap.  The GPU tests (test_gpu_collider_ref64.py) hold the engine to the same values.
 """
 import ctypes as C
@@ -15,19 +15,9 @@ import pytest
 
 import ref64
 import ref64_cases as S
-from test_ref64_cpu import BRANCH_MARGIN, DT_ULPS, F_ALLOW, KAPPA, STRESS_ALLOW, check_counts, check_report, ref_models
+from ref64_checks import COLLIDER_VEL_KAPPA, MAX_NEAR_NODES, oracle_substep_check, ref_models
 
-# the collider's grid velocity per component: the oracle's worst |oracle - ref64| / (2^-24 E) over KERNEL_MATRIX is 2.62
-# (box, boundary 0, static), against 2.13 for the grid update without a collider (VEL_KAPPA 4 there, as here)
-COLLIDER_VEL_KAPPA = 4.0
 COLLIDER_MAX_REL = 4.0     # the max |v|^2 within 4 x 2^-24 relative of [mx_lo, mx_hi] (the near nodes' branch choices)
-MAX_NEAR_NODES = 0.01      # share of the resolved nodes that may lie near a discontinuity
-MAX_TAINTED = 0.05         # share of the particle updates (and of the grid cells) that may read (write) such a node
-# Per sub-step: test_ref64_cpu's kappa, except F (J, F, logJp): 8 in place of 4.  The oracle's worst F is 5.9 on
-# walls_boundary1, which has no collider: a wall band's edge runs through its models, so the grid velocity jumps from v to 0
-# between two nodes, and F's M has no term for the last bit of the stored position (the momentum's has one) while G2P's
-# weights carry that bit times |v| / dx into A.  The collider cases stay under 4.6 (moving_floor_frame_end, sphere_separate).
-COLLIDER_KAPPA = dict(KAPPA, F=8.0)
 
 DOMAIN_BITS = 6
 FIELDS = {
@@ -197,75 +187,9 @@ def test_collider_kernel_reaches_every_branch(oracle):
 
 
 # ---- per sub-step: the collider oracle through COLLIDER_CASES ---------------------------------------------------------------
-def check_dt_range(impl_dt, r, label):
-    """The implementation's dt lies in [dt(mx_hi), dt(mx_lo)] (the near nodes' branch choices) within DT_ULPS, the max
-    widened by COLLIDER_VEL_KAPPA 2^-24 mx_err (dt scales as max^-1/2 where it is CFL-bound)."""
-    lo, hi = r["dt_range"]
-    info = r.get("collider_info", r)
-    err = COLLIDER_VEL_KAPPA * ref64.EPS32 * info.get("mx_err", 0.0)
-    if info["mx_hi"] > 0 and err > 0:
-        lo *= np.sqrt(info["mx_hi"] / (info["mx_hi"] + err))
-        hi *= np.sqrt(info["mx_lo"] / max(info["mx_lo"] - err, info["mx_lo"] * 0.5)) if info["mx_lo"] > 0 else 1.0
-    ulp = float(np.spacing(np.float32(r["new_dt"])))
-    assert lo - DT_ULPS * ulp <= impl_dt <= hi + DT_ULPS * ulp, f"{label}: dt {impl_dt!r} outside [{lo!r}, {hi!r}] (ref64 {r['new_dt']!r})"
-
-
-def collider_report(case, label, counts):
-    total = sum(len(m["pos"]) for m in case["models"]) * len(case["steps"])
-    print(f"{label}: near nodes {counts['near']} of {counts['resolved']}, tainted particles {counts['tainted_particles']} of {total}, "
-          f"tainted cells {counts['tainted_cells']}, worst x test_ref64_cpu's KAPPA {counts['worst']}")
-    assert counts["near"] <= case.get("max_near_nodes", MAX_NEAR_NODES) * max(counts["resolved"], 1), f"{label}: {counts}"
-    assert counts["tainted_particles"] <= case.get("max_tainted", MAX_TAINTED) * total, f"{label}: {counts}"
-    assert counts["near_branch"] <= case.get("max_near_branch", 0.01) * total, f"{label}: {counts}"
-
-
-def substep_compare(case, r, keys, grid, before, after, dt_after, label, counts):
-    check_counts(r, before, after, case["max_ppc"], label)
-    rep = ref64.compare(r, keys, grid, after, COLLIDER_KAPPA, STRESS_ALLOW, [F_ALLOW[m["material"]] for m in case["models"]], margin=BRANCH_MARGIN,
-                        max_ppc=case["max_ppc"])
-    check_report(rep, label)
-    check_dt_range(dt_after, r, label)
-    info = r["collider_info"]
-    if info["near"] is not None:
-        counts["near"] += int(info["near"].sum())
-        counts["resolved"] += int((info["branch"] != "").sum())   # nodes with mass: the ones the collider resolves
-    for q in ("tainted_particles", "tainted_cells", "near_branch"):
-        counts[q] += rep[q]
-    for q in ("mass", "momentum", "pos", "F"):
-        counts["worst"][q] = round(max(counts["worst"].get(q, 0.0), rep[q] * COLLIDER_KAPPA[q] / KAPPA[q]), 3)
-
-
-def new_counts():
-    return dict(near=0, resolved=0, tainted_particles=0, tainted_cells=0, near_branch=0, worst={})
-
-
-def oracle_collider_check(ob, case, label):
-    osim = S.build_oracle(ob, case)
-    clock = S.OracleClock(osim)
-    ccol, objs = S.ref_collider(case), S.ref_objects(case)
-    nm = len(case["models"])
-    done = 0
-    counts = new_counts()
-    for k in case["steps"]:
-        clock.step(k - done)
-        t = np.float32(osim.sim_time) if ccol is not None or objs else 0.0
-        _, nbc, _ = osim.block_counts()
-        before = [osim.particle_state(i) for i in range(nm)]
-        r = ref64.substep(osim.cfg, ref_models(case, before), osim.active_keys()[:nbc], osim.grid(), osim.dt, case["dt"], clock.time_left(), ccol, t,
-                          objects=objs)
-        clock.step(1)
-        done = k + 1
-        _, nbc, _ = osim.block_counts()
-        after = [osim.particle_state(i) for i in range(nm)]
-        substep_compare(case, r, osim.active_keys()[:nbc], osim.grid(), before, after, osim.dt, f"{label} sub-step {k}", counts)
-    osim.close()
-    collider_report(case, label, counts)
-    return counts
-
-
 @pytest.mark.parametrize("name", list(S.COLLIDER_CASES))
 def test_ref64_collider_cases_match_oracle(oracle, name):
-    oracle_collider_check(oracle, S.COLLIDER_CASES[name], name)
+    oracle_substep_check(oracle, S.COLLIDER_CASES[name], name)
 
 
 def test_collider_cases_act():

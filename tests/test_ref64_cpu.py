@@ -1,97 +1,24 @@
 """The float64 reference (tests/ref64.py) against the FP32 oracle, one sub-step at a time, and its own identities.
 
 For every case: the oracle's state at sub-step k -> ref64 for one sub-step -> compared with the oracle at k + 1 per grid
-cell (by key) and per particle (matched by position), each against its own bound kappa * 2^-24 * M (ref64.compare).
-The kappa values below are the smallest round values the FP32 oracle passes over this whole matrix; the GPU tests
-(test_gpu_ref64.py) hold the engine to the same values.
+cell (by key) and per particle (matched by position), each against its own bound kappa * 2^-24 * M (ref64.compare), in
+ref64_checks.oracle_substep_check.  ref64_checks.KAPPA holds the smallest round values the FP32 oracle passes over this whole
+matrix; the GPU tests (test_gpu_ref64.py) hold the engine to the same values.
 """
 import numpy as np
 import pytest
 
 import ref64
 import ref64_cases as S
+from ref64_checks import BRANCH_MARGIN, F_ALLOW, KAPPA, RASTER_KAPPA, STRESS_ALLOW, check_report, oracle_substep_check, ref_models
 
-# kappa per quantity; beside each, the oracle's worst |oracle - ref64| / (2^-24 M) over CASES
-KAPPA = dict(
-    mass=1.0,       # oracle worst 0.63 (domain_bits_5)
-    momentum=0.2,   # oracle worst 0.127 (fluid_clamp); M includes the sensitivity to the stored position's last bit
-    pos=2.0,        # oracle worst 1.89 (fluid_clamp)
-    F=4.0,          # oracle worst 3.4 (cfl_bound; J, F, logJp)
-)
-# set-up rasterisation sums up to 27 x 8 terms per node in any order, and its M has no position-sensitivity term
-RASTER_KAPPA = dict(mass=32.0, momentum=32.0, pos=1.0, F=1.0)   # oracle worst 19.4 (walls)
-# a constitutive model's own error, in units of its stress scale (DESIGN.md section 3, device math unit tests):
-# fixed-corotated 3e-5 of (2 mu + lambda) vol |F|^2; sand and NACC 3e-5 of the stress, 2e-5 of F and logJp
-STRESS_ALLOW = 3e-5
-F_ALLOW = {ref64.J_FLUID: 0.0, ref64.FIXED_COROTATED: 0.0, ref64.SAND: 2e-5, ref64.NACC: 2e-5}
-BRANCH_MARGIN = 1e-4
-# The new dt is sqrt, then a division, after the max of FP32 |v|^2: three roundings, so one ulp (what a single correctly
-# rounded operation would give) is not reachable in FP32.  The oracle's worst case is 1.01 ulp (cfl_bound); 2 is the next
-# whole number of ulps.
-DT_ULPS = 2.0
 # grid update (kernel level): v = mv * (1 / m), masked, + g dt: a few roundings of the magnitude |mv / m| + |g dt|
 VEL_KAPPA = 4.0   # oracle worst 2.13; the max |v|^2 within 4 x 2^-24 relative (oracle worst 1.63)
 
 
-def check_report(rep, label):
-    for q in ("mass", "momentum", "pos", "F"):
-        assert rep[q] <= 1.0, f"{label}: {q} error is {rep[q]:.3g} x its bound ({rep['worst']})"
-
-
-def check_dt(impl_dt, ref_dt, label):
-    ulp = float(np.spacing(np.float32(ref_dt)))
-    assert abs(impl_dt - ref_dt) <= DT_ULPS * ulp, f"{label}: dt {impl_dt!r} vs reference {ref_dt!r} ({(impl_dt - ref_dt) / ulp:.2f} ulp)"
-
-
-def check_counts(r, before, after, max_ppc, label):
-    """No particle disappears unless ref64 says so: the count after a sub-step is n - lost - what overflowing cells drop."""
-    for m, (res, b, a) in enumerate(zip(r["models"], before, after)):
-        _, n_over, kept = ref64.cell_overflow(res, max_ppc)
-        lost = int(res["lost"].sum())
-        assert len(a) == kept, (f"{label}: model {m} has {len(a)} particles after the sub-step, {len(b)} before; ref64 predicts {kept} "
-                                f"({lost} lost, {len(b) - lost - kept} dropped from {n_over} cells over max_ppc = {max_ppc})")
-
-
-def ref_models(case, states):
-    return [dict(material=m["material"], params=S.ref_params(m), state=s) for m, s in zip(case["models"], states)]
-
-
-def oracle_substep_check(ob, case, label):
-    """Run the oracle through case['steps']; at each, one ref64 sub-step against the oracle's next one."""
-    osim = S.build_oracle(ob, case)
-    clock = S.OracleClock(osim)
-    nm = len(case["models"])
-    done = 0
-    near = 0
-    worst = dict(mass=0.0, momentum=0.0, pos=0.0, F=0.0)
-    for k in case["steps"]:
-        clock.step(k - done)
-        _, nbc, _ = osim.block_counts()
-        before = [osim.particle_state(i) for i in range(nm)]
-        r = ref64.substep(osim.cfg, ref_models(case, before), osim.active_keys()[:nbc], osim.grid(), osim.dt, case["dt"], clock.time_left())
-        clock.step(1)
-        done = k + 1
-        _, nbc, _ = osim.block_counts()
-        after = [osim.particle_state(i) for i in range(nm)]
-        check_counts(r, before, after, case["max_ppc"], f"{label} sub-step {k}")
-        rep = ref64.compare(r, osim.active_keys()[:nbc], osim.grid(), after, KAPPA, STRESS_ALLOW, [F_ALLOW[m["material"]] for m in case["models"]],
-                            margin=BRANCH_MARGIN, max_ppc=case["max_ppc"])
-        check_report(rep, f"{label} sub-step {k}")
-        check_dt(osim.dt, r["new_dt"], f"{label} sub-step {k}")
-        near += rep["near_branch"]
-        for q in worst:
-            worst[q] = max(worst[q], rep[q])
-    osim.close()
-    return worst, near
-
-
 @pytest.mark.parametrize("name", [n for n, c in S.CASES.items() if c.get("oracle", True)])
 def test_ref64_matches_oracle(oracle, name):
-    case = S.CASES[name]
-    worst, near = oracle_substep_check(oracle, case, name)
-    total = sum(len(m["pos"]) for m in case["models"]) * len(case["steps"])
-    # the branch-point exclusion is for the odd particle; a case where it hides a large share proves nothing
-    assert near <= case.get("max_near_branch", 0.01) * total, f"{name}: {near} of {total} particle updates within {BRANCH_MARGIN} of a branch point"
+    oracle_substep_check(oracle, S.CASES[name], name)
 
 
 @pytest.mark.parametrize("cases,want", [(("sand_floor",), {"tip", "elastic", "yield"}),
@@ -131,7 +58,7 @@ def grid_mass(grid):
 @pytest.mark.parametrize("name", ["overflow_fc_in_block", "overflow_fluid_cross_block"])
 def test_cell_overflow_in_g2p2g_oracle(oracle, name):
     """A cell that receives more than max_ppc particles in g2p2g keeps max_ppc of them (ref64.compare with max_ppc in
-    oracle_substep_check); the grid of that sub-step has every particle's mass, the next one is short by exactly the mass of
+    ref64_checks.oracle_substep_check); the grid of that sub-step has every particle's mass, the next one is short by exactly the mass of
     the dropped particles."""
     case = S.CASES[name]
     osim = S.build_oracle(oracle, case)

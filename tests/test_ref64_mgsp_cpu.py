@@ -13,7 +13,7 @@ import ref64_cases as S
 import ref64_mgsp as M
 from claymore_b200 import mgsp
 from claymore_b200._capi import Config
-from test_ref64_cpu import BRANCH_MARGIN, DT_ULPS, F_ALLOW, KAPPA, RASTER_KAPPA, STRESS_ALLOW, check_report
+from ref64_checks import BRANCH_MARGIN, DT_ULPS, F_ALLOW, KAPPA, RASTER_KAPPA, STRESS_ALLOW, check_report, rank_models
 
 
 # ---- splits of a case ------------------------------------------------------------------------------------------------------
@@ -31,10 +31,6 @@ def split_case(case, world, kind):
             part = mgsp.partition_scene_global(scene, r, world)
         out.append([dict(case["models"][p["model"]], pos=p["pos"], model=p["model"]) for p in part["models"]])
     return out
-
-
-def rank_models(parts, states):
-    return [dict(model=p["model"], material=p["material"], params=S.ref_params(p), state=s) for p, s in zip(parts, states)]
 
 
 # ---- synthetic shards from ref64's own output --------------------------------------------------------------------------------

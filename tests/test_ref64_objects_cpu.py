@@ -5,7 +5,7 @@ masses log-uniform from 1e-12 to 1 with zero and subnormal nodes, velocities N(0
 {0, 0.3, -0.2} x {static, combined motion} x t {0, 0.37, 3.1} x boundary {2, 0}, plus the 16-object list and the level-set
 collider with two objects.  Per node: |v - ref64| <= COLLIDER_VEL_KAPPA 2^-24 E, nodes near a discontinuity (ref64's margin)
 left out and counted; the max within COLLIDER_MAX_REL of [mx_lo, mx_hi].  Per sub-step: the oracle with the objects through
-OBJECT_CASES with COLLIDER_KAPPA.  The kappa values are test_ref64_collider_cpu's: the oracle's worst ratios over this matrix
+OBJECT_CASES with COLLIDER_KAPPA.  The kappa values are the collider's (ref64_checks, test_ref64_collider_cpu): the oracle's worst ratios over this matrix
 stay under them (printed per entry).  The GPU tests (test_gpu_objects_ref64.py) hold the engine to the same values.
 """
 import ctypes as C
@@ -15,9 +15,8 @@ import pytest
 
 import ref64
 import ref64_cases as S
-from test_ref64_collider_cpu import (FIELDS, FRICTIONS, MAX_NEAR_NODES, MOTIONS, TIMES, TYPES, block_field, check_collider_update, collider_of,
-                                     oracle_collider_check)
-from test_ref64_cpu import ref_models
+from ref64_checks import MAX_NEAR_NODES, oracle_substep_check, ref_models
+from test_ref64_collider_cpu import FIELDS, FRICTIONS, MOTIONS, TIMES, TYPES, block_field, check_collider_update, collider_of
 
 DOMAIN_BITS = 6
 SHAPES = {
@@ -201,7 +200,7 @@ def test_objects_kernel_reaches_every_branch(oracle):
 # ---- per sub-step: the oracle with the objects through OBJECT_CASES --------------------------------------------------------
 @pytest.mark.parametrize("name", list(S.OBJECT_CASES))
 def test_ref64_object_cases_match_oracle(oracle, name):
-    oracle_collider_check(oracle, S.OBJECT_CASES[name], name)
+    oracle_substep_check(oracle, S.OBJECT_CASES[name], name)
 
 
 def test_object_cases_act():
