@@ -1,10 +1,12 @@
 """The scene runner, the reference's `gmpm -f scene.json` (Projects/GMPM/gmpm.cu):
 
-    python -m claymore_b200 -f scene.json [--out DIR] [--attributes v,J] [--resume CKPT]
+    python -m claymore_b200 -f scene.json [--out DIR] [--attributes v,J] [--resume CKPT] [--forces]
 
 parse_scene, then main_loop: every finished frame is written to DIR (default: the working directory) as
 model_id[i]_frame[f].bgeo, with the per-particle attributes listed (v: velocity, J: volume ratio).  --resume continues a
-checkpoint of the same scene and writes only its remaining frames.
+checkpoint of the same scene and writes only its remaining frames.  --forces also writes DIR/forces.csv: per finished frame and
+body (0: the "collider", then the "boundaries" in document order) the mean force and torque the material exerted on it over the
+frame (scene.force_recorder); a resumed run appends its frames' rows, a fresh run truncates the file.
 
     python -m claymore_b200 mesh2sdf in.obj out.sdf --h H [--padding P] [--exact-band B]
 
@@ -15,7 +17,7 @@ import argparse
 import os
 import sys
 
-from .scene import parse_scene
+from .scene import force_recorder, parse_scene
 
 
 def mesh2sdf(argv):
@@ -46,6 +48,7 @@ def main(argv=None):
     ap.add_argument("--out", default=".", help="directory of the .bgeo files")
     ap.add_argument("--attributes", default="", help="comma-separated per-particle attributes: v, J")
     ap.add_argument("--resume", default=None, help="checkpoint of this scene to continue from")
+    ap.add_argument("--forces", action="store_true", help="write the mean force and torque on each collision body per frame to DIR/forces.csv")
     args = ap.parse_args(argv)
     attributes = [a for a in args.attributes.split(",") if a]
     for a in attributes:
@@ -53,11 +56,16 @@ def main(argv=None):
             ap.error(f"unknown attribute {a!r} (known: v, J)")
     if not os.path.isdir(args.out):
         ap.error(f"output directory {args.out!r} does not exist")
-    sim = parse_scene(args.file, resume=args.resume)
+    sim = parse_scene(args.file, resume=args.resume, forces=args.forces)
+    on_frame, fh = None, None
     try:
-        sim.main_loop(output=args.out, attributes=attributes)
+        if args.forces:
+            on_frame, fh = force_recorder(sim, os.path.join(args.out, "forces.csv"), append=args.resume is not None)
+        sim.main_loop(on_frame=on_frame, output=args.out, attributes=attributes)
         err = sim.stats().error
     finally:
+        if fh is not None:
+            fh.close()
         sim.close()
     if err:
         print(f"simulation stopped with error bits {err}", file=sys.stderr)

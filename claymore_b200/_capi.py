@@ -77,6 +77,7 @@ class Collider(C.Structure):
 
 SHAPE_PLANE, SHAPE_BOX, SHAPE_SPHERE, SHAPE_CYLINDER = 0, 1, 2, 3   # CB200_SHAPE_*
 MAX_COLLISION_OBJECTS = 16                                           # CB200_MAX_COLLISION_OBJECTS
+FORCE_COMPONENTS = 6                                                 # CB200_FORCE_COMPONENTS: (Jx, Jy, Jz, Lx, Ly, Lz) per body
 SHAPE_LEVELSET = 4                                                   # CB200_SHAPE_LEVELSET
 MAX_COLLISION_LEVELSETS = 16                                         # CB200_MAX_COLLISION_LEVELSETS
 
@@ -167,6 +168,8 @@ _SIGNATURES = {
     "cb200_update_grid_velocity_query_max_objects": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), C.POINTER(CollisionObject), _I, _F, _P, _P],
     "cb200_update_grid_velocity_query_max_levelsets": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), C.POINTER(CollisionObject), _I,
                                                        C.POINTER(LevelSetLattice), _I, _F, _P, _P],
+    "cb200_update_grid_velocity_query_max_forces": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), C.POINTER(CollisionObject), _I,
+                                                    C.POINTER(LevelSetLattice), _I, _F, _P, _P, _P],
     "cb200_levelset_prepare": [C.POINTER(SdfHeader), _P, _P, _P],
     "cb200_clear_grid": [_I, _P, _P],
     "cb200_cell_bucket_to_block": [_CFG, _I, _P, _P, _P, _P, _P],
@@ -217,6 +220,8 @@ _SIGNATURES = {
     "cb200_sim_add_collision_levelset": [_P, C.POINTER(SdfHeader), _P, C.POINTER(_I)],
     "cb200_sim_clear_collision_levelsets": [_P],
     "cb200_sim_time": [_P, C.POINTER(C.c_double)],
+    "cb200_sim_set_force_report": [_P, _I],
+    "cb200_sim_collision_forces": [_P, _P, _I, C.POINTER(_I), C.POINTER(C.c_double)],
     "cb200_sim_mgsp_inbox": [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_size_t)],
     "cb200_sim_mgsp_ipc_handle": [_P, _P],
     "cb200_sim_mgsp_open_peers": [_P, _P],

@@ -122,8 +122,9 @@ int cb200_g2p2g(const cb200_config* c, float dt, float new_dt, int pbc, cb200_pa
 
 // The four kernel-level grid updates: the level set when collider is non-null (valid, with a field), then objs[0, n), placed at time;
 // level-set objects index lattices[0, n_lattices)
+// impulses (nullable): the report's device rows, added into (section 2.13)
 static int update_grid_boundaries(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream,
-                                  const cb200_levelset* lattices = nullptr, int n_lattices = 0) {
+                                  const cb200_levelset* lattices = nullptr, int n_lattices = 0, double* impulses = nullptr) {
 	CB_CFG(c);
 	if(n_lattices < 0 || n_lattices > CB200_MAX_COLLISION_LEVELSETS || (n_lattices > 0 && !lattices)) return (int) cudaErrorInvalidValue;
 	LevelSets ls {};
@@ -153,7 +154,8 @@ static int update_grid_boundaries(const cb200_config* c, int block_count, float*
 	a.clear_grid = nullptr;
 	a.n_clear = 0;
 	a.time = time;
-	launch_grid_update(a, bd, ls, grid_for(block_count, kGridThreads / 32), (cudaStream_t) stream);
+	const ForceArgs fa {impulses, nullptr, 0u};
+	launch_grid_update(a, bd, ls, grid_for(block_count, kGridThreads / 32), (cudaStream_t) stream, impulses ? &fa : nullptr);
 	return (int) cudaGetLastError();
 }
 
@@ -172,6 +174,11 @@ int cb200_update_grid_velocity_query_max_objects(const cb200_config* c, int bloc
 
 int cb200_update_grid_velocity_query_max_levelsets(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, float time, float* max_vel, void* stream) {
 	return update_grid_boundaries(c, block_count, grid, partition, dt, collider, objs, n, time, max_vel, stream, levelsets, n_levelsets);
+}
+
+int cb200_update_grid_velocity_query_max_forces(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, float time, float* max_vel, double* impulses, void* stream) {
+	if(!impulses) return (int) cudaErrorInvalidValue;
+	return update_grid_boundaries(c, block_count, grid, partition, dt, collider, objs, n, time, max_vel, stream, levelsets, n_levelsets, impulses);
 }
 
 int cb200_levelset_prepare(const cb200_sdf_header* header, const float* phi, float* lattice, void* stream) {

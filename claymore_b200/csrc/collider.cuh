@@ -404,6 +404,36 @@ __device__ __forceinline__ void boundaries_resolve(const Boundaries& b, const Bo
 	}
 }
 
+// The chain over the two cells a lane holds, (nx, ny, nz) and (nx, ny, nz + 1) (hx / hy: which have mass), one body at a time: each
+// body resolves both cells through the same collider_resolve as boundaries_resolve, then stage(k, f, in0, in1, in2) sees body k
+// (0: the level-set collider, 1 + i: object i), its frame f and the velocities it received (channels 0-2, .x / .y the two cells);
+// v0-v2 hold the velocities it left.  Each cell goes through the same calls in the same order as with boundaries_resolve.
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS, class Stage>
+__device__ __forceinline__ void boundaries_resolve_pair(const Boundaries& b, const BoundaryFrames& s, const Cfg& cfg, int nx, int ny, int nz, bool hx, bool hy, float2& v0, float2& v1,
+                                                        float2& v2, Stage&& stage) {
+	static_assert(OBJECTS || !LEVELSETS, "level-set objects are objects");
+	if constexpr(COLLIDE) {
+		const float2 i0 = v0, i1 = v1, i2 = v2;
+		auto q = [&](const float* x, float* n) { return collider_query(b.col, cfg, x, n); };
+		if(hx) collider_resolve(b.col, s.col, cfg.dx, nx, ny, nz, v0.x, v1.x, v2.x, q);
+		if(hy) collider_resolve(b.col, s.col, cfg.dx, nx, ny, nz + 1, v0.y, v1.y, v2.y, q);
+		stage(0, s.col, i0, i1, i2);
+	}
+	if constexpr(OBJECTS) {
+		for(int i = 0; i < b.objects.n; ++i) {
+			const cb200_collision_object& o = s.o[i];
+			const float2 i0 = v0, i1 = v1, i2 = v2;
+			auto q = [&](const float* x, float* n) {
+				if constexpr(LEVELSETS) return object_query_levelsets(o, x, n);
+				else return object_query(o, x, n);
+			};
+			if(hx) collider_resolve(o, s.f[i], cfg.dx, nx, ny, nz, v0.x, v1.x, v2.x, q);
+			if(hy) collider_resolve(o, s.f[i], cfg.dx, nx, ny, nz + 1, v0.y, v1.y, v2.y, q);
+			stage(1 + i, s.f[i], i0, i1, i2);
+		}
+	}
+}
+
 // grid-update velocity of one cell (wall mask, gravity on y, the chain) and its |v|^2, NaN -> +inf; no mass -> 0
 template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
 __device__ __forceinline__ float cell_vel_sq_boundaries(float m, float p0, float p1, float p2, bool wx, bool wy, bool wz, float gdt, const Boundaries& bd, const BoundaryFrames& s, const Cfg& cfg, int nx, int ny, int nz) {

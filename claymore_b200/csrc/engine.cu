@@ -384,6 +384,10 @@ struct cb200_sim {
 	// the lattices of the level-set collision objects (cb200_sim_add_collision_levelset), owned by this simulator, in registry order
 	LevelSets levelsets {};
 	long long frames_done = 0;  // frames finished by cb200_sim_advance_frame (restored from a checkpoint)
+	// the boundary impulse report (cb200_sim_set_force_report): its sums, [kForceBodies][kForceComps] doubles, then the simulated time of
+	// its last reset (force_reset)
+	bool force_report = false;
+	double* forces = nullptr;
 	// the rows each particle block starts at in every read-out, per model: the scans of the bucket sizes, [kMaxModels][max_blocks + 1]
 	int* ck_base = nullptr;
 	// checkpoint (cb200_sim_checkpoint_begin / _end): the blob, copied to the host on the staging's own stream
@@ -460,7 +464,8 @@ DevArrays sim_arrays(cb200_sim* s, size_t mb) {
 	        dev_array(s->grid[1], (mb + 1) * kGridBlockFloats, 0),
 	        dev_array(s->tile_sums, tiles * kScanComps, kNoFill),
 	        dev_array(s->block_totals, (size_t) kMaxModels * mb, kNoFill),
-	        dev_array(s->ck_base, (size_t) kMaxModels * (mb + 1), kNoFill)};
+	        dev_array(s->ck_base, (size_t) kMaxModels * (mb + 1), kNoFill),
+	        dev_array(s->forces, (size_t) kForceBodies * kForceComps + 1, 0)};
 }
 
 int fill_arrays(cb200_sim* s, const DevArrays& a) {
@@ -585,6 +590,14 @@ G2P2GArgs make_g2p2g_args(cb200_sim* s, int material, int R) {
 	return a;
 }
 
+// zeroes the report's sums and starts its span at StepState::sim_time, stream-ordered
+int force_reset(cb200_sim* s) {
+	constexpr size_t n = (size_t) kForceBodies * kForceComps;
+	CK(cudaMemsetAsync(s->forces, 0, n * sizeof(double), s->stream));
+	CK(cudaMemcpyAsync(s->forces + n, &s->d_state->sim_time, sizeof(double), cudaMemcpyDeviceToDevice, s->stream));
+	return 0;
+}
+
 // ---- phase A: grid update (+ fused clears) -------------------------------------------------------
 int enqueue_grid_update(cb200_sim* s, int R) {
 	const int Rn = R ^ 1;
@@ -603,7 +616,9 @@ int enqueue_grid_update(cb200_sim* s, int R) {
 	}
 	gu.n_clear = (int) s->models.size();
 	for(size_t m = 0; m < s->models.size(); ++m) gu.clear_counts[m] = s->models[m].pb[Rn].cell_particle_counts;
-	launch_grid_update(gu, s->boundaries, s->levelsets, grid_blocks(4), s->stream);  // placed at StepState::sim_time, the start of this sub-step
+	// MGSP: a block every rank holding it resolves counts on the lowest of them (the marks the previous sub-step's tagging left)
+	const ForceArgs fa {s->forces, s->desc.mgsp_world > 1 ? s->part[R].overlap_marks : nullptr, (1u << s->desc.mgsp_rank) - 1u};
+	launch_grid_update(gu, s->boundaries, s->levelsets, grid_blocks(4), s->stream, s->force_report ? &fa : nullptr);  // placed at StepState::sim_time, the start of this sub-step
 	++s->launches;
 	return (int) cudaGetLastError();
 }
@@ -1333,7 +1348,7 @@ int cb200_sim_initial_setup(cb200_sim* s) {
 	if(!s) return (int) cudaErrorInvalidValue;
 	CK(setup_impl(s, s->restore.start()));
 	s->restore.release();  // (setup_impl has synchronised: a staged state is in the bins and the grid now)
-	return 0;
+	return force_reset(s);  // a restore starts the report's span at the restored clock; adding or removing particles keeps the sums
 }
 
 static int set_frame_roll(cb200_sim* s, int on) {
@@ -1490,6 +1505,7 @@ int cb200_sim_set_collider(cb200_sim* s, const cb200_collider* params, const flo
 	s->boundaries.col = *params;
 	s->boundaries.col.sdf = s->sdf;
 	s->boundaries.has_collider = true;
+	CK(force_reset(s));
 	return recapture(s);
 }
 int cb200_sim_clear_collider(cb200_sim* s) {
@@ -1499,6 +1515,7 @@ int cb200_sim_clear_collider(cb200_sim* s) {
 	s->boundaries.col = ColliderView {};
 	g_pool.release(s->sdf);
 	s->sdf = nullptr;
+	CK(force_reset(s));
 	return recapture(s);
 }
 int cb200_sim_set_collision_objects(cb200_sim* s, const cb200_collision_object* objs, int n) {
@@ -1506,6 +1523,7 @@ int cb200_sim_set_collision_objects(cb200_sim* s, const cb200_collision_object* 
 	if(!s || !objects_prepare(objs, n, l, s->levelsets.count)) return (int) cudaErrorInvalidValue;
 	CK(cudaStreamSynchronize(s->stream));
 	s->boundaries.objects = l;
+	CK(force_reset(s));
 	return recapture(s);
 }
 // phi is uploaded into scratch, the lattice built from it on the device; the registry takes the lattice only once it is complete
@@ -1545,6 +1563,27 @@ int cb200_sim_time(cb200_sim* s, double* time) {
 	*time = s->h_state->sim_time;
 	return 0;
 }
+// ---- the boundary impulse report (DESIGN.md section 2.13) ---------------------------------------------------------------------
+int cb200_sim_set_force_report(cb200_sim* s, int enable) {
+	if(!s) return (int) cudaErrorInvalidValue;
+	CK(cudaStreamSynchronize(s->stream));
+	s->force_report = enable != 0;
+	CK(force_reset(s));
+	return recapture(s);
+}
+int cb200_sim_collision_forces(cb200_sim* s, double* out, int capacity, int* n_bodies, double* elapsed) {
+	const int rows = s ? 1 + s->boundaries.objects.n : 0;
+	if(!s || !s->force_report || !out || !n_bodies || !elapsed || capacity < rows) return (int) cudaErrorInvalidValue;
+	constexpr size_t n = (size_t) kForceBodies * kForceComps;
+	double h[n + 1];
+	CK(cudaMemcpyAsync(h, s->forces, sizeof(h), cudaMemcpyDeviceToHost, s->stream));
+	CK(pull_state(s));  // synchronises
+	memcpy(out, h, (size_t) rows * kForceComps * sizeof(double));
+	*n_bodies = rows;
+	*elapsed = s->h_state->sim_time - h[n];
+	return force_reset(s);
+}
+
 // ---- checkpoint / restore (format and kernels: checkpoint.cuh) ---------------------------------------------------------------
 int cb200_checkpoint_inspect(const void* blob, size_t bytes, cb200_checkpoint_info* info) { return ck_parse(blob, bytes, info); }
 

@@ -27,6 +27,58 @@ struct GridUpdateArgs {
 template<bool COLLIDE, bool OBJECTS>
 constexpr int kBoundaryMinCtas = OBJECTS ? 2 : 4;
 
+// ---- the boundary impulse report (DESIGN.md section 2.13) ----------------------------------------------------------------------
+// Body 0 is the level-set collider, body 1 + i object i of the list.  Per body the grid update adds J = sum m (v_in - v_out) and
+// L = sum (p - b(t)) x m (v_in - v_out) over the nodes with mass, v_in the velocity the body receives in the chain and v_out the one it
+// leaves, p = n dx and b(t) = trans + trans_vel t the pivot its omega turns about; (Jx, Jy, Jz, Lx, Ly, Lz) per body.
+constexpr int kForceBodies = 1 + CB200_MAX_COLLISION_OBJECTS;
+constexpr int kForceComps = 6;
+// A kernel parameter of its own beside Boundaries, so that GridUpdateArgs and the instances without the report keep their block.
+struct ForceArgs {
+	double* impulses;          // [kForceBodies][6], added into (one atomicAdd per CTA and non-zero component)
+	const int* overlap_marks;  // nullable (MGSP): bit p of block b set when peer p also resolves b; b counts on the lowest rank holding it
+	unsigned lower_ranks;      // (1u << rank) - 1
+};
+// the CTA's per-warp sums: each warp's lane 0 adds to its own slot, the CTA adds the 8 slots at its end
+__device__ __forceinline__ double (*force_slots())[kForceBodies * kForceComps] {
+	__shared__ double s[kGridThreads / 32][kForceBodies * kForceComps];
+	return s;
+}
+__device__ __forceinline__ void force_slots_clear() {
+	double* s = &force_slots()[0][0];
+	for(int i = threadIdx.x; i < (kGridThreads / 32) * kForceBodies * kForceComps; i += kGridThreads) s[i] = 0.0;
+}
+// body k's impulse on the two cells a lane holds (velocities in i*, out o*; hx / hy: which have mass) added to the warp's slot k; the
+// offset p - b is collider_material_point's xm.  A warp in which no lane changed a velocity skips the reduction (a lane's two
+// contributions may cancel in J and not in L, so the test is on the velocities, not on the sums).
+__device__ __forceinline__ void warp_body_impulse(double* slot, int lane, float dx, int nx, int ny, int nz, float2 m, bool hx, bool hy, const ColliderFrame& f, float2 i0, float2 i1, float2 i2,
+                                                  float2 o0, float2 o1, float2 o2) {
+	float r[kForceComps] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+	auto cell = [&](float mc, int z, float d0, float d1, float d2) {
+		const float j[3] = {mc * d0, mc * d1, mc * d2};
+		const float xm[3] = {(float) nx * dx - f.b[0], (float) ny * dx - f.b[1], (float) z * dx - f.b[2]};
+		r[0] += j[0];
+		r[1] += j[1];
+		r[2] += j[2];
+		r[3] += xm[1] * j[2] - xm[2] * j[1];
+		r[4] += xm[2] * j[0] - xm[0] * j[2];
+		r[5] += xm[0] * j[1] - xm[1] * j[0];
+	};
+	const bool cx = hx && (i0.x != o0.x || i1.x != o1.x || i2.x != o2.x), cy = hy && (i0.y != o0.y || i1.y != o1.y || i2.y != o2.y);
+	if(!__any_sync(0xffffffffu, cx || cy)) return;
+	if(cx) cell(m.x, nz, i0.x - o0.x, i1.x - o1.x, i2.x - o2.x);
+	if(cy) cell(m.y, nz + 1, i0.y - o0.y, i1.y - o1.y, i2.y - o2.y);
+#pragma unroll
+	for(int c = 0; c < kForceComps; ++c) {
+#pragma unroll
+		for(int off = 16; off > 0; off >>= 1) r[c] += __shfl_xor_sync(0xffffffffu, r[c], off);
+	}
+	if(lane == 0) {
+#pragma unroll
+		for(int c = 0; c < kForceComps; ++c) slot[c] += (double) r[c];
+	}
+}
+
 // update_grid_velocity_query_max (mgmpm_kernels.cuh:325-420): one warp per grid block, two cells per lane as
 // one 8-byte access per channel; warp max by redux, one atomicMax per CTA on the float's bit pattern.
 // Quirks kept: wall blocks zero the masked component BEFORE gravity is added to y (Appendix B #1);
@@ -34,9 +86,13 @@ constexpr int kBoundaryMinCtas = OBJECTS ? 2 : 4;
 // COLLIDE / OBJECTS: the MGSP form with a Boundary (mgmpm_kernels.cuh:323-399): after gravity, cells with mass resolve against the
 // boundary chain of `bd` (collider.cuh: the SignedDistanceGrid, then the analytic objects of DESIGN.md section 2.9); the max is |v|^2
 // where that kernel reports 2|v|^2 (Appendix B #11).
-template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
-__device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const Boundaries* bd) {
+// FORCES: the chain runs one body at a time over both cells of a lane (boundaries_resolve_pair) and each body's impulse is added to
+// fa->impulses (section 2.13); the velocities are those of the instance without it.
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false, bool FORCES = false>
+__device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const Boundaries* bd, const ForceArgs* fa = nullptr) {
+	static_assert(!FORCES || COLLIDE || OBJECTS, "the report needs a body");
 	__shared__ unsigned s_max[kGridThreads / 32];
+	if constexpr(FORCES) force_slots_clear();  // published by the frame builder's barrier
 	const BoundaryFrames* fr = nullptr;
 	if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, a.state ? (float) a.state->sim_time : a.time);
 	const Cfg& cfg = a.cfg;
@@ -57,21 +113,44 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 			float2 v0 = blk[32 + lane], v1 = blk[64 + lane], v2 = blk[96 + lane];
 			float sq0 = 0.f, sq1 = 0.f;
 			const bool hx = node_has_mass(m.x), hy = node_has_mass(m.y);
-			if(hx) {
-				const float mi = 1.f / m.x;
-				v0.x = wx ? 0.f : v0.x * mi;
-				v1.x = (wy ? 0.f : v1.x * mi) + gdt;
-				v2.x = wz ? 0.f : v2.x * mi;
-				if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
-				sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
-			}
-			if(hy) {
-				const float mi = 1.f / m.y;
-				v0.y = wx ? 0.f : v0.y * mi;
-				v1.y = (wy ? 0.f : v1.y * mi) + gdt;
-				v2.y = wz ? 0.f : v2.y * mi;
-				if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
-				sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
+			if constexpr(FORCES) {
+				if(hx) {
+					const float mi = 1.f / m.x;
+					v0.x = wx ? 0.f : v0.x * mi;
+					v1.x = (wy ? 0.f : v1.x * mi) + gdt;
+					v2.x = wz ? 0.f : v2.x * mi;
+				}
+				if(hy) {
+					const float mi = 1.f / m.y;
+					v0.y = wx ? 0.f : v0.y * mi;
+					v1.y = (wy ? 0.f : v1.y * mi) + gdt;
+					v2.y = wz ? 0.f : v2.y * mi;
+				}
+				const int nx = 4 * kx + (lane >> 3), ny = 4 * ky + ((lane >> 1) & 3), nz = 4 * kz + 2 * (lane & 1);
+				const bool counted = !fa->overlap_marks || (fa->overlap_marks[b] & fa->lower_ranks) == 0u;  // warp-uniform
+				double* slots = force_slots()[warp];
+				boundaries_resolve_pair<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, nx, ny, nz, hx, hy, v0, v1, v2, [&](int k, const ColliderFrame& f, float2 i0, float2 i1, float2 i2) {
+					if(counted) warp_body_impulse(slots + k * kForceComps, lane, cfg.dx, nx, ny, nz, m, hx, hy, f, i0, i1, i2, v0, v1, v2);
+				});
+				if(hx) sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
+				if(hy) sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
+			} else {
+				if(hx) {
+					const float mi = 1.f / m.x;
+					v0.x = wx ? 0.f : v0.x * mi;
+					v1.x = (wy ? 0.f : v1.x * mi) + gdt;
+					v2.x = wz ? 0.f : v2.x * mi;
+					if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
+					sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
+				}
+				if(hy) {
+					const float mi = 1.f / m.y;
+					v0.y = wx ? 0.f : v0.y * mi;
+					v1.y = (wy ? 0.f : v1.y * mi) + gdt;
+					v2.y = wz ? 0.f : v2.y * mi;
+					if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
+					sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
+				}
 			}
 			if(hx || hy) {
 				blk[32 + lane] = v0;
@@ -100,6 +179,14 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 		for(int i = 1; i < kGridThreads / 32; ++i) m = max(m, s_max[i]);
 		if(m) atomicMax(reinterpret_cast<unsigned*>(a.max_vel), m);
 	}
+	if constexpr(FORCES) {  // behind the max's barrier: every warp's slots are complete
+		for(int i = threadIdx.x; i < kForceBodies * kForceComps; i += kGridThreads) {
+			double sum = 0.0;
+#pragma unroll
+			for(int w = 0; w < kGridThreads / 32; ++w) sum += force_slots()[w][i];
+			if(sum != 0.0) atomicAdd(fa->impulses + i, sum);
+		}
+	}
 }
 __global__ void __launch_bounds__(kGridThreads) grid_update_kernel(const GridUpdateArgs a) { grid_update_body<false, false>(a, nullptr); }
 // the same with the boundaries of bd (COLLIDE: bd.has_collider; OBJECTS: bd.objects.n >= 1)
@@ -115,6 +202,19 @@ __global__ void __launch_bounds__(kGridThreads, (kBoundaryMinCtas<COLLIDE, true>
 	grid_update_body<COLLIDE, true, true>(a, &bd);
 }
 static_assert(sizeof(GridUpdateArgs) + sizeof(Boundaries) + sizeof(LevelSets) <= 4096, "the level-set grid update's parameters must fit the 4 KiB kernel-parameter limit");
+// the two with the impulse report of fa (section 2.13)
+template<bool COLLIDE, bool OBJECTS>
+__global__ void __launch_bounds__(kGridThreads, (kBoundaryMinCtas<COLLIDE, OBJECTS>)) grid_update_boundary_forces_kernel(const GridUpdateArgs a, const __grid_constant__ Boundaries bd, const __grid_constant__ ForceArgs fa) {
+	grid_update_body<COLLIDE, OBJECTS, false, true>(a, &bd, &fa);
+}
+static_assert(sizeof(GridUpdateArgs) + sizeof(Boundaries) + sizeof(ForceArgs) <= 4096, "the reporting boundary grid update's parameters must fit the 4 KiB kernel-parameter limit");
+template<bool COLLIDE>
+__global__ void __launch_bounds__(kGridThreads, (kBoundaryMinCtas<COLLIDE, true>)) grid_update_levelset_forces_kernel(const GridUpdateArgs a, const __grid_constant__ Boundaries bd, const __grid_constant__ LevelSets ls,
+                                                                                                                     const __grid_constant__ ForceArgs fa) {
+	levelset_views_cta(ls);
+	grid_update_body<COLLIDE, true, true, true>(a, &bd, &fa);
+}
+static_assert(sizeof(GridUpdateArgs) + sizeof(Boundaries) + sizeof(LevelSets) + sizeof(ForceArgs) <= 4096, "the reporting level-set grid update's parameters must fit the 4 KiB kernel-parameter limit");
 
 // clear_grid (mgmpm_kernels.cuh:106-115)
 __global__ void clear_grid_kernel(int block_count, float* grid) {
@@ -259,12 +359,18 @@ void for_each_boundary_instance(F&& f) {
 	f(std::false_type(), std::true_type());
 	f(std::true_type(), std::true_type());
 }
-// ls: the lattices bd's level-set objects index (read only when one is)
-inline void launch_grid_update(const GridUpdateArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st) {
+// ls: the lattices bd's level-set objects index (read only when one is); fa (nullable): report the impulses there (no body: nothing)
+inline void launch_grid_update(const GridUpdateArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st, const ForceArgs* fa = nullptr) {
 	with_boundaries(bd, [&](auto C, auto O, auto L) {
-		if constexpr(L) grid_update_levelset_kernel<C><<<ctas, kGridThreads, 0, st>>>(a, bd, ls);
-		else if constexpr(C || O) grid_update_boundary_kernel<C, O><<<ctas, kGridThreads, 0, st>>>(a, bd);
-		else grid_update_kernel<<<ctas, kGridThreads, 0, st>>>(a);
+		if constexpr(L) {
+			if(fa) grid_update_levelset_forces_kernel<C><<<ctas, kGridThreads, 0, st>>>(a, bd, ls, *fa);
+			else grid_update_levelset_kernel<C><<<ctas, kGridThreads, 0, st>>>(a, bd, ls);
+		} else if constexpr(C || O) {
+			if(fa) grid_update_boundary_forces_kernel<C, O><<<ctas, kGridThreads, 0, st>>>(a, bd, *fa);
+			else grid_update_boundary_kernel<C, O><<<ctas, kGridThreads, 0, st>>>(a, bd);
+		} else {
+			grid_update_kernel<<<ctas, kGridThreads, 0, st>>>(a);
+		}
 	});
 }
 inline void launch_carry_grid(const CarryArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st) {

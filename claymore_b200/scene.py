@@ -54,6 +54,7 @@ count), before the sources emit, the sinks due at that frame with the same "mode
 CB200_MAX_COLLISION_OBJECTS sinks in one such group).  A resumed run applies exactly the frames after the checkpoint's frame.  Bad
 keys or values, too many sinks in one group, or "sinks" in MGSP mode raise ValueError before any device work.
 """
+import csv
 import json
 import os
 
@@ -396,11 +397,42 @@ def _check_resume(doc, cfg, resume):
     return inf
 
 
-def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_kwargs):
+FORCE_COLUMNS = ("frame", "time", "body", "shape", "Fx", "Fy", "Fz", "Tx", "Ty", "Tz")
+
+
+def force_bodies(doc):
+    """The shape of each body of the impulse report: the "collider" (body 0, "none" without one), then the "boundaries" entries in
+    document order."""
+    return ["collider" if "collider" in doc else "none"] + [b.get("shape", "") for b in doc.get("boundaries", [])]
+
+
+def force_recorder(sim, path, append=False):
+    """(on_frame, file): main_loop's per-frame hook that writes one CSV row per body of sim.force_bodies to `path` (FORCE_COLUMNS): the
+    frame, the simulated time at its end and the mean force and torque over the frame, the impulses read and reset once per frame.
+    append: continue the file of an interrupted run (a resumed run's frames follow its checkpoint's); else it is truncated."""
+    f = open(path, "a" if append else "w", newline="")
+    w = csv.writer(f)
+    if f.tell() == 0:
+        w.writerow(FORCE_COLUMNS)
+    shapes = sim.force_bodies
+
+    def on_frame(s, frame):
+        elapsed, imp = s.collision_forces()
+        t = s.sim_time()
+        mean = imp / elapsed if elapsed > 0 else np.zeros_like(imp)
+        for k, row in enumerate(mean):
+            w.writerow([frame, "%.17g" % t, k, shapes[k]] + ["%.17g" % x for x in row])
+        f.flush()
+    return on_frame, f
+
+
+def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, forces=False, **sim_kwargs):
     """parse_scene (gmpm.cu:60-165): returns an initialised GmpmSimulator with every model registered.
     resume: path of a checkpoint of this scene.  It is checked against the document before any simulator exists; the scene's
     collider and boundaries are set and the checkpoint restored in place of the models (max_blocks defaults to the saved capacity).  MGSP runs
-    resume rank by rank instead: GmpmSimulator.from_checkpoint, wire the peers, restore."""
+    resume rank by rank instead: GmpmSimulator.from_checkpoint, wire the peers, restore.
+    forces: turn on the boundary impulse report (GmpmSimulator.report_forces); sim.force_bodies names its bodies (force_bodies).  Not
+    in MGSP mode (ValueError)."""
     if isinstance(path_or_dict, dict):
         doc, base = path_or_dict, os.getcwd()
     else:
@@ -413,6 +445,8 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
         raise ValueError("\"emit\" is not supported in MGSP mode")
     if doc.get("sinks") and sim_kwargs.get("mgsp_world", 1) > 1:
         raise ValueError("\"sinks\" are not supported in MGSP mode")
+    if forces and sim_kwargs.get("mgsp_world", 1) > 1:
+        raise ValueError("the force report is not supported in MGSP mode by the scene runner")
     models = [m for m in doc.get("models", []) if m.get("type", "particles") in PARTICLE_TYPES]
     # {path or (path, h, padding, band): LevelSet} of the "levelset" boundaries and sinks and the .obj models: one build and one
     # registration per distinct level set
@@ -431,6 +465,7 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
             sim.set_collision_objects(objs)
         sim.restore(resume)
         sim.emitters = ([sink] if sink else []) + emitters
+        _report_forces(sim, doc, forces)
         return sim
     for model in models:
         if model.get("constitutive") not in CONSTITUTIVE:
@@ -463,4 +498,11 @@ def parse_scene(path_or_dict, config=None, max_blocks=10000, resume=None, **sim_
     if objs:
         sim.set_collision_objects(objs)
     sim.emitters = ([sink] if sink else []) + emitters
+    _report_forces(sim, doc, forces)
     return sim
+
+
+def _report_forces(sim, doc, forces):
+    sim.force_bodies = force_bodies(doc)
+    if forces:
+        sim.report_forces(True)

@@ -302,6 +302,21 @@ class GmpmSimulator:
         check(self.L.cb200_sim_time(self.h, C.byref(t)), "sim_time")
         return t.value
 
+    # ---- boundary impulse report (DESIGN.md section 2.13) ---------------------------------------------------------------
+    def report_forces(self, enable=True):
+        """Turns the per-body impulse report of the grid update on or off and resets it (synchronises).  Body 0 is the level-set
+        collider, body 1 + i collision object i."""
+        check(self.L.cb200_sim_set_force_report(self.h, 1 if enable else 0), "report_forces")
+
+    def collision_forces(self):
+        """(elapsed, impulses) since the last reset, then resets: the simulated time covered and a float64 (1 + n_objects, 6) array
+        of (Jx, Jy, Jz, Lx, Ly, Lz) per body, the impulse the material gave it and the angular impulse about its pivot
+        trans + trans_vel t.  Mean force is J / elapsed, mean torque L / elapsed.  Synchronises; needs report_forces()."""
+        out = np.zeros((_capi.MAX_COLLISION_OBJECTS + 1, _capi.FORCE_COMPONENTS), np.float64)
+        n, elapsed = C.c_int(0), C.c_double(0.0)
+        check(self.L.cb200_sim_collision_forces(self.h, out.ctypes.data_as(C.c_void_p), len(out), C.byref(n), C.byref(elapsed)), "collision_forces")
+        return elapsed.value, out[:n.value].copy()
+
     # ---- checkpoint / restore (format: include/claymore_b200.h, reader: claymore_b200.checkpoint) -------------------
     def checkpoint_begin(self):
         """Snapshot at the current sub-step boundary; returns the blob's size without waiting for its copy to the host, so

@@ -165,6 +165,18 @@ CB200_API int cb200_levelset_prepare(const struct cb200_sdf_header* header, cons
 /* cb200_update_grid_velocity_query_max_objects where objs may hold CB200_SHAPE_LEVELSET entries, whose b[1] indexes
  * levelsets[0, n_levelsets) (at most CB200_MAX_COLLISION_LEVELSETS prepared lattices). */
 CB200_API int cb200_update_grid_velocity_query_max_levelsets(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, float time, float* max_vel, void* stream);
+/* The boundary impulse report (DESIGN.md section 2.13).  Body 0 is the level-set collider (all zeros without one), body 1 + i is
+ * object i of the list (analytic or CB200_SHAPE_LEVELSET); sinks and the wall band are not bodies.  Per body and grid update:
+ *   J = sum m (v_in - v_out)                 over the nodes with mass,
+ *   L = sum (p - b(t)) x m (v_in - v_out),   p = n dx the node, b(t) = trans + trans_vel t the pivot the body's omega turns about,
+ * v_in the velocity the body receives in the chain (after the wall mask, gravity and every earlier body), v_out the one it leaves.
+ * A row is (Jx, Jy, Jz, Lx, Ly, Lz); a body that changes no node's velocity reports exactly 0.  Mean force over a span of simulated
+ * time is J / span, mean torque L / span. */
+#define CB200_FORCE_COMPONENTS 6
+/* cb200_update_grid_velocity_query_max_levelsets that also ADDS each body's (J, L) of this grid update into the DEVICE
+ * impulses[(1 + n) * CB200_FORCE_COMPONENTS] (double).  The velocities and the max are those of the entry without the report.
+ * cudaErrorInvalidValue, nothing launched, for a null impulses or what that entry rejects. */
+CB200_API int cb200_update_grid_velocity_query_max_forces(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, float time, float* max_vel, double* impulses, void* stream);
 
 /* clear_grid  mgmpm_kernels.cuh:106-115 via GridBuffer::reset  grid_buffer.cuh:32-35 */
 CB200_API int cb200_clear_grid(int block_count, float* grid, void* stream);
@@ -299,6 +311,17 @@ CB200_API int cb200_sim_add_collision_levelset(cb200_sim* sim, const struct cb20
 CB200_API int cb200_sim_clear_collision_levelsets(cb200_sim* sim);
 /* simulated time since initial_setup: the sum of the dt of every finished sub-step (synchronises) */
 CB200_API int cb200_sim_time(cb200_sim* sim, double* time);
+/* Turns the boundary impulse report (cb200_update_grid_velocity_query_max_forces) of every sub-step's grid update on (enable != 0) or
+ * off, and resets its accumulator.  Off (the default) the grid update is the one without the report.  Synchronises and re-captures
+ * the sub-step graphs; call it between sub-steps. */
+CB200_API int cb200_sim_set_force_report(cb200_sim* sim, int enable);
+/* Copies the report accumulated since its last reset, n_bodies = 1 + the number of collision objects rows of (Jx, Jy, Jz, Lx, Ly, Lz)
+ * summed in double over the sub-steps, into out[capacity * CB200_FORCE_COMPONENTS], the simulated time those sub-steps cover into
+ * *elapsed, then resets it.  Synchronises.  cudaErrorInvalidValue, nothing written or reset, when the report is off, for a null
+ * pointer or for capacity < 1 + the number of objects.  cb200_sim_set_force_report, cb200_sim_set_collider,
+ * cb200_sim_clear_collider, cb200_sim_set_collision_objects and a restore reset it as well (the rows change meaning); adding or
+ * removing particles keeps it; a checkpoint does not store it.  Under MGSP each rank reports the blocks it is the lowest rank to hold: the ranks' rows sum to the whole. */
+CB200_API int cb200_sim_collision_forces(cb200_sim* sim, double* out, int capacity, int* n_bodies, double* elapsed);
 /* number of kernels this library launched on behalf of `sim` since creation */
 CB200_API long long cb200_sim_launch_count(cb200_sim* sim);
 

@@ -19,6 +19,11 @@ dragon-shaped obstacle (two_dragons.sdf's 77 x 118 x 401 nodes, two ellipsoids, 
 halves, with the grid update's kernel time and the device memory each adds, as --objects.
 
     python tools/collider_bench.py --levelsets [--steps 50] [--warmup 10] [--rounds 3]
+
+--forces compares, in alternating rounds, the boundary impulse report off and on (GmpmSimulator.report_forces, DESIGN.md
+section 2.13) for the level-set floor, the analytic floor box and 4 and 16 analytic objects, with the grid update's kernel time.
+
+    python tools/collider_bench.py --forces [--steps 50] [--warmup 10] [--rounds 3]
 """
 import ctypes as C
 import argparse
@@ -30,7 +35,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
-def run(scene, field, args, stream, objs=None):
+def run(scene, field, args, stream, objs=None, forces=False):
     import torch
     from claymore_b200 import scenes
     sim = scenes.build_engine(scene, dt=args.dt, max_blocks=scenes.max_blocks_for(scene), stream=stream.cuda_stream, auto_grow=False)
@@ -40,6 +45,8 @@ def run(scene, field, args, stream, objs=None):
         sim.set_collider(field[0], field[1], type="sticky")
     if objs:
         sim.set_collision_objects(objs)
+    if forces:
+        sim.report_forces(True)
     torch.cuda.synchronize()
     added = free0 - torch.cuda.mem_get_info()[0]
     sim.step(args.warmup)
@@ -56,7 +63,7 @@ def run(scene, field, args, stream, objs=None):
     sim.profile_read()
     sim.profile(False)
     kernel_ms = None
-    if args.objects or args.levelsets:
+    if args.objects or args.levelsets or args.forces:
         from torch.profiler import ProfilerActivity, profile
         sim.sync()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -127,6 +134,7 @@ def main():
     ap.add_argument("--dt", type=float, default=1e-4)
     ap.add_argument("--objects", action="store_true", help="also the analytic floor box, 4 and 16 analytic objects")
     ap.add_argument("--levelsets", action="store_true", help="also the analytic floor box, the floor as a level-set object and a dragon")
+    ap.add_argument("--forces", action="store_true", help="the impulse report off and on: level-set floor, analytic floor, 4 and 16 objects")
     args = ap.parse_args()
 
     import torch
@@ -145,6 +153,14 @@ def main():
     sets = object_sets(top) if args.objects else {}
     if args.levelsets:
         sets = {"analytic_floor": object_sets(top)["analytic_floor"], **levelset_sets(top, 1.0 / (1 << scene["domain_bits"]))}
+    if args.forces:
+        sets = object_sets(top)
+        names = [(n, f) for n in ["floor"] + sorted(sets) for f in (False, True)]
+        for r in range(args.rounds):
+            for name, forces in (names if r % 2 == 0 else names[::-1]):
+                res = run(scene, field if name == "floor" else None, args, stream, sets.get(name), forces=forces)
+                print(json.dumps({"round": r, "collider": name, "forces": forces, "steps": args.steps, **res}), flush=True)
+        return
     names = ["floor", "none"] + sorted(sets)
     for r in range(args.rounds):
         order = names if r % 2 == 0 else names[::-1]
