@@ -89,6 +89,26 @@ class CollisionObject(C.Structure):
                 ("dsdt", C.c_float), ("scale", C.c_float)]
 
 
+TRACK_LINEAR, TRACK_SMOOTH, TRACK_PERIODIC = 0, 1, 2                 # CB200_TRACK_*
+MAX_TRACK_KEYS = 4096                                                # CB200_MAX_TRACK_KEYS
+
+
+class TrackKey(C.Structure):
+    """cb200_track_key: a keyframed pose of a collision object's track, rot the quaternion (w, x, y, z)."""
+    _fields_ = [("t", C.c_float), ("pos", C.c_float * 3), ("rot", C.c_float * 4)]
+
+
+class TrackRecord(C.Structure):
+    """cb200_track_record: one key as cb200_track_prepare prepares it for the device (64 B)."""
+    _fields_ = [("t", C.c_float), ("pos", C.c_float * 3), ("rot", C.c_float * 4), ("tangent", C.c_float * 3), ("rotvec", C.c_float * 3),
+                ("reserved", C.c_float * 2)]
+
+
+class TrackSpan(C.Structure):
+    """cb200_track_span: object i's records in the table the kernel-level entry takes (count 0: not tracked)."""
+    _fields_ = [("offset", C.c_int), ("count", C.c_int), ("flags", C.c_int)]
+
+
 OUTPUT_V, OUTPUT_J = 1, 2        # CB200_OUTPUT_V / CB200_OUTPUT_J: per-particle attributes of a frame's .bgeo files
 ERROR_OUTPUT_IO = 2000           # CB200_ERROR_OUTPUT_IO
 
@@ -170,6 +190,9 @@ _SIGNATURES = {
                                                        C.POINTER(LevelSetLattice), _I, _F, _P, _P],
     "cb200_update_grid_velocity_query_max_forces": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), C.POINTER(CollisionObject), _I,
                                                     C.POINTER(LevelSetLattice), _I, _F, _P, _P, _P],
+    "cb200_update_grid_velocity_query_max_tracks": [_CFG, _I, _P, Partition, _F, C.POINTER(Collider), C.POINTER(CollisionObject), _I,
+                                                    C.POINTER(LevelSetLattice), _I, _P, C.POINTER(TrackSpan), _F, _P, _P, _P],
+    "cb200_track_prepare": [C.POINTER(TrackKey), _I, _I, C.POINTER(TrackRecord)],
     "cb200_levelset_prepare": [C.POINTER(SdfHeader), _P, _P, _P],
     "cb200_clear_grid": [_I, _P, _P],
     "cb200_cell_bucket_to_block": [_CFG, _I, _P, _P, _P, _P, _P],
@@ -221,6 +244,7 @@ _SIGNATURES = {
     "cb200_sim_clear_collision_levelsets": [_P],
     "cb200_sim_time": [_P, C.POINTER(C.c_double)],
     "cb200_sim_set_force_report": [_P, _I],
+    "cb200_sim_set_object_track": [_P, _I, C.POINTER(TrackKey), _I, _I],
     "cb200_sim_collision_forces": [_P, _P, _I, C.POINTER(_I), C.POINTER(C.c_double)],
     "cb200_sim_mgsp_inbox": [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_size_t)],
     "cb200_sim_mgsp_ipc_handle": [_P, _P],

@@ -123,8 +123,9 @@ int cb200_g2p2g(const cb200_config* c, float dt, float new_dt, int pbc, cb200_pa
 // The four kernel-level grid updates: the level set when collider is non-null (valid, with a field), then objs[0, n), placed at time;
 // level-set objects index lattices[0, n_lattices)
 // impulses (nullable): the report's device rows, added into (section 2.13)
+// tracks (nullable): the objects' tracks (section 2.14), already checked against objs
 static int update_grid_boundaries(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, float time, float* max_vel, void* stream,
-                                  const cb200_levelset* lattices = nullptr, int n_lattices = 0, double* impulses = nullptr) {
+                                  const cb200_levelset* lattices = nullptr, int n_lattices = 0, double* impulses = nullptr, const Tracks* tracks = nullptr) {
 	CB_CFG(c);
 	if(n_lattices < 0 || n_lattices > CB200_MAX_COLLISION_LEVELSETS || (n_lattices > 0 && !lattices)) return (int) cudaErrorInvalidValue;
 	LevelSets ls {};
@@ -155,7 +156,7 @@ static int update_grid_boundaries(const cb200_config* c, int block_count, float*
 	a.n_clear = 0;
 	a.time = time;
 	const ForceArgs fa {impulses, nullptr, 0u};
-	launch_grid_update(a, bd, ls, grid_for(block_count, kGridThreads / 32), (cudaStream_t) stream, impulses ? &fa : nullptr);
+	launch_grid_update(a, bd, ls, grid_for(block_count, kGridThreads / 32), (cudaStream_t) stream, impulses ? &fa : nullptr, tracks);
 	return (int) cudaGetLastError();
 }
 
@@ -179,6 +180,26 @@ int cb200_update_grid_velocity_query_max_levelsets(const cb200_config* c, int bl
 int cb200_update_grid_velocity_query_max_forces(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, float time, float* max_vel, double* impulses, void* stream) {
 	if(!impulses) return (int) cudaErrorInvalidValue;
 	return update_grid_boundaries(c, block_count, grid, partition, dt, collider, objs, n, time, max_vel, stream, levelsets, n_levelsets, impulses);
+}
+
+int cb200_track_prepare(const cb200_track_key* keys, int n, int flags, cb200_track_record* out) {
+	return track_prepare(keys, n, flags, out) ? 0 : (int) cudaErrorInvalidValue;
+}
+
+int cb200_update_grid_velocity_query_max_tracks(const cb200_config* c, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, const cb200_track_record* records, const cb200_track_span* spans,
+                                                float time, float* max_vel, double* impulses, void* stream) {
+	if(n < 0 || n > CB200_MAX_COLLISION_OBJECTS || (n > 0 && (!spans || !objs))) return (int) cudaErrorInvalidValue;
+	Tracks tr {};
+	tr.rec = reinterpret_cast<const float4*>(records);
+	for(int i = 0; i < n; ++i) {
+		const cb200_track_span& sp = spans[i];
+		if(sp.count < 0 || sp.count > CB200_MAX_TRACK_KEYS || sp.offset < 0 || (sp.flags & ~(CB200_TRACK_SMOOTH | CB200_TRACK_PERIODIC))) return (int) cudaErrorInvalidValue;
+		if(sp.count > 0 && (!records || !track_object_ok(objs[i]) || ((sp.flags & CB200_TRACK_PERIODIC) && sp.count < 2))) return (int) cudaErrorInvalidValue;
+		tr.off[i] = sp.offset;
+		tr.n[i] = sp.count;
+		tr.flags[i] = sp.flags;
+	}
+	return update_grid_boundaries(c, block_count, grid, partition, dt, collider, objs, n, time, max_vel, stream, levelsets, n_levelsets, impulses, &tr);
 }
 
 int cb200_levelset_prepare(const cb200_sdf_header* header, const float* phi, float* lattice, void* stream) {

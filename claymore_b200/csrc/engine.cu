@@ -388,6 +388,12 @@ struct cb200_sim {
 	// its last reset (force_reset)
 	bool force_report = false;
 	double* forces = nullptr;
+	// the objects' motion tracks (cb200_sim_set_object_track): each tracked object's prepared keys, and their concatenation in object
+	// order on the device (track_table, CB200_MAX_TRACK_KEYS records) that `tracks` indexes
+	std::vector<cb200_track_record> track_keys[CB200_MAX_COLLISION_OBJECTS];
+	int track_flags[CB200_MAX_COLLISION_OBJECTS] = {};
+	cb200_track_record* track_table = nullptr;
+	Tracks tracks {};
 	// the rows each particle block starts at in every read-out, per model: the scans of the bucket sizes, [kMaxModels][max_blocks + 1]
 	int* ck_base = nullptr;
 	// checkpoint (cb200_sim_checkpoint_begin / _end): the blob, copied to the host on the staging's own stream
@@ -465,7 +471,8 @@ DevArrays sim_arrays(cb200_sim* s, size_t mb) {
 	        dev_array(s->tile_sums, tiles * kScanComps, kNoFill),
 	        dev_array(s->block_totals, (size_t) kMaxModels * mb, kNoFill),
 	        dev_array(s->ck_base, (size_t) kMaxModels * (mb + 1), kNoFill),
-	        dev_array(s->forces, (size_t) kForceBodies * kForceComps + 1, 0)};
+	        dev_array(s->forces, (size_t) kForceBodies * kForceComps + 1, 0),
+	        dev_array(s->track_table, (size_t) CB200_MAX_TRACK_KEYS, kNoFill)};
 }
 
 int fill_arrays(cb200_sim* s, const DevArrays& a) {
@@ -618,7 +625,7 @@ int enqueue_grid_update(cb200_sim* s, int R) {
 	for(size_t m = 0; m < s->models.size(); ++m) gu.clear_counts[m] = s->models[m].pb[Rn].cell_particle_counts;
 	// MGSP: a block every rank holding it resolves counts on the lowest of them (the marks the previous sub-step's tagging left)
 	const ForceArgs fa {s->forces, s->desc.mgsp_world > 1 ? s->part[R].overlap_marks : nullptr, (1u << s->desc.mgsp_rank) - 1u};
-	launch_grid_update(gu, s->boundaries, s->levelsets, grid_blocks(4), s->stream, s->force_report ? &fa : nullptr);  // placed at StepState::sim_time, the start of this sub-step
+	launch_grid_update(gu, s->boundaries, s->levelsets, grid_blocks(4), s->stream, s->force_report ? &fa : nullptr, &s->tracks);  // placed at StepState::sim_time, the start of this sub-step
 	++s->launches;
 	return (int) cudaGetLastError();
 }
@@ -741,7 +748,7 @@ int enqueue_carry_and_exterior(cb200_sim* s, int R) {
 		a.new_grid = s->grid[0];
 		a.next_max_vel = mgsp ? &scr->local_max : nullptr;
 		// MGSP: the boundaries, so that the predicted max is the one the next grid update finds; a single domain predicts nothing
-		launch_carry_grid(a, mgsp ? s->boundaries : Boundaries {}, s->levelsets, grid_blocks(4), st);
+		launch_carry_grid(a, mgsp ? s->boundaries : Boundaries {}, s->levelsets, grid_blocks(4), st, mgsp ? &s->tracks : nullptr);
 		++s->launches;
 	}
 	if(mgsp) {
@@ -1332,7 +1339,7 @@ static int setup_impl(cb200_sim* s, const StartSrc& src) {
 	CK(push_state(s));
 	if(mgsp) {
 		// global max |v|^2 of the start grid (later sub-steps get it from the end-of-step exchange of the previous one)
-		launch_grid_max(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->boundaries, s->levelsets, grid_blocks(2), st);
+		launch_grid_max(cfg, s->d_state, s->grid[0], s->part[R].active_keys, &s->d_state->max_vel_sq, s->boundaries, s->levelsets, grid_blocks(2), st, &s->tracks);
 		mgsp_allreduce_maxvel_kernel<<<1, 32, 0, st>>>(mgsp_view(s), &s->d_state->max_vel_sq);
 		s->launches += 2;
 	}
@@ -1523,6 +1530,40 @@ int cb200_sim_set_collision_objects(cb200_sim* s, const cb200_collision_object* 
 	if(!s || !objects_prepare(objs, n, l, s->levelsets.count)) return (int) cudaErrorInvalidValue;
 	CK(cudaStreamSynchronize(s->stream));
 	s->boundaries.objects = l;
+	for(int i = 0; i < CB200_MAX_COLLISION_OBJECTS; ++i) s->track_keys[i].clear();  // a new list: every track is cleared
+	s->tracks = Tracks {};
+	CK(force_reset(s));
+	return recapture(s);
+}
+// ---- motion tracks (DESIGN.md section 2.14) -----------------------------------------------------------------------------------
+int cb200_sim_set_object_track(cb200_sim* s, int object, const cb200_track_key* keys, int n, int flags) {
+	if(!s || object < 0 || object >= s->boundaries.objects.n || n < 0 || n > CB200_MAX_TRACK_KEYS) return (int) cudaErrorInvalidValue;
+	std::vector<cb200_track_record> rec((size_t) n);
+	if(n > 0 && (!track_object_ok(s->boundaries.objects.o[object]) || !track_prepare(keys, n, flags, rec.data()))) return (int) cudaErrorInvalidValue;
+	size_t total = rec.size();
+	for(int i = 0; i < s->boundaries.objects.n; ++i)
+		if(i != object) total += s->track_keys[i].size();
+	if(total > CB200_MAX_TRACK_KEYS) return (int) cudaErrorInvalidValue;
+	// the table in object order, and the spans into it
+	std::vector<cb200_track_record> table;
+	table.reserve(total);
+	Tracks tr {};
+	tr.rec = reinterpret_cast<const float4*>(s->track_table);
+	for(int i = 0; i < s->boundaries.objects.n; ++i) {
+		const std::vector<cb200_track_record>& k = i == object ? rec : s->track_keys[i];
+		tr.off[i] = (int) table.size();
+		tr.n[i] = (int) k.size();
+		tr.flags[i] = i == object ? flags : s->track_flags[i];
+		table.insert(table.end(), k.begin(), k.end());
+	}
+	CK(cudaStreamSynchronize(s->stream));
+	if(!table.empty()) {
+		CK(cudaMemcpyAsync(s->track_table, table.data(), table.size() * sizeof(cb200_track_record), cudaMemcpyHostToDevice, s->stream));
+		CK(cudaStreamSynchronize(s->stream));
+	}
+	s->track_keys[object] = std::move(rec);
+	s->track_flags[object] = flags;
+	s->tracks = tr;
 	CK(force_reset(s));
 	return recapture(s);
 }

@@ -88,13 +88,15 @@ __device__ __forceinline__ void warp_body_impulse(double* slot, int lane, float 
 // where that kernel reports 2|v|^2 (Appendix B #11).
 // FORCES: the chain runs one body at a time over both cells of a lane (boundaries_resolve_pair) and each body's impulse is added to
 // fa->impulses (section 2.13); the velocities are those of the instance without it.
-template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false, bool FORCES = false>
-__device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const Boundaries* bd, const ForceArgs* fa = nullptr) {
+// TRACKS (OBJECTS): the objects with a track in tr move on it (section 2.14), the pivot of their impulse report is c(t).
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false, bool FORCES = false, bool TRACKS = false>
+__device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const Boundaries* bd, const ForceArgs* fa = nullptr, const Tracks* tr = nullptr) {
 	static_assert(!FORCES || COLLIDE || OBJECTS, "the report needs a body");
 	__shared__ unsigned s_max[kGridThreads / 32];
 	if constexpr(FORCES) force_slots_clear();  // published by the frame builder's barrier
 	const BoundaryFrames* fr = nullptr;
-	if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, a.state ? (float) a.state->sim_time : a.time);
+	if constexpr(TRACKS) fr = &boundary_frames_tracks_cta<COLLIDE>(*bd, *tr, a.state ? (float) a.state->sim_time : a.time);
+	else if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, a.state ? (float) a.state->sim_time : a.time);
 	const Cfg& cfg = a.cfg;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int nbc = a.state ? a.state->nbc : a.nbc;
@@ -129,9 +131,16 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 				const int nx = 4 * kx + (lane >> 3), ny = 4 * ky + ((lane >> 1) & 3), nz = 4 * kz + 2 * (lane & 1);
 				const bool counted = !fa->overlap_marks || (fa->overlap_marks[b] & fa->lower_ranks) == 0u;  // warp-uniform
 				double* slots = force_slots()[warp];
-				boundaries_resolve_pair<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, nx, ny, nz, hx, hy, v0, v1, v2, [&](int k, const ColliderFrame& f, float2 i0, float2 i1, float2 i2) {
-					if(counted) warp_body_impulse(slots + k * kForceComps, lane, cfg.dx, nx, ny, nz, m, hx, hy, f, i0, i1, i2, v0, v1, v2);
-				});
+				if constexpr(TRACKS) {
+					auto stage = [&](int k, const ColliderFrame& f, float2 i0, float2 i1, float2 i2) {
+						if(counted) warp_body_impulse(slots + k * kForceComps, lane, cfg.dx, nx, ny, nz, m, hx, hy, f, i0, i1, i2, v0, v1, v2);
+					};
+					boundaries_resolve_pair<COLLIDE, OBJECTS, LEVELSETS, decltype(stage)&, true>(*bd, *fr, cfg, nx, ny, nz, hx, hy, v0, v1, v2, stage, tr);
+				} else {
+					boundaries_resolve_pair<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, nx, ny, nz, hx, hy, v0, v1, v2, [&](int k, const ColliderFrame& f, float2 i0, float2 i1, float2 i2) {
+						if(counted) warp_body_impulse(slots + k * kForceComps, lane, cfg.dx, nx, ny, nz, m, hx, hy, f, i0, i1, i2, v0, v1, v2);
+					});
+				}
 				if(hx) sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
 				if(hy) sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
 			} else {
@@ -140,7 +149,7 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 					v0.x = wx ? 0.f : v0.x * mi;
 					v1.x = (wy ? 0.f : v1.x * mi) + gdt;
 					v2.x = wz ? 0.f : v2.x * mi;
-					if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x);
+					if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS, TRACKS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1), v0.x, v1.x, v2.x, tr);
 					sq0 = v0.x * v0.x + v1.x * v1.x + v2.x * v2.x;
 				}
 				if(hy) {
@@ -148,7 +157,7 @@ __device__ __forceinline__ void grid_update_body(const GridUpdateArgs& a, const 
 					v0.y = wx ? 0.f : v0.y * mi;
 					v1.y = (wy ? 0.f : v1.y * mi) + gdt;
 					v2.y = wz ? 0.f : v2.y * mi;
-					if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y);
+					if constexpr(COLLIDE || OBJECTS) boundaries_resolve<COLLIDE, OBJECTS, LEVELSETS, TRACKS>(*bd, *fr, cfg, 4 * kx + (lane >> 3), 4 * ky + ((lane >> 1) & 3), 4 * kz + 2 * (lane & 1) + 1, v0.y, v1.y, v2.y, tr);
 					sq1 = v0.y * v0.y + v1.y * v1.y + v2.y * v2.y;
 				}
 			}
@@ -215,6 +224,14 @@ __global__ void __launch_bounds__(kGridThreads, (kBoundaryMinCtas<COLLIDE, true>
 	grid_update_body<COLLIDE, true, true, true>(a, &bd, &fa);
 }
 static_assert(sizeof(GridUpdateArgs) + sizeof(Boundaries) + sizeof(LevelSets) + sizeof(ForceArgs) <= 4096, "the reporting level-set grid update's parameters must fit the 4 KiB kernel-parameter limit");
+// the same with the objects' tracks tr (section 2.14), with or without level-set objects (ls) and the report (fa); COLLIDE: bd.has_collider
+template<bool COLLIDE, bool LEVELSETS, bool FORCES>
+__global__ void __launch_bounds__(kGridThreads, (kBoundaryMinCtas<COLLIDE, true>)) grid_update_tracks_kernel(const GridUpdateArgs a, const __grid_constant__ Boundaries bd, const __grid_constant__ LevelSets ls,
+                                                                                                            const __grid_constant__ ForceArgs fa, const __grid_constant__ Tracks tr) {
+	if constexpr(LEVELSETS) levelset_views_cta(ls);  // published by the frame builder's barrier
+	grid_update_body<COLLIDE, true, LEVELSETS, FORCES, true>(a, &bd, &fa, &tr);
+}
+static_assert(sizeof(GridUpdateArgs) + sizeof(Boundaries) + sizeof(LevelSets) + sizeof(ForceArgs) + sizeof(Tracks) <= 4096, "the tracked grid update's parameters must fit the 4 KiB kernel-parameter limit");
 
 // clear_grid (mgmpm_kernels.cuh:106-115)
 __global__ void clear_grid_kernel(int block_count, float* grid) {
@@ -245,8 +262,8 @@ struct CarryArgs {
 	int* overlap_marks;
 };
 // COLLIDE / OBJECTS (MGSP): the predictor applies the boundaries of bd at the time the next grid update sees
-template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
-__device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Boundaries* bd) {
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false, bool TRACKS = false>
+__device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Boundaries* bd, const Tracks* tr = nullptr) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int n = *a.new_count;
 	const int old_nbc = a.state->nbc;
@@ -255,7 +272,8 @@ __device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Bounda
 	float gdt = 0.f;
 	if(a.next_max_vel) gdt = a.cfg.gravity * device_compute_dt(a.cfg, a.state->max_vel_sq, a.state->step_time, a.state->frame_time, a.state->dt_default);
 	const BoundaryFrames* fr = nullptr;
-	if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, (float) (a.state->sim_time + (double) a.state->dt));  // the clock rolls by this sub-step's dt
+	if constexpr(TRACKS) fr = &boundary_frames_tracks_cta<COLLIDE>(*bd, *tr, (float) (a.state->sim_time + (double) a.state->dt));
+	else if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, (float) (a.state->sim_time + (double) a.state->dt));  // the clock rolls by this sub-step's dt
 	unsigned vmax = 0u;
 	for(int j = blockIdx.x * 8 + warp; j < n; j += gridDim.x * 8) {
 		const int kx = a.new_keys[3 * j], ky = a.new_keys[3 * j + 1], kz = a.new_keys[3 * j + 2];
@@ -272,7 +290,7 @@ __device__ __forceinline__ void carry_grid_body(const CarryArgs& a, const Bounda
 			if(a.next_max_vel) {
 				const float2* s2 = reinterpret_cast<const float2*>(s);
 				const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
-				if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS, LEVELSETS>(a.cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+				if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS, LEVELSETS, TRACKS>(a.cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt, tr)));
 				else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 			}
 		} else {
@@ -297,21 +315,28 @@ __global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, true>)) carry_
 	carry_grid_body<COLLIDE, true, true>(a, &bd);
 }
 static_assert(sizeof(CarryArgs) + sizeof(Boundaries) + sizeof(LevelSets) <= 4096, "the level-set carry's parameters must fit the 4 KiB kernel-parameter limit");
+template<bool COLLIDE, bool LEVELSETS>
+__global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, true>)) carry_grid_tracks_kernel(const CarryArgs a, const __grid_constant__ Boundaries bd, const __grid_constant__ LevelSets ls, const __grid_constant__ Tracks tr) {
+	if constexpr(LEVELSETS) levelset_views_cta(ls);
+	carry_grid_body<COLLIDE, true, LEVELSETS, true>(a, &bd, &tr);
+}
+static_assert(sizeof(CarryArgs) + sizeof(Boundaries) + sizeof(LevelSets) + sizeof(Tracks) <= 4096, "the tracked carry's parameters must fit the 4 KiB kernel-parameter limit");
 
 // max |v|^2 the grid update will find, without touching the grid (MGSP start-up)
-template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false>
-__device__ __forceinline__ void grid_max_body(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries* bd) {
+template<bool COLLIDE, bool OBJECTS, bool LEVELSETS = false, bool TRACKS = false>
+__device__ __forceinline__ void grid_max_body(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries* bd, const Tracks* tr = nullptr) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int g = cfg.gsize, bc = cfg.boundary;
 	const float gdt = cfg.gravity * state->dt;
 	const BoundaryFrames* fr = nullptr;
-	if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, (float) state->sim_time);
+	if constexpr(TRACKS) fr = &boundary_frames_tracks_cta<COLLIDE>(*bd, *tr, (float) state->sim_time);
+	else if constexpr(COLLIDE || OBJECTS) fr = &boundary_frames_cta<COLLIDE, OBJECTS>(*bd, (float) state->sim_time);
 	unsigned vmax = 0u;
 	for(int b = blockIdx.x * 8 + warp; b < state->nbc; b += gridDim.x * 8) {
 		const int kx = keys[3 * b], ky = keys[3 * b + 1], kz = keys[3 * b + 2];
 		const bool wx = (kx < bc) | (kx >= g - bc), wy = (ky < bc) | (ky >= g - bc), wz = (kz < bc) | (kz >= g - bc);
 		const float2* s2 = reinterpret_cast<const float2*>(grid + (size_t) b * kGridBlockFloats);
-		if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS, LEVELSETS>(cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt)));
+		if constexpr(COLLIDE || OBJECTS) vmax = max(vmax, __float_as_uint(cell_pair_vel_sq_boundaries<COLLIDE, OBJECTS, LEVELSETS, TRACKS>(cfg, *bd, *fr, s2, lane, kx, ky, kz, wx, wy, wz, gdt, tr)));
 		else vmax = max(vmax, __float_as_uint(cell_pair_vel_sq(s2[lane], s2[32 + lane], s2[64 + lane], s2[96 + lane], wx, wy, wz, gdt)));
 	}
 	vmax = __reduce_max_sync(0xffffffffu, vmax);
@@ -328,6 +353,12 @@ template<bool COLLIDE>
 __global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, true>)) grid_max_levelset_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const __grid_constant__ Boundaries bd, const __grid_constant__ LevelSets ls) {
 	levelset_views_cta(ls);
 	grid_max_body<COLLIDE, true, true>(cfg, state, grid, keys, max_vel, &bd);
+}
+template<bool COLLIDE, bool LEVELSETS>
+__global__ void __launch_bounds__(256, (kBoundaryMinCtas<COLLIDE, true>)) grid_max_tracks_kernel(Cfg cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const __grid_constant__ Boundaries bd,
+                                                                                                const __grid_constant__ LevelSets ls, const __grid_constant__ Tracks tr) {
+	if constexpr(LEVELSETS) levelset_views_cta(ls);
+	grid_max_body<COLLIDE, true, LEVELSETS, true>(cfg, state, grid, keys, max_vel, &bd, &tr);
 }
 
 // ---- launching the three boundary passes ---------------------------------------------------------------------------------------
@@ -352,6 +383,17 @@ void with_boundaries(const Boundaries& bd, F&& f) {
 	else if(bd.objects.n > 0) f(N(), T(), N());
 	else f(N(), N(), N());
 }
+// f(COLLIDE, LEVELSETS), two std::bool_constant, for the tracked instances that apply bd (section 2.14)
+template<class F>
+void with_tracks(const Boundaries& bd, F&& f) {
+	using T = std::true_type;
+	using N = std::false_type;
+	if(has_levelset_objects(bd)) {
+		if(bd.has_collider) f(T(), T());
+		else f(N(), T());
+	} else if(bd.has_collider) f(T(), N());
+	else f(N(), N());
+}
 // f(COLLIDE, OBJECTS) for each boundary instance without level sets
 template<class F>
 void for_each_boundary_instance(F&& f) {
@@ -360,7 +402,16 @@ void for_each_boundary_instance(F&& f) {
 	f(std::true_type(), std::true_type());
 }
 // ls: the lattices bd's level-set objects index (read only when one is); fa (nullable): report the impulses there (no body: nothing)
-inline void launch_grid_update(const GridUpdateArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st, const ForceArgs* fa = nullptr) {
+// tr (nullable): the objects' tracks; the tracked instances run only when one of bd's objects has a track
+inline void launch_grid_update(const GridUpdateArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st, const ForceArgs* fa = nullptr, const Tracks* tr = nullptr) {
+	if(tracks_any(tr)) {
+		const ForceArgs none {};
+		with_tracks(bd, [&](auto C, auto L) {
+			if(fa) grid_update_tracks_kernel<C, L, true><<<ctas, kGridThreads, 0, st>>>(a, bd, ls, *fa, *tr);
+			else grid_update_tracks_kernel<C, L, false><<<ctas, kGridThreads, 0, st>>>(a, bd, ls, none, *tr);
+		});
+		return;
+	}
 	with_boundaries(bd, [&](auto C, auto O, auto L) {
 		if constexpr(L) {
 			if(fa) grid_update_levelset_forces_kernel<C><<<ctas, kGridThreads, 0, st>>>(a, bd, ls, *fa);
@@ -373,14 +424,23 @@ inline void launch_grid_update(const GridUpdateArgs& a, const Boundaries& bd, co
 		}
 	});
 }
-inline void launch_carry_grid(const CarryArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st) {
+inline void launch_carry_grid(const CarryArgs& a, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st, const Tracks* tr = nullptr) {
+	if(tracks_any(tr)) {
+		with_tracks(bd, [&](auto C, auto L) { carry_grid_tracks_kernel<C, L><<<ctas, 256, 0, st>>>(a, bd, ls, *tr); });
+		return;
+	}
 	with_boundaries(bd, [&](auto C, auto O, auto L) {
 		if constexpr(L) carry_grid_levelset_kernel<C><<<ctas, 256, 0, st>>>(a, bd, ls);
 		else if constexpr(C || O) carry_grid_boundary_kernel<C, O><<<ctas, 256, 0, st>>>(a, bd);
 		else carry_grid_kernel<<<ctas, 256, 0, st>>>(a);
 	});
 }
-inline void launch_grid_max(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st) {
+inline void launch_grid_max(const Cfg& cfg, const StepState* state, const float* grid, const int* keys, float* max_vel, const Boundaries& bd, const LevelSets& ls, int ctas, cudaStream_t st,
+                            const Tracks* tr = nullptr) {
+	if(tracks_any(tr)) {
+		with_tracks(bd, [&](auto C, auto L) { grid_max_tracks_kernel<C, L><<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel, bd, ls, *tr); });
+		return;
+	}
 	with_boundaries(bd, [&](auto C, auto O, auto L) {
 		if constexpr(L) grid_max_levelset_kernel<C><<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel, bd, ls);
 		else if constexpr(C || O) grid_max_boundary_kernel<C, O><<<ctas, 256, 0, st>>>(cfg, state, grid, keys, max_vel, bd);

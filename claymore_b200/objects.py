@@ -8,13 +8,17 @@ scale, dsdt.
 
 objects.levelset places an SDFGen level set (claymore_b200.sdf.LevelSet) as an obstacle (DESIGN.md section 2.11): the simulator
 registers its lattice on first use and writes the registry index into the object it passes on.
+
+objects.track(keys, interp, periodic) is a motion track (DESIGN.md section 2.14): keyframed poses of the object's pivot and rotation
+that the grid update evaluates at each sub-step's time.  Every constructor takes it as track=; the object then places its shape with
+R(t) = Q(t) rot about the pivot c(t) (x = R(t)^T (p - c(t)) scale + trans) and moves rigidly, so trans_vel, omega and dsdt must be 0.
 """
 import math
 
 import numpy as np
 
-from ._capi import (MAX_COLLISION_LEVELSETS, MAX_COLLISION_OBJECTS, SEPARATE, SHAPE_BOX, SHAPE_CYLINDER, SHAPE_LEVELSET, SHAPE_PLANE,
-                    SHAPE_SPHERE, SLIP, STICKY, CollisionObject)
+from ._capi import (MAX_COLLISION_LEVELSETS, MAX_COLLISION_OBJECTS, MAX_TRACK_KEYS, SEPARATE, SHAPE_BOX, SHAPE_CYLINDER, SHAPE_LEVELSET,
+                    SHAPE_PLANE, SHAPE_SPHERE, SLIP, STICKY, TRACK_LINEAR, TRACK_PERIODIC, TRACK_SMOOTH, CollisionObject, TrackKey)
 
 BOUNDARY_TYPES = {"sticky": STICKY, "slip": SLIP, "separate": SEPARATE}
 SHAPES = {"plane": SHAPE_PLANE, "box": SHAPE_BOX, "sphere": SHAPE_SPHERE, "cylinder": SHAPE_CYLINDER}
@@ -28,7 +32,7 @@ def _vec(v, n=3, what="vector"):
 
 
 def _make(shape, a, b, type="sticky", friction=0.3, trans=(0.0, 0.0, 0.0), trans_vel=(0.0, 0.0, 0.0), omega=(0.0, 0.0, 0.0), rot=None,
-          scale=1.0, dsdt=0.0):
+          scale=1.0, dsdt=0.0, track=None):
     o = CollisionObject()
     o.shape = shape
     if isinstance(type, str):
@@ -43,7 +47,103 @@ def _make(shape, a, b, type="sticky", friction=0.3, trans=(0.0, 0.0, 0.0), trans
     o.trans[:], o.trans_vel[:], o.omega[:] = _vec(trans, what="trans"), _vec(trans_vel, what="trans_vel"), _vec(omega, what="omega")
     o.scale, o.dsdt = float(scale), float(dsdt)
     validate(o)
+    if track is not None:
+        if not isinstance(track, Track):
+            raise ValueError("track must come from objects.track")
+        if any(o.trans_vel) or any(o.omega) or o.dsdt != 0.0:
+            raise ValueError("a tracked object must have trans_vel = omega = 0 and dsdt = 0: the track moves it")
+        o.track = track
     return o
+
+
+# ---- motion tracks (DESIGN.md section 2.14) -----------------------------------------------------------------------------------
+INTERP = {"linear": TRACK_LINEAR, "smooth": TRACK_SMOOTH}
+
+
+class Track:
+    """A validated motion track: keys (a ctypes array of cb200_track_key), n and flags (CB200_TRACK_*), as
+    GmpmSimulator.set_object_track passes them on."""
+
+    def __init__(self, keys, flags):
+        self.keys, self.n, self.flags = keys, len(keys), flags
+
+
+def quaternion(rotation):
+    """The unit quaternion (w, x, y, z) of a rotation given as a quaternion (4 values) or a 3x3 rotation matrix (row i, column j), in
+    double; a zero quaternion or a matrix that is not a rotation raises ValueError."""
+    r = np.asarray(rotation, np.float64)
+    if r.shape == (4,):
+        if not np.isfinite(r).all():
+            raise ValueError("every value of a track key must be finite")
+        n = np.linalg.norm(r)
+        if not n > 0:
+            raise ValueError("a track key's quaternion must not be zero")
+        return r / n
+    if r.shape != (3, 3):
+        raise ValueError(f"a rotation is a quaternion (w, x, y, z) or a 3x3 matrix, not shape {r.shape}")
+    if not np.isfinite(r).all():
+        raise ValueError("every value of a track key must be finite")
+    if not (np.allclose(r @ r.T, np.eye(3), atol=1e-5) and np.linalg.det(r) > 0):
+        raise ValueError("a track key's matrix must be a rotation")
+    # the largest of w, x, y, z first (Shepperd), then the rest from the off-diagonal terms
+    tr = np.trace(r)
+    cand = [tr, r[0, 0], r[1, 1], r[2, 2]]
+    i = int(np.argmax(cand))
+    if i == 0:
+        w = np.sqrt(1.0 + tr) / 2
+        q = [w, (r[2, 1] - r[1, 2]) / (4 * w), (r[0, 2] - r[2, 0]) / (4 * w), (r[1, 0] - r[0, 1]) / (4 * w)]
+    else:
+        a, b, c = [(0, 1, 2), (1, 2, 0), (2, 0, 1)][i - 1]
+        v = np.sqrt(1.0 + r[a, a] - r[b, b] - r[c, c]) / 2
+        q = np.zeros(4)
+        q[0] = (r[c, b] - r[b, c]) / (4 * v)
+        q[1 + a] = v
+        q[1 + b] = (r[b, a] + r[a, b]) / (4 * v)
+        q[1 + c] = (r[c, a] + r[a, c]) / (4 * v)
+    q = np.asarray(q, np.float64)
+    return q / np.linalg.norm(q)
+
+
+def track(keys, interp="linear", periodic=False):
+    """A motion track from keys [(t, position, rotation)], rotation a quaternion (w, x, y, z) or a 3x3 rotation matrix: the checks of
+    cb200_track_prepare as ValueError (1 to MAX_TRACK_KEYS keys with strictly increasing t, finite values, no zero quaternion, no two
+    neighbouring rotations 180 degrees apart, a periodic track's last pose equal to its first, quaternions up to sign).  interp:
+    "linear" (piecewise linear positions) or "smooth" (cubic Hermite); every segment's rotation is a slerp."""
+    if interp not in INTERP:
+        raise ValueError(f"unknown interpolation {interp!r} (known: {', '.join(INTERP)})")
+    keys = list(keys)
+    if not 1 <= len(keys) <= MAX_TRACK_KEYS:
+        raise ValueError(f"a track has 1 to {MAX_TRACK_KEYS} keys, not {len(keys)}")
+    if periodic and len(keys) < 2:
+        raise ValueError("a periodic track needs at least 2 keys")
+    arr = (TrackKey * len(keys))()
+    qs = []
+    for k, key in enumerate(keys):
+        if len(key) != 3:
+            raise ValueError("a track key is (t, position, rotation)")
+        t, pos, rot = key
+        pos = _vec(pos, what="position")
+        if not (math.isfinite(float(t)) and all(math.isfinite(v) for v in pos)):
+            raise ValueError("every value of a track key must be finite")
+        q = quaternion(rot)
+        arr[k].t, arr[k].pos[:], arr[k].rot[:] = float(t), pos, [float(v) for v in q]
+        if k > 0 and not arr[k].t > arr[k - 1].t:
+            raise ValueError(f"track key times must increase strictly (as float32): {arr[k - 1].t} then {arr[k].t}")
+        qs.append(np.asarray(list(arr[k].rot), np.float64))
+    for k in range(1, len(qs)):
+        a = qs[k - 1] / np.linalg.norm(qs[k - 1])
+        b = qs[k] / np.linalg.norm(qs[k])
+        if float(a @ b) == 0.0:
+            raise ValueError(f"track keys {k - 1} and {k} are 180 degrees apart: the rotation between them is ambiguous")
+        if float(a @ b) < 0.0:
+            qs[k] = -qs[k]
+    if periodic:
+        f32 = lambda v: np.asarray(v, np.float64) / np.linalg.norm(np.asarray(v, np.float64))  # noqa: E731
+        first, last = arr[0], arr[len(keys) - 1]
+        q0, q1 = f32(list(first.rot)).astype(np.float32), f32(list(last.rot)).astype(np.float32)
+        if list(first.pos) != list(last.pos) or not (np.array_equal(q0, q1) or np.array_equal(q0, -q1)):
+            raise ValueError("a periodic track's last pose must equal its first")
+    return Track(arr, INTERP[interp] | (TRACK_PERIODIC if periodic else 0))
 
 
 def plane(point, normal, **motion):

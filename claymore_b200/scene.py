@@ -23,6 +23,16 @@ into [offset, offset + span] as a model's is (DESIGN.md section 2.11), but it ma
 its lattice registered once per simulator.  Unknown keys or shapes, too many entries, an unreadable file or a bad value raise
 ValueError before any device work; "collider" and "boundaries" may both be present.
 
+A "boundaries" entry may move on a keyframed track (claymore_b200.objects.track, DESIGN.md section 2.14):
+
+     "track": {"keys": [{"t": 0.0, "position": [3], "rotation": [3]}, ...], "interp": "linear"|"smooth", "periodic": false}
+
+The pivot of a tracked entry is the centre of its [offset, offset + span] box (for a plane: offset); the shape is placed as it is
+without a track and turned and moved about that pivot.  "position" is where the pivot is at time "t" (default: where it is placed,
+the centre), "rotation" a rotation vector in radians (default [0, 0, 0]), applied in world space after the entry's rest orientation;
+a "scale" scales the shape about the pivot.
+A tracked entry has no "velocity", "omega" or "dsdt"; a bad track raises ValueError before any device work.
+
 A "file": "<name>.obj" model, boundary or sink is a Wavefront OBJ triangle mesh turned into a level set on the device
 (claymore_b200.mesh, SDFGen's make_level_set3 bit for bit, DESIGN.md section 2.12) with the optional keys "h" (node spacing in mesh
 units; default: the mesh's longest extent x dx / the longest span, about one simulation cell per level-set cell), "padding" (1) and
@@ -163,7 +173,37 @@ def _collider(sim, c, cfg, base_dir):
                      omega=c.get("omega", [0, 0, 0]), scale=c.get("scale", 1.0), dsdt=c.get("dsdt", 0.0))
 
 
-BOUNDARY_KEYS = ("shape", "offset", "span", "normal", "type", "friction", "velocity", "omega", "scale", "dsdt")
+BOUNDARY_KEYS = ("shape", "offset", "span", "normal", "type", "friction", "velocity", "omega", "scale", "dsdt", "track")
+TRACK_KEYS = ("keys", "interp", "periodic")
+TRACK_KEY_KEYS = ("t", "position", "rotation")
+
+
+def _track(tr, pivot):
+    """objects.track of a "track" entry whose keys' positions default to pivot and whose rotations are rotation vectors (ValueError on a
+    bad entry)."""
+    from . import objects
+    if not isinstance(tr, dict):
+        raise ValueError(f"\"track\" must be an object with keys {', '.join(TRACK_KEYS)}")
+    unknown = sorted(set(tr) - set(TRACK_KEYS))
+    if unknown:
+        raise ValueError(f"track: unknown keys {unknown} (known: {', '.join(TRACK_KEYS)})")
+    keys = tr.get("keys")
+    if not isinstance(keys, list) or not keys:
+        raise ValueError("track: \"keys\" must be a non-empty list")
+    out = []
+    for k, key in enumerate(keys):
+        if not isinstance(key, dict) or "t" not in key:
+            raise ValueError(f"track key {k} must be an object with \"t\" and optional \"position\", \"rotation\"")
+        unknown = sorted(set(key) - set(TRACK_KEY_KEYS))
+        if unknown:
+            raise ValueError(f"track key {k}: unknown keys {unknown} (known: {', '.join(TRACK_KEY_KEYS)})")
+        r = np.asarray(key.get("rotation", [0.0, 0.0, 0.0]), np.float64).reshape(3)
+        th = float(np.linalg.norm(r))
+        q = [1.0, 0.0, 0.0, 0.0] if th == 0.0 else [np.cos(th / 2)] + list(np.sin(th / 2) * r / th)
+        out.append((float(key["t"]), np.asarray(key.get("position", pivot), np.float64).reshape(3), q))
+    if not isinstance(tr.get("periodic", False), bool):
+        raise ValueError("track: \"periodic\" must be true or false")
+    return objects.track(out, tr.get("interp", "linear"), tr.get("periodic", False))
 LEVELSET_KEYS = ("file",) + MESH_KEYS   # with "shape": "levelset"
 
 
@@ -205,6 +245,9 @@ def _object(b, what, keys, base_dir=None, cache=None, dx=None):
         span = np.asarray(b.get("span", [1, 1, 1]), dtype=np.float64).reshape(3)
         motion = dict(type=b.get("type", "sticky"), friction=float(b.get("friction", 0.3)), trans_vel=b.get("velocity", [0, 0, 0]),
                       omega=b.get("omega", [0, 0, 0]), scale=float(b.get("scale", 1.0)), dsdt=float(b.get("dsdt", 0.0)))
+        if "track" in b:  # placed about its pivot: x = R(t)^T (p - c(t)) scale + pivot, the rest pose at c = pivot is the untracked one
+            pivot = offset if shape == "plane" else offset + span / 2
+            motion.update(trans=pivot, track=_track(b["track"], pivot))
         if shape == "levelset":
             ls = _obstacle_level_set(b, what, base_dir, {} if cache is None else cache, span, dx)
             return objects.levelset(ls, offset, span, **motion)

@@ -258,6 +258,18 @@ class GmpmSimulator:
         From the next sub-step on the grid update resolves the level-set collider, then these in list order (synchronises)."""
         objs = list(objs)
         check(self.L.cb200_sim_set_collision_objects(self.h, self._objects_array(objs), len(objs)), "set_collision_objects")
+        for i, o in enumerate(objs):
+            tr = getattr(o, "track", None)
+            if tr is not None:
+                self.set_object_track(i, tr)
+
+    def set_object_track(self, index, track):
+        """Moves collision object `index` of the list set_collision_objects set along `track` (claymore_b200.objects.track; None
+        clears it).  Resets the force report and synchronises (DESIGN.md section 2.14)."""
+        if track is None:
+            check(self.L.cb200_sim_set_object_track(self.h, int(index), None, 0, 0), "set_object_track")
+        else:
+            check(self.L.cb200_sim_set_object_track(self.h, int(index), track.keys, track.n, track.flags), "set_object_track")
 
     def clear_collision_objects(self):
         check(self.L.cb200_sim_set_collision_objects(self.h, None, 0), "clear_collision_objects")

@@ -178,6 +178,51 @@ CB200_API int cb200_update_grid_velocity_query_max_levelsets(const cb200_config*
  * cudaErrorInvalidValue, nothing launched, for a null impulses or what that entry rejects. */
 CB200_API int cb200_update_grid_velocity_query_max_forces(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, float time, float* max_vel, double* impulses, void* stream);
 
+/* Motion tracks of collision objects (DESIGN.md section 2.14): keyframed poses the grid update evaluates at the sub-step's time.
+ * A key is (t, pos, rot): the simulated time, where the object's pivot is then and a unit quaternion rot = (w, x, y, z) (normalised in
+ * double by cb200_track_prepare).  A track holds 1 to CB200_MAX_TRACK_KEYS keys with strictly increasing t; flags is
+ * CB200_TRACK_LINEAR or CB200_TRACK_SMOOTH, optionally | CB200_TRACK_PERIODIC.
+ *   position c(t): LINEAR piecewise linear; SMOOTH cubic Hermite with tangents m_k = (c_{k+1} - c_{k-1}) / (t_{k+1} - t_{k-1}),
+ *                  one-sided at the ends (a PERIODIC track's wrap around: the last key is the first);
+ *   rotation Q(t): consecutive quaternions are aligned to one hemisphere; segment k is q_k (x) exp(u theta_k a_k / 2),
+ *                  u = (t - t_k) / (t_{k+1} - t_k), so the world angular velocity R(q_k) a_k theta_k / (t_{k+1} - t_k) is constant on it;
+ *   outside: before the first key the first pose, from the last key on the last pose, both at rest; PERIODIC maps t >= t_last to
+ *            t_0 + fmodf(t - t_0, t_last - t_0) (float) first.
+ * The object's pivot is c(t) and its rotation Q(t) R0 (R0 its rot_mat): its material-space point is R(t)^T (p - c(t)) scale + trans and
+ * its velocity the rigid c'(t) + omega(t) x (p - c(t)); the force report's torque is about c(t).  A tracked object must have
+ * trans_vel = omega = 0 and dsdt = 0.  Rejected (cudaErrorInvalidValue, nothing changed): keys not strictly increasing, a non-finite
+ * value, a zero quaternion, neighbouring quaternions exactly 180 degrees apart (q_k . q_{k+1} = 0), a PERIODIC track with fewer than 2
+ * keys or whose last pose differs from its first (quaternions equal up to sign), more than CB200_MAX_TRACK_KEYS keys, unknown flags. */
+typedef struct cb200_track_key {
+	float t;
+	float pos[3];
+	float rot[4];
+} cb200_track_key;
+enum { CB200_TRACK_LINEAR = 0, CB200_TRACK_SMOOTH = 1, CB200_TRACK_PERIODIC = 2 };
+#define CB200_MAX_TRACK_KEYS 4096
+/* one prepared key (64 B): the key's t and pos, its hemisphere-aligned unit quaternion, the position tangent m_k (SMOOTH; 0 for
+ * LINEAR) and the rotation vector theta_k a_k of the segment it starts (0 on the last key) */
+typedef struct cb200_track_record {
+	float t;
+	float pos[3];
+	float rot[4];
+	float tangent[3];
+	float rotvec[3];
+	float reserved[2];
+} cb200_track_record;
+/* object i's records: table[offset, offset + count); count 0: not tracked */
+typedef struct cb200_track_span {
+	int offset, count, flags;
+} cb200_track_span;
+/* Host only: validates keys[0, n) with flags (the rejections above) and writes n records to out.  cudaErrorInvalidValue, out
+ * untouched, on a rejection or a null pointer. */
+CB200_API int cb200_track_prepare(const cb200_track_key* keys, int n, int flags, cb200_track_record* out);
+/* cb200_update_grid_velocity_query_max_forces (impulses may be NULL: no report) where object i with spans[i].count > 0 moves on its
+ * track: records is the DEVICE table the spans index (prepared by cb200_track_prepare), spans a HOST array of n.  Allocates nothing.
+ * cudaErrorInvalidValue, nothing launched, for what that entry rejects, a null spans, a span with count < 0, count >
+ * CB200_MAX_TRACK_KEYS, offset < 0 or unknown flags, a tracked object with trans_vel, omega or dsdt set, or a null records. */
+CB200_API int cb200_update_grid_velocity_query_max_tracks(const cb200_config* cfg, int block_count, float* grid, cb200_partition partition, float dt, const cb200_collider* collider, const cb200_collision_object* objs, int n, const cb200_levelset* levelsets, int n_levelsets, const cb200_track_record* records, const cb200_track_span* spans, float time, float* max_vel, double* impulses, void* stream);
+
 /* clear_grid  mgmpm_kernels.cuh:106-115 via GridBuffer::reset  grid_buffer.cuh:32-35 */
 CB200_API int cb200_clear_grid(int block_count, float* grid, void* stream);
 
@@ -301,6 +346,14 @@ CB200_API int cb200_sim_clear_collider(cb200_sim* sim);
  * at the simulated time at the start of the sub-step.  Synchronises and re-captures the sub-step graphs; call it between
  * sub-steps.  Objects are scene input: a checkpoint does not store them, set them before cb200_sim_restore. */
 CB200_API int cb200_sim_set_collision_objects(cb200_sim* sim, const cb200_collision_object* objs, int n);
+/* Moves collision object `object` (an index into the list cb200_sim_set_collision_objects set) along keys[0, n) with flags (the
+ * semantics of cb200_track_key); n = 0 clears its track.  The simulator keeps the prepared keys of all its tracks, at most
+ * CB200_MAX_TRACK_KEYS together, on the device.  cudaErrorInvalidValue, nothing changed, for what cb200_track_prepare rejects, an
+ * object index outside the list, a tracked object with trans_vel, omega or dsdt set, or a total above CB200_MAX_TRACK_KEYS.
+ * The grid update, the MGSP carry predictor and the set-up predictor evaluate the track at the time they place objects at.  Resets
+ * the force report.  Synchronises and re-captures the sub-step graphs; call it between sub-steps.  Replacing the object list clears
+ * every track.  Tracks are scene input, as objects are: a checkpoint does not store them; under MGSP set the same on every rank. */
+CB200_API int cb200_sim_set_object_track(cb200_sim* sim, int object, const cb200_track_key* keys, int n, int flags);
 /* Registers a level set for CB200_SHAPE_LEVELSET objects and sinks: phi_host (ni nj nk floats of `header`) is uploaded, its lattice
  * prepared on the device (16 B per node, kept until cb200_sim_destroy or cb200_sim_clear_collision_levelsets) and its index written to
  * *id.  cudaErrorInvalidValue, nothing changed, for a bad header (as cb200_sdf_parse), a null pointer or a full registry

@@ -24,6 +24,12 @@ halves, with the grid update's kernel time and the device memory each adds, as -
 section 2.13) for the level-set floor, the analytic floor box and 4 and 16 analytic objects, with the grid update's kernel time.
 
     python tools/collider_bench.py --forces [--steps 50] [--warmup 10] [--rounds 3]
+
+--tracks compares, in alternating rounds, the analytic floor box and 4 and 16 analytic objects untracked against the same objects each
+on a smooth motion track (DESIGN.md section 2.14; a slow drift and turn, so that the scene stays the same), with the grid update's
+kernel time.
+
+    python tools/collider_bench.py --tracks [--steps 50] [--warmup 10] [--rounds 3]
 """
 import ctypes as C
 import argparse
@@ -63,7 +69,7 @@ def run(scene, field, args, stream, objs=None, forces=False):
     sim.profile_read()
     sim.profile(False)
     kernel_ms = None
-    if args.objects or args.levelsets or args.forces:
+    if args.objects or args.levelsets or args.forces or args.tracks:
         from torch.profiler import ProfilerActivity, profile
         sim.sync()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -91,6 +97,22 @@ def object_sets(top):
         else:
             extra.append(objects.plane((0.5, 0.1 - 0.005 * i, 0.5), (0.0, 1.0, 0.0), type="slip"))
     return {"analytic_floor": [floor], "objects4": [floor] + extra[:3], "objects16": [floor] + extra}
+
+
+def tracked(objs):
+    """copies of objs, each on a three-key smooth track from its rest pose (a drift of 1e-3 and a turn of 0.01 rad per second);
+    omega, the one velocity object_sets gives, is dropped (a tracked object moves only along its track)"""
+    from claymore_b200 import objects
+    from claymore_b200._capi import CollisionObject
+    out = []
+    for o in objs:
+        c = CollisionObject.from_buffer_copy(o)
+        c.omega[:] = [0.0, 0.0, 0.0]
+        p = list(c.trans)
+        c.track = objects.track([(0.0, p, (1, 0, 0, 0)), (1.0, [p[0], p[1] + 1e-3, p[2]], (0.99999, 0.0, 0.005, 0.0)),
+                                 (2.0, [p[0] + 1e-3, p[1] + 1e-3, p[2]], (0.99995, 0.0, 0.01, 0.0))], "smooth")
+        out.append(c)
+    return out
 
 
 def _level_set(phi, h):
@@ -135,6 +157,7 @@ def main():
     ap.add_argument("--objects", action="store_true", help="also the analytic floor box, 4 and 16 analytic objects")
     ap.add_argument("--levelsets", action="store_true", help="also the analytic floor box, the floor as a level-set object and a dragon")
     ap.add_argument("--forces", action="store_true", help="the impulse report off and on: level-set floor, analytic floor, 4 and 16 objects")
+    ap.add_argument("--tracks", action="store_true", help="untracked against tracked: analytic floor, 4 and 16 objects")
     args = ap.parse_args()
 
     import torch
@@ -160,6 +183,14 @@ def main():
             for name, forces in (names if r % 2 == 0 else names[::-1]):
                 res = run(scene, field if name == "floor" else None, args, stream, sets.get(name), forces=forces)
                 print(json.dumps({"round": r, "collider": name, "forces": forces, "steps": args.steps, **res}), flush=True)
+        return
+    if args.tracks:
+        sets = object_sets(top)
+        names = [(n, t) for n in sorted(sets) for t in (False, True)]
+        for r in range(args.rounds):
+            for name, tr in (names if r % 2 == 0 else names[::-1]):
+                res = run(scene, None, args, stream, tracked(sets[name]) if tr else sets[name])
+                print(json.dumps({"round": r, "collider": name, "tracks": tr, "steps": args.steps, **res}), flush=True)
         return
     names = ["floor", "none"] + sorted(sets)
     for r in range(args.rounds):
