@@ -1141,6 +1141,14 @@ int cb200_sim_init_model(cb200_sim* s, int material, const float* positions_host
 	});
 }
 
+static int recapture(cb200_sim* s);
+// make_g2p2g_args passes each model's parameters by value, so the sub-step graphs hold the ones they were captured with: a setter
+// called between sub-steps re-captures them (after the sub-steps issued before it), and the change applies from the next sub-step
+// in graph and stream mode alike.  The clock and the force report are kept.
+static int params_changed(cb200_sim* s) {
+	CK(cudaStreamSynchronize(s->stream));
+	return recapture(s);
+}
 static int set_elastic(cb200_sim* s, int model, int material, float rho, float vol, float ym, float pr) {
 	if(!s || model < 0 || model >= (int) s->models.size() || s->models[model].material != material) return (int) cudaErrorInvalidValue;
 	for(int i = 0; i < 2; ++i) {
@@ -1154,8 +1162,14 @@ static int set_elastic(cb200_sim* s, int model, int material, float rho, float v
 	return 0;
 }
 // ParticleBuffer<FIXED_COROTATED>::update_parameters  particle_buffer.cuh:178-184
-int cb200_sim_update_fr_parameters(cb200_sim* s, int model, float rho, float vol, float ym, float pr) { return set_elastic(s, model, CB200_FIXED_COROTATED, rho, vol, ym, pr); }
-int cb200_sim_update_sand_parameters(cb200_sim* s, int model, float rho, float vol, float ym, float pr) { return set_elastic(s, model, CB200_SAND, rho, vol, ym, pr); }
+int cb200_sim_update_fr_parameters(cb200_sim* s, int model, float rho, float vol, float ym, float pr) {
+	CK(set_elastic(s, model, CB200_FIXED_COROTATED, rho, vol, ym, pr));
+	return params_changed(s);
+}
+int cb200_sim_update_sand_parameters(cb200_sim* s, int model, float rho, float vol, float ym, float pr) {
+	CK(set_elastic(s, model, CB200_SAND, rho, vol, ym, pr));
+	return params_changed(s);
+}
 // ParticleBuffer<J_FLUID>::update_parameters  particle_buffer.cuh:152-159
 int cb200_sim_update_j_fluid_parameters(cb200_sim* s, int model, float rho, float vol, float bulk, float gamma, float visc) {
 	if(!s || model < 0 || model >= (int) s->models.size() || s->models[model].material != CB200_J_FLUID) return (int) cudaErrorInvalidValue;
@@ -1168,7 +1182,7 @@ int cb200_sim_update_j_fluid_parameters(cb200_sim* s, int model, float rho, floa
 		pb.gamma = gamma;
 		pb.viscosity = visc;
 	}
-	return 0;
+	return params_changed(s);
 }
 // ParticleBuffer<NACC>::update_parameters  particle_buffer.cuh:250-259
 int cb200_sim_update_nacc_parameters(cb200_sim* s, int model, float rho, float vol, float ym, float pr, float beta, float xi) {
@@ -1180,7 +1194,7 @@ int cb200_sim_update_nacc_parameters(cb200_sim* s, int model, float rho, float v
 		pb.beta = beta;
 		pb.xi = xi;
 	}
-	return 0;
+	return params_changed(s);
 }
 
 // register_blocks_kernel over the (lo, span) ring of the first pbc blocks of partition p; returns p's new block count in *out
@@ -1481,7 +1495,8 @@ int cb200_sim_grid(cb200_sim* s, float* grid_host, int capacity_blocks, int* n_o
 }
 long long cb200_sim_launch_count(cb200_sim* s) { return s ? s->launches : 0; }
 
-// The sub-step graphs hold the grid-update and carry launches of the collider and object state they were captured with: drop them and,
+// The sub-step graphs hold the grid-update and carry launches of the collider and object state they were captured with, and the
+// g2p2g launches of the material parameters: drop them and,
 // once set up, instantiate both roll parities again right away (never later, while an MGSP peer may be waiting on this rank).
 static int recapture(cb200_sim* s) {
 	drop_graphs(s);

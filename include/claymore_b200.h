@@ -300,7 +300,11 @@ CB200_API int cb200_sim_create(const cb200_sim_desc* desc, void* stream, cb200_s
 CB200_API int cb200_sim_destroy(cb200_sim* sim);
 /* GmpmSimulator::init_model<M>(positions, v0)  gmpm_simulator.cuh:168-209; positions: HOST float[3*n] */
 CB200_API int cb200_sim_init_model(cb200_sim* sim, int material, const float* positions_host, int n, const float* v0_host3, int* model_id);
-/* update_{fr,j_fluid,nacc}_parameters  gmpm_simulator.cuh:211-254 (sand: defaults as in gmpm.cu:134-135, or this call) */
+/* update_{fr,j_fluid,nacc}_parameters  gmpm_simulator.cuh:211-254 (sand: defaults as in gmpm.cu:134-135, or this call).
+ * Each may also be called between sub-steps of a set-up simulator: the change applies from the next sub-step, in graph and
+ * stream mode alike (the call synchronises and re-captures the sub-step graphs).  The clock and the force report are kept.
+ * Under MGSP every rank that holds the model must make the same call before its next step.  A wrong material for the model,
+ * a model index out of range or no model at all is refused (cudaErrorInvalidValue) and changes nothing. */
 CB200_API int cb200_sim_update_fr_parameters(cb200_sim* sim, int model, float rho, float vol, float youngs, float poisson);
 CB200_API int cb200_sim_update_sand_parameters(cb200_sim* sim, int model, float rho, float vol, float youngs, float poisson);
 CB200_API int cb200_sim_update_j_fluid_parameters(cb200_sim* sim, int model, float rho, float vol, float bulk, float gamma, float viscosity);

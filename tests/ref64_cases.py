@@ -4,7 +4,8 @@ A case is dict(domain_bits, models=[dict(material, pos, v0, rho, vol, args)], dt
 are the material setter's arguments after (rho, vol); ``steps`` the sub-steps k at which one sub-step is checked.  A case with
 a ``collider`` = dict(field=(kind, *args), type, friction, rot_mat, trans, trans_vel, omega, dsdt, scale) has a signed-distance
 collider (collider_field, collider_struct; the other keys default to SignedDistanceGrid's).  A case with ``objects`` has
-analytic collision objects after it (OBJECT_CASES, object_structs).
+analytic collision objects after it (OBJECT_CASES, object_structs).  A case with ``updates`` changes material parameters between
+sub-steps (_updated).
 """
 import numpy as np
 
@@ -143,6 +144,65 @@ def _overflow(material, x_full):
 NACC_SOFT = (0.12, 0.3, 2.0, 0.079)
 
 
+# ---- material parameters changed between sub-steps ------------------------------------------------------------------------
+# A case with ``updates`` = {k: [(scene model, rho, vol, args), ...]} calls the model's material setter right before sub-step k
+# (ref64_checks.apply_updates), args in SETTER order after (rho, vol).  Sub-steps k and k + 1 are checked: the two roll parities
+# read the parameters of one particle buffer each.  Each update changes one parameter group, on deformed material, so that one
+# stale field cannot hide behind another (test_params_cpu.py: ref64 with the parameters before the update is off by 10x its bound).
+def _updated(case, updates, steps):
+    return dict(case, updates=updates, steps=sorted(set(steps) | {j for k in updates for j in (k, k + 1)}))
+
+
+def _fc_floor_params():
+    c = _floor(FIXED_COROTATED, [])
+    v = c["models"][0]["vol"]
+    return _updated(c, {20: [(0, 2.5e3, v, (5e3, 0.4))],              # rho: the mass
+                        23: [(0, 5e3, v / 2, (5e3, 0.4))],            # vol x 0.5, rho x 2: the same mass, half the stress volume
+                        26: [(0, 5e3, v / 2, (2e4, 0.4))],            # E
+                        29: [(0, 5e3, v / 2, (2e4, 0.25))]}, [])      # nu
+
+
+def _fluid_floor_params():
+    c = _floor(J_FLUID, [])
+    v = c["models"][0]["vol"]
+    return _updated(c, {20: [(0, 1e3, v, (1e5, 7.15, 0.01))],         # bulk
+                        23: [(0, 1e3, v, (1e5, 3.0, 0.01))],          # gamma
+                        26: [(0, 1e3, v, (1e5, 3.0, 10.0))],          # viscosity
+                        29: [(0, 1.5e3, v, (1e5, 3.0, 10.0))]}, [])   # rho
+
+
+def _fluid_clamp_params():
+    """fluid_clamp with its viscosity raised at sub-step 1, in the slam.  A change of bulk, gamma or rho there leaves the FP32
+    oracle's sub-step 2 within a few percent of the bounds or over them (F, lost particles), and so do the sub-steps after 2
+    without a change; those groups are changed on fluid_floor_params."""
+    c = CASES["fluid_clamp"]
+    return _updated(c, {1: [(0, 1e3, c["models"][0]["vol"], (4e4, 7.15, 2.0))]}, [])
+
+
+def _sand_floor_params():
+    c = CASES["sand_floor"]
+    v = c["models"][0]["vol"]
+    return _updated(c, {56: [(0, 1e3, v, (2e4, 0.4))], 59: [(0, 1e3, v, (2e4, 0.25))]}, [])   # E, nu; ~100 particles on the yield branch
+
+
+def _nacc_shear_params():
+    c = CASES["nacc_shear"]
+    v = c["models"][0]["vol"]
+    ups = {}
+    for k, args in ((4, (5e3, 0.4, 2.0, 0.8)), (7, (5e3, 0.4, 2.0, 0.3)), (10, (2e4, 0.4, 2.0, 0.3)), (13, (2e4, 0.25, 2.0, 0.3))):   # beta, xi, E, nu
+        ups[k] = [(0, 1e3, v, args), (1, 1e3, v, args)]
+    return _updated(c, ups, [])
+
+
+def _multi_model_params():
+    """multi_model_8 with rho changes to the second fixed-corotated model, the second fluid and the NACC model only: each update
+    must reach its own slot of its material's g2p2g launch."""
+    c = CASES["multi_model_8"]
+    m = c["models"]
+    return _updated(c, {1: [(1, 1e3, m[1]["vol"], m[1]["args"])],
+                        2: [(4, 1.6e3, m[4]["vol"], m[4]["args"]), (6, 500.0, m[6]["vol"], m[6]["args"])]}, [0, 3])
+
+
 CASES = {
     "fc_cube": _cube(FIXED_COROTATED, steps=[0, 3]),
     "fluid_cube": _cube(J_FLUID, steps=[0, 3]),
@@ -191,6 +251,15 @@ CASES = {
                                  model(NACC, box(1.0 / 64, (24, 26, 24), (36, 32, 36)), (-2.0, 0.01, 0.0), 1.0 / 64, args=NACC_SOFT)], [4, 7],
                              max_near_branch=0.25),
 }
+# parameter changes between sub-steps: odd and even update steps, each checked with the sub-step after it
+CASES.update({
+    "fc_floor_params": _fc_floor_params(),
+    "fluid_floor_params": _fluid_floor_params(),
+    "fluid_clamp_params": _fluid_clamp_params(),
+    "sand_floor_params": _sand_floor_params(),
+    "nacc_shear_params": _nacc_shear_params(),
+    "multi_model_8_params": _multi_model_params(),
+})
 
 
 class OracleClock:

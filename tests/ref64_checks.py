@@ -96,12 +96,32 @@ def check_counts(r, before, after, max_ppc, label):
                                 f"({lost} lost, {len(b) - lost - kept} dropped from {n_over} cells over max_ppc = {max_ppc})")
 
 
-def ref_models(case, states):
-    return [dict(material=m["material"], params=S.ref_params(m), state=s) for m, s in zip(case["models"], states)]
+def ref_models(case, states, models=None):
+    """ref64's models of the case's particle ``states``, with the parameters of ``models`` (current_models) or else the case's."""
+    return [dict(material=m["material"], params=S.ref_params(m), state=s) for m, s in zip(case["models"] if models is None else models, states)]
 
 
-def rank_models(parts, states):
-    return [dict(model=p["model"], material=p["material"], params=S.ref_params(p), state=s) for p, s in zip(parts, states)]
+def rank_models(parts, states, models=None):
+    """ref64_mgsp's models of a rank's ``parts``, with the parameters of the scene models ``models`` (current_models) or else the parts'."""
+    return [dict(model=p["model"], material=p["material"], params=S.ref_params(p if models is None else models[p["model"]]), state=s)
+            for p, s in zip(parts, states)]
+
+
+# ---- parameter changes between sub-steps (case["updates"], ref64_cases) -------------------------------------------------------
+def current_models(case):
+    """The case's models as set up; apply_updates keeps their rho, vol and args at the parameters in effect."""
+    return [dict(m) for m in case["models"]]
+
+
+def apply_updates(case, k, models, call):
+    """The case's updates before sub-step k: call(scene model, material setter name, rho, vol, args) for each, and ``models``
+    (current_models) follows.  Every update step k and k + 1 must be checked steps: the two roll parities read the parameters of
+    pb[0] and pb[1] in turn."""
+    for mi, rho, vol, args in case.get("updates", {}).get(k, ()):
+        assert k >= 1 and k in case["steps"] and k + 1 in case["steps"], f"an update at sub-step {k} needs sub-steps {k} and {k + 1} checked"
+        m = models[mi]
+        call(mi, S.SETTER[m["material"]], rho, vol, tuple(args))
+        m.update(rho=rho, vol=vol, args=tuple(args))
 
 
 def new_counts():
@@ -158,12 +178,14 @@ def oracle_substep_check(ob, case, label):
     nm = len(case["models"])
     done = 0
     counts = new_counts()
+    models = current_models(case)
     for k in case["steps"]:
         clock.step(k - done)
+        apply_updates(case, k, models, lambda mi, setter, rho, vol, args: getattr(osim, setter)(mi, rho, vol, *args))
         t = np.float32(osim.sim_time) if ccol is not None or objs else 0.0
         _, nbc, _ = osim.block_counts()
         before = [osim.particle_state(i) for i in range(nm)]
-        r = ref64.substep(osim.cfg, ref_models(case, before), osim.active_keys()[:nbc], osim.grid(), osim.dt, case["dt"], clock.time_left(), ccol, t,
+        r = ref64.substep(osim.cfg, ref_models(case, before, models), osim.active_keys()[:nbc], osim.grid(), osim.dt, case["dt"], clock.time_left(), ccol, t,
                           objects=objs)
         clock.step(1)
         done = k + 1
@@ -174,23 +196,28 @@ def oracle_substep_check(ob, case, label):
     collider_report(case, label, counts)
 
 
-def engine_substep_check(case, use_graph, label):
+def engine_substep_check(case, use_graph, label, sim=None, before_step=None, start=0):
     """The step driver through case['steps'], the boundaries placed at the simulated time the engine reports before each
-    checked sub-step: error bits, the clock, particles and cells, dt."""
-    sim = S.build_engine(case, use_graph=use_graph)
+    checked sub-step: error bits, the clock, particles and cells, dt.  ``sim``: a simulator of the case, set up, at sub-step ``start``
+    (default: S.build_engine, at 0); ``before_step(sim, k)`` runs after the updates of each checked sub-step k, right before the state is read."""
+    sim = S.build_engine(case, use_graph=use_graph) if sim is None else sim
     ccol, objs = S.ref_collider(case), S.ref_objects(case)
     nm = len(case["models"])
-    done = 0
+    done = start
     expect = 0   # a particle that moves more than one cell (quirk #4) or leaves its block's neighbourhood is flagged lost,
     #              a cell that gets more than max_ppc particles in g2p2g sets the overflow bit
     counts = new_counts()
+    models = current_models(case)
     for k in case["steps"]:
         sim.step(k - done)
+        apply_updates(case, k, models, lambda mi, setter, rho, vol, args: getattr(sim, setter)(rho, vol, *args, model=mi))
+        if before_step is not None:
+            before_step(sim, k)
         st = sim.stats()
         assert st.error == expect, f"{label}: error bits {st.error} at sub-step {k}, expected {expect}"
         keys, grid, before = engine_state(sim, nm)
         t = sim.sim_time()
-        r = ref64.substep(sim.cfg, ref_models(case, before), keys, grid, st.dt, case["dt"], S.engine_time_left(sim, case), ccol, np.float32(t),
+        r = ref64.substep(sim.cfg, ref_models(case, before, models), keys, grid, st.dt, case["dt"], S.engine_time_left(sim, case), ccol, np.float32(t),
                           objects=objs)
         sim.step(1)
         done = k + 1
@@ -242,6 +269,14 @@ def build_ranks(case, parts, use_graph, halo_cap=0, max_blocks=6000):
     return sims
 
 
+def rank_update(sims, parts, mi, setter, rho, vol, args):
+    """A parameter change of scene model ``mi`` on every rank that holds it (its local model id is its index in the rank's parts)."""
+    for s, ps in zip(sims, parts):
+        for i, p in enumerate(ps):
+            if p["model"] == mi:
+                getattr(s, setter)(rho, vol, *args, model=i)
+
+
 def rank_errors(sims, expect, label):
     got = [s.stats().error for s in sims]
     assert not any(e & ERR_HALO_MAP for e in got), f"{label}: kErrHaloMap on a rank ({got})"
@@ -265,14 +300,16 @@ def mgsp_substep_check(case, parts, use_graph, label):
     check_report(M.compare(cfg, ref, [dict(zip(("keys", "grid"), rank_grid(s))) for s in sims], RASTER_KAPPA, 0.0, []), f"{label} set-up")
     done, near_branch, near, tainted = 0, 0, 0, 0
     f_allow = [F_ALLOW[m["material"]] for m in case["models"]]
+    models = current_models(case)
     for k in case["steps"]:
         if k > done:
             on_threads(sims, lambda s: (s.step(k - done), s.sync()))
+        apply_updates(case, k, models, lambda mi, setter, rho, vol, args: rank_update(sims, parts, mi, setter, rho, vol, args))
         rank_errors(sims, expect, f"{label} at sub-step {k}")
         ranks = []
         for s, ps in zip(sims, parts):
             keys, grid = rank_grid(s)
-            ranks.append(dict(keys=keys, grid=grid, models=rank_models(ps, [s.particle_state(i) for i in range(len(ps))])))
+            ranks.append(dict(keys=keys, grid=grid, models=rank_models(ps, [s.particle_state(i) for i in range(len(ps))], models)))
         dts = [s.stats().dt for s in sims]
         M.check_dts(dts, dts[0], 0)
         t = sims[0].sim_time()

@@ -67,6 +67,8 @@ MATRIX = {
     "walls-2x": (S.CASES["walls"], 2, "x", dict(owners=2)),
     "high_faces-2x": (_high_faces_by_group(), 2, "x", dict(owners=2)),
     "multi_model_8-2global": (S.CASES["multi_model_8"], 2, "global", dict(owners=2, models_differ=True)),
+    # rho changes between sub-steps on the ranks that hold the model (ref64_checks.rank_update); a rank without it makes no call
+    "multi_model_8_params-2global": (S.CASES["multi_model_8_params"], 2, "global", dict(owners=2, models_differ=True)),
     "block_sizes-2x": (S.CASES["block_sizes"], 2, "x", dict(owners=2, models_differ=True)),
     "slabs_into_each_other-2global": (_slabs_into_each_other(), 2, "global", dict(owners=2, fresh=True)),
     "movers-2x": (_movers(), 2, "x", dict(owners=2, fresh=True)),
